@@ -161,7 +161,7 @@ def run(a, ClockSampler) -> dict:
         "config": {"model": f"llama-{a.model}", "global_batch": a.batch * world, "per_worker_batch": a.batch,
                    "micro_batch": a.micro_batch, "grad_accum": accum, "seq_len": a.seq, "parallelism": f"diloco{world}x1",
                    "local_steps": H, "outer_steps_in_timed_window": 1 if H <= total_steps and H > a.warmup else 0},
-        "notes": {"entry": "open_diloco.train_diloco_torch.main (unmodified, baseline/_ref)", "l2": "per-step working set >> 126 MB L2",
+        "notes": {"entry": "open_diloco.train_diloco_torch.main (unmodified, baseline/_ref)", "l2": "per-step working set >> 50 MB L2",
                   "inner_opt": "AdamW lr4e-4 wd0.1 b(0.9,0.95) clip1.0 cosine(1000,88000)", "outer_opt": "SGD lr0.7 m0.9 nesterov"},
         "tokens_per_sec_per_gpu": value / world,
         "clocks": marks.get("clocks"),

@@ -45,12 +45,14 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--compression", default=None)
     ap.add_argument("--no-fused-collective", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write what the last timed step computed to DIR/<name>.npy (rank 0)")
     return ap.parse_args()
 
 
 # --------------------------------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md 'clocks' line)."""
+    """nvidia-smi sampling DURING the timed region (SM clock, power draw, throttle reasons)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -104,6 +106,26 @@ def baseline_number():
         return float(v) if v else None
     except Exception:
         return None
+
+
+# --------------------------------------------------------------------------------------------------- output dump
+DUMP_SAMPLE = 4 << 20          # fp32 parameters sampled for the dump (16 MB)
+
+
+def dump_outputs(out_dir: str, loss, model) -> None:
+    """What the timed path hands its caller after the last timed step: the loss it returned and the updated fp32
+    parameters (a fixed, seeded sample of the flat parameter vector when it is larger than DUMP_SAMPLE)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(loss.float().item())], dtype=np.float32))
+    flat = model.arena.master.detach().reshape(-1)
+    if flat.numel() > DUMP_SAMPLE:
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randint(flat.numel(), (DUMP_SAMPLE,), generator=g).sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "params.npy"), flat.float().cpu().numpy())
 
 
 # --------------------------------------------------------------------------------------------------- our arm
@@ -178,9 +200,11 @@ def run_ours(a) -> dict:
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
     for _ in range(a.steps):
-        tr.train_step(it)
+        last_loss = tr.train_step(it)
     ev1.record()
     sync()
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, last_loss, model)
     my_ms = ev0.elapsed_time(ev1)
     dev_ms = max_over_ranks(my_ms)
     per_rank_ms = [my_ms / a.steps]
@@ -253,7 +277,7 @@ def run_ours(a) -> dict:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    sustained = peaks.get("bf16_tflops_sustained", 1400.0)
+    sustained = peaks.get("bf16_tflops_sustained")
     out = {
         "metric": "tokens_per_sec (DiLoCo inner steps incl. one outer sync in the timed window)",
         "value": value, "unit": "tokens/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
@@ -264,18 +288,18 @@ def run_ours(a) -> dict:
         "config": {"model": f"llama-{a.model}", "global_batch": a.batch * world, "per_worker_batch": a.batch,
                    "micro_batch": a.micro_batch, "grad_accum": accum, "seq_len": a.seq, "parallelism": f"diloco{world}x1",
                    "local_steps": H, "outer_steps_in_timed_window": outer_in_window},
-        "notes": {"l2": "per-step working set (>10 GB activations + 3.4 GB optimizer state) >> 126 MB L2; no flush needed",
+        "notes": {"l2": "per-step working set (>10 GB activations + 3.4 GB optimizer state) >> 50 MB L2; no flush needed",
                   "inner_opt": "AdamW lr4e-4 wd0.1 b(0.9,0.95) clip1.0 cosine(1000,88000)", "outer_opt": "SGD lr0.7 m0.9 nesterov",
                   "entry": "opendiloco_b200.trainer.DiLoCoTrainer.train_step"},
         "per_rank_ms_per_step": per_rank_ms, "params_equal_across_ranks": params_equal,
         "tokens_per_sec_per_gpu": value / world,
-        "mfu_vs_measured_sustained": (value / world) * flops_tok / (sustained * 1e12),
+        "mfu_vs_measured_sustained": (value / world) * flops_tok / (sustained * 1e12) if sustained else None,
         "outer_sync_ms": outer_ms, "outer_sync_with_handshake_ms": outer_hs_ms,
         "outer_sync_eff_GBps": (nparam * 4 / (outer_ms / 1e3) / 1e9) if outer_ms else None,
         "outer_fused_collective": bool(getattr(tr.optimizer, "_fused", None)) if tr.is_diloco else None,
         "outer_kernel": (("sharded in-place (ZeRO-1 outer optimizer over NVLS)" if tr.optimizer._fused.sharded else "replicated update")
                          if tr.is_diloco and getattr(tr.optimizer, "_fused", None) else None),
-        "clocks": clocks, "e2e": e2e, "gpu_launches": launches,
+        "gpu": torch.cuda.get_device_name(dev), "clocks": clocks, "e2e": e2e, "gpu_launches": launches,
     }
     if world > 1:
         dist.destroy_process_group()
@@ -306,6 +330,8 @@ def run_reference(a) -> dict:
 
 def main():
     a = parse_args()
+    if a.dump_outputs and a.impl != "ours":
+        sys.exit("--dump-outputs is implemented for --impl ours only")
     out = run_ours(a) if a.impl == "ours" else run_reference(a)
     if out:
         print(json.dumps(out), flush=True)

@@ -1,4 +1,4 @@
-"""opendiloco_b200 - a B200-native (sm_100a) DiLoCo training framework with the capabilities of OpenDiLoCo.
+"""opendiloco_b200 - an H100-native (sm_90a) DiLoCo training framework with the capabilities of OpenDiLoCo.
 
     from opendiloco_b200 import LlamaForCausalLM, LlamaConfig, DiLoCoOptimizer, DiLoCoTrainer
 """

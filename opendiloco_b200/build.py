@@ -1,15 +1,15 @@
-"""In-tree build of the sm_100a native libraries.
+"""In-tree build of the sm_90a native libraries.
 
     python -m opendiloco_b200.build            # build everything that is stale
     python -m opendiloco_b200.build --force    # rebuild
 
-Two shared objects are produced next to this file (git-ignored, but shipped to the GPU box by gpurun):
+Two shared objects are produced next to this file (git-ignored build products):
 
-  * ``_C/libodb200.so``   - every CUDA kernel (nvcc, ``-gencode arch=compute_100a,code=sm_100a -lineinfo``),
+  * ``_C/libodb200.so``   - every CUDA kernel (nvcc, ``-gencode arch=compute_90a,code=sm_90a -lineinfo``),
                             plain C ABI, loaded with ctypes (raw device pointers + stream handles, no pybind).
   * ``_C/libodbhost.so``  - host runtime in C++17 (safetensors reader, synthetic-token prefetcher, TCP rendezvous).
 
-nvcc cross-compiles without a GPU, so this is also the driver's "does it build" check (``__graft_entry__.build``).
+nvcc cross-compiles without a GPU, so the libraries can be built on a machine without one (``__graft_entry__.build``).
 """
 from __future__ import annotations
 
@@ -31,7 +31,7 @@ NVCC = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nv
 CXX = os.environ.get("CXX") or shutil.which("g++") or "g++"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "--expt-extended-lambda",
     "-Xcompiler", "-fPIC,-fvisibility=hidden",
@@ -102,7 +102,7 @@ def build_cuda(force: bool = False, verbose: bool = False) -> Path:
         results = list(ex.map(compile_one, cu))
     objs = [o for o, _ in results]
     if force or any(c for _, c in results) or not target.exists():
-        _run([NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(target), *map(str, objs),
+        _run([NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(target), *map(str, objs),
               "-Xcompiler", "-fPIC", "-cudart", "static", "-ldl", "-lpthread"])
     if verbose:
         for src in cu:

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels of opendiloco_b200.
+// Shared device helpers for the sm_90a kernels of opendiloco_b200.
 // Everything here is header-only; each .cu is compiled on its own into libodb200.so.
 #pragma once
 #include <cuda_runtime.h>
@@ -132,13 +132,11 @@ __device__ __forceinline__ float block_max(float v, float* sm) {
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // Every kernel of the micro-step raises `launch_dependents` on entry and executes `griddepcontrol.wait` before its first
 // global-memory access; launched with the programmatic-serialization attribute, the NEXT kernel's CTAs are scheduled as soon
-// as SM resources free up and run their prologue (barrier init, TMEM allocation, tensor-map prefetch, index math) while the
+// as SM resources free up and run their prologue (barrier init, tensor-map prefetch, index math) while the
 // previous kernel drains its last wave.  The wait returns only when the previous grid has completed and flushed, so the
 // data dependence is exactly the stream order (also inside a captured CUDA graph, where the edge becomes programmatic).
-// MEASURED (round 2, B200, Llama-150M step inside the CUDA graph): 781.3 k tok/s without the attribute, 763.2 k with it
-// (-2.3 %, two runs each, same box) - the early-resident CTAs of the next kernel cost more than the overlapped prologues win
-// when every GEMM is a one-CTA-per-SM persistent kernel.  The attribute is therefore OFF by default (ODB_PDL=1 turns it on);
-// without it both instructions are no-ops and the launch is an ordinary one.
+// The attribute is OFF by default (ODB_PDL=1 turns it on); without it both instructions are no-ops and the launch is an
+// ordinary one.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
@@ -151,19 +149,30 @@ inline int pdl_enabled() {
   return v;
 }
 
+// cluster_x > 1: the grid is launched in clusters of cluster_x CTAs along x
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int cluster_x,
+                                      Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled();
+  attr[1].id = cudaLaunchAttributeClusterDimension;
+  attr[1].val.clusterDim.x = cluster_x;
+  attr[1].val.clusterDim.y = 1;
+  attr[1].val.clusterDim.z = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cfg.numAttrs = cluster_x > 1 ? 2 : 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  return launch_pdl_cluster(kernel, grid, block, smem, st, 1, static_cast<Args&&>(args)...);
 }
 
 inline int sm_count() {
@@ -171,7 +180,7 @@ inline int sm_count() {
   if (n == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }

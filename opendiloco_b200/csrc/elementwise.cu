@@ -1,4 +1,4 @@
-// Bandwidth-bound Llama kernels for sm_100a: embedding, (residual+)RMSNorm fwd/bwd, RoPE, SwiGLU.
+// Bandwidth-bound Llama kernels for sm_90a: embedding, (residual+)RMSNorm fwd/bwd, RoPE, SwiGLU.
 // All activations are bf16, all statistics / reductions fp32. 16-byte vector accesses everywhere;
 // one warp owns one token row so there is no block-level synchronisation on the forward path.
 //
@@ -126,10 +126,7 @@ __global__ void __launch_bounds__(256) rmsnorm_fwd_kernel(const __nv_bfloat16* x
 // dres (the gradient flowing down the residual stream) is updated in place: dres <- bf16(dres + dx).
 // If dres_in == nullptr the kernel writes dres = dx (used for the final norm, where no skip path exists).
 // Each warp keeps per-lane dw partial sums in registers across its rows; one smem reduction + atomics per CTA.
-// ncu: 59 % of the measured HBM copy bandwidth at h = 1024 (190 registers, one CTA per SM).  A column-owner rewrite (one
-// 8-column vector per thread, four rows in flight, row dots through shared memory, 126 registers) was measured in round 2
-// at 71 us against this kernel's 67 us per 32768 x 1024 call - the two block barriers per row group cost what the extra
-// occupancy bought - and was not kept.
+// 190 registers, one CTA per SM at h = 1024.
 template <int NCH, bool kRegAcc>
 __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy,
                                                           const __nv_bfloat16* __restrict__ x,

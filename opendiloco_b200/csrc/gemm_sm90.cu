@@ -1,0 +1,599 @@
+// wgmma / TMA / mbarrier GEMM family for sm_90a with fused Llama epilogues (SURVEY.md §2.5 K3, K4, K6, K7).
+//
+//   C[M,N] = A[M,K] * B[N,K]^T      bf16 operands, fp32 accumulation in registers
+//
+// One CTA per 128 x 256 output tile, 384 threads in three warpgroups:
+//   warpgroup 0    TMA producer (one thread): A tile 128x64, B tile 256x64 per stage (128-byte swizzle), mbarrier
+//                  full/empty ring of STAGES stages; gives its registers to the MMA warpgroups (setmaxnreg)
+//   warpgroups 1-2 MMA + epilogue: each issues wgmma m64n256k16 for its 64 rows of the tile (4 per 64-deep k-block),
+//                  keeps one wgmma group in flight, then runs the fused epilogue straight from the accumulator registers
+//
+// CL = 2 (odb_gemm2_*: forward projections with at least one wave of 256 x 256 tiles): a cluster of two CTAs computes a 256 x 256 tile,
+// the two m-halves of the same B tile.  Each CTA loads its own A and ONE half of B, multicast into both CTAs, so the B
+// traffic from L2 per CTA halves; a stage is refilled only when the MMA warpgroups of both CTAs have released it.
+//
+// Operand layouts (template flags, the shared-memory descriptor expresses both - no transposed copies are made):
+//   A_MN = false : A is [M, K] row-major (K-major)          A_MN = true : A is [K, M] row-major (MN-major, wgrad)
+//   B_MN = false : B is [N, K] row-major (K-major)          B_MN = true : B is [K, N] row-major (MN-major, dgrad)
+//
+// Epilogues:
+//   kStore   : plain bf16 store
+//   kSwiGLU  : B rows are [gate rows n0..n0+127 | up rows I+n0..I+n0+127]; writes gate|up (needed by backward) AND
+//              act = silu(gate) * up, so the SwiGLU kernel and its re-read of the 2I-wide tensor disappear
+//   kSwiGLUBwd: the GEMM result is d(act) of the down projection; the epilogue reads the matching gate / up values of
+//              C = gu [M, 2I] and turns them IN PLACE into d(gate) / d(up) - d(act) never reaches memory
+//   kRoPE    : C is the packed qkv buffer; 64-column chunks are heads; chunks below `rope_cols` are rotated with the
+//              HF rotate-half convention using fp32 cos/sin tables (position = row % S)
+//   kLCEFwd  : fused linear-cross-entropy forward.  The accumulator holds a tile of LM-head logits z; the epilogue turns
+//              it into shifted exponentials e = exp(z - c_row) (c_row = the row's label logit, so sum_v e >= 1 and
+//              loss_row = log sum_v e), writes the tile's row sums into one partial plane per 256-column tile and
+//              (training only) stores bf16(e).  Logits are never written.
+//   kLCEdX   : dgrad of the LM head on the shifted exponentials: out = rowscale * acc - g * W[label]
+//   kWgradAcc: fp32 reduce-add of the tile into dW (gradient accumulation across micro-batches + split-K over tokens)
+#include <stdlib.h>
+
+#include "common.cuh"
+#include "sm90_ptx.cuh"
+
+using namespace odb;
+using namespace sm90;
+
+namespace gemm {
+
+constexpr int BM = 128, BN = 256, BK = 64;
+constexpr int A_BYTES = BM * BK * 2;       // 16 KB
+constexpr int B_BYTES = BN * BK * 2;       // 32 KB
+constexpr int BOX_BYTES = 64 * 64 * 2;     // one 64 x 64 box of an MN-major operand
+constexpr int STAGES = 4;
+constexpr int THREADS = 384;
+constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 1024 /*align*/ + 256 /*barriers*/;
+constexpr int GROUP_M = 8;                 // rasterisation: 8 m-blocks x all n-blocks per super-block (L2 reuse of A and B)
+
+enum Epi { kStore = 0, kSwiGLU = 1, kRoPE = 2, kSwiGLUBwd = 3, kLCEFwd = 4, kLCEdX = 5, kWgradAcc = 6 };
+
+// group_m > 0: groups of group_m m-blocks x all n-blocks, m fastest inside a group (A and B tiles of a group stay in L2).
+// group_m == 0: n fastest over the whole problem - for a few n-blocks and a very deep K (the LM-head dX: 4 n-blocks,
+// K = vocabulary) the CTAs that share an A row-block then run side by side and A is fetched from HBM once.
+__device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int group_m, int& m_blk, int& n_blk) {
+  if (group_m == 0) {
+    m_blk = tile / num_n;
+    n_blk = tile - m_blk * num_n;
+    return;
+  }
+  const int group_size = group_m * num_n;
+  const int group_id = tile / group_size;
+  const int first_m = group_id * group_m;
+  const int gsz = (num_m - first_m) < group_m ? (num_m - first_m) : group_m;
+  const int r = tile - group_id * group_size;
+  m_blk = first_m + r % gsz;
+  n_blk = r / gsz;
+}
+
+struct Params {
+  int M, N, K;
+  int num_m, num_n;          // tile counts
+  int group_m;               // rasterisation (see tile_coords)
+  int splits, kb_per_split;  // split-K (kWgradAcc): work item = tile * splits + split
+  void* C; long long ldc;
+  void* aux; long long ldaux;
+  int I;                     // kSwiGLU / kSwiGLUBwd: intermediate size
+  int S, rope_cols;          // kRoPE: sequence length, number of leading columns that get rotated
+  const float* cos_t;        // [S, 32] fp32 (head_dim 64)
+  const float* sin_t;
+  int ks1, ks2;              // A split along K (A_MN = false) or along M (A_MN = true) into up to three tensors:
+                             // blocks [0,ks1) from A, [ks1,ks2) from A1, [ks2,..) from A2 (0/0 = single tensor)
+  const float* row_shift;    // kLCEFwd: c_row [M] (label logit; 0 for ignored rows)
+  float* partials;           // kLCEFwd: [num_n (+ num_n when want_sumsq)][M] partial row sums of exp(z - c)
+  int want_sumsq;            // kLCEFwd: also accumulate sum z^2 into the second half of partials
+  int store;                 // kLCEFwd: 1 = write bf16(e) to C (training) ; 0 = statistics only (evaluation)
+  const float* rowscale;     // kLCEdX: s_row [M] = gscale / sum_v e  (0 for ignored rows)
+  const long long* labels;   // kLCEdX: [M], < 0 = ignored
+  const float* gscale;       // kLCEdX: device scalar loss_scale / n_valid
+  const __nv_bfloat16* wlab; // kLCEdX: the LM-head weight [V, N] (row stride ldwlab) for the one-hot gather
+  long long ldwlab;
+};
+
+__device__ __forceinline__ void red_add_f2(float* p, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void st_bf2(void* p, float a, float b) { *reinterpret_cast<uint32_t*>(p) = f2_to_bf2(a, b); }
+__device__ __forceinline__ float2 ld_bf2(const void* p) { return bf2_to_f2(*reinterpret_cast<const uint32_t*>(p)); }
+
+template <int EPI, bool A_MN, bool B_MN, int CL>
+__device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_a, uint8_t* smem_b, uint64_t* full_bar,
+                                                 uint64_t* empty_bar, int wg, int m0, int n0, int n_blk, int kb0, int kb1);
+
+template <int EPI, bool A_MN, bool B_MN, int CL>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a1,
+            const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_b, Params p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + STAGES * A_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + STAGES * B_BYTES);
+  uint64_t* empty_bar = full_bar + STAGES;
+
+  pdl_launch_dependents();
+  static_assert(CL == 1 || (CL == 2 && !B_MN && !A_MN), "clusters share a K-major B tile");
+  const int wg = threadIdx.x >> 7;
+  const uint32_t rank = CL == 2 ? cluster_ctarank() : 0;
+  const int work = blockIdx.x / CL;
+  const int tile = work / p.splits, split = work - tile * p.splits;
+  int m_blk, n_blk;
+  tile_coords(tile, (p.num_m + CL - 1) / CL, p.num_n, p.group_m, m_blk, n_blk);
+  m_blk = m_blk * CL + (int)rank;                // CL = 2: this CTA's m-half of the cluster tile (may lie beyond M)
+  const int m0 = m_blk * BM, n0 = n_blk * BN;
+  const int num_k_total = (p.K + BK - 1) / BK;
+  const int kb0 = split * p.kb_per_split;
+  const int kb1 = min(num_k_total, kb0 + p.kb_per_split);
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2 * CL); }
+    fence_barrier_init();
+  }
+  if constexpr (CL == 2) cluster_sync();         // the peer multicasts into our stages and arrives on our barriers
+  else __syncthreads();
+  pdl_wait();
+
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      // which A tensor this tile reads (A_MN: the split is along M, so it is fixed per tile)
+      const CUtensorMap* ta_m = &tmap_a;
+      int am0 = m0;
+      if constexpr (A_MN) {
+        if (p.ks1 && m_blk >= p.ks2) { ta_m = &tmap_a2; am0 = m0 - p.ks2 * BM; }
+        else if (p.ks1 && m_blk >= p.ks1) { ta_m = &tmap_a1; am0 = m0 - p.ks1 * BM; }
+      }
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
+        uint8_t* sa = smem_a + stage * A_BYTES;
+        uint8_t* sb = smem_b + stage * B_BYTES;
+        if constexpr (A_MN) {       // [K rows, M cols]: two 64(m) x 64(k) boxes
+          tma_load_2d(sa, ta_m, &full_bar[stage], am0, kb * BK);
+          tma_load_2d(sa + BOX_BYTES, ta_m, &full_bar[stage], am0 + 64, kb * BK);
+        } else {
+          if (p.ks1 == 0 || kb < p.ks1) tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BK, m0);
+          else if (kb < p.ks2) tma_load_2d(sa, &tmap_a1, &full_bar[stage], (kb - p.ks1) * BK, m0);
+          else tma_load_2d(sa, &tmap_a2, &full_bar[stage], (kb - p.ks2) * BK, m0);
+        }
+        if constexpr (B_MN) {       // [K rows, N cols]: four 64(n) x 64(k) boxes
+#pragma unroll
+          for (int j = 0; j < 4; ++j) tma_load_2d(sb + j * BOX_BYTES, &tmap_b, &full_bar[stage], n0 + 64 * j, kb * BK);
+        } else if constexpr (CL == 2) {   // this CTA's half of B (gate | up for kSwiGLU) into both CTAs
+          const int b_row = EPI == kSwiGLU ? (rank == 0 ? n_blk * (BN / 2) : p.I + n_blk * (BN / 2)) : n0 + (int)rank * (BN / 2);
+          tma_load_2d_multicast(sb + rank * (B_BYTES / 2), &tmap_b, &full_bar[stage], kb * BK, b_row, (uint16_t)0x3);
+        } else if constexpr (EPI == kSwiGLU) {
+          const int g0 = n_blk * (BN / 2);
+          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BK, g0);
+          tma_load_2d(sb + B_BYTES / 2, &tmap_b, &full_bar[stage], kb * BK, p.I + g0);
+        } else {
+          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BK, n0);
+        }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else {
+    mma_and_epilogue<EPI, A_MN, B_MN, CL>(p, smem_a, smem_b, full_bar, empty_bar, wg, m0, n0, n_blk, kb0, kb1);
+  }
+  if constexpr (CL == 2) cluster_sync();         // no CTA leaves while its peer may still arrive on its barriers
+}
+
+template <int EPI, bool A_MN, bool B_MN, int CL>
+__device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_a, uint8_t* smem_b, uint64_t* full_bar,
+                                                 uint64_t* empty_bar, int wg, int m0, int n0, int n_blk, int kb0, int kb1) {
+  reg_alloc<232>();
+  const int cw = wg - 1;                         // this warpgroup's 64 rows of the tile
+  float acc[128];
+  {
+    int stage = 0, prev_stage = 0;
+    uint32_t phase = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_base = smem_u32(smem_a + stage * A_BYTES) + (A_MN ? cw * BOX_BYTES : cw * 64 * 128);
+      const uint32_t b_base = smem_u32(smem_b + stage * B_BYTES);
+      const uint64_t adesc = A_MN ? make_smem_desc_sw128(a_base, BOX_BYTES, 1024) : make_smem_desc_sw128(a_base, 16, 1024);
+      const uint64_t bdesc = B_MN ? make_smem_desc_sw128(b_base, BOX_BYTES, 1024) : make_smem_desc_sw128(b_base, 16, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        // K-major: 16 bf16 = 32 bytes further along the 128-byte swizzle row (+2 descriptor units);
+        // MN-major: 16 rows of 128 B further (+128 units)
+        wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc + (A_MN ? 128 : 2) * k, bdesc + (B_MN ? 128 : 2) * k,
+                                                     (kb > kb0 || k > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                           // the previous k-block's MMAs have retired: release its stage
+      if (kb > kb0 && (threadIdx.x & 127) == 0) {
+        mbar_arrive(&empty_bar[prev_stage]);
+        if constexpr (CL == 2) mbar_arrive_cluster(&empty_bar[prev_stage], cluster_ctarank() ^ 1);
+      }
+      prev_stage = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+  }
+
+  // -------------------------------------------------------------------- epilogue from the accumulator registers
+  // Fragment of m64n256: acc[4*i + 2*h + e] is row (16*warp + lane/4 + 8*h), column (8*i + 2*(lane%4) + e).
+  const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
+  const int rbase = m0 + cw * 64 + warp * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+
+  if constexpr (EPI == kStore || EPI == kRoPE) {
+    __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C);
+    const bool rope_tile = EPI == kRoPE && n0 < p.rope_cols;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rbase + 8 * h;
+      if (row >= p.M) continue;
+      if (EPI == kRoPE && rope_tile) {
+        const int pos = row % p.S;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          if (n0 + c * 64 >= p.rope_cols) continue;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int j = 8 * i + cq + e;
+              float& va = acc[4 * (8 * c + i) + 2 * h + e];
+              float& vb = acc[4 * (8 * c + i + 4) + 2 * h + e];
+              const float a = bf16_round(va), b = bf16_round(vb);   // match the unfused path: rotate the bf16 projection
+              const float cs = p.cos_t[(size_t)pos * 32 + j], sn = p.sin_t[(size_t)pos * 32 + j];
+              va = a * cs - b * sn;
+              vb = b * cs + a * sn;
+            }
+          }
+        }
+      }
+      __nv_bfloat16* crow = C + (size_t)row * p.ldc;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = n0 + 8 * i + cq;
+        if (col + 1 < p.N) st_bf2(crow + col, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+        else if (col < p.N) crow[col] = __float2bfloat16_rn(acc[4 * i + 2 * h]);
+      }
+    }
+  } else if constexpr (EPI == kSwiGLU) {
+    // tile columns [0,128) are gate columns g0.., [128,256) the matching up columns
+    __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.C);
+    __nv_bfloat16* act = reinterpret_cast<__nv_bfloat16*>(p.aux);
+    const int g0 = n_blk * (BN / 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rbase + 8 * h;
+      if (row >= p.M) continue;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const int col = g0 + 8 * i + cq;
+        if (col >= p.I) continue;                // I % 64 == 0: pairs never straddle the end
+        const float ga = acc[4 * i + 2 * h], gb = acc[4 * i + 2 * h + 1];
+        const float ua = acc[4 * (i + 16) + 2 * h], ub = acc[4 * (i + 16) + 2 * h + 1];
+        st_bf2(gu + (size_t)row * p.ldc + col, ga, gb);
+        st_bf2(gu + (size_t)row * p.ldc + p.I + col, ua, ub);
+        // the activation is computed from the bf16 values the backward will see
+        const float ga_r = bf16_round(ga), gb_r = bf16_round(gb), ua_r = bf16_round(ua), ub_r = bf16_round(ub);
+        st_bf2(act + (size_t)row * p.ldaux + col, ga_r * fast_sigmoid(ga_r) * ua_r, gb_r * fast_sigmoid(gb_r) * ub_r);
+      }
+    }
+  } else if constexpr (EPI == kSwiGLUBwd) {
+    __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.C);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rbase + 8 * h;
+      if (row >= p.M) continue;
+      __nv_bfloat16* grow = gu + (size_t)row * p.ldc;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = n0 + 8 * i + cq;
+        if (col >= p.I) continue;
+        const float2 g = ld_bf2(grow + col), u = ld_bf2(grow + p.I + col);
+        float og[2], ou[2];
+        const float gg[2] = {g.x, g.y}, uu[2] = {u.x, u.y};
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float dj = bf16_round(acc[4 * i + 2 * h + e]);   // the un-fused path rounds d(act) to bf16 first
+          const float sg = fast_sigmoid(gg[e]);
+          og[e] = dj * uu[e] * sg * (1.f + gg[e] * (1.f - sg));
+          ou[e] = dj * gg[e] * sg;
+        }
+        st_bf2(grow + col, og[0], og[1]);
+        st_bf2(grow + p.I + col, ou[0], ou[1]);
+      }
+    }
+  } else if constexpr (EPI == kLCEFwd) {
+    constexpr float L2E = 1.4426950408889634f;
+    __nv_bfloat16* E = reinterpret_cast<__nv_bfloat16*>(p.C);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rbase + 8 * h;
+      const bool row_ok = row < p.M;
+      const float shift = row_ok ? p.row_shift[row] * L2E : 0.f;
+      float psum = 0.f, psq = 0.f;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = n0 + 8 * i + cq;
+        float ev[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float v = acc[4 * i + 2 * h + e];
+          const bool ok = col + e < p.N;
+          // clamp: a row whose label is > 69 nats below its best logit would overflow the fp32 row sum otherwise
+          float x;
+          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(x) : "f"(fminf(fmaf(v, L2E, -shift), 100.f)));
+          ev[e] = ok ? x : 0.f;
+          psum += ev[e];
+          psq += ok ? v * v : 0.f;
+        }
+        if (p.store && row_ok) {
+          __nv_bfloat16* erow = E + (size_t)row * p.ldc;
+          if (col + 1 < p.N) st_bf2(erow + col, ev[0], ev[1]);
+          else if (col < p.N) erow[col] = __float2bfloat16_rn(ev[0]);
+        }
+      }
+      psum += __shfl_xor_sync(0xffffffffu, psum, 1);
+      psum += __shfl_xor_sync(0xffffffffu, psum, 2);
+      psq += __shfl_xor_sync(0xffffffffu, psq, 1);
+      psq += __shfl_xor_sync(0xffffffffu, psq, 2);
+      if (row_ok && (lane & 3) == 0) {
+        p.partials[(size_t)n_blk * p.M + row] = psum;
+        if (p.want_sumsq) p.partials[((size_t)p.num_n + n_blk) * p.M + row] = psq;
+      }
+    }
+  } else if constexpr (EPI == kLCEdX) {
+    __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rbase + 8 * h;
+      if (row >= p.M) continue;
+      const float rs = p.rowscale[row];
+      const long long y = p.labels[row];
+      const float g = y >= 0 ? *p.gscale : 0.f;
+      const __nv_bfloat16* wl = p.wlab + (size_t)(y >= 0 ? y : 0) * p.ldwlab;
+      __nv_bfloat16* crow = C + (size_t)row * p.ldc;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = n0 + 8 * i + cq;
+        if (col >= p.N) continue;                // N % 64 == 0
+        const float2 w = y >= 0 ? ld_bf2(wl + col) : make_float2(0.f, 0.f);
+        st_bf2(crow + col, fmaf(rs, acc[4 * i + 2 * h], -g * w.x), fmaf(rs, acc[4 * i + 2 * h + 1], -g * w.y));
+      }
+    }
+  } else if constexpr (EPI == kWgradAcc) {
+    float* dW = reinterpret_cast<float*>(p.C);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rbase + 8 * h;
+      if (row >= p.M) continue;
+      float* drow = dW + (size_t)row * p.ldc;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = n0 + 8 * i + cq;
+        if (col + 1 < p.N) red_add_f2(drow + col, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+        else if (col < p.N) atomicAdd(drow + col, acc[4 * i + 2 * h]);
+      }
+    }
+  }
+}
+
+struct ASplit {
+  const void* A1 = nullptr; const void* A2 = nullptr;
+  long long lda1 = 0, lda2 = 0;
+  int K0 = 0, K1 = 0, K2 = 0;      // extents of the three A tensors along the split dimension; K0 == 0 => no split
+};
+
+struct LceArgs {
+  const float* row_shift = nullptr; float* partials = nullptr; int want_sumsq = 0; int store = 1;
+  const float* rowscale = nullptr; const long long* labels = nullptr; const float* gscale = nullptr;
+  const void* wlab = nullptr; long long ldwlab = 0;
+};
+
+template <int EPI, bool A_MN, bool B_MN, int CL = 1>
+static int launch(const void* A, const void* B, void* C, void* aux, int M, int N, int K, long long lda, long long ldb,
+                  long long ldc, long long ldaux, int I, int S, int rope_cols, const float* cos_t, const float* sin_t,
+                  cudaStream_t st, const ASplit& sp = ASplit(), const LceArgs& lce = LceArgs()) {
+  CUtensorMap ta, ta1, ta2, tb;
+  int rc;
+  if (A_MN) {          // A given as [K rows, M cols] (possibly three tensors side by side along M)
+    if ((rc = make_tmap_2d(&ta, A, K, sp.K0 ? sp.K0 : M, lda * 2, 64, 64, 2))) return rc;
+  } else {
+    if ((rc = make_tmap_2d(&ta, A, M, sp.K0 ? sp.K0 : K, lda * 2, BM, BK, 2))) return rc;
+  }
+  ta1 = ta; ta2 = ta;
+  if (sp.K0) {
+    if (A_MN) {
+      if (sp.K1 && (rc = make_tmap_2d(&ta1, sp.A1, K, sp.K1, sp.lda1 * 2, 64, 64, 2))) return rc;
+      if (sp.K2 && (rc = make_tmap_2d(&ta2, sp.A2, K, sp.K2, sp.lda2 * 2, 64, 64, 2))) return rc;
+    } else {
+      if ((rc = make_tmap_2d(&ta1, sp.A1, M, sp.K1, sp.lda1 * 2, BM, BK, 2))) return rc;
+      if ((rc = make_tmap_2d(&ta2, sp.A2, M, sp.K2, sp.lda2 * 2, BM, BK, 2))) return rc;
+    }
+  }
+  if (B_MN) {
+    if ((rc = make_tmap_2d(&tb, B, K, N, ldb * 2, 64, 64, 2))) return rc;            // [K rows, N cols], 64 x 64 boxes
+  } else if (EPI == kSwiGLU) {
+    if ((rc = make_tmap_2d(&tb, B, 2 * I, K, ldb * 2, BN / 2, BK, 2))) return rc;
+  } else if (CL == 2) {
+    if ((rc = make_tmap_2d(&tb, B, N, K, ldb * 2, BN / 2, BK, 2))) return rc;      // each CTA of the pair loads one half
+  } else {
+    if ((rc = make_tmap_2d(&tb, B, N, K, ldb * 2, BN, BK, 2))) return rc;
+  }
+  Params p{};
+  p.M = M; p.N = N; p.K = K;
+  p.num_m = ceil_div(M, BM);
+  p.num_n = (EPI == kSwiGLU) ? ceil_div(I, BN / 2) : ceil_div(N, BN);
+  p.group_m = EPI == kLCEdX ? 0 : GROUP_M;
+  p.C = C; p.ldc = ldc; p.aux = aux; p.ldaux = ldaux;
+  p.I = I; p.S = S > 0 ? S : 1; p.rope_cols = rope_cols; p.cos_t = cos_t; p.sin_t = sin_t;
+  const int split_blk = A_MN ? BM : BK;
+  p.ks1 = sp.K0 ? sp.K0 / split_blk : 0;
+  p.ks2 = sp.K0 ? (sp.K0 + sp.K1) / split_blk : 0;
+  p.row_shift = lce.row_shift; p.partials = lce.partials; p.want_sumsq = lce.want_sumsq; p.store = lce.store;
+  p.rowscale = lce.rowscale; p.labels = lce.labels; p.gscale = lce.gscale;
+  p.wlab = (const __nv_bfloat16*)lce.wlab; p.ldwlab = lce.ldwlab;
+  const int tiles = p.num_m * p.num_n;
+  const int kb_total = ceil_div(K, BK);
+  p.splits = 1;
+  p.kb_per_split = kb_total;
+  if (EPI == kWgradAcc) {
+    // split-K over the tokens so that tiles * splits is close to a whole number of waves, >= 16 k-blocks per work item
+    int best = 1;
+    double best_eff = 0.0;
+    for (int s = 1; s <= 64 && kb_total / s >= 16; ++s) {
+      const int work = tiles * s;
+      const int waves = ceil_div(work, sm_count());
+      const double eff = (double)work / (double)(waves * sm_count());
+      if (eff > best_eff + 0.02) { best_eff = eff; best = s; }
+    }
+    p.kb_per_split = ceil_div(kb_total, best);
+    p.splits = ceil_div(kb_total, p.kb_per_split);   // no empty slices
+  }
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_kernel<EPI, A_MN, B_MN, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    if (e != cudaSuccess) return (int)e;
+    attr_set = true;
+  }
+  const int cluster_tiles = ceil_div(p.num_m, CL) * p.num_n;
+  launch_pdl_cluster(gemm_kernel<EPI, A_MN, B_MN, CL>, dim3(cluster_tiles * CL * p.splits), dim3(THREADS), SMEM_BYTES, st, CL,
+                     ta, ta1, ta2, tb, p);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : (int)e;
+}
+
+}  // namespace gemm
+
+// C[M,N] (bf16, row stride ldc) = A[M,K] (row stride lda) * B[N,K]^T (row stride ldb); strides in elements.
+ODB_EXPORT int odb_gemm_bf16_tn(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb,
+                                long long ldc, cudaStream_t st) {
+  if (K % 8 || lda % 8 || ldb % 8 || ldc % 8) return -1;
+  return gemm::launch<gemm::kStore, false, false>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st);
+}
+
+// as odb_gemm_bf16_tn, computed by clusters of two CTAs that share (multicast) the B tile
+ODB_EXPORT int odb_gemm2_bf16_tn(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb,
+                                 long long ldc, cudaStream_t st) {
+  if (K % 8 || lda % 8 || ldb % 8 || ldc % 8) return -1;
+  return gemm::launch<gemm::kStore, false, false, 2>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st);
+}
+
+// gu[M,2I] = x[M,K] * Wgu[2I,K]^T and act[M,I] = silu(gu[:, :I]) * gu[:, I:]   (I % 64 == 0)
+ODB_EXPORT int odb_gemm_swiglu(const void* X, const void* Wgu, void* gu, void* act, int M, int I, int K, cudaStream_t st) {
+  if (K % 8 || I % 64) return -1;
+  return gemm::launch<gemm::kSwiGLU, false, false>(X, Wgu, gu, act, M, 2 * I, K, K, K, 2 * I, I, I, 0, 0, nullptr, nullptr, st);
+}
+
+// as odb_gemm_swiglu, computed by clusters of two CTAs (one loads the gate half of B, the other the up half)
+ODB_EXPORT int odb_gemm2_swiglu(const void* X, const void* Wgu, void* gu, void* act, int M, int I, int K, cudaStream_t st) {
+  if (K % 8 || I % 64) return -1;
+  return gemm::launch<gemm::kSwiGLU, false, false, 2>(X, Wgu, gu, act, M, 2 * I, K, K, K, 2 * I, I, I, 0, 0, nullptr, nullptr, st);
+}
+
+// Backward of the SwiGLU MLP's middle: gu[M,2I] (gate|up, bf16) is replaced IN PLACE by d(gate)|d(up), where
+// d(act)[M,I] = dY[M,K] * WdT[I,K]^T is formed in registers only (I % 64 == 0).
+ODB_EXPORT int odb_gemm_swiglu_bwd(const void* dY, const void* WdT, void* gu, int M, int I, int K, long long lda, long long ldb,
+                                   cudaStream_t st) {
+  if (K % 8 || I % 64 || lda % 8 || ldb % 8) return -1;
+  return gemm::launch<gemm::kSwiGLUBwd, false, false>(dY, WdT, gu, nullptr, M, I, K, lda, ldb, 2 * I, 0, I, 0, 0, nullptr, nullptr, st);
+}
+
+// qkv[M,N] = x[M,K] * Wqkv[N,K]^T with RoPE applied to the first rope_cols columns (head_dim 64, position = row % S)
+ODB_EXPORT int odb_gemm_qkv_rope(const void* X, const void* W, void* qkv, int M, int N, int K, int S, int rope_cols,
+                                 const void* cos_t, const void* sin_t, cudaStream_t st) {
+  if (K % 8 || N % 64 || rope_cols % 64) return -1;
+  return gemm::launch<gemm::kRoPE, false, false>(X, W, qkv, nullptr, M, N, K, K, K, N, 0, 0, S, rope_cols, (const float*)cos_t,
+                                                 (const float*)sin_t, st);
+}
+
+// as odb_gemm_qkv_rope, computed by clusters of two CTAs that share (multicast) the B tile
+ODB_EXPORT int odb_gemm2_qkv_rope(const void* X, const void* W, void* qkv, int M, int N, int K, int S, int rope_cols,
+                                  const void* cos_t, const void* sin_t, cudaStream_t st) {
+  if (K % 8 || N % 64 || rope_cols % 64) return -1;
+  return gemm::launch<gemm::kRoPE, false, false, 2>(X, W, qkv, nullptr, M, N, K, K, K, N, 0, 0, S, rope_cols, (const float*)cos_t,
+                                                    (const float*)sin_t, st);
+}
+
+// C[M,N] = [A0 | A1 | A2][M, K0+K1+K2] * B[N, K0+K1+K2]^T with the three A pieces read in place (K0, K1, K2 % 64 == 0)
+ODB_EXPORT int odb_gemm_bf16_tn_a3(const void* A0, const void* A1, const void* A2, long long lda0, long long lda1, long long lda2,
+                                   int K0, int K1, int K2, const void* B, void* C, int M, int N, long long ldb, long long ldc,
+                                   cudaStream_t st) {
+  if (K0 % 64 || K1 % 64 || K2 % 64 || K0 <= 0 || K1 <= 0 || K2 <= 0) return -1;
+  gemm::ASplit sp;
+  sp.A1 = A1; sp.A2 = A2; sp.lda1 = lda1; sp.lda2 = lda2; sp.K0 = K0; sp.K1 = K1; sp.K2 = K2;
+  return gemm::launch<gemm::kStore, false, false>(A0, B, C, nullptr, M, N, K0 + K1 + K2, lda0, ldb, ldc, 0, 0, 0, 0, nullptr,
+                                                  nullptr, st, sp);
+}
+
+// C[M,N] = A[M,K] * B[K,N] with B row-major (the dgrad dX = dY W on the forward [out, in] weight layout)
+ODB_EXPORT int odb_gemm_bf16_nn(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb,
+                                long long ldc, cudaStream_t st) {
+  if (K % 8 || N % 8 || lda % 8 || ldb % 8 || ldc % 8) return -1;
+  return gemm::launch<gemm::kStore, false, true>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st);
+}
+
+// as odb_gemm_bf16_tn_a3 with B = W[K0+K1+K2, N] in its forward layout (dgrad of the fused QKV projection)
+ODB_EXPORT int odb_gemm_bf16_nn_a3(const void* A0, const void* A1, const void* A2, long long lda0, long long lda1, long long lda2,
+                                   int K0, int K1, int K2, const void* B, void* C, int M, int N, long long ldb, long long ldc,
+                                   cudaStream_t st) {
+  if (K0 % 64 || K1 % 64 || K2 % 64 || K0 <= 0 || K1 <= 0 || K2 <= 0 || N % 8 || ldb % 8) return -1;
+  gemm::ASplit sp;
+  sp.A1 = A1; sp.A2 = A2; sp.lda1 = lda1; sp.lda2 = lda2; sp.K0 = K0; sp.K1 = K1; sp.K2 = K2;
+  return gemm::launch<gemm::kStore, false, true>(A0, B, C, nullptr, M, N, K0 + K1 + K2, lda0, ldb, ldc, 0, 0, 0, 0, nullptr,
+                                                 nullptr, st, sp);
+}
+
+// as odb_gemm_swiglu_bwd with the down-projection weight Wd[K, I] in its forward layout (MN-major B operand)
+ODB_EXPORT int odb_gemm_swiglu_bwd_nn(const void* dY, const void* Wd, void* gu, int M, int I, int K, long long lda, long long ldb,
+                                      cudaStream_t st) {
+  if (K % 8 || I % 64 || lda % 8 || ldb % 8) return -1;
+  return gemm::launch<gemm::kSwiGLUBwd, false, true>(dY, Wd, gu, nullptr, M, I, K, lda, ldb, 2 * I, 0, I, 0, 0, nullptr, nullptr, st);
+}
+
+// ---------------------------------------------------------------------------------------------------- fused linear-cross-entropy
+// E[M,V] = exp(X W^T - row_shift) (bf16, only when store) and the partial row sums of E (one plane per 256 vocabulary columns)
+ODB_EXPORT int odb_lce_fwd(const void* X, const void* W, void* E, int M, int V, int K, long long ldx, long long ldw, long long lde,
+                           const void* row_shift, void* partials, int want_sumsq, int store, cudaStream_t st) {
+  if (K % 8 || ldx % 8 || ldw % 8 || (store && (lde % 8 || !E))) return -1;
+  gemm::LceArgs a;
+  a.row_shift = (const float*)row_shift; a.partials = (float*)partials; a.want_sumsq = want_sumsq; a.store = store;
+  return gemm::launch<gemm::kLCEFwd, false, false>(X, W, E, nullptr, M, V, K, ldx, ldw, lde, 0, 0, 0, 0, nullptr, nullptr, st,
+                                                   gemm::ASplit(), a);
+}
+
+ODB_EXPORT int odb_lce_planes(int V) { return (V + gemm::BN - 1) / gemm::BN; }
+
+// dX[M,N] (bf16) = rowscale[M] * (E[M,V] * W[V,N]) - gscale * [label >= 0] * W[label]     (N % 64 == 0)
+ODB_EXPORT int odb_lce_dx(const void* E, const void* W, void* dX, int M, int N, int V, long long lde, long long ldw, long long ldd,
+                          const void* rowscale, const void* labels, const void* gscale, cudaStream_t st) {
+  if (V % 8 || N % 64 || lde % 8 || ldw % 8 || ldd % 8) return -1;
+  gemm::LceArgs a;
+  a.rowscale = (const float*)rowscale; a.labels = (const long long*)labels; a.gscale = (const float*)gscale;
+  a.wlab = W; a.ldwlab = ldw;
+  return gemm::launch<gemm::kLCEdX, false, true>(E, W, dX, nullptr, M, N, V, lde, ldw, ldd, 0, 0, 0, 0, nullptr, nullptr, st,
+                                                 gemm::ASplit(), a);
+}
+
+// ---------------------------------------------------------------------------------------------------- weight gradient
+// dW[N_out, K_out] (fp32, row stride ldw) += [dY0 | dY1 | dY2][T, N_out]^T * X[T, K_out]
+// Both operands are MN-major for the tensor core (the reduction index t is the slow memory dimension).  n1, n2: column
+// counts of the 2nd / 3rd dY tensors (0 = unused; then dY0 has all N_out columns); when used, every piece must be a
+// multiple of 256 columns.  T, N_out, K_out need no alignment beyond 8 elements (TMA clips).
+ODB_EXPORT int odb_wgrad_bf16(const void* dY0, const void* dY1, const void* dY2, long long ld0, long long ld1, long long ld2,
+                              int n0, int n1, int n2, const void* X, long long ldx, void* dW, long long ldw, int T, int K_out,
+                              cudaStream_t st) {
+  const int N_out = n0 + n1 + n2;
+  if ((n1 || n2) && (n0 % 256 || n1 % 256 || n2 % 256)) return -1;
+  if (ld0 % 8 || ldx % 8 || ldw % 4 || T <= 0) return -1;
+  gemm::ASplit sp;
+  if (n1 || n2) { sp.A1 = dY1; sp.A2 = dY2; sp.lda1 = ld1; sp.lda2 = ld2; sp.K0 = n0; sp.K1 = n1; sp.K2 = n2; }
+  return gemm::launch<gemm::kWgradAcc, true, true>(dY0, X, dW, nullptr, N_out, K_out, T, ld0, ldx, ldw, 0, 0, 0, 0, nullptr,
+                                                   nullptr, st, sp);
+}

@@ -201,7 +201,7 @@ ODB_EXPORT int odb_ce_fwd(const void* logits, const void* labels, int rows, int 
 }
 
 // =============================================================================================== fused linear-cross-entropy
-// Host-free bookkeeping + the two thin passes around the LCE GEMMs of gemm2_sm100.cu (kLCEFwd / kLCEdX):
+// Host-free bookkeeping + the two thin passes around the LCE GEMMs of gemm_sm90.cu (kLCEFwd / kLCEdX):
 //
 //   lce_prep       labels -> HF-shifted labels (position s predicts token s+1, last position ignored), n_valid,
 //                  gscale = loss_scale / max(n_valid, 1), loss_sum = 0             (replaces eight ATen launches)
@@ -349,7 +349,7 @@ ODB_EXPORT int odb_lce_prep(const void* labels_in, void* labels_out, int B, int 
 ODB_EXPORT int odb_lce_label_dot(const void* x, long long ldx, const void* W, long long ldw, const void* labels, void* c, int T,
                                  int h, cudaStream_t st) {
   if (h % 8 || ldx % 8 || ldw % 8) return -1;
-  const int blocks = ceil_div(T, 8) < 148 * 8 ? ceil_div(T, 8) : 148 * 8;
+  const int blocks = ceil_div(T, 8) < sm_count() * 8 ? ceil_div(T, 8) : sm_count() * 8;
   launch_pdl(lce_label_dot_kernel, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)W, ldw,
              (const long long*)labels, (float*)c, T, h);
   ODB_CHECK_LAST();

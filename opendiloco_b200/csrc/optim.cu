@@ -1,4 +1,4 @@
-// Flat-arena optimizer kernels for sm_100a (SURVEY.md §2.5 K9-K12, K14).
+// Flat-arena optimizer kernels for sm_90a (SURVEY.md §2.5 K9-K12, K14).
 //
 //  * grad_sqnorm:   one pass over the fp32 gradient arena -> per-CTA partial sums of squares + non-finite flag
 //  * adamw_step:    one launch: (clip coefficient from the partials) -> AdamW on fp32 master weights ->

@@ -263,8 +263,7 @@ __global__ void __launch_bounds__(512) fused_outer_kernel(float* __restrict__ th
 // =====================================================================================================================
 // Pipelined version: the vector is cut into `nchunk` chunks and the three stages run as a software pipeline over chunks,
 // on disjoint sets of CTAs, so the NVLink/NVSwitch reduction of chunk c overlaps the HBM-bound delta / Nesterov work on
-// the other chunks (stage times at 8 GPUs, 860 MB fp32: delta 0.5 ms, in-switch reduce+broadcast 2.0 ms, Nesterov 0.85 ms;
-// run back-to-back by the kernel above, overlapped here).
+// the other chunks (run back-to-back by the kernel above, overlapped here).
 //
 //   local CTAs :  for c: delta(chunk c) -> window ; last CTA to finish chunk c raises ready[c] on every rank
 //                 for c: wait done[c] from every rank ; Nesterov(chunk c)
@@ -555,9 +554,8 @@ ODB_EXPORT int odb_fused_outer_sharded(void* theta_outer, void* buf, void* theta
   if (e != cudaSuccess) return (int)e;
   if (per_sm < 1) return -3;
   const int grid = sm_count() * (per_sm > 2 ? 2 : per_sm);
-  // owner CTAs: the NVLS round trips saturate with well under 100 CTAs (860 MB vector, 8 GPUs: 64 -> 2.27 ms, 96 -> 2.34,
-  // 120 -> 2.33, 197 -> 2.54, 250 -> 2.91; 2 GPUs: flat between 32 and 100, 16 -> 4.3); the rest of the grid runs the
-  // HBM-bound post pass
+  // owner CTAs: the NVLS round trips saturate with well under 100 CTAs, so 64 own the slabs and the rest of the grid runs
+  // the HBM-bound post pass (a choice not yet measured on H100 / NVLink 4)
   if (n_comm <= 0 || n_comm >= grid) n_comm = grid / 3 < 64 ? grid / 3 : 64;
   float* a0 = (float*)theta_outer; float* a1 = (float*)buf; float* a2 = (float*)theta_local;
   __nv_bfloat16* a3 = (__nv_bfloat16*)shadow; float* a4 = (float*)theta_mc; int* tf = (int*)timeout_flag;

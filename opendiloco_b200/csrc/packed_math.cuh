@@ -1,4 +1,5 @@
-// Packed fp32x2 arithmetic (Blackwell FFMA2 / FADD2 / FMUL2) and exp2 helpers shared by the attention and cross-entropy kernels.
+// fp32 pairs carried in one 64-bit register (two scalar FFMA / FADD / FMUL on sm_90) and exp2 helpers of the
+// cross-entropy kernels.
 #pragma once
 #include "common.cuh"
 
@@ -11,22 +12,7 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-// 2^x for x <= 0 on the FMA/ALU pipes (Cody-Waite split + degree-3 polynomial, rel. error 6e-4 - far below the bf16
-// rounding of P).  Half of the exponentials go through this path so the 16-lane MUFU and the FMA pipe work in parallel
-// (the softmax of a 128x128 tile needs 16384 exponentials = 1024 MUFU cycles per SM otherwise).
-__device__ __forceinline__ float poly_exp2(float x) {
-  x = fmaxf(x, -126.f);
-  const float magic = 12582912.f;                       // 1.5 * 2^23: adding it rounds x to the nearest integer
-  const float t = x + magic;
-  const float n = t - magic;
-  const float r = x - n;                                // [-0.5, 0.5]
-  float pl = fmaf(r, 0.0555041087f, 0.2402265070f);
-  pl = fmaf(r, pl, 0.6931471806f);
-  pl = fmaf(r, pl, 1.0f);
-  return __int_as_float(__float_as_int(pl) + (__float_as_int(t) - __float_as_int(magic)) * 8388608);
-}
-
-// ---- packed fp32x2 helpers (Blackwell FFMA2 / FADD2): one instruction, two lanes of a 64-bit register pair
+// ---- fp32 pair helpers: two lanes of a 64-bit register pair
 __device__ __forceinline__ uint64_t pack2(float a, float b) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
@@ -39,49 +25,24 @@ __device__ __forceinline__ uint64_t pack2u(uint32_t a, uint32_t b) {
 }
 __device__ __forceinline__ void unpack2(uint64_t v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
 __device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+  return pack2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t fadd2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(a0 + b0, a1 + b1);
 }
 __device__ __forceinline__ uint32_t cvt_bf16x2(uint64_t v) {
   float a, b;
   unpack2(v, a, b);
   return f2_to_bf2(a, b);
 }
-// 2^y for two values y <= ~8 on the FMA / ALU pipes: n = round(y), r = y - n in [-0.5, 0.5], 2^r by a degree-3 polynomial
-// (rel. error 6e-4, far below the bf16 rounding of P), then n is added to the exponent field.
-__device__ __forceinline__ uint64_t poly_exp2x2(uint64_t y) {
-  float y0, y1;
-  unpack2(y, y0, y1);
-  y = pack2(fmaxf(y0, -126.f), fmaxf(y1, -126.f));
-  const float magic = 12582912.f;                               // 1.5 * 2^23
-  const uint64_t mg = pack2(magic, magic), nmg = pack2(-magic, -magic);
-  const uint64_t t = fadd2(y, mg);
-  const uint64_t n = fadd2(t, nmg);
-  float n0, n1;
-  unpack2(n, n0, n1);
-  const uint64_t r = fadd2(y, pack2(-n0, -n1));
-  uint64_t pl = ffma2(r, pack2(0.0555041087f, 0.0555041087f), pack2(0.2402265070f, 0.2402265070f));
-  pl = ffma2(r, pl, pack2(0.6931471806f, 0.6931471806f));
-  pl = ffma2(r, pl, pack2(1.0f, 1.0f));
-  float p0, p1, t0, t1;
-  unpack2(pl, p0, p1);
-  unpack2(t, t0, t1);
-  const int mi = __float_as_int(magic);
-  p0 = __int_as_float(__float_as_int(p0) + (__float_as_int(t0) - mi) * 8388608);
-  p1 = __int_as_float(__float_as_int(p1) + (__float_as_int(t1) - mi) * 8388608);
-  return pack2(p0, p1);
-}
-
 __device__ __forceinline__ uint64_t fmul2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(a0 * b0, a1 * b1);
 }
 
 }  // namespace packed_math

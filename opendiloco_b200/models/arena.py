@@ -5,7 +5,7 @@
   grad    fp32 [P]   - gradient accumulator (wgrad GEMMs accumulate straight into it)
 
 There is no transposed copy of the weights: the dgrad GEMMs read ``shadow`` in its forward [out, in] layout as an MN-major
-tcgen05 operand (``ops.tc_gemm.linear_nn``).
+wgmma operand (``ops.tc_gemm.linear_nn``).
 
 One buffer => one fused optimizer launch, one collective per outer step (the reference sends 111 per-tensor
 messages: train_diloco_torch.py:342-346, SURVEY.md §2.5 N2), and q|k|v / gate|up weights that are physically

@@ -1,4 +1,4 @@
-"""Llama causal LM on the flat arena: hand-scheduled forward/backward over sm_100a kernels.
+"""Llama causal LM on the flat arena: hand-scheduled forward/backward over sm_90a kernels.
 
 There is no autograd graph on the hot path.  ``LlamaEngine`` runs the layer program explicitly
 (K1..K8 of SURVEY.md §2.5), keeps activations in shape-keyed static workspaces (CUDA-graph friendly) and
@@ -33,9 +33,8 @@ IGNORE_INDEX = -100
 
 
 def _use_graph() -> bool:
-    """CUDA-graph replay of the micro-step (default on; ODB_CUDA_GRAPH=0 for the eager launch sequence).  Measured on B200,
-    Llama-150M: GPU busy 98.4 % -> 99.7 % of the step window (4052 inter-kernel gaps of ~2.2 us -> 193), +1.0 % tokens/s
-    (profiles/r2_idle_gap.txt)."""
+    """CUDA-graph replay of the micro-step (default on; ODB_CUDA_GRAPH=0 for the eager launch sequence): the thousands of
+    short inter-kernel gaps of an eagerly launched step collapse into one graph launch (profiles/idle_gap.py measures it)."""
     return os.environ.get("ODB_CUDA_GRAPH", "1") == "1"
 
 
@@ -157,7 +156,7 @@ class LlamaEngine:
             K.rmsnorm_fwd(x_prev, ar.w(p + "input_layernorm.weight"), cfg.rms_norm_eps, delta=delta, out=ws.xn1[l],
                           rstd=ws.rstd1[l], x_out=ws.xa[l])
             if D == 64 and TC.usable(ws.xn1[l], ar.qkv_w(l)):
-                # tcgen05 GEMM with the rotary embedding applied in the epilogue (no separate RoPE pass over q|k)
+                # wgmma GEMM with the rotary embedding applied in the epilogue (no separate RoPE pass over q|k)
                 TC.linear_qkv_rope(ws.xn1[l], ar.qkv_w(l), ws.qkv[l], ws.cos, ws.sin, S, (Hq + Hkv) * D)
             else:
                 G.mm_nt(ws.xn1[l], ar.qkv_w(l), out=ws.qkv[l])
@@ -233,7 +232,7 @@ class LlamaEngine:
         return (ws.loss_sum / ws.n_valid)[0]
 
     def _head_loss_fused(self, ws: _Workspace, w_lm: torch.Tensor, g_lm: torch.Tensor | None, want_norm: bool) -> None:
-        """Fused linear-cross-entropy on tcgen05 (SURVEY K7).  Per chunk of rows:
+        """Fused linear-cross-entropy on the wgmma GEMM (SURVEY K7).  Per chunk of rows:
 
           c_t   = x_t . W[y_t]                               (lce_label_dot: the label logit, 2 x T x h bytes)
           E     = exp(X W^T - c)   + partial row sums        (ONE GEMM, epilogue in registers; bf16 E only when training)

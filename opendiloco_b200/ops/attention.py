@@ -5,9 +5,9 @@ Layout contract (chosen so that no transpose is ever materialised): the fused QK
 attention output is written token-major ``[T, Hq*D]`` so it feeds the o-proj GEMM directly.
 
 Back-ends:
-  * ``tc``     - our tcgen05 kernel (``csrc/attn_sm100.cu``), used when built and the shape qualifies
-  * ``cudnn``  - cuDNN fused attention through aten (sm_100 kernels; measured 495/444 TF/s fwd/bwd at B32 S1024 H16 D64)
-  * ``flash``  - flash-attn 2.8 library kernels (sm_80 mma.sync code: 266/196 TF/s on B200), ODB_ATTN_LIB=flash
+  * ``tc``     - our kernels (``csrc/attn_sm90.cu``, ``csrc/attn_bwd_sm90.cu``), used when built and the shape qualifies
+  * ``cudnn``  - cuDNN fused attention through aten (comparison baseline)
+  * ``flash``  - flash-attn library kernels (comparison baseline), ODB_ATTN_LIB=flash
   * ``math``   - fp32 PyTorch reference (CPU, tests)
 The reference framework itself calls a library here (torch SDPA / flash-attn: train_fsdp.py:107,173).
 """
@@ -23,7 +23,7 @@ import ctypes
 from .. import _lib
 
 _FLASH = None
-# Back-end of the bf16 CUDA path: "tc" = our tcgen05 kernels (csrc/attn_sm100.cu, attn_bwd_sm100.cu; head_dim 64,
+# Back-end of the bf16 CUDA path: "tc" = our kernels (csrc/attn_sm90.cu, attn_bwd_sm90.cu; head_dim 64,
 # S % 128 == 0), "cudnn" / "flash" = the library kernels (kept as comparison baselines and for other head sizes).
 _LIB = os.environ.get("ODB_ATTN_LIB", "tc")
 
@@ -38,7 +38,7 @@ def bwd_applies_rope(aux) -> bool:
     return isinstance(aux[0], str) and aux[0] == "tc"
 
 _lib.register_optional("odb_attn_fwd", [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                        ctypes.c_int, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p])
+                                        ctypes.c_int, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_float, ctypes.c_void_p])
 
 
 _lib.register_optional("odb_attn_bwd", [ctypes.c_void_p] * 11 + [ctypes.c_int] * 4 + [ctypes.c_longlong] * 4 + [ctypes.c_float, ctypes.c_void_p])
@@ -58,7 +58,7 @@ def _bwd_scratch(dev, T: int, Hq: int, D: int):
 
 def tc_attention_bwd(dout: torch.Tensor, qkv: torch.Tensor, out: torch.Tensor, lse: torch.Tensor, B: int, S: int, Hq: int, Hkv: int,
                      D: int = 64, dqkv: torch.Tensor | None = None, cos: torch.Tensor | None = None, sin: torch.Tensor | None = None):
-    """Our tcgen05 attention backward (csrc/attn_bwd_sm100.cu): pre-pass (row statistics, zero dQ accumulator), main
+    """Our attention backward (csrc/attn_bwd_sm90.cu): pre-pass (row statistics, zero dQ accumulator), main
     kernel, post-pass (dQ fp32 -> bf16).  With ``dqkv`` the three gradients land in the column blocks of that packed
     [T, (Hq+2*Hkv)*D] buffer (returned); otherwise returns dense (dq, dk, dv).  With ``cos``/``sin`` the post-pass also
     undoes the RoPE rotation of dq and dk (the backward of the fused QKV+RoPE projection epilogue)."""
@@ -82,14 +82,13 @@ def tc_attention_bwd(dout: torch.Tensor, qkv: torch.Tensor, out: torch.Tensor, l
     return dqkv if dqkv is not None else (dq, dk, dv)
 
 
-def tc_attention_fwd(qkv: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int = 64, dbg: torch.Tensor | None = None):
-    """Our tcgen05 causal attention forward.  Returns (out [T, Hq*D] bf16, lse [B, Hq, S] fp32, natural log)."""
+def tc_attention_fwd(qkv: torch.Tensor, B: int, S: int, Hq: int, Hkv: int, D: int = 64):
+    """Our causal attention forward (csrc/attn_sm90.cu).  Returns (out [T, Hq*D] bf16, lse [B, Hq, S] fp32, natural log)."""
     assert D == 64 and S % 128 == 0 and qkv.dtype == torch.bfloat16 and qkv.stride(1) == 1
     out = torch.empty(B * S, Hq * D, dtype=qkv.dtype, device=qkv.device)
     lse = torch.empty(B, Hq, S, dtype=torch.float32, device=qkv.device)
     _lib.check(_lib.cuda_lib().odb_attn_fwd(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, S, Hq, Hkv, qkv.stride(0),
-                                            out.stride(0), 1.0 / math.sqrt(D), dbg.data_ptr() if dbg is not None else None,
-                                            _lib.stream_ptr(qkv)), "attn_fwd")
+                                            out.stride(0), 1.0 / math.sqrt(D), _lib.stream_ptr(qkv)), "attn_fwd")
     _lib.count_launch()
     return out, lse
 

@@ -6,9 +6,9 @@ Three shapes of GEMM appear in a Llama step (SURVEY.md §2.5 K3/K6/K7):
   * ``mm_nn``      y[M,K]  = a[M,N] @ b[N,K]            dgrad                 (b is N-major)
   * ``mm_tn_acc``  w[N,K] += a[T,N]^T @ b[T,K]  (fp32)  wgrad, accumulated straight into the fp32 gradient arena
 
-CUDA bf16 operands always run on the tcgen05 kernels of ``csrc/gemm2_sm100.cu`` / ``gemm_sm100.cu`` /
-``wgrad_sm100.cu`` (:mod:`opendiloco_b200.ops.tc_gemm`): ``mm_nt`` with K-major operands, ``mm_nn`` with the weight read
-as an MN-major B operand (no transposed copy), ``mm_tn_acc`` with both operands MN-major and a TMA reduce-add epilogue.
+CUDA bf16 operands always run on the wgmma kernels of ``csrc/gemm_sm90.cu`` (:mod:`opendiloco_b200.ops.tc_gemm`):
+``mm_nt`` with K-major operands, ``mm_nn`` with the weight read as an MN-major B operand (no transposed copy),
+``mm_tn_acc`` with both operands MN-major and an fp32 reduce-add epilogue.
 ``torch.mm`` (cuBLAS / ATen) is only the fp32 / fp16 / CPU path and the ``ODB_TC_GEMM=0`` comparison baseline.
 """
 from __future__ import annotations
@@ -21,7 +21,7 @@ _ADDMM_DTYPE_OK: bool | None = None
 
 
 def mm_nt(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
-    """a[M,K] @ b[N,K]^T : our tcgen05 kernel for CUDA bf16 operands, cuBLAS/ATen otherwise (fp32, fp16, CPU)."""
+    """a[M,K] @ b[N,K]^T : our wgmma kernel for CUDA bf16 operands, cuBLAS/ATen otherwise (fp32, fp16, CPU)."""
     if TC.usable(a, b) and (out is None or TC.usable(out)):
         return TC.linear(a, b, out)
     if out is None:
@@ -30,8 +30,8 @@ def mm_nt(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor | None = None) -> 
 
 
 def mm_nn(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
-    """a[M,N] @ b[N,K] (dgrad): the weight ``b`` stays in its forward [out, in] layout and is fed to tcgen05 as an
-    MN-major operand (UMMA descriptor LBO/SBO), so no transposed weight copy exists."""
+    """a[M,N] @ b[N,K] (dgrad): the weight ``b`` stays in its forward [out, in] layout and is fed to wgmma as an
+    MN-major operand (shared-memory descriptor LBO/SBO), so no transposed weight copy exists."""
     if TC.nn_usable(a, b, out):
         return TC.linear_nn(a, b, out)
     if out is None:
@@ -43,7 +43,7 @@ def mm_tn_acc(a: torch.Tensor, b: torch.Tensor, acc: torch.Tensor, alpha: float 
     """acc (fp32 [N,K]) += alpha * a^T @ b with low-precision a [T,N], b [T,K] and fp32 accumulation/output."""
     global _ADDMM_DTYPE_OK
     if alpha == 1.0 and acc.dtype == torch.float32 and acc.stride(-1) == 1 and TC.wgrad_usable(a, b):
-        TC.wgrad_acc(a, b, acc)          # tcgen05, MN-major operands, split-K, fp32 TMA reduce-add into the grad arena
+        TC.wgrad_acc(a, b, acc)          # wgmma, MN-major operands, split-K, fp32 reduce-add into the grad arena
         return
     if a.dtype == acc.dtype:
         acc.addmm_(a.t(), b, alpha=alpha)

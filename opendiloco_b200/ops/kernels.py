@@ -1,4 +1,4 @@
-"""Python front-end of the sm_100a kernels (``csrc/*.cu``) with a PyTorch reference beside each op.
+"""Python front-end of the sm_90a kernels (``csrc/*.cu``) with a PyTorch reference beside each op.
 
 Dispatch rule (there is exactly one): CUDA tensors -> our kernel (raises if the library is not built);
 CPU tensors -> the reference implementation below, written to reproduce the same rounding points

@@ -1,6 +1,6 @@
-"""Python front-end of the tcgen05 GEMM family (``csrc/gemm_sm100.cu``).
+"""Python front-end of the wgmma GEMM family (``csrc/gemm_sm90.cu``).
 
-``linear``         y = x @ W^T                                  (bf16 in/out, fp32 accumulate in TMEM)
+``linear``         y = x @ W^T                                  (bf16 in/out, fp32 accumulate)
 ``linear_swiglu``  gu = x @ Wgu^T ; act = silu(gate) * up        (one kernel: the SwiGLU pass is the GEMM epilogue)
 ``linear_qkv_rope`` qkv = x @ Wqkv^T with RoPE on the q|k heads   (RoPE is the GEMM epilogue; head_dim 64)
 
@@ -23,18 +23,18 @@ _lib.register_optional("odb_gemm_qkv_rope", [c_void_p, c_void_p, c_void_p, c_int
 for _n in ("odb_gemm2_bf16_tn", "odb_gemm2_swiglu", "odb_gemm2_qkv_rope"):
     _lib.register_optional(_n, _lib._OPTIONAL_SIGS[_n.replace("gemm2", "gemm")])
 
-_lib.register_optional("odb_gemm2_bf16_tn_a3", [c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_void_p, c_void_p,
-                                               c_int, c_int, c_ll, c_ll, c_void_p])
+_lib.register_optional("odb_gemm_bf16_tn_a3", [c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_void_p, c_void_p,
+                                              c_int, c_int, c_ll, c_ll, c_void_p])
 
 _lib.register_optional("odb_wgrad_bf16", [c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_void_p, c_ll, c_void_p,
                                          c_ll, c_int, c_int, c_void_p])
 
-_lib.register_optional("odb_gemm2_swiglu_bwd", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_void_p])
+_lib.register_optional("odb_gemm_swiglu_bwd", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_void_p])
 
-_lib.register_optional("odb_gemm2_bf16_nn", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_void_p])
-_lib.register_optional("odb_gemm2_bf16_nn_a3", [c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_void_p, c_void_p,
+_lib.register_optional("odb_gemm_bf16_nn", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_void_p])
+_lib.register_optional("odb_gemm_bf16_nn_a3", [c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_void_p, c_void_p,
                                                c_int, c_int, c_ll, c_ll, c_void_p])
-_lib.register_optional("odb_gemm2_swiglu_bwd_nn", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_void_p])
+_lib.register_optional("odb_gemm_swiglu_bwd_nn", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_void_p])
 _lib.register_optional("odb_lce_fwd", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_void_p, c_void_p, c_int,
                                       c_int, c_void_p])
 _lib.register_optional("odb_lce_planes", [c_int])
@@ -43,22 +43,26 @@ _lib.register_optional("odb_lce_dx", [c_void_p, c_void_p, c_void_p, c_int, c_int
 
 ENABLED = os.environ.get("ODB_TC_GEMM", "1") != "0"
 FUSE_SWIGLU_BWD = os.environ.get("ODB_TC_SWIGLU_BWD", "1") != "0"
-TWO_CTA = os.environ.get("ODB_TC_GEMM_2CTA", "1") != "0"     # CTA-pair (cta_group::2, 256x256 tiles) kernels
+# 2-CTA cluster kernels (256x256 tiles, B tile multicast): off by default.  Llama-150M bench.py step, H100 SXM at 700 W,
+# three alternating runs each: 1652-1658 ms with the 1-CTA kernels vs 1728-1740 ms with the cluster kernels (-4.7 %
+# tokens/s): with one 193 KB CTA per SM, co-scheduling CTA pairs costs more than the halved B traffic wins.
+TWO_CTA = os.environ.get("ODB_TC_GEMM_2CTA", "0") == "1"
 
 
 _PAIRS: int | None = None
 
 
 def _pairs() -> int:
-    """CTA pairs the device runs at once (SM count // 2): below one full wave the 128x256 single-CTA tiles fill it better."""
+    """CTA pairs the device runs at once (SM count // 2): below one full wave of pair tiles the 128x256 single-CTA tiles
+    fill it better."""
     global _PAIRS
     if _PAIRS is None:
-        _PAIRS = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count // 2 if torch.cuda.is_available() else 74
+        _PAIRS = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count // 2 if torch.cuda.is_available() else 66
     return _PAIRS
 
 
 def _fn(name: str, M: int = 1 << 30, N: int = 1 << 30):
-    """CTA-pair kernel (256x256 tiles) for problems with at least one full wave of pair-tiles, else 128x256 tiles."""
+    """2-CTA cluster kernel (256x256 tiles) for problems with at least one full wave of pair tiles, else 128x256 tiles."""
     lib = _lib.cuda_lib()
     pair_tiles = ((M + 255) // 256) * ((N + 255) // 256)
     two = TWO_CTA and pair_tiles >= _pairs()
@@ -94,20 +98,20 @@ def linear_swiglu(x: torch.Tensor, w_gu: torch.Tensor, gu: torch.Tensor, act: to
 
 
 def swiglu_bwd_usable(dy: torch.Tensor, w_down: torch.Tensor, gu: torch.Tensor) -> bool:
-    """The fused down-proj dgrad + SwiGLU backward (CTA-pair kernel; ``w_down`` is the weight in its forward [h, I] layout)."""
-    if not (FUSE_SWIGLU_BWD and TWO_CTA and usable(dy, w_down, gu)):
+    """The fused down-proj dgrad + SwiGLU backward (``w_down`` is the weight in its forward [h, I] layout)."""
+    if not (FUSE_SWIGLU_BWD and usable(dy, w_down, gu)):
         return False
     I = w_down.shape[1]
-    return I % 64 == 0 and gu.is_contiguous() and gu.shape[1] == 2 * I and _lib.has_symbol("odb_gemm2_swiglu_bwd_nn")
+    return I % 64 == 0 and gu.is_contiguous() and gu.shape[1] == 2 * I and _lib.has_symbol("odb_gemm_swiglu_bwd_nn")
 
 
 def linear_swiglu_bwd(dy: torch.Tensor, w_down: torch.Tensor, gu: torch.Tensor) -> None:
-    """gu [M, 2I] (gate|up) <- d(gate)|d(up) in place, with d(act) = dy @ w_down formed in tensor memory only
+    """gu [M, 2I] (gate|up) <- d(gate)|d(up) in place, with d(act) = dy @ w_down formed in registers only
     (replaces the down-proj dgrad GEMM + the stand-alone swiglu_bwd kernel: d(act) is neither written nor re-read).
     ``w_down`` [h, I] is read as an MN-major B operand, i.e. exactly as the forward pass stores it."""
     M, K = dy.shape
     I = w_down.shape[1]
-    _lib.check(_lib.cuda_lib().odb_gemm2_swiglu_bwd_nn(dy.data_ptr(), w_down.data_ptr(), gu.data_ptr(), M, I, K, dy.stride(0),
+    _lib.check(_lib.cuda_lib().odb_gemm_swiglu_bwd_nn(dy.data_ptr(), w_down.data_ptr(), gu.data_ptr(), M, I, K, dy.stride(0),
                                                        w_down.stride(0), _lib.stream_ptr(dy)), "gemm_swiglu_bwd_nn")
     _lib.count_launch()
 
@@ -116,25 +120,25 @@ def linear_swiglu_bwd_t(dy: torch.Tensor, w_down_t: torch.Tensor, gu: torch.Tens
     """Same with the weight given transposed ([I, h], K-major B) - kept for the kernel tests."""
     M, K = dy.shape
     I = w_down_t.shape[0]
-    _lib.check(_lib.cuda_lib().odb_gemm2_swiglu_bwd(dy.data_ptr(), w_down_t.data_ptr(), gu.data_ptr(), M, I, K, dy.stride(0),
+    _lib.check(_lib.cuda_lib().odb_gemm_swiglu_bwd(dy.data_ptr(), w_down_t.data_ptr(), gu.data_ptr(), M, I, K, dy.stride(0),
                                                     w_down_t.stride(0), _lib.stream_ptr(dy)), "gemm_swiglu_bwd")
     _lib.count_launch()
 
 
 def nn_usable(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor | None = None) -> bool:
-    return (TWO_CTA and usable(a, b) and (out is None or usable(out)) and b.shape[1] % 8 == 0 and a.shape[1] % 8 == 0
-            and _lib.has_symbol("odb_gemm2_bf16_nn"))
+    return (usable(a, b) and (out is None or usable(out)) and b.shape[1] % 8 == 0 and a.shape[1] % 8 == 0
+            and _lib.has_symbol("odb_gemm_bf16_nn"))
 
 
 def linear_nn(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
     """out[M, N] = a[M, K] @ b[K, N] with b row-major (the dgrad dX = dY W on the forward weight layout): B is fed to
-    tcgen05 as an MN-major operand, no transposed weight copy exists anywhere."""
+    wgmma as an MN-major operand, no transposed weight copy exists anywhere."""
     M, K = a.shape
     N = b.shape[1]
     if out is None:
         out = torch.empty(M, N, dtype=a.dtype, device=a.device)
-    _lib.check(_lib.cuda_lib().odb_gemm2_bf16_nn(a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0),
-                                                 out.stride(0), _lib.stream_ptr(a)), "gemm2_bf16_nn")
+    _lib.check(_lib.cuda_lib().odb_gemm_bf16_nn(a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0),
+                                                 out.stride(0), _lib.stream_ptr(a)), "gemm_bf16_nn")
     _lib.count_launch()
     return out
 
@@ -143,16 +147,16 @@ def linear_nn_a3(a0: torch.Tensor, a1: torch.Tensor, a2: torch.Tensor, w: torch.
     """out = cat([a0, a1, a2], dim=1) @ w with w [K0+K1+K2, N] row-major; the three A pieces are read in place."""
     M = a0.shape[0]
     N = w.shape[1]
-    _lib.check(_lib.cuda_lib().odb_gemm2_bf16_nn_a3(a0.data_ptr(), a1.data_ptr(), a2.data_ptr(), a0.stride(0), a1.stride(0),
+    _lib.check(_lib.cuda_lib().odb_gemm_bf16_nn_a3(a0.data_ptr(), a1.data_ptr(), a2.data_ptr(), a0.stride(0), a1.stride(0),
                                                     a2.stride(0), a0.shape[1], a1.shape[1], a2.shape[1], w.data_ptr(), out.data_ptr(),
-                                                    M, N, w.stride(0), out.stride(0), _lib.stream_ptr(out)), "gemm2_bf16_nn_a3")
+                                                    M, N, w.stride(0), out.stride(0), _lib.stream_ptr(out)), "gemm_bf16_nn_a3")
     _lib.count_launch()
     return out
 
 
 # ------------------------------------------------------------------------------------------------ fused linear-cross-entropy
 def lce_usable(x: torch.Tensor, w: torch.Tensor) -> bool:
-    return TWO_CTA and usable(x, w) and w.shape[1] % 64 == 0 and w.shape[0] % 8 == 0 and _lib.has_symbol("odb_lce_fwd")
+    return usable(x, w) and w.shape[1] % 64 == 0 and w.shape[0] % 8 == 0 and _lib.has_symbol("odb_lce_fwd")
 
 
 def lce_planes(V: int) -> int:
@@ -162,7 +166,7 @@ def lce_planes(V: int) -> int:
 def lce_fwd(x: torch.Tensor, w: torch.Tensor, shift: torch.Tensor, partials: torch.Tensor, e_out: torch.Tensor | None,
             want_sumsq: bool = False) -> None:
     """LM-head GEMM whose epilogue emits e = exp(x @ w^T - shift[:, None]) (bf16, only when ``e_out`` is given) and the
-    partial row sums of e (``partials`` [planes(, x2 with want_sumsq), M] fp32).  Logits are never written."""
+    partial row sums of e (``partials`` [planes(, x2 with want_sumsq), M] fp32; one plane per 256 vocabulary columns).  Logits are never written."""
     M, K = x.shape
     V = w.shape[0]
     assert partials.dtype == torch.float32 and partials.numel() >= lce_planes(V) * M * (2 if want_sumsq else 1)
@@ -198,9 +202,9 @@ def linear_a3(a0: torch.Tensor, a1: torch.Tensor, a2: torch.Tensor, w: torch.Ten
     """out = cat([a0, a1, a2], dim=1) @ w^T with the three A pieces read in place (dq|dk|dv -> dgrad of the fused QKV)."""
     M = a0.shape[0]
     N = w.shape[0]
-    _lib.check(_lib.cuda_lib().odb_gemm2_bf16_tn_a3(a0.data_ptr(), a1.data_ptr(), a2.data_ptr(), a0.stride(0), a1.stride(0),
+    _lib.check(_lib.cuda_lib().odb_gemm_bf16_tn_a3(a0.data_ptr(), a1.data_ptr(), a2.data_ptr(), a0.stride(0), a1.stride(0),
                                                     a2.stride(0), a0.shape[1], a1.shape[1], a2.shape[1], w.data_ptr(), out.data_ptr(),
-                                                    M, N, w.stride(0), out.stride(0), _lib.stream_ptr(out)), "gemm2_bf16_tn_a3")
+                                                    M, N, w.stride(0), out.stride(0), _lib.stream_ptr(out)), "gemm_bf16_tn_a3")
     _lib.count_launch()
     return out
 

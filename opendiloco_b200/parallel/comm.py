@@ -1,6 +1,6 @@
 """Process topology and collectives.
 
-One process per GPU, ``torch.distributed`` (NCCL over NVLink 5 / NVSwitch; gloo on CPU) for the plumbing.  The job is
+One process per GPU, ``torch.distributed`` (NCCL over NVLink / NVSwitch; gloo on CPU) for the plumbing.  The job is
 a grid ``galaxy_size x gpus_per_worker``:
 
     rank = world_rank * gpus_per_worker + local_rank

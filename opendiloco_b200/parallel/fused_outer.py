@@ -1,7 +1,7 @@
 """Host side of the fused outer step (``csrc/outer_comm.cu``): NVLink symmetric-memory windows + launch.
 
 ``torch.distributed._symmetric_memory`` is used purely as plumbing: it allocates the same-sized window on every rank of
-the outer group, exchanges the handles, maps every peer's window into this process (P2P over NVLink 5) and - when the
+the outer group, exchanges the handles, maps every peer's window into this process (P2P over NVLink) and - when the
 fabric supports NVLS - binds them to one multicast address.  The kernel that touches those pointers is ours.
 """
 from __future__ import annotations

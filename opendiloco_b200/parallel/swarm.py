@@ -1,7 +1,7 @@
 """Swarm membership for DiLoCo workers on one NVLink domain.
 
 The reference discovers peers through hivemind's Kademlia DHT + a Go libp2p daemon and tracks training progress in DHT
-records (SURVEY.md E11/E12, hivemind_diloco.py:174-282).  On a single 8xB200 box the workers are ranks of one NCCL
+records (SURVEY.md E11/E12, hivemind_diloco.py:174-282).  On a single 8-GPU box the workers are ranks of one NCCL
 world, so "the DHT" reduces to (a) the outer process group and (b) the c10d key-value store that already backs the
 rendezvous — used here for arrival handshakes, straggler time-outs and drop detection.
 

@@ -1,5 +1,5 @@
 """Self-contained DiLoCo trainer: every rank is one worker (the reference's ``train_diloco_torch.py``, SURVEY.md §3.4 /
-C7), on the B200-native engine.  Works on NCCL (GPUs) and on gloo (CPUs - BASELINE.json config #1).
+C7), on the H100-native engine.  Works on NCCL (GPUs) and on gloo (CPUs - BASELINE.json config #1).
 
     torchrun --nproc_per_node=8 -m opendiloco_b200.train_diloco_torch --model-name-or-path 150m --precision bf16-mixed \
         --per-device-train-batch-size 32 --batch-size 512 --local-steps 500 --fake-data

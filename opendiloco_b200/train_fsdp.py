@@ -1,4 +1,4 @@
-"""Pre-training entry point with the reference's ``train_fsdp.py`` CLI (SURVEY.md §5.6) on the B200-native engine.
+"""Pre-training entry point with the reference's ``train_fsdp.py`` CLI (SURVEY.md §5.6) on the H100-native engine.
 
     torchrun --nproc_per_node=2 -m opendiloco_b200.train_fsdp --per-device-train-batch-size 8 --total-batch-size 128 \
         --lr 1e-2 --path-model 2m --fake-data --max-steps 20
@@ -15,7 +15,7 @@ Differences from the reference driver that are intentional:
   * ``--sharding-strategy`` is honoured together with ``--hv`` (the reference forces NO_SHARD, train_fsdp.py:192-194),
     which is what BASELINE.json config #4 (1B, 4 workers x 2 GPUs ZeRO-2) needs;
   * ``--torch-compile`` / ``--attn-implementation`` are accepted for CLI compatibility and ignored: the model math is
-    hand-written sm_100a kernels, there is no tracing compiler on the hot path.
+    hand-written sm_90a kernels, there is no tracing compiler on the hot path.
 """
 from __future__ import annotations
 

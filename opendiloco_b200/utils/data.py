@@ -8,7 +8,7 @@ Reference behaviour being reproduced (SURVEY.md E7, Appendix A):
     (train_fsdp.py:151-156);
   * resumable loader state (torchdata StatefulDataLoader: train_fsdp.py:163-168, ckpt_utils.py:83-87).
 
-``SyntheticTokenLoader`` is the B200-side fast path: batches are produced directly as pinned [B, S] int64 tensors
+``SyntheticTokenLoader`` is the GPU-side fast path: batches are produced directly as pinned [B, S] int64 tensors
 (by the C++ prefetcher in ``libodbhost.so`` when built) so the H2D copy is a single async DMA per micro-batch.
 """
 from __future__ import annotations
@@ -215,7 +215,7 @@ def write_token_shard(path: str, tokens, bytes_per_token: int | None = None) -> 
 class TokenFileLoader(_RingLoader):
     """Causal-LM batches straight from pre-tokenised shards (``csrc/host/tokenfile.cc``): mmap + prefetch thread, windows
     of ``seq_len`` tokens, seeded shuffle that visits every window once per epoch, disjoint samples per rank.  Feeds the
-    ~6 M tokens/s an 8xB200 box consumes, which on-the-fly tokenisation (the reference's pipeline) cannot.
+    ~6 M tokens/s an 8-GPU box consumes, which on-the-fly tokenisation (the reference's pipeline) cannot.
 
     ``paths``: shard files, or one glob pattern.  Shards come from ``write_token_shard`` / ``scripts/tokenize_corpus.py``;
     header-less ``.bin`` files of uint16 / uint32 tokens work with ``raw_bytes_per_token``."""

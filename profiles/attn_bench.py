@@ -1,4 +1,4 @@
-"""Library attention candidates on B200 at the flagship shape (B=32,S=1024,H=16,D=64): flash-attn 2.8 vs cuDNN SDPA."""
+"""Library attention candidates on the GPU at the flagship shape (B=32,S=1024,H=16,D=64): flash-attn 2.8 vs cuDNN SDPA."""
 import math, sys, os, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 B, S, H, D = 32, 1024, 16, 64

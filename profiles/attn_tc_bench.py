@@ -1,4 +1,4 @@
-"""Our tcgen05 attention forward vs cuDNN / fp32 math: numerics and timing."""
+"""Our attention forward vs cuDNN / fp32 math: numerics and timing."""
 import math, os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from opendiloco_b200.ops import attention as A

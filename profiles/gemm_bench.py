@@ -1,4 +1,4 @@
-"""tcgen05 GEMM family vs cuBLAS (torch.mm): numerics + CUDA-event timing at the Llama-150M / 1B shapes."""
+"""wgmma GEMM family vs cuBLAS (torch.mm): numerics + CUDA-event timing at the Llama-150M / 1B shapes."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from opendiloco_b200.ops import tc_gemm as T, kernels as K
@@ -16,8 +16,6 @@ def timeit(fn, n=20):
 
 def rel(a, b): return ((a.float() - b.float()).norm() / b.float().norm()).item()
 
-T.TWO_CTA = os.environ.get("ODB_TC_GEMM_2CTA", "1") != "0"
-print("two_cta =", T.TWO_CTA)
 print("== plain TN GEMM")
 for (M, N, Kd) in [(300, 520, 200), (128, 256, 64), (4096, 1024, 1024), (32768, 1024, 1024), (32768, 3072, 1024), (32768, 5376, 1024),
                    (32768, 1024, 2688), (2048, 32000, 1024), (16384, 2560, 2048), (16384, 2048, 5632)]:
@@ -73,7 +71,7 @@ ref = torch.cat([dq, dk, dv], 1).float().t() @ x.float()
 out = torch.zeros(3072, Kd, device=dev); T.wgrad_acc((dq, dk, dv), x, out); torch.cuda.synchronize()
 print("3-source wgrad rel_err", rel(out, ref), "time", timeit(lambda: T.wgrad_acc((dq, dk, dv), x, out)) * 1e3, "us")
 
-print("== down-proj dgrad + SwiGLU backward epilogue (d(act) never leaves tensor memory)")
+print("== down-proj dgrad + SwiGLU backward epilogue (d(act) never leaves the registers)")
 for (M, I, Kd) in [(32768, 2688, 1024), (16384, 5632, 2048)]:
     dy = torch.randn(M, Kd, device=dev).to(BF); wt = (torch.randn(I, Kd, device=dev) * 0.05).to(BF)
     gu = torch.randn(M, 2 * I, device=dev).to(BF)

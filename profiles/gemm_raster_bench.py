@@ -1,4 +1,4 @@
-"""Rasterisation sweep of the CTA-pair GEMM at the Llama-150M micro-batch shapes (run once per ODB_GEMM_GROUP_M value; the
+"""Rasterisation sweep of the GEMM at the Llama-150M micro-batch shapes (run once per ODB_GEMM_GROUP_M value; the
 kernel reads the variable at its first launch).  L2 is flushed between timed launches."""
 import os
 import sys

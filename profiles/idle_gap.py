@@ -1,7 +1,7 @@
 """GPU busy fraction inside one un-graphed training step (nsys is not in the image: torch.profiler's CUPTI activity
 records give every kernel's start / end on the device, including the ctypes-launched ones of libodb200.so).
 
-    python profiles/idle_gap.py [--graph]      -> gpurun_out/idle_gap.json
+    python profiles/idle_gap.py [--graph]      -> profiles_out/idle_gap.json
 
 Reports, for ONE optimizer step (16 micro-batches + AdamW) after warm-up: window (first kernel start -> last kernel end),
 sum of kernel durations, busy %, number of kernels, and the distribution of the gaps between consecutive kernels.
@@ -60,7 +60,7 @@ out = {"graph": "--graph" in sys.argv, "kernels": len(spans), "window_ms": (t1 -
        "busy_pct": 100.0 * busy / (t1 - t0), "idle_ms": (t1 - t0 - busy) / 1e3, "gaps": len(gaps),
        "gap_us_median": gaps[len(gaps) // 2] if gaps else 0, "gap_us_p90": gaps[int(len(gaps) * 0.9)] if gaps else 0,
        "gap_us_max": gaps[-1] if gaps else 0, "gaps_over_10us": sum(1 for x in gaps if x > 10)}
-os.makedirs("gpurun_out", exist_ok=True)
-name = "gpurun_out/idle_gap_graph.json" if out["graph"] else "gpurun_out/idle_gap.json"
+os.makedirs("profiles_out", exist_ok=True)
+name = "profiles_out/idle_gap_graph.json" if out["graph"] else "profiles_out/idle_gap.json"
 json.dump(out, open(name, "w"), indent=1)
 print(json.dumps(out))

@@ -3,9 +3,9 @@ torch.autocast(bf16), torch AdamW / cosine schedule / clip / SGD-Nesterov outer 
 IDENTICAL initial weights (one random-init HF checkpoint), an IDENTICAL token stream (torch.Generator seeded per step) and
 identical hyper-parameters.  BASELINE.md asks for |d loss| <= 1e-3 at step 1000.
 
-    python profiles/loss_parity.py --impl reference --steps 1000 --out gpurun_out/parity_ref.jsonl
-    python profiles/loss_parity.py --impl ours      --steps 1000 --out gpurun_out/parity_ours.jsonl
-    python profiles/loss_parity.py --compare gpurun_out/parity_ref.jsonl gpurun_out/parity_ours.jsonl
+    python profiles/loss_parity.py --impl reference --steps 1000 --out profiles_out/parity_ref.jsonl
+    python profiles/loss_parity.py --impl ours      --steps 1000 --out profiles_out/parity_ours.jsonl
+    python profiles/loss_parity.py --compare profiles_out/parity_ref.jsonl profiles_out/parity_ours.jsonl
 
 Protocol: Llama-150M, 1 worker (the outer step is the solo form), 32 x 1024 tokens per optimizer step (one micro-batch),
 H = 50, lr 4e-4 with 100 warm-up steps of a 1000-step cosine, bf16-mixed.  (The full 512 x 1024 batch would cost the
@@ -28,7 +28,7 @@ ap.add_argument("--seq", type=int, default=1024)
 ap.add_argument("--local-steps", type=int, default=50)
 ap.add_argument("--warmup", type=int, default=100)
 ap.add_argument("--model", default="150m")
-ap.add_argument("--out", default="gpurun_out/parity.jsonl")
+ap.add_argument("--out", default="profiles_out/parity.jsonl")
 ap.add_argument("--compare", nargs=2)
 a = ap.parse_args()
 

@@ -1,6 +1,6 @@
 """One-shot drivers for `ncu --set full` captures of individual kernels at the Llama-150M micro-batch shapes.
 
-    ncu --set full --clock-control none --import-source on -k regex:<kernel> -s 2 -c 1 -o gpurun_out/<name> \
+    ncu --set full --clock-control none --import-source on -k regex:<kernel> -s 2 -c 1 -o profiles_out/<name> \
         python profiles/ncu_one.py <which>
 
 which: lce | bandwidth (AdamW, grad norm, RMSNorm fwd/bwd, embedding fwd/bwd, LCE helpers, Nesterov solo, cast)

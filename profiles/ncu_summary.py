@@ -1,7 +1,7 @@
 """Summarise an `ncu --set full` report (read on the CPU box): per kernel duration, DRAM bytes, achieved GB/s, % of the
 measured HBM copy bandwidth (MEASURED_PEAKS.json), tensor-pipe %, registers.
 
-    python profiles/ncu_summary.py gpurun_out/x.ncu-rep > profiles/r2_ncu_x.txt
+    python profiles/ncu_summary.py profiles_out/x.ncu-rep > profiles_out/ncu_x.txt
 """
 import csv
 import io

@@ -1,6 +1,6 @@
 """One micro-batch (fwd+bwd) + optimizer step of Llama-150M between cudaProfilerStart/Stop, for
-    ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv python profiles/profile_step.py
-(serialised, cold-cache: compare SHARES, not absolutes - B200_PROFILING.md)."""
+    ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file profiles_out/launches.csv python profiles/profile_step.py
+(serialised, cold-cache: compare SHARES, not absolutes)."""
 import os
 import sys
 

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on a B200 via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -25,4 +25,7 @@ def pytest_collection_modifyitems(config, items):
 
 @pytest.fixture(scope="session")
 def ref_model_dir():
-    return "/root/reference/tests/models/llama-2m-fresh" if os.path.isdir("/root/reference/tests/models/llama-2m-fresh") else None
+    """The reference's fresh Llama-2M test checkpoint (HF layout), vocabulary cut to its first 512 rows to stay small."""
+    path = os.path.join(ROOT, "tests", "golden", "llama-2m-fresh")
+    assert os.path.isfile(os.path.join(path, "model.safetensors")) and os.path.isfile(os.path.join(path, "config.json")), path
+    return path

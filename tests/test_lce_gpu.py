@@ -1,4 +1,4 @@
-"""Fused linear-cross-entropy (tcgen05 GEMM with the exponentials in the epilogue; csrc/gemm2_sm100.cu kLCEFwd / kLCEdX,
+"""Fused linear-cross-entropy (wgmma GEMM with the exponentials in the epilogue; csrc/gemm_sm90.cu kLCEFwd / kLCEdX,
 csrc/lce.cu) against a plain fp32 PyTorch cross-entropy of the same op (reference call site train_diloco_torch.py:313-314)."""
 import pytest
 import torch

@@ -12,15 +12,11 @@ def _hf():
 
 def test_matches_hf_llama_fp32(ref_model_dir, tmp_path):
     tr = _hf()
-    if ref_model_dir is None:
-        cfg = LlamaConfig(hidden_size=64, intermediate_size=256, num_hidden_layers=2, num_attention_heads=2, vocab_size=1024)
-        LlamaForCausalLM(cfg, precision="32-true", seed=1).save_pretrained(str(tmp_path))
-        ref_model_dir = str(tmp_path)
     torch.manual_seed(0)
     ours = LlamaForCausalLM.from_pretrained(ref_model_dir, precision="32-true")
     hf = tr.LlamaForCausalLM.from_pretrained(ref_model_dir, attn_implementation="sdpa").float()
     ours.train(), hf.train()
-    ids = torch.randint(3, 1024, (2, 48))
+    ids = torch.randint(3, hf.config.vocab_size, (2, 48))
     o1, o2 = ours(input_ids=ids, labels=ids), hf(input_ids=ids, labels=ids)
     assert abs(o1.loss.item() - o2.loss.item()) < 1e-5
     o1.loss.backward(), o2.loss.backward()

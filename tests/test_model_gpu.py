@@ -1,4 +1,4 @@
-"""End-to-end model numerics on a B200: the kernel path (CUDA, bf16) against the PyTorch reference path of the same engine."""
+"""End-to-end model numerics on an H100: the kernel path (CUDA, bf16) against the PyTorch reference path of the same engine."""
 import pytest
 import torch
 

@@ -1,4 +1,5 @@
-"""tcgen05 GEMM family (1-CTA and CTA-pair kernels, fused SwiGLU / RoPE epilogues) against fp32 PyTorch references."""
+"""wgmma GEMM family (1-CTA and 2-CTA cluster kernels, fused SwiGLU / RoPE epilogues, weight gradient, MN-major operands)
+against fp32 PyTorch references."""
 import pytest
 import torch
 
@@ -120,7 +121,7 @@ def test_swiglu_backward_epilogue(M, I, Kd):
 @pytest.mark.parametrize("M,N,Kd", [(128, 256, 64), (300, 520, 200), (1000, 136, 72), (4096, 1024, 1024), (20000, 1024, 2688),
                                     (8192, 1024, 32000)])
 def test_linear_nn_mn_major_b(M, N, Kd):
-    """dgrad form: out = a @ b with b [K, N] row-major, fed to tcgen05 as an MN-major operand (no transposed copy)."""
+    """dgrad form: out = a @ b with b [K, N] row-major, fed to wgmma as an MN-major operand (no transposed copy)."""
     torch.manual_seed(6)
     a = torch.randn(M, Kd, device="cuda").to(BF)
     b = (torch.randn(Kd, N, device="cuda") * 0.1).to(BF)
