@@ -1,0 +1,271 @@
+"""KV-cached autoregressive generation for :class:`~opendiloco_b200.models.llama.LlamaForCausalLM`.
+
+Prefill runs the prompt through the training layer program (fused QKV+RoPE GEMM, the causal attention forward, the
+SwiGLU GEMM) on buffers of this module's own, copies k|v into per-layer caches and samples the first token.  Every later
+token is one decode step over ``[B, ·]`` buffers:
+
+    embedding -> per layer: rmsnorm -> QKV GEMM -> rope+append -> split-KV attention -> o-proj -> rmsnorm(+residual)
+              -> gate|up SwiGLU GEMM -> down -> final norm -> LM head -> sampler
+
+All the per-step scalars (positions, step counters, finished flags, sampler settings) live in device memory, so the step
+is captured once into a CUDA graph and replayed (``ODB_CUDA_GRAPH=0``: eager launches).  CUDA bf16 models run the
+kernels of ``csrc/decode_sm90.cu`` and the training GEMMs; other precisions and devices run the same program on the
+PyTorch references of :mod:`opendiloco_b200.ops`.
+
+Nothing here goes through ``LlamaEngine.workspace`` or its captured training graphs: generating between training steps
+leaves the training buffers and graph untouched.
+"""
+from __future__ import annotations
+
+import os
+
+import torch
+
+from ..ops import attention as A
+from ..ops import decode as DK
+from ..ops import gemm as G
+from ..ops import kernels as K
+from ..ops import tc_gemm as TC
+
+FINISHED_CHECK_EVERY = 16           # decode steps between host checks of "every row has finished"
+
+
+def _round_up(x: int, m: int) -> int:
+    return (x + m - 1) // m * m
+
+
+def _use_graph() -> bool:
+    return os.environ.get("ODB_CUDA_GRAPH", "1") == "1"
+
+
+class _PrefillBuffers:
+    """Transient [B*Sp, ·] activations of one prefill (no per-layer saved activations)."""
+
+    def __init__(self, cfg, T: int, device, dtype):
+        e = lambda *shape: torch.empty(*shape, dtype=dtype, device=device)  # noqa: E731
+        h, i = cfg.hidden_size, cfg.intermediate_size
+        self.T = T
+        self.ids = torch.empty(T, dtype=torch.int64, device=device)
+        self.res, self.xn, self.proj = e(T, h), e(T, h), e(T, h)
+        self.rstd = torch.empty(T, dtype=torch.float32, device=device)
+        self.qkv, self.gu, self.act = e(T, cfg.qkv_dim), e(T, 2 * i), e(T, i)
+
+
+class DecodeState:
+    """KV caches, decode buffers and device-side control scalars for B rows of up to Smax positions."""
+
+    def __init__(self, cfg, B: int, Smax: int, device, dtype):
+        L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+        h, i, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
+        e = lambda *shape: torch.empty(*shape, dtype=dtype, device=device)  # noqa: E731
+        i32 = lambda: torch.zeros(B, dtype=torch.int32, device=device)      # noqa: E731
+        self.cfg, self.B, self.Smax, self.device, self.dtype = cfg, B, Smax, torch.device(device), dtype
+        self.key = (B, Smax, str(device), dtype)
+        self.kc = [torch.zeros(B, Hkv, Smax, D, dtype=dtype, device=device) for _ in range(L)]
+        self.vc = [torch.zeros(B, Hkv, Smax, D, dtype=dtype, device=device) for _ in range(L)]
+        n_rope = _round_up(max(cfg.max_position_embeddings, Smax), 128)
+        self.cos, self.sin = K.rope_tables(n_rope, D, cfg.rope_theta, device)
+        # one-token-per-row buffers of the decode step
+        self.ids = torch.zeros(B, dtype=torch.int64, device=device)
+        self.res, self.xn, self.proj = e(B, h), e(B, h), e(B, h)
+        self.rstd = torch.empty(B, dtype=torch.float32, device=device)
+        self.qkv, self.att, self.gu, self.act = e(B, cfg.qkv_dim), e(B, cfg.q_dim), e(B, 2 * i), e(B, i)
+        self.logits = e(B, V)
+        self.pos, self.gen, self.finished, self.lens = i32(), i32(), i32(), i32()
+        self.out = torch.zeros(B, Smax, dtype=torch.int64, device=device)
+        self.ictl, self.fctl = DK.make_controls(False, 1.0, 0, 1.0, 0, 0, [], device)
+        self.kernels = DK.usable(self.res, D, Hq, Hkv)
+        self.part_o = self.part_ml = None
+        if self.kernels:
+            nch = DK.attn_chunks(Smax)
+            self.part_o = torch.empty(B, Hq, nch, D, dtype=torch.float32, device=device)
+            self.part_ml = torch.empty(B, Hq, nch, 2, dtype=torch.float32, device=device)
+        self._prefill: _PrefillBuffers | None = None
+        self.graph = None
+        self.graph_key = None
+
+    def prefill_buffers(self, T: int) -> _PrefillBuffers:
+        if self._prefill is None or self._prefill.T != T:
+            self._prefill = None                      # free the old buffers before allocating the new ones
+            self._prefill = _PrefillBuffers(self.cfg, T, self.device, self.dtype)
+        return self._prefill
+
+    def set_controls(self, do_sample: bool, temperature: float, top_k: int, top_p: float, seed: int, pad: int, eos: list[int]):
+        ictl, fctl = DK.make_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, "cpu")
+        self.ictl.copy_(ictl)
+        self.fctl.copy_(fctl)
+
+
+def decode_state(model, B: int, Smax: int) -> DecodeState:
+    """The model's decode state for (B, Smax), allocated on first use; at most one is resident."""
+    eng, ar = model.engine, model.arena
+    key = (B, Smax, str(ar.device), ar.compute_dtype)
+    st = eng.decode_state
+    if st is None or st.key != key:
+        eng.decode_state = None                       # free the old caches before allocating the new ones
+        st = eng.decode_state = DecodeState(model.config, B, Smax, ar.device, ar.compute_dtype)
+    return st
+
+
+# ------------------------------------------------------------------------------------------------ prefill
+@torch.no_grad()
+def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor) -> None:
+    """ids [B, Sp]: prompts compacted to start at position 0 and right-padded; lens [B] real lengths.  Fills the caches,
+    computes the logits at position lens[b]-1 and samples the first new token (st.pos ends at lens)."""
+    cfg, ar = model.config, model.arena
+    B, Sp = ids.shape
+    L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    eps = cfg.rms_norm_eps
+    T = B * Sp
+    pb = st.prefill_buffers(T)
+    st.lens.copy_(lens)
+    st.pos.copy_(lens - 1)
+    st.gen.zero_()
+    st.finished.zero_()
+    pb.ids.copy_(ids.reshape(-1))
+    cos, sin = st.cos[:Sp], st.sin[:Sp]
+    K.embedding_fwd(pb.ids, ar.w("model.embed_tokens.weight"), out=pb.res)
+    delta = None
+    for l in range(L):
+        p = f"model.layers.{l}."
+        K.rmsnorm_fwd(pb.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
+        if st.kernels and TC.usable(pb.xn, ar.qkv_w(l)):
+            TC.linear_qkv_rope(pb.xn, ar.qkv_w(l), pb.qkv, cos, sin, Sp, (Hq + Hkv) * D)
+        else:
+            G.mm_nt(pb.xn, ar.qkv_w(l), out=pb.qkv)
+            K.rope_(pb.qkv, cos, sin, Sp, Hq + Hkv, D)
+        DK.kv_fill(pb.qkv, st.lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D)
+        att, _ = A.attention_fwd(pb.qkv, B, Sp, Hq, Hkv, D)
+        G.mm_nt(att, ar.w(p + "self_attn.o_proj.weight"), out=pb.proj)
+        K.rmsnorm_fwd(pb.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=pb.proj, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
+        _mlp(cfg, ar, l, pb.xn, pb.gu, pb.act)
+        G.mm_nt(pb.act, ar.w(p + "mlp.down_proj.weight"), out=pb.proj)
+        delta = pb.proj
+    # only the last real position of every row feeds the LM head: gather its residual and delta rows
+    last = torch.arange(B, device=st.device, dtype=torch.int64) * Sp + st.lens.long() - 1
+    K.embedding_fwd(last, pb.res, out=st.res)
+    K.embedding_fwd(last, delta, out=st.proj)
+    _head_and_sample(cfg, ar, st, st.proj)
+
+
+def _mlp(cfg, ar, l: int, xn, gu, act) -> None:
+    if cfg.intermediate_size % 64 == 0 and TC.usable(xn, ar.gu_w(l)):
+        TC.linear_swiglu(xn, ar.gu_w(l), gu, act)
+    else:
+        G.mm_nt(xn, ar.gu_w(l), out=gu)
+        K.swiglu_fwd(gu, out=act)
+
+
+def _head_and_sample(cfg, ar, st: DecodeState, delta) -> None:
+    K.rmsnorm_fwd(st.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=st.xn, rstd=st.rstd, x_out=st.res)
+    G.mm_nt(st.xn, ar.w("lm_head.weight"), out=st.logits)
+    DK.sample(st.logits, st.ictl, st.fctl, st.pos, st.gen, st.finished, st.out, st.ids)
+
+
+# ------------------------------------------------------------------------------------------------ decode step
+def _step_eager(model, st: DecodeState) -> None:
+    cfg, ar = model.config, model.arena
+    L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    eps = cfg.rms_norm_eps
+    K.embedding_fwd(st.ids, ar.w("model.embed_tokens.weight"), out=st.res)
+    delta = None
+    for l in range(L):
+        p = f"model.layers.{l}."
+        K.rmsnorm_fwd(st.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=st.xn, rstd=st.rstd, x_out=st.res)
+        G.mm_nt(st.xn, ar.qkv_w(l), out=st.qkv)
+        DK.rope_append(st.qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D)
+        DK.attention(st.qkv, st.kc[l], st.vc[l], st.pos, st.att, Hq, Hkv, D, st.part_o, st.part_ml)
+        G.mm_nt(st.att, ar.w(p + "self_attn.o_proj.weight"), out=st.proj)
+        K.rmsnorm_fwd(st.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=st.proj, out=st.xn, rstd=st.rstd, x_out=st.res)
+        _mlp(cfg, ar, l, st.xn, st.gu, st.act)
+        G.mm_nt(st.act, ar.w(p + "mlp.down_proj.weight"), out=st.proj)
+        delta = st.proj
+    _head_and_sample(cfg, ar, st, delta)
+
+
+@torch.no_grad()
+def step(model, st: DecodeState, graph: bool | None = None) -> None:
+    """One decode step: consume st.ids at st.pos, sample the next token into st.ids / st.out.  With the kernels and
+    ``graph`` (default: ``ODB_CUDA_GRAPH`` != 0) the first call runs eagerly (warm-up), the second captures the step and
+    every call replays it."""
+    if graph is None:
+        graph = _use_graph()
+    if not (graph and st.kernels):
+        _step_eager(model, st)
+        return
+    key = (model.arena.version, model.arena.shadow.data_ptr())
+    if st.graph is None or st.graph_key != key:
+        if st.graph_key != ("warm",) + key:
+            st.graph, st.graph_key = None, ("warm",) + key
+            _step_eager(model, st)
+            return
+        torch.cuda.synchronize(st.device)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, capture_error_mode="thread_local"):
+            _step_eager(model, st)
+        st.graph, st.graph_key = g, key
+    st.graph.replay()
+
+
+# ------------------------------------------------------------------------------------------------ generate
+def _eos_list(eos) -> list[int]:
+    if eos is None:
+        return []
+    if isinstance(eos, int):
+        return [eos]
+    return [int(e) for e in eos]
+
+
+@torch.no_grad()
+def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, max_new_tokens: int = 20,
+             do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
+             pad_token_id: int | None = None, seed: int = 0) -> torch.Tensor:
+    """See :meth:`LlamaForCausalLM.generate`."""
+    cfg, ar = model.config, model.arena
+    if ar.param_sharded:
+        raise ValueError("generate() needs the full compute weights on this rank; the arena is parameter-sharded (FULL_SHARD)")
+    if input_ids.dim() != 2:
+        raise ValueError(f"input_ids must be [batch, prompt_length], got shape {tuple(input_ids.shape)}")
+    B, P = input_ids.shape
+    if max_new_tokens < 1:
+        raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
+    if P + max_new_tokens > cfg.max_position_embeddings:
+        raise ValueError(f"prompt length {P} + max_new_tokens {max_new_tokens} exceeds max_position_embeddings "
+                         f"{cfg.max_position_embeddings}")
+    if do_sample and not temperature > 0:
+        raise ValueError(f"temperature must be > 0 when sampling, got {temperature}")
+    if do_sample and not 0 < top_p <= 1:
+        raise ValueError(f"top_p must be in (0, 1], got {top_p}")
+    dev = ar.device
+    ids = input_ids.to(dev)
+    if attention_mask is None:
+        lens = torch.full((B,), P, dtype=torch.int32, device=dev)
+    else:
+        m = attention_mask.to(dev).bool()
+        if m.shape != ids.shape:
+            raise ValueError(f"attention_mask shape {tuple(m.shape)} differs from input_ids {tuple(ids.shape)}")
+        if not bool((m[:, 1:] >= m[:, :-1]).all()) or not bool(m[:, -1].all()):
+            raise ValueError("attention_mask must be left-padded: zeros (padding) before ones in every row")
+        lens = m.sum(dim=1).to(torch.int32)
+    eos = _eos_list(cfg.eos_token_id if eos_token_id is None else eos_token_id)
+    pad = pad_token_id if pad_token_id is not None else (eos[0] if eos else 0)
+
+    # compact each row to start at position 0, right-pad to the prefill length
+    kernels = DK.usable(ar.shadow if ar.shadow is not None else ar.master, cfg.head_dim, cfg.num_attention_heads,
+                        cfg.num_key_value_heads)
+    max_len = int(lens.max())
+    Sp = _round_up(max_len, 128) if kernels else max_len
+    Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))
+    st = decode_state(model, B, Smax)
+    col = (P - lens.long())[:, None] + torch.arange(Sp, device=dev)[None, :]
+    comp = ids.gather(1, col.clamp(max=P - 1))
+    comp = comp.masked_fill(torch.arange(Sp, device=dev)[None, :] >= lens.long()[:, None], 0)
+
+    st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos)
+    st.out.fill_(pad)
+    prefill(model, st, comp, lens)
+    for t in range(1, max_new_tokens):
+        if eos and t % FINISHED_CHECK_EVERY == 0 and bool(st.finished.all()):
+            break
+        step(model, st)
+    return torch.cat([ids, st.out[:, :max_new_tokens].clone()], dim=1)

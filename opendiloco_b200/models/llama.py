@@ -121,6 +121,7 @@ class LlamaEngine:
         self.module_hooks: dict[str, Any] = {}     # name -> holder module with user forward hooks
         self.head_grad_tmp: torch.Tensor | None = None
         self._graphs: dict[tuple, dict] = {}       # (B, S, loss_scale, labels-alias) -> captured micro-step
+        self.decode_state = None                   # generation's KV caches + decode graph (models/generation.py)
 
     def workspace(self, B: int, S: int) -> _Workspace:
         key = (B, S, str(self.arena.device), self.arena.compute_dtype)
@@ -562,6 +563,7 @@ class LlamaForCausalLM(nn.Module):
                 self.arena.migrate(device)
                 self.engine._ws.clear()
                 self.engine._graphs.clear()
+                self.engine.decode_state = None
                 self.engine.head_grad_tmp = None
                 self._rebind()
         return self
@@ -606,6 +608,26 @@ class LlamaForCausalLM(nn.Module):
                 and not self.arena.param_sharded):
             return self.engine.forward_backward_graphed(input_ids, labels, loss_scale)
         return self.engine.forward_backward(input_ids, labels, loss_scale, attention_mask)
+
+    @torch.no_grad()
+    def generate(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, max_new_tokens: int = 20,
+                 do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
+                 pad_token_id: int | None = None, seed: int = 0) -> torch.Tensor:
+        """KV-cached text generation with HF ``generate`` keyword names.  Returns LongTensor [B, P + max_new_tokens]: the
+        prompt as given, then the new tokens.
+
+        Prompts may be left-padded with an ``attention_mask``.  ``do_sample=False`` is greedy (ties to the lowest id);
+        otherwise temperature, top-k (0 = off) and top-p are applied in HF's order and tokens are drawn with ``seed``.
+        ``eos_token_id`` (int or list) defaults to ``config.eos_token_id``; after a row emits it, the row is filled with
+        ``pad_token_id`` (default: the first EOS id).  Reads the current compute weights.  bf16-mixed CUDA models run the
+        decode kernels (csrc/decode_sm90.cu) with the step replayed from a CUDA graph; other precisions and devices run the
+        PyTorch reference path.  Raises ValueError for a parameter-sharded (FULL_SHARD) model, a prompt plus
+        ``max_new_tokens`` longer than ``max_position_embeddings``, or a mask that is not left-padded."""
+        from .generation import generate
+
+        return generate(self, input_ids, attention_mask=attention_mask, max_new_tokens=max_new_tokens, do_sample=do_sample,
+                        temperature=temperature, top_k=top_k, top_p=top_p, eos_token_id=eos_token_id, pad_token_id=pad_token_id,
+                        seed=seed)
 
     # ------------------------------------------------------------------ state dict / checkpoints
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):

@@ -1,0 +1,114 @@
+#!/usr/bin/env python
+"""Generate text with a Llama model: an HF directory, a preset (random weights from --init-seed), or a training checkpoint.
+
+    python scripts/generate.py --model 150m --checkpoint outputs/model_step_1000 --weights outer --prompt-ids "1 450 4996"
+    python scripts/generate.py --model /models/llama-150m --prompt "The capital of" --tokenizer /models/llama-150m \\
+        --max-new-tokens 64 --do-sample --temperature 0.8 --top-p 0.95
+
+``--checkpoint`` reads a checkpoint directory written by train_fsdp / utils/ckpt.save_checkpoint (the one holding the
+``*.distcp`` shards, i.e. ``model_step_N`` or its ``diloco_rank_R`` sub-directory).  ``--weights local`` takes the
+worker's own weights (``model``), ``--weights outer`` the DiLoCo global model (``theta_outer``).  Tokenizers are only
+read from a local directory.
+"""
+import argparse
+import json
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import torch  # noqa: E402
+
+from opendiloco_b200.models.config import LlamaConfig  # noqa: E402
+from opendiloco_b200.models.llama import LlamaForCausalLM  # noqa: E402
+
+
+def load_checkpoint_weights(model: LlamaForCausalLM, ckpt_dir: str, weights: str) -> None:
+    """Copy the flat ``model`` (local) or ``theta_outer`` (outer) range of a checkpoint into the model's master weights."""
+    from opendiloco_b200.utils import ckpt
+
+    meta_path = os.path.join(ckpt_dir, ckpt.METADATA_FILE)
+    if not os.path.isfile(meta_path):
+        raise SystemExit(f"error: {ckpt_dir} has no {ckpt.METADATA_FILE}: not a flat-arena checkpoint directory")
+    with open(meta_path) as f:
+        meta = json.load(f)
+    numel = int(meta["numel"])
+    if numel != model.arena.numel:
+        raise SystemExit(f"error: checkpoint holds {numel} parameters, model --model has {model.arena.numel}: wrong --model?")
+    key = {"local": "model", "outer": "theta_outer"}[weights]
+    ckpt._SHARD_CACHE.clear()
+    try:
+        flat = ckpt._assemble(ckpt_dir, key, 0, numel, "cpu")
+    finally:
+        ckpt._SHARD_CACHE.clear()
+    if flat is None:
+        raise SystemExit(f"error: checkpoint {ckpt_dir} has no '{key}' weights"
+                         + (" (it was written without a DiLoCo optimizer, so there is no outer model)" if weights == "outer" else ""))
+    with torch.no_grad():
+        model.arena.master.copy_(flat.to(model.arena.device))
+    model.arena.sync_shadow()
+
+
+def main(argv=None) -> None:
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--model", required=True, help="HF model directory or preset name (150m, 1b, ...)")
+    ap.add_argument("--checkpoint", default=None, help="training checkpoint directory to take the weights from")
+    ap.add_argument("--weights", choices=["local", "outer"], default="local", help="with --checkpoint: local or DiLoCo outer weights")
+    ap.add_argument("--init-seed", type=int, default=0, help="seed of the random weights of a preset without weights")
+    ap.add_argument("--device", default="cuda" if torch.cuda.is_available() else "cpu")
+    ap.add_argument("--precision", default=None, help="bf16-mixed (default on CUDA), 32-true (default on CPU), fp16-mixed")
+    ap.add_argument("--prompt-ids", action="append", default=None, help='space-separated token ids; repeat for a batch')
+    ap.add_argument("--prompt", action="append", default=None, help="prompt text (needs --tokenizer); repeat for a batch")
+    ap.add_argument("--tokenizer", default=None, help="local tokenizer directory (never downloaded)")
+    ap.add_argument("--max-new-tokens", type=int, default=20)
+    ap.add_argument("--do-sample", action="store_true")
+    ap.add_argument("--temperature", type=float, default=1.0)
+    ap.add_argument("--top-k", type=int, default=50)
+    ap.add_argument("--top-p", type=float, default=1.0)
+    ap.add_argument("--eos-token-id", type=int, default=None)
+    ap.add_argument("--pad-token-id", type=int, default=None)
+    ap.add_argument("--seed", type=int, default=0)
+    a = ap.parse_args(argv)
+
+    tok = None
+    if a.tokenizer is not None:
+        from transformers import AutoTokenizer
+
+        tok = AutoTokenizer.from_pretrained(a.tokenizer, local_files_only=True)
+    if (a.prompt is None) == (a.prompt_ids is None):
+        ap.error("give exactly one of --prompt-ids or --prompt")
+    if a.prompt is not None and tok is None:
+        ap.error("--prompt needs --tokenizer")
+    prompts = ([[int(t) for t in p.split()] for p in a.prompt_ids] if a.prompt_ids is not None
+               else [tok(p)["input_ids"] for p in a.prompt])
+    if any(len(p) == 0 for p in prompts):
+        ap.error("empty prompt")
+
+    device = torch.device(a.device)
+    precision = a.precision or ("bf16-mixed" if device.type == "cuda" else "32-true")
+    cfg = LlamaConfig.from_pretrained(a.model)
+    if a.checkpoint is not None:
+        model = LlamaForCausalLM(cfg, device=device, precision=precision, init=False)
+        load_checkpoint_weights(model, a.checkpoint, a.weights)
+    else:
+        model = LlamaForCausalLM.from_pretrained(a.model, config=cfg, device=device, precision=precision, seed=a.init_seed)
+    model.eval()
+
+    # left-pad the batch to a common length
+    P = max(len(p) for p in prompts)
+    ids = torch.zeros(len(prompts), P, dtype=torch.int64)
+    mask = torch.zeros(len(prompts), P, dtype=torch.int64)
+    for i, p in enumerate(prompts):
+        ids[i, P - len(p):] = torch.tensor(p)
+        mask[i, P - len(p):] = 1
+    out = model.generate(ids.to(device), attention_mask=mask.to(device), max_new_tokens=a.max_new_tokens, do_sample=a.do_sample,
+                         temperature=a.temperature, top_k=a.top_k, top_p=a.top_p, eos_token_id=a.eos_token_id,
+                         pad_token_id=a.pad_token_id, seed=a.seed).cpu()
+    for i, p in enumerate(prompts):
+        new = out[i, P:].tolist()
+        print("ids:", " ".join(str(t) for t in p + new))
+        if tok is not None:
+            print("text:", tok.decode(p + new, skip_special_tokens=True))
+
+
+if __name__ == "__main__":
+    main()
