@@ -29,7 +29,11 @@
 //              loss_row = log sum_v e), writes the tile's row sums into one partial plane per 256-column tile and
 //              (training only) stores bf16(e).  Logits are never written.
 //   kLCEdX   : dgrad of the LM head on the shifted exponentials: out = rowscale * acc - g * W[label]
+//   kLCEScore: scoring (evaluation) statistics of the LM head, per row and 256-column plane: the plane maximum m, its lowest
+//              column, s = sum exp(z - m) (every exponent <= 0: exact for any logit range, no clamp) and the label logit z_y
+//              taken from the same accumulator.  Nothing of size [M, N] is written.
 //   kWgradAcc: fp32 reduce-add of the tile into dW (gradient accumulation across micro-batches + split-K over tokens)
+#include <limits.h>
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -49,7 +53,7 @@ constexpr int THREADS = 384;
 constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 1024 /*align*/ + 256 /*barriers*/;
 constexpr int GROUP_M = 8;                 // rasterisation: 8 m-blocks x all n-blocks per super-block (L2 reuse of A and B)
 
-enum Epi { kStore = 0, kSwiGLU = 1, kRoPE = 2, kSwiGLUBwd = 3, kLCEFwd = 4, kLCEdX = 5, kWgradAcc = 6 };
+enum Epi { kStore = 0, kSwiGLU = 1, kRoPE = 2, kSwiGLUBwd = 3, kLCEFwd = 4, kLCEdX = 5, kWgradAcc = 6, kLCEScore = 7 };
 
 // group_m > 0: groups of group_m m-blocks x all n-blocks, m fastest inside a group (A and B tiles of a group stay in L2).
 // group_m == 0: n fastest over the whole problem - for a few n-blocks and a very deep K (the LM-head dX: 4 n-blocks,
@@ -91,6 +95,10 @@ struct Params {
   const float* gscale;       // kLCEdX: device scalar loss_scale / n_valid
   const __nv_bfloat16* wlab; // kLCEdX: the LM-head weight [V, N] (row stride ldwlab) for the one-hot gather
   long long ldwlab;
+  float* sc_max;             // kLCEScore: [num_n][M] plane maxima (labels: [M], < 0 = no label logit written)
+  float* sc_sum;             // kLCEScore: [num_n][M] sum over the plane of exp(z - plane maximum)
+  int* sc_idx;               // kLCEScore: [num_n][M] lowest column holding the plane maximum
+  float* sc_zlab;            // kLCEScore: [M] the label logit
 };
 
 __device__ __forceinline__ void red_add_f2(float* p, float a, float b) {
@@ -367,6 +375,65 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
         st_bf2(crow + col, fmaf(rs, acc[4 * i + 2 * h], -g * w.x), fmaf(rs, acc[4 * i + 2 * h + 1], -g * w.y));
       }
     }
+  } else if constexpr (EPI == kLCEScore) {
+    constexpr float L2E = 1.4426950408889634f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rbase + 8 * h;
+      const bool row_ok = row < p.M;
+      const long long y = row_ok ? p.labels[row] : -1;
+      // columns relative to this thread's first one (n0 + cq): the compares below are against constants
+      const int lim = p.N - n0 - cq;
+      const long long yr = y - n0 - cq;
+      const int lab = (y >= 0 && yr >= 0 && yr < BN) ? (int)yr : -1;
+      // this thread's 64 columns of the row, in increasing order: the maximum (strict > keeps the lowest column) ...
+      float m = -INFINITY, zl = 0.f;
+      int idx = INT_MAX;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float v = acc[4 * i + 2 * h + e];
+          if (8 * i + e < lim && v > m) { m = v; idx = 8 * i + e; }
+          if (8 * i + e == lab) zl = v;
+        }
+      }
+      if (idx != INT_MAX) idx += n0 + cq;
+      // ... then the sum of exp(z - m) with every exponent <= 0
+      const float mb = m * L2E;
+      float s = 0.f;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float x;
+          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(x) : "f"(fmaf(acc[4 * i + 2 * h + e], L2E, -mb)));
+          s += 8 * i + e < lim ? x : 0.f;
+        }
+      }
+      // merge (max, column, sum) over the quad that shares the row
+#pragma unroll
+      for (int off = 1; off <= 2; off <<= 1) {
+        const float mo = __shfl_xor_sync(0xffffffffu, m, off), so = __shfl_xor_sync(0xffffffffu, s, off);
+        const int io = __shfl_xor_sync(0xffffffffu, idx, off);
+        const float mn = fmaxf(m, mo);
+        if (mn != -INFINITY) {
+          float a, b;
+          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(a) : "f"((m - mn) * L2E));
+          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(b) : "f"((mo - mn) * L2E));
+          s = s * a + so * b;
+        }
+        idx = (mo > m || (mo == m && io < idx)) ? io : idx;
+        m = mn;
+      }
+      if (row_ok && (lane & 3) == 0) {
+        const size_t o = (size_t)n_blk * p.M + row;
+        p.sc_max[o] = m;
+        p.sc_sum[o] = s;
+        p.sc_idx[o] = idx;
+      }
+      if (row_ok && lab >= 0 && (lab & 6) == 0) p.sc_zlab[row] = zl;     // this thread owns the label column
+    }
   } else if constexpr (EPI == kWgradAcc) {
     float* dW = reinterpret_cast<float*>(p.C);
 #pragma unroll
@@ -394,6 +461,7 @@ struct LceArgs {
   const float* row_shift = nullptr; float* partials = nullptr; int want_sumsq = 0; int store = 1;
   const float* rowscale = nullptr; const long long* labels = nullptr; const float* gscale = nullptr;
   const void* wlab = nullptr; long long ldwlab = 0;
+  float* sc_max = nullptr; float* sc_sum = nullptr; int* sc_idx = nullptr; float* sc_zlab = nullptr;
 };
 
 template <int EPI, bool A_MN, bool B_MN, int CL = 1>
@@ -439,6 +507,7 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
   p.row_shift = lce.row_shift; p.partials = lce.partials; p.want_sumsq = lce.want_sumsq; p.store = lce.store;
   p.rowscale = lce.rowscale; p.labels = lce.labels; p.gscale = lce.gscale;
   p.wlab = (const __nv_bfloat16*)lce.wlab; p.ldwlab = lce.ldwlab;
+  p.sc_max = lce.sc_max; p.sc_sum = lce.sc_sum; p.sc_idx = lce.sc_idx; p.sc_zlab = lce.sc_zlab;
   const int tiles = p.num_m * p.num_n;
   const int kb_total = ceil_div(K, BK);
   p.splits = 1;
@@ -579,6 +648,19 @@ ODB_EXPORT int odb_lce_dx(const void* E, const void* W, void* dX, int M, int N, 
   a.wlab = W; a.ldwlab = ldw;
   return gemm::launch<gemm::kLCEdX, false, true>(E, W, dX, nullptr, M, N, V, lde, ldw, ldd, 0, 0, 0, 0, nullptr, nullptr, st,
                                                  gemm::ASplit(), a);
+}
+
+// Scoring statistics of logits Z = X W^T without writing Z: per row and 256-column plane pl (planes = odb_lce_planes(V))
+// pmax[pl][M] = max of the plane, pidx[pl][M] = its lowest column, psum[pl][M] = sum exp(z - pmax), and zlab[M] = z[label]
+// (rows with label < 0 leave zlab untouched).  Merged into log-probabilities by odb_lce_score_finalize (lce.cu).
+ODB_EXPORT int odb_lce_score(const void* X, const void* W, int M, int V, int K, long long ldx, long long ldw, const void* labels,
+                             void* pmax, void* psum, void* pidx, void* zlab, cudaStream_t st) {
+  if (K % 8 || ldx % 8 || ldw % 8) return -1;
+  gemm::LceArgs a;
+  a.labels = (const long long*)labels;
+  a.sc_max = (float*)pmax; a.sc_sum = (float*)psum; a.sc_idx = (int*)pidx; a.sc_zlab = (float*)zlab;
+  return gemm::launch<gemm::kLCEScore, false, false>(X, W, nullptr, nullptr, M, V, K, ldx, ldw, 0, 0, 0, 0, 0, nullptr, nullptr, st,
+                                                     gemm::ASplit(), a);
 }
 
 // ---------------------------------------------------------------------------------------------------- weight gradient

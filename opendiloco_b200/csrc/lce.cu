@@ -5,6 +5,8 @@
 //   row r (label y, -100 = ignore):  lse = log sum_j exp(x_j) ;  loss_r = lse - x_y
 //   dlogits_j = (softmax_j - [j == y]) * gscale        gscale = loss_scale / n_valid  (read from device memory)
 // One CTA per row; the whole row is cached in registers (V <= 256*8*NV) so HBM sees one read and one write.
+#include <limits.h>
+
 #include "common.cuh"
 #include "packed_math.cuh"
 
@@ -364,6 +366,68 @@ ODB_EXPORT int odb_lce_finalize(const void* partials, int planes, int T, const v
   launch_pdl(lce_finalize_kernel, dim3(ceil_div(T, LCE_FIN_ROWS)), dim3(256), 0, st, (const float*)partials, planes, T,
              (const long long*)labels, (const float*)gscale, (float*)loss_sum, (float*)sumsq, (float*)rowscale,
              (const __nv_bfloat16*)x, ldx, (__nv_bfloat16*)xs, ldxs, (float*)dW, lddw, h);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+// =============================================================================================== scoring (per-token log-likelihood)
+// Merge of the per-plane statistics of the kLCEScore GEMM epilogue (gemm_sm90.cu), per row t:
+//   M* = max_p m_p ; argmax = lowest idx_p among the planes with m_p == M* ; lse = M* + log sum_p s_p exp(m_p - M*)
+//   logprob[t] = z_label - lse ; greedy[t] = (argmax == label) ; rows with label < 0 give 0 / false
+// Every exponent is <= 0, so the result holds for any logit range.  Same layout as lce_finalize: 256 threads = 4 plane-slices
+// x 64 rows, coalesced over the rows of a plane.
+__device__ __forceinline__ void score_merge(float& m, float& s, int& i, float m2, float s2, int i2) {
+  if (m2 > m) {
+    s = s * expf(m - m2) + s2;
+    m = m2;
+    i = i2;
+  } else if (m2 != -INFINITY) {
+    s += s2 * expf(m2 - m);
+    if (m2 == m && i2 < i) i = i2;
+  }
+}
+
+__global__ void __launch_bounds__(256) lce_score_finalize_kernel(const float* __restrict__ pmax, const float* __restrict__ psum,
+                                                                 const int* __restrict__ pidx, const float* __restrict__ zlab,
+                                                                 int planes, int T, const long long* __restrict__ labels,
+                                                                 float* __restrict__ logprob, bool* __restrict__ greedy,
+                                                                 float* __restrict__ lse_out, int* __restrict__ argmax_out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ float s_m[4][LCE_FIN_ROWS], s_s[4][LCE_FIN_ROWS];
+  __shared__ int s_i[4][LCE_FIN_ROWS];
+  const int r = threadIdx.x & (LCE_FIN_ROWS - 1), q = threadIdx.x >> 6;
+  const int t = blockIdx.x * LCE_FIN_ROWS + r;
+  float m = -INFINITY, s = 0.f;
+  int i = INT_MAX;
+  if (t < T) {
+    for (int pl = q; pl < planes; pl += 4) {
+      const size_t o = (size_t)pl * T + t;
+      score_merge(m, s, i, pmax[o], psum[o], pidx[o]);
+    }
+  }
+  s_m[q][r] = m;
+  s_s[q][r] = s;
+  s_i[q][r] = i;
+  __syncthreads();
+  if (q != 0 || t >= T) return;
+#pragma unroll
+  for (int k = 1; k < 4; ++k) score_merge(m, s, i, s_m[k][r], s_s[k][r], s_i[k][r]);
+  const float lse = m + logf(s);
+  const long long y = labels[t];
+  logprob[t] = y >= 0 ? zlab[t] - lse : 0.f;
+  greedy[t] = y >= 0 && (long long)i == y;
+  if (lse_out) lse_out[t] = lse;
+  if (argmax_out) argmax_out[t] = i;
+}
+
+ODB_EXPORT int odb_lce_score_finalize(const void* pmax, const void* psum, const void* pidx, const void* zlab, int planes, int T,
+                                      const void* labels, void* logprob, void* greedy, void* lse, void* argmax, cudaStream_t st) {
+  if (planes <= 0 || T < 0) return -1;
+  if (T == 0) return 0;
+  launch_pdl(lce_score_finalize_kernel, dim3(ceil_div(T, LCE_FIN_ROWS)), dim3(256), 0, st, (const float*)pmax, (const float*)psum,
+             (const int*)pidx, (const float*)zlab, planes, T, (const long long*)labels, (float*)logprob, (bool*)greedy, (float*)lse,
+             (int*)argmax);
   ODB_CHECK_LAST();
   return 0;
 }

@@ -114,8 +114,7 @@ def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor) -> No
     computes the logits at position lens[b]-1 and samples the first new token (st.pos ends at lens)."""
     cfg, ar = model.config, model.arena
     B, Sp = ids.shape
-    L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-    eps = cfg.rms_norm_eps
+    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     T = B * Sp
     pb = st.prefill_buffers(T)
     st.lens.copy_(lens)
@@ -123,29 +122,42 @@ def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor) -> No
     st.gen.zero_()
     st.finished.zero_()
     pb.ids.copy_(ids.reshape(-1))
-    cos, sin = st.cos[:Sp], st.sin[:Sp]
+    delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
+                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, st.lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D))
+    # only the last real position of every row feeds the LM head: gather its residual and delta rows
+    last = torch.arange(B, device=st.device, dtype=torch.int64) * Sp + st.lens.long() - 1
+    K.embedding_fwd(last, pb.res, out=st.res)
+    K.embedding_fwd(last, delta, out=st.proj)
+    _head_and_sample(cfg, ar, st, st.proj)
+
+
+def forward_layers(model, pb: _PrefillBuffers, B: int, Sp: int, cos, sin, fused_rope: bool, on_qkv=None):
+    """The forward-only layer program over pb.ids [B*Sp] (rows start at position 0; causal attention keeps right padding
+    from reaching real positions): embedding, then per layer rmsnorm -> QKV(+RoPE) GEMM -> attention -> o-proj ->
+    rmsnorm(+residual) -> SwiGLU GEMM -> down.  ``on_qkv(l, qkv)`` sees the rotated projections of layer l.  Returns the
+    last layer's output delta; the residual before it is in pb.res."""
+    cfg, ar = model.config, model.arena
+    L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    eps = cfg.rms_norm_eps
     K.embedding_fwd(pb.ids, ar.w("model.embed_tokens.weight"), out=pb.res)
     delta = None
     for l in range(L):
         p = f"model.layers.{l}."
         K.rmsnorm_fwd(pb.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
-        if st.kernels and TC.usable(pb.xn, ar.qkv_w(l)):
+        if fused_rope and TC.usable(pb.xn, ar.qkv_w(l)):
             TC.linear_qkv_rope(pb.xn, ar.qkv_w(l), pb.qkv, cos, sin, Sp, (Hq + Hkv) * D)
         else:
             G.mm_nt(pb.xn, ar.qkv_w(l), out=pb.qkv)
             K.rope_(pb.qkv, cos, sin, Sp, Hq + Hkv, D)
-        DK.kv_fill(pb.qkv, st.lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D)
+        if on_qkv is not None:
+            on_qkv(l, pb.qkv)
         att, _ = A.attention_fwd(pb.qkv, B, Sp, Hq, Hkv, D)
         G.mm_nt(att, ar.w(p + "self_attn.o_proj.weight"), out=pb.proj)
         K.rmsnorm_fwd(pb.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=pb.proj, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
         _mlp(cfg, ar, l, pb.xn, pb.gu, pb.act)
         G.mm_nt(pb.act, ar.w(p + "mlp.down_proj.weight"), out=pb.proj)
         delta = pb.proj
-    # only the last real position of every row feeds the LM head: gather its residual and delta rows
-    last = torch.arange(B, device=st.device, dtype=torch.int64) * Sp + st.lens.long() - 1
-    K.embedding_fwd(last, pb.res, out=st.res)
-    K.embedding_fwd(last, delta, out=st.proj)
-    _head_and_sample(cfg, ar, st, st.proj)
+    return delta
 
 
 def _mlp(cfg, ar, l: int, xn, gu, act) -> None:

@@ -122,6 +122,7 @@ class LlamaEngine:
         self.head_grad_tmp: torch.Tensor | None = None
         self._graphs: dict[tuple, dict] = {}       # (B, S, loss_scale, labels-alias) -> captured micro-step
         self.decode_state = None                   # generation's KV caches + decode graph (models/generation.py)
+        self.score_state = None                    # scoring buffers (models/scoring.py)
 
     def workspace(self, B: int, S: int) -> _Workspace:
         key = (B, S, str(self.arena.device), self.arena.compute_dtype)
@@ -564,6 +565,7 @@ class LlamaForCausalLM(nn.Module):
                 self.engine._ws.clear()
                 self.engine._graphs.clear()
                 self.engine.decode_state = None
+                self.engine.score_state = None
                 self.engine.head_grad_tmp = None
                 self._rebind()
         return self
@@ -628,6 +630,23 @@ class LlamaForCausalLM(nn.Module):
         return generate(self, input_ids, attention_mask=attention_mask, max_new_tokens=max_new_tokens, do_sample=do_sample,
                         temperature=temperature, top_k=top_k, top_p=top_p, eos_token_id=eos_token_id, pad_token_id=pad_token_id,
                         seed=seed)
+
+    @torch.no_grad()
+    def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None):
+        """Per-token log-likelihoods.  Returns ``ScoreOutput`` with ``logprobs`` (fp32 [B, S], log p(target_t | tokens < t))
+        and ``greedy`` (bool [B, S], the argmax of the prediction at t-1, lowest index on ties, equals target_t), on the
+        model's device.
+
+        Targets follow HF ``labels``: entry t is about token t; ``labels`` (``-100`` = ignored) default to ``input_ids``.
+        Position 0, padded and ignored positions give 0.0 / False.  ``attention_mask`` may hold any one contiguous run of
+        ones per row (left, right or no padding); each row is scored like its unpadded tokens alone, positions from 0.
+        Reads the current compute weights.  bf16-mixed CUDA models run the scoring LM-head kernels (no logits are written,
+        exact for any logit range); other precisions and devices run the PyTorch reference path.  Raises ValueError for a
+        parameter-sharded (FULL_SHARD) model, a sequence longer than ``max_position_embeddings``, mismatched shapes, a mask
+        that is not one run per row, or token / label ids outside the vocabulary."""
+        from .scoring import score
+
+        return score(self, input_ids, attention_mask=attention_mask, labels=labels)
 
     # ------------------------------------------------------------------ state dict / checkpoints
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):

@@ -288,6 +288,39 @@ def lce_finalize(partials: torch.Tensor, planes: int, labels: torch.Tensor, gsca
     _lib.count_launch()
 
 
+_lib.register_optional("odb_lce_score_finalize", [_ct.c_void_p, _ct.c_void_p, _ct.c_void_p, _ct.c_void_p, _ct.c_int, _ct.c_int,
+                                                 _ct.c_void_p, _ct.c_void_p, _ct.c_void_p, _ct.c_void_p, _ct.c_void_p, _ct.c_void_p])
+
+
+def lce_score_finalize(pmax: torch.Tensor, psum: torch.Tensor, pidx: torch.Tensor, zlab: torch.Tensor, planes: int,
+                       labels: torch.Tensor, logprob: torch.Tensor, greedy: torch.Tensor, lse: torch.Tensor | None = None,
+                       argmax: torch.Tensor | None = None) -> None:
+    """Merge the plane statistics of ``tc_gemm.lce_score`` for the T = labels.numel() rows:  lse = M* + log sum_p s_p
+    exp(m_p - M*), argmax = the lowest column holding M*, logprob = zlab - lse (fp32), greedy = (argmax == label) (bool);
+    rows with label < 0 give 0.0 / False.  Optional outputs: lse (fp32) and argmax (int32).  The inputs are fp32
+    statistics whatever the model's precision, so CUDA tensors always run the kernel; CPU tensors the reference."""
+    T = labels.numel()
+    if pmax.is_cuda:
+        assert greedy.dtype == torch.bool and logprob.dtype == torch.float32 and labels.dtype == torch.int64
+        assert argmax is None or argmax.dtype == torch.int32
+        _lib.check(_lib.cuda_lib().odb_lce_score_finalize(_p(pmax), _p(psum), _p(pidx), _p(zlab), planes, T, _p(labels), _p(logprob),
+                                                          _p(greedy), _p(lse), _p(argmax), _lib.stream_ptr(pmax)),
+                   "lce_score_finalize")
+        _lib.count_launch()
+        return
+    m, s, i = (t[: planes * T].view(planes, T) for t in (pmax, psum, pidx))
+    mx = m.amax(dim=0)
+    l = mx + torch.log((s * torch.exp(m - mx)).sum(dim=0))
+    am = torch.where(m == mx, i, torch.iinfo(torch.int32).max).amin(dim=0)
+    valid = labels >= 0
+    logprob.copy_(torch.where(valid, zlab[:T] - l, torch.zeros_like(l)))
+    greedy.copy_(valid & (am.long() == labels))
+    if lse is not None:
+        lse.copy_(l)
+    if argmax is not None:
+        argmax.copy_(am)
+
+
 # ------------------------------------------------------------------------------------------------ optimizer kernels
 HP_LR, HP_B1, HP_B2, HP_EPS, HP_WD, HP_BC1, HP_BC2, HP_MAXNORM, HP_INVSCALE = range(9)
 HP_SIZE = 16

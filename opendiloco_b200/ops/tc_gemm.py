@@ -40,6 +40,9 @@ _lib.register_optional("odb_lce_fwd", [c_void_p, c_void_p, c_void_p, c_int, c_in
 _lib.register_optional("odb_lce_planes", [c_int])
 _lib.register_optional("odb_lce_dx", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_void_p, c_void_p, c_void_p,
                                      c_void_p])
+_lib.register_optional("odb_lce_score", [c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p])
+SCORE_PLANE = 256                   # vocabulary columns per plane of the scoring statistics (the GEMM's tile width)
 
 ENABLED = os.environ.get("ODB_TC_GEMM", "1") != "0"
 FUSE_SWIGLU_BWD = os.environ.get("ODB_TC_SWIGLU_BWD", "1") != "0"
@@ -186,6 +189,36 @@ def lce_dx(e: torch.Tensor, w: torch.Tensor, rowscale: torch.Tensor, labels: tor
                                           out.stride(0), rowscale.data_ptr(), labels.data_ptr(), gscale.data_ptr(),
                                           _lib.stream_ptr(e)), "lce_dx")
     _lib.count_launch()
+
+
+def lce_score(x: torch.Tensor, w: torch.Tensor, labels: torch.Tensor, pmax: torch.Tensor, psum: torch.Tensor, pidx: torch.Tensor,
+              zlab: torch.Tensor) -> None:
+    """Scoring statistics of the logits z = x @ w^T without writing them.  Per row and plane of 256 vocabulary columns
+    (``planes = ceil(V / 256)``; the flat buffers hold [planes, M] with row stride M): ``pmax`` = the plane maximum,
+    ``pidx`` (int32) = its lowest column, ``psum`` = sum exp(z - pmax); ``zlab[:M]`` = z[label] (untouched where label < 0).
+
+    CUDA bf16: the kLCEScore epilogue of the wgmma GEMM.  Other dtypes / CPU: the reference on the fp32 logits chunk."""
+    M = x.shape[0]
+    V = w.shape[0]
+    planes = (V + SCORE_PLANE - 1) // SCORE_PLANE
+    assert pmax.numel() >= planes * M and psum.numel() >= planes * M and pidx.numel() >= planes * M and zlab.numel() >= M
+    assert pidx.dtype == torch.int32 and labels.dtype == torch.int64 and labels.is_contiguous()
+    if lce_usable(x, w) and _lib.has_symbol("odb_lce_score"):
+        _lib.check(_lib.cuda_lib().odb_lce_score(x.data_ptr(), w.data_ptr(), M, V, x.shape[1], x.stride(0), w.stride(0), labels.data_ptr(),
+                                                 pmax.data_ptr(), psum.data_ptr(), pidx.data_ptr(), zlab.data_ptr(), _lib.stream_ptr(x)),
+                   "lce_score")
+        _lib.count_launch()
+        return
+    z = x.float() @ w.float().t()                                                  # [M, V] fp32 logits chunk
+    zp = torch.nn.functional.pad(z, (0, planes * SCORE_PLANE - V), value=float("-inf")).view(M, planes, SCORE_PLANE)
+    m = zp.amax(dim=-1)
+    pmax[: planes * M].view(planes, M).copy_(m.t())
+    psum[: planes * M].view(planes, M).copy_(torch.exp(zp - m[..., None]).sum(dim=-1).t())
+    first = torch.arange(planes, device=z.device, dtype=torch.int64) * SCORE_PLANE
+    pidx[: planes * M].view(planes, M).copy_((zp.argmax(dim=-1) + first).t())     # argmax: the first maximal index
+    valid = labels >= 0
+    zl = z.gather(1, labels.clamp(min=0)[:, None])[:, 0]
+    zlab[:M].copy_(torch.where(valid, zl, zlab[:M]))
 
 
 def linear_qkv_rope(x: torch.Tensor, w: torch.Tensor, qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, S: int,

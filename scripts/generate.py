@@ -48,14 +48,32 @@ def load_checkpoint_weights(model: LlamaForCausalLM, ckpt_dir: str, weights: str
     model.arena.sync_shadow()
 
 
-def main(argv=None) -> None:
-    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+def add_model_args(ap: argparse.ArgumentParser) -> None:
+    """The options that choose the model and its weights (shared with scripts/evaluate.py)."""
     ap.add_argument("--model", required=True, help="HF model directory or preset name (150m, 1b, ...)")
     ap.add_argument("--checkpoint", default=None, help="training checkpoint directory to take the weights from")
     ap.add_argument("--weights", choices=["local", "outer"], default="local", help="with --checkpoint: local or DiLoCo outer weights")
     ap.add_argument("--init-seed", type=int, default=0, help="seed of the random weights of a preset without weights")
     ap.add_argument("--device", default="cuda" if torch.cuda.is_available() else "cpu")
     ap.add_argument("--precision", default=None, help="bf16-mixed (default on CUDA), 32-true (default on CPU), fp16-mixed")
+
+
+def load_model(a: argparse.Namespace) -> LlamaForCausalLM:
+    """The model chosen by the ``add_model_args`` options, in eval mode."""
+    device = torch.device(a.device)
+    precision = a.precision or ("bf16-mixed" if device.type == "cuda" else "32-true")
+    cfg = LlamaConfig.from_pretrained(a.model)
+    if a.checkpoint is not None:
+        model = LlamaForCausalLM(cfg, device=device, precision=precision, init=False)
+        load_checkpoint_weights(model, a.checkpoint, a.weights)
+    else:
+        model = LlamaForCausalLM.from_pretrained(a.model, config=cfg, device=device, precision=precision, seed=a.init_seed)
+    return model.eval()
+
+
+def main(argv=None) -> None:
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    add_model_args(ap)
     ap.add_argument("--prompt-ids", action="append", default=None, help='space-separated token ids; repeat for a batch')
     ap.add_argument("--prompt", action="append", default=None, help="prompt text (needs --tokenizer); repeat for a batch")
     ap.add_argument("--tokenizer", default=None, help="local tokenizer directory (never downloaded)")
@@ -84,14 +102,7 @@ def main(argv=None) -> None:
         ap.error("empty prompt")
 
     device = torch.device(a.device)
-    precision = a.precision or ("bf16-mixed" if device.type == "cuda" else "32-true")
-    cfg = LlamaConfig.from_pretrained(a.model)
-    if a.checkpoint is not None:
-        model = LlamaForCausalLM(cfg, device=device, precision=precision, init=False)
-        load_checkpoint_weights(model, a.checkpoint, a.weights)
-    else:
-        model = LlamaForCausalLM.from_pretrained(a.model, config=cfg, device=device, precision=precision, seed=a.init_seed)
-    model.eval()
+    model = load_model(a)
 
     # left-pad the batch to a common length
     P = max(len(p) for p in prompts)
