@@ -33,6 +33,15 @@
 //              column, s = sum exp(z - m) (every exponent <= 0: exact for any logit range, no clamp) and the label logit z_y
 //              taken from the same accumulator.  Nothing of size [M, N] is written.
 //   kWgradAcc: fp32 reduce-add of the tile into dW (gradient accumulation across micro-batches + split-K over tokens)
+//
+// Element type (ELEM): 0 = bf16 operands (everything above).  1 / 2 = FP8 operands, A e4m3 / e5m2, B e4m3, both K-major
+// (odb_gemm_fp8_*, odb_wgrad_fp8).  An FP8 k-block is 128 elements deep: the same 128-byte swizzle rows as bf16.  The
+// tensor core's FP8 accumulation is narrower than fp32, so each consumer warpgroup issues every k-block as 4 x m64n128k32
+// into a fresh 64-register scratch accumulator, waits, and adds it into its fp32 accumulator: partial sums are promoted to
+// fp32 once per 128 products.  Scratch plus accumulator must fit the 168 registers ptxas allots each thread of a
+// 384-thread CTA (setmaxnreg does not raise that limit at compile time), so the FP8 tile is 128 x 128 (64 + 64 registers)
+// instead of 128 x 256; the epilogues take the tile width as a constant.  They first multiply the accumulator by the two
+// dequantisation factors (device scalars inv_a * inv_b, powers of two), then run as for bf16.
 #include <limits.h>
 #include <stdlib.h>
 
@@ -45,6 +54,7 @@ using namespace sm90;
 namespace gemm {
 
 constexpr int BM = 128, BN = 256, BK = 64;
+constexpr int BK8 = 128;                   // k-block depth of the FP8 kernels (128 one-byte elements = one swizzle row)
 constexpr int A_BYTES = BM * BK * 2;       // 16 KB
 constexpr int B_BYTES = BN * BK * 2;       // 32 KB
 constexpr int BOX_BYTES = 64 * 64 * 2;     // one 64 x 64 box of an MN-major operand
@@ -99,6 +109,8 @@ struct Params {
   float* sc_sum;             // kLCEScore: [num_n][M] sum over the plane of exp(z - plane maximum)
   int* sc_idx;               // kLCEScore: [num_n][M] lowest column holding the plane maximum
   float* sc_zlab;            // kLCEScore: [M] the label logit
+  const float* inv_a;        // FP8: device scalars 1 / scale of A and of B (dequantisation in the epilogue)
+  const float* inv_b;
 };
 
 __device__ __forceinline__ void red_add_f2(float* p, float a, float b) {
@@ -107,11 +119,11 @@ __device__ __forceinline__ void red_add_f2(float* p, float a, float b) {
 __device__ __forceinline__ void st_bf2(void* p, float a, float b) { *reinterpret_cast<uint32_t*>(p) = f2_to_bf2(a, b); }
 __device__ __forceinline__ float2 ld_bf2(const void* p) { return bf2_to_f2(*reinterpret_cast<const uint32_t*>(p)); }
 
-template <int EPI, bool A_MN, bool B_MN, int CL>
+template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM>
 __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_a, uint8_t* smem_b, uint64_t* full_bar,
                                                  uint64_t* empty_bar, int wg, int m0, int n0, int n_blk, int kb0, int kb1);
 
-template <int EPI, bool A_MN, bool B_MN, int CL>
+template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM = 0>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a1,
             const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_b, Params p) {
@@ -124,6 +136,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 
   pdl_launch_dependents();
   static_assert(CL == 1 || (CL == 2 && !B_MN && !A_MN), "clusters share a K-major B tile");
+  static_assert(ELEM == 0 || (CL == 1 && !A_MN && !B_MN), "FP8 wgmma takes K-major operands only");
+  constexpr int KB = ELEM ? BK8 : BK;            // elements per k-block
+  constexpr int BNE = ELEM ? BN / 2 : BN;        // tile columns
   const int wg = threadIdx.x >> 7;
   const uint32_t rank = CL == 2 ? cluster_ctarank() : 0;
   const int work = blockIdx.x / CL;
@@ -131,8 +146,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   int m_blk, n_blk;
   tile_coords(tile, (p.num_m + CL - 1) / CL, p.num_n, p.group_m, m_blk, n_blk);
   m_blk = m_blk * CL + (int)rank;                // CL = 2: this CTA's m-half of the cluster tile (may lie beyond M)
-  const int m0 = m_blk * BM, n0 = n_blk * BN;
-  const int num_k_total = (p.K + BK - 1) / BK;
+  const int m0 = m_blk * BM, n0 = n_blk * BNE;
+  const int num_k_total = (p.K + KB - 1) / KB;
   const int kb0 = split * p.kb_per_split;
   const int kb1 = min(num_k_total, kb0 + p.kb_per_split);
 
@@ -161,14 +176,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       uint32_t phase = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
-        mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
+        mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + BNE * 128);
         uint8_t* sa = smem_a + stage * A_BYTES;
         uint8_t* sb = smem_b + stage * B_BYTES;
         if constexpr (A_MN) {       // [K rows, M cols]: two 64(m) x 64(k) boxes
           tma_load_2d(sa, ta_m, &full_bar[stage], am0, kb * BK);
           tma_load_2d(sa + BOX_BYTES, ta_m, &full_bar[stage], am0 + 64, kb * BK);
         } else {
-          if (p.ks1 == 0 || kb < p.ks1) tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BK, m0);
+          if (p.ks1 == 0 || kb < p.ks1) tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * KB, m0);
           else if (kb < p.ks2) tma_load_2d(sa, &tmap_a1, &full_bar[stage], (kb - p.ks1) * BK, m0);
           else tma_load_2d(sa, &tmap_a2, &full_bar[stage], (kb - p.ks2) * BK, m0);
         }
@@ -177,30 +192,57 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           for (int j = 0; j < 4; ++j) tma_load_2d(sb + j * BOX_BYTES, &tmap_b, &full_bar[stage], n0 + 64 * j, kb * BK);
         } else if constexpr (CL == 2) {   // this CTA's half of B (gate | up for kSwiGLU) into both CTAs
           const int b_row = EPI == kSwiGLU ? (rank == 0 ? n_blk * (BN / 2) : p.I + n_blk * (BN / 2)) : n0 + (int)rank * (BN / 2);
-          tma_load_2d_multicast(sb + rank * (B_BYTES / 2), &tmap_b, &full_bar[stage], kb * BK, b_row, (uint16_t)0x3);
+          tma_load_2d_multicast(sb + rank * (B_BYTES / 2), &tmap_b, &full_bar[stage], kb * KB, b_row, (uint16_t)0x3);
         } else if constexpr (EPI == kSwiGLU) {
-          const int g0 = n_blk * (BN / 2);
-          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BK, g0);
-          tma_load_2d(sb + B_BYTES / 2, &tmap_b, &full_bar[stage], kb * BK, p.I + g0);
+          const int g0 = n_blk * (BNE / 2);
+          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, g0);
+          tma_load_2d(sb + BNE / 2 * 128, &tmap_b, &full_bar[stage], kb * KB, p.I + g0);
         } else {
-          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BK, n0);
+          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, n0);
         }
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
   } else {
-    mma_and_epilogue<EPI, A_MN, B_MN, CL>(p, smem_a, smem_b, full_bar, empty_bar, wg, m0, n0, n_blk, kb0, kb1);
+    mma_and_epilogue<EPI, A_MN, B_MN, CL, ELEM>(p, smem_a, smem_b, full_bar, empty_bar, wg, m0, n0, n_blk, kb0, kb1);
   }
   if constexpr (CL == 2) cluster_sync();         // no CTA leaves while its peer may still arrive on its barriers
 }
 
-template <int EPI, bool A_MN, bool B_MN, int CL>
+template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM>
 __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_a, uint8_t* smem_b, uint64_t* full_bar,
                                                  uint64_t* empty_bar, int wg, int m0, int n0, int n_blk, int kb0, int kb1) {
   reg_alloc<232>();
   const int cw = wg - 1;                         // this warpgroup's 64 rows of the tile
+  constexpr int NI = ELEM ? 16 : 32;             // 8-column groups of the tile: acc[4*i + 2*h + e], i < NI
+  constexpr int BNE = 8 * NI;
   float acc[128];
-  {
+  if constexpr (ELEM != 0) {
+    // FP8: per k-block 4 x k32 into `part` (same fragment layout as acc[0..63]), then acc += part in fp32 (promotion)
+    float part[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint64_t adesc = make_smem_desc_sw128(smem_u32(smem_a + stage * A_BYTES) + cw * 64 * 128, 16, 1024);
+      const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smem_b + stage * B_BYTES), 16, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK8 / 32; ++k)         // 32 fp8 = 32 bytes further along the swizzle row (+2 descriptor units)
+        wgmma_m64n128k32_f8<ELEM>(part, adesc + 2 * k, bdesc + 2 * k, k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);     // the k-block has retired: release the stage
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] += part[j];
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    const float dq = *p.inv_a * *p.inv_b;
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc[j] *= dq;
+  } else {
     int stage = 0, prev_stage = 0;
     uint32_t phase = 0;
     for (int kb = kb0; kb < kb1; ++kb) {
@@ -245,7 +287,7 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
       if (EPI == kRoPE && rope_tile) {
         const int pos = row % p.S;
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
+        for (int c = 0; c < NI / 8; ++c) {
           if (n0 + c * 64 >= p.rope_cols) continue;
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
@@ -264,27 +306,27 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
       }
       __nv_bfloat16* crow = C + (size_t)row * p.ldc;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
+      for (int i = 0; i < NI; ++i) {
         const int col = n0 + 8 * i + cq;
         if (col + 1 < p.N) st_bf2(crow + col, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
         else if (col < p.N) crow[col] = __float2bfloat16_rn(acc[4 * i + 2 * h]);
       }
     }
   } else if constexpr (EPI == kSwiGLU) {
-    // tile columns [0,128) are gate columns g0.., [128,256) the matching up columns
+    // tile columns [0,BNE/2) are gate columns g0.., [BNE/2,BNE) the matching up columns
     __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.C);
     __nv_bfloat16* act = reinterpret_cast<__nv_bfloat16*>(p.aux);
-    const int g0 = n_blk * (BN / 2);
+    const int g0 = n_blk * (BNE / 2);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = rbase + 8 * h;
       if (row >= p.M) continue;
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
+      for (int i = 0; i < NI / 2; ++i) {
         const int col = g0 + 8 * i + cq;
         if (col >= p.I) continue;                // I % 64 == 0: pairs never straddle the end
         const float ga = acc[4 * i + 2 * h], gb = acc[4 * i + 2 * h + 1];
-        const float ua = acc[4 * (i + 16) + 2 * h], ub = acc[4 * (i + 16) + 2 * h + 1];
+        const float ua = acc[4 * (i + NI / 2) + 2 * h], ub = acc[4 * (i + NI / 2) + 2 * h + 1];
         st_bf2(gu + (size_t)row * p.ldc + col, ga, gb);
         st_bf2(gu + (size_t)row * p.ldc + p.I + col, ua, ub);
         // the activation is computed from the bf16 values the backward will see
@@ -300,7 +342,7 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
       if (row >= p.M) continue;
       __nv_bfloat16* grow = gu + (size_t)row * p.ldc;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
+      for (int i = 0; i < NI; ++i) {
         const int col = n0 + 8 * i + cq;
         if (col >= p.I) continue;
         const float2 g = ld_bf2(grow + col), u = ld_bf2(grow + p.I + col);
@@ -318,6 +360,7 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
       }
     }
   } else if constexpr (EPI == kLCEFwd) {
+    static_assert(ELEM == 0, "bf16 only");
     constexpr float L2E = 1.4426950408889634f;
     __nv_bfloat16* E = reinterpret_cast<__nv_bfloat16*>(p.C);
 #pragma unroll
@@ -442,7 +485,7 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
       if (row >= p.M) continue;
       float* drow = dW + (size_t)row * p.ldc;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
+      for (int i = 0; i < NI; ++i) {
         const int col = n0 + 8 * i + cq;
         if (col + 1 < p.N) red_add_f2(drow + col, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
         else if (col < p.N) atomicAdd(drow + col, acc[4 * i + 2 * h]);
@@ -464,13 +507,19 @@ struct LceArgs {
   float* sc_max = nullptr; float* sc_sum = nullptr; int* sc_idx = nullptr; float* sc_zlab = nullptr;
 };
 
-template <int EPI, bool A_MN, bool B_MN, int CL = 1>
+template <int EPI, bool A_MN, bool B_MN, int CL = 1, int ELEM = 0>
 static int launch(const void* A, const void* B, void* C, void* aux, int M, int N, int K, long long lda, long long ldb,
                   long long ldc, long long ldaux, int I, int S, int rope_cols, const float* cos_t, const float* sin_t,
-                  cudaStream_t st, const ASplit& sp = ASplit(), const LceArgs& lce = LceArgs()) {
+                  cudaStream_t st, const ASplit& sp = ASplit(), const LceArgs& lce = LceArgs(), const float* inv_a = nullptr,
+                  const float* inv_b = nullptr) {
+  constexpr int EB = ELEM ? 1 : 2;               // operand bytes per element
+  constexpr int KB = ELEM ? BK8 : BK;
+  constexpr int BNE = ELEM ? BN / 2 : BN;        // tile columns
   CUtensorMap ta, ta1, ta2, tb;
   int rc;
-  if (A_MN) {          // A given as [K rows, M cols] (possibly three tensors side by side along M)
+  if (ELEM) {          // FP8: K-major A and B, no split, no cluster
+    if ((rc = make_tmap_2d(&ta, A, M, K, lda, BM, KB, EB))) return rc;
+  } else if (A_MN) {          // A given as [K rows, M cols] (possibly three tensors side by side along M)
     if ((rc = make_tmap_2d(&ta, A, K, sp.K0 ? sp.K0 : M, lda * 2, 64, 64, 2))) return rc;
   } else {
     if ((rc = make_tmap_2d(&ta, A, M, sp.K0 ? sp.K0 : K, lda * 2, BM, BK, 2))) return rc;
@@ -488,16 +537,16 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
   if (B_MN) {
     if ((rc = make_tmap_2d(&tb, B, K, N, ldb * 2, 64, 64, 2))) return rc;            // [K rows, N cols], 64 x 64 boxes
   } else if (EPI == kSwiGLU) {
-    if ((rc = make_tmap_2d(&tb, B, 2 * I, K, ldb * 2, BN / 2, BK, 2))) return rc;
+    if ((rc = make_tmap_2d(&tb, B, 2 * I, K, ldb * EB, BNE / 2, KB, EB))) return rc;
   } else if (CL == 2) {
     if ((rc = make_tmap_2d(&tb, B, N, K, ldb * 2, BN / 2, BK, 2))) return rc;      // each CTA of the pair loads one half
   } else {
-    if ((rc = make_tmap_2d(&tb, B, N, K, ldb * 2, BN, BK, 2))) return rc;
+    if ((rc = make_tmap_2d(&tb, B, N, K, ldb * EB, BNE, KB, EB))) return rc;
   }
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.num_m = ceil_div(M, BM);
-  p.num_n = (EPI == kSwiGLU) ? ceil_div(I, BN / 2) : ceil_div(N, BN);
+  p.num_n = (EPI == kSwiGLU) ? ceil_div(I, BNE / 2) : ceil_div(N, BNE);
   p.group_m = EPI == kLCEdX ? 0 : GROUP_M;
   p.C = C; p.ldc = ldc; p.aux = aux; p.ldaux = ldaux;
   p.I = I; p.S = S > 0 ? S : 1; p.rope_cols = rope_cols; p.cos_t = cos_t; p.sin_t = sin_t;
@@ -508,8 +557,9 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
   p.rowscale = lce.rowscale; p.labels = lce.labels; p.gscale = lce.gscale;
   p.wlab = (const __nv_bfloat16*)lce.wlab; p.ldwlab = lce.ldwlab;
   p.sc_max = lce.sc_max; p.sc_sum = lce.sc_sum; p.sc_idx = lce.sc_idx; p.sc_zlab = lce.sc_zlab;
+  p.inv_a = inv_a; p.inv_b = inv_b;
   const int tiles = p.num_m * p.num_n;
-  const int kb_total = ceil_div(K, BK);
+  const int kb_total = ceil_div(K, KB);
   p.splits = 1;
   p.kb_per_split = kb_total;
   if (EPI == kWgradAcc) {
@@ -527,12 +577,13 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
   }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_kernel<EPI, A_MN, B_MN, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gemm_kernel<EPI, A_MN, B_MN, CL, ELEM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         SMEM_BYTES);
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
   const int cluster_tiles = ceil_div(p.num_m, CL) * p.num_n;
-  launch_pdl_cluster(gemm_kernel<EPI, A_MN, B_MN, CL>, dim3(cluster_tiles * CL * p.splits), dim3(THREADS), SMEM_BYTES, st, CL,
+  launch_pdl_cluster(gemm_kernel<EPI, A_MN, B_MN, CL, ELEM>, dim3(cluster_tiles * CL * p.splits), dim3(THREADS), SMEM_BYTES, st, CL,
                      ta, ta1, ta2, tb, p);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : (int)e;
@@ -678,4 +729,57 @@ ODB_EXPORT int odb_wgrad_bf16(const void* dY0, const void* dY1, const void* dY2,
   if (n1 || n2) { sp.A1 = dY1; sp.A2 = dY2; sp.lda1 = ld1; sp.lda2 = ld2; sp.K0 = n0; sp.K1 = n1; sp.K2 = n2; }
   return gemm::launch<gemm::kWgradAcc, true, true>(dY0, X, dW, nullptr, N_out, K_out, T, ld0, ldx, ldw, 0, 0, 0, 0, nullptr,
                                                    nullptr, st, sp);
+}
+
+// ---------------------------------------------------------------------------------------------------- FP8 (e4m3 / e5m2)
+// Operands are FP8 bytes, K-major (row strides in elements = bytes, multiples of 16); inv_a / inv_b are device fp32 scalars
+// (1 / scale of each operand, written by odb_fp8_cast) that the epilogue multiplies into the fp32 accumulator.
+// a_e5m2 = 0: A is e4m3 (forward), 1: A is e5m2 (gradients).  B is always e4m3.  Outputs are as for the bf16 exports.
+static bool fp8_ok(int K, long long lda, long long ldb) { return K % 16 == 0 && lda % 16 == 0 && ldb % 16 == 0; }
+
+// C[M,N] (bf16) = A[M,K] * B[N,K]^T
+ODB_EXPORT int odb_gemm_fp8_tn(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
+                               int a_e5m2, const void* inv_a, const void* inv_b, cudaStream_t st) {
+  if (!fp8_ok(K, lda, ldb) || ldc % 8) return -1;
+  if (a_e5m2)
+    return gemm::launch<gemm::kStore, false, false, 1, 2>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st,
+                                                          gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a, (const float*)inv_b);
+  return gemm::launch<gemm::kStore, false, false, 1, 1>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st,
+                                                        gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a, (const float*)inv_b);
+}
+
+// as odb_gemm_qkv_rope with e4m3 x[M,K] and Wqkv[N,K]
+ODB_EXPORT int odb_gemm_fp8_qkv_rope(const void* X, const void* W, void* qkv, int M, int N, int K, int S, int rope_cols,
+                                     const void* cos_t, const void* sin_t, const void* inv_a, const void* inv_b, cudaStream_t st) {
+  if (!fp8_ok(K, K, K) || N % 64 || rope_cols % 64) return -1;
+  return gemm::launch<gemm::kRoPE, false, false, 1, 1>(X, W, qkv, nullptr, M, N, K, K, K, N, 0, 0, S, rope_cols, (const float*)cos_t,
+                                                       (const float*)sin_t, st, gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a,
+                                                       (const float*)inv_b);
+}
+
+// as odb_gemm_swiglu with e4m3 x[M,K] and Wgu[2I,K]
+ODB_EXPORT int odb_gemm_fp8_swiglu(const void* X, const void* Wgu, void* gu, void* act, int M, int I, int K, const void* inv_a,
+                                   const void* inv_b, cudaStream_t st) {
+  if (!fp8_ok(K, K, K) || I % 64) return -1;
+  return gemm::launch<gemm::kSwiGLU, false, false, 1, 1>(X, Wgu, gu, act, M, 2 * I, K, K, K, 2 * I, I, I, 0, 0, nullptr, nullptr, st,
+                                                         gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a, (const float*)inv_b);
+}
+
+// as odb_gemm_swiglu_bwd with e5m2 dY[M,K] and e4m3 WdT[I,K] (the transposed down-projection weight)
+ODB_EXPORT int odb_gemm_fp8_swiglu_bwd(const void* dY, const void* WdT, void* gu, int M, int I, int K, long long lda, long long ldb,
+                                       const void* inv_a, const void* inv_b, cudaStream_t st) {
+  if (!fp8_ok(K, lda, ldb) || I % 64) return -1;
+  return gemm::launch<gemm::kSwiGLUBwd, false, false, 1, 2>(dY, WdT, gu, nullptr, M, I, K, lda, ldb, 2 * I, 0, I, 0, 0, nullptr, nullptr,
+                                                            st, gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a,
+                                                            (const float*)inv_b);
+}
+
+// dW[N_out, K_out] (fp32, row stride ldw) += dYt[N_out, T] * Xt[K_out, T]^T with e5m2 dYt and e4m3 Xt: the transposed
+// copies written by odb_fp8_cast, so that the reduction over tokens is the K-major dimension.  Split-K over T as for bf16.
+ODB_EXPORT int odb_wgrad_fp8(const void* dYt, const void* Xt, void* dW, int N_out, int K_out, int T, long long ld_dyt, long long ld_xt,
+                             long long ldw, const void* inv_a, const void* inv_b, cudaStream_t st) {
+  if (!fp8_ok(T, ld_dyt, ld_xt) || ldw % 4 || T <= 0) return -1;
+  return gemm::launch<gemm::kWgradAcc, false, false, 1, 2>(dYt, Xt, dW, nullptr, N_out, K_out, T, ld_dyt, ld_xt, ldw, 0, 0, 0, 0,
+                                                           nullptr, nullptr, st, gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a,
+                                                           (const float*)inv_b);
 }

@@ -23,6 +23,7 @@ from torch import nn
 
 from .. import _lib
 from ..ops import attention as A
+from ..ops import fp8 as F
 from ..ops import gemm as G
 from ..ops import kernels as K
 from ..ops import tc_gemm as TC
@@ -92,6 +93,7 @@ class _Workspace:
         self.n_valid = torch.ones(1, dtype=f32, device=device)
         self.sumsq = torch.zeros(1, dtype=f32, device=device)
         self.cos, self.sin = K.rope_tables(S, cfg.head_dim, cfg.rope_theta, device)
+        self.fp8: _Fp8Workspace | None = None      # precision="fp8-mixed" only
 
     @property
     def logits(self) -> torch.Tensor:
@@ -109,9 +111,77 @@ class _Workspace:
         return self._lce
 
 
+class _Fp8Workspace:
+    """FP8 buffers of one (B, S) workspace (``precision="fp8-mixed"``, see ops/fp8.py for the recipe).
+
+    Saved per layer: the transposed e4m3 copies of the four projection inputs (xn1, att, xn2, act), the K-major B operands
+    of the weight gradients.  Transient: one row-major e4m3 activation copy, one row-major and one transposed e4m3 weight
+    copy, and the row-major and transposed e5m2 copies of one gradient; each is consumed by the GEMMs right after its cast.
+    Device scalars per layer (amax / inv, index = ``_F8_*``): four activations, four weights (the backward's transposed
+    weight cast reuses the forward's amax), four gradients."""
+
+    def __init__(self, cfg: LlamaConfig, T: int, device):
+        h, I, L, qd, n_qkv = cfg.hidden_size, cfg.intermediate_size, cfg.num_hidden_layers, cfg.q_dim, cfg.qkv_dim
+        e = lambda *shape, dt=F.E4M3: torch.empty(*shape, dtype=dt, device=device)  # noqa: E731
+        self.T = T
+        self.xn1_t = [e(h, T) for _ in range(L)]
+        self.att_t = [e(qd, T) for _ in range(L)]
+        self.xn2_t = [e(h, T) for _ in range(L)]
+        self.act_t = [e(I, T) for _ in range(L)]
+        self.a_row = e(T * max(h, qd, I))
+        w_max = max(n_qkv * h, h * qd, 2 * I * h)
+        self.w_row, self.w_t = e(w_max), e(w_max)
+        g_max = T * max(h, 2 * I, n_qkv)
+        self.g_row, self.g_t = e(g_max, dt=F.E5M2), e(g_max, dt=F.E5M2)
+        self.amax = torch.zeros(L, 12, dtype=torch.float32, device=device)
+        self.inv = torch.ones(L, 12, dtype=torch.float32, device=device)
+
+    def _slot(self, l: int, i: int):
+        return self.amax[l, i:i + 1], self.inv[l, i:i + 1]
+
+    def act(self, l: int, i: int, x: torch.Tensor, x_t: torch.Tensor):
+        """e4m3 copies of a projection input: row-major (transient, returned) and transposed (``x_t``, saved)."""
+        T, n = x.shape
+        row = self.a_row[: T * n].view(T, n)
+        slot, inv = self._slot(l, i)
+        F.quantize(x, slot, inv, F.E4M3, out=row, out_t=x_t)
+        return row, inv
+
+    def weight(self, l: int, i: int, w: torch.Tensor):
+        """Row-major e4m3 copy of a compute weight for the forward GEMM."""
+        row = self.w_row[: w.numel()].view(w.shape)
+        slot, inv = self._slot(l, 4 + i)
+        F.quantize(w, slot, inv, F.E4M3, out=row)
+        return row, inv
+
+    def weight_t(self, l: int, i: int, w: torch.Tensor):
+        """Transposed e4m3 copy of a compute weight for the dgrad GEMM, scaled with the forward's amax."""
+        t = self.w_t[: w.numel()].view(w.shape[1], w.shape[0])
+        slot, inv = self._slot(l, 4 + i)
+        F.cast(w, slot, F.E4M3, inv, out_t=t)
+        return t, inv
+
+    def grad(self, l: int, i: int, g: torch.Tensor):
+        """e5m2 copies of a gradient: row-major (dgrad A operand) and transposed (weight-gradient A operand)."""
+        T, n = g.shape
+        row, t = self.g_row[: T * n].view(T, n), self.g_t[: T * n].view(n, T)
+        slot, inv = self._slot(l, 8 + i)
+        F.quantize(g, slot, inv, F.E5M2, out=row, out_t=t)
+        return row, t, inv
+
+    def act_inv(self, l: int, i: int) -> torch.Tensor:
+        return self.inv[l, i:i + 1]
+
+
+# slot indices of the four projection groups (activation i, weight 4 + i, gradient 8 + i)
+_F8_QKV, _F8_O, _F8_GU, _F8_DOWN = 0, 1, 2, 3
+
+
 class LlamaEngine:
-    def __init__(self, cfg: LlamaConfig, arena: ParamArena, lce_chunk: int = 32768):
+    def __init__(self, cfg: LlamaConfig, arena: ParamArena, lce_chunk: int = 32768, fp8: bool = False):
         self.cfg, self.arena = cfg, arena
+        # precision="fp8-mixed": the q|k|v, o, gate|up and down projections run as FP8 GEMMs (forward, dgrad, wgrad)
+        self.fp8 = fp8
         # rows of the logits tile of the chunked linear-cross-entropy (ODB_LCE_CHUNK overrides: larger = fewer, fuller GEMM
         # launches and less reduce-add traffic into the lm_head gradient, at 64 KB of bf16 logits per row)
         self.lce_chunk = int(os.environ.get("ODB_LCE_CHUNK", lce_chunk))
@@ -133,7 +203,11 @@ class LlamaEngine:
                 self._ws.pop(old)
                 for gk in [k for k in self._graphs if k[:2] == old[:2]]:      # graphs captured on the evicted buffers
                     del self._graphs[gk]
+            if self.fp8 and self.arena.device.type == "cuda":
+                F.check_tokens(B * S)
             ws = _Workspace(self.cfg, B, S, self.arena.device, self.arena.compute_dtype, self.lce_chunk)
+            if self.fp8:
+                ws.fp8 = _Fp8Workspace(self.cfg, B * S, self.arena.device)
             self._ws[key] = ws
         return ws
 
@@ -148,6 +222,7 @@ class LlamaEngine:
         cfg, ar = self.cfg, self.arena
         B, S, L = ws.B, ws.S, cfg.num_hidden_layers
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+        f8 = ws.fp8
         ws.ids.copy_(ids.reshape(-1), non_blocking=True)
         K.embedding_fwd(ws.ids, ar.w("model.embed_tokens.weight"), out=ws.xa[0])
         delta = None
@@ -157,7 +232,11 @@ class LlamaEngine:
             # --- attention block:  xa = x_prev + delta ; xn1 = norm(xa)
             K.rmsnorm_fwd(x_prev, ar.w(p + "input_layernorm.weight"), cfg.rms_norm_eps, delta=delta, out=ws.xn1[l],
                           rstd=ws.rstd1[l], x_out=ws.xa[l])
-            if D == 64 and TC.usable(ws.xn1[l], ar.qkv_w(l)):
+            if f8 is not None:
+                xq, ix = f8.act(l, _F8_QKV, ws.xn1[l], f8.xn1_t[l])
+                wq, iw = f8.weight(l, _F8_QKV, ar.qkv_w(l))
+                F.linear_qkv_rope(xq, wq, ix, iw, ws.qkv[l], ws.cos, ws.sin, S, Hq + Hkv, D)
+            elif D == 64 and TC.usable(ws.xn1[l], ar.qkv_w(l)):
                 # wgmma GEMM with the rotary embedding applied in the epilogue (no separate RoPE pass over q|k)
                 TC.linear_qkv_rope(ws.xn1[l], ar.qkv_w(l), ws.qkv[l], ws.cos, ws.sin, S, (Hq + Hkv) * D)
             else:
@@ -167,19 +246,32 @@ class LlamaEngine:
                 ws.att[l], ws.aux[l] = A.attention_fwd(ws.qkv[l], B, S, Hq, Hkv, D)
             else:
                 ws.att[l], ws.aux[l] = _masked_attention_fwd(ws.qkv[l], attention_mask, B, S, Hq, Hkv, D)
-            G.mm_nt(ws.att[l], ar.w(p + "self_attn.o_proj.weight"), out=ws.proj)
+            if f8 is not None:
+                xq, ix = f8.act(l, _F8_O, ws.att[l], f8.att_t[l])
+                wq, iw = f8.weight(l, _F8_O, ar.w(p + "self_attn.o_proj.weight"))
+                F.linear(xq, wq, ix, iw, out=ws.proj)
+            else:
+                G.mm_nt(ws.att[l], ar.w(p + "self_attn.o_proj.weight"), out=ws.proj)
             if self.collect_act_norms:
                 self.act_norms[f"activation/{p}self_attn"] = ws.proj.float().norm(p=2)
             self._fire_hooks(p + "self_attn", ws.proj)
             # --- MLP block:  xm = xa + proj ; xn2 = norm(xm)
             K.rmsnorm_fwd(ws.xa[l], ar.w(p + "post_attention_layernorm.weight"), cfg.rms_norm_eps, delta=ws.proj,
                           out=ws.xn2[l], rstd=ws.rstd2[l], x_out=ws.xm[l])
-            if cfg.intermediate_size % 64 == 0 and TC.usable(ws.xn2[l], ar.gu_w(l)):
-                TC.linear_swiglu(ws.xn2[l], ar.gu_w(l), ws.gu[l], ws.act[l])     # SwiGLU is the GEMM epilogue
+            if f8 is not None:
+                xq, ix = f8.act(l, _F8_GU, ws.xn2[l], f8.xn2_t[l])
+                wq, iw = f8.weight(l, _F8_GU, ar.gu_w(l))
+                F.linear_swiglu(xq, wq, ix, iw, ws.gu[l], ws.act[l])
+                xq, ix = f8.act(l, _F8_DOWN, ws.act[l], f8.act_t[l])
+                wq, iw = f8.weight(l, _F8_DOWN, ar.w(p + "mlp.down_proj.weight"))
+                F.linear(xq, wq, ix, iw, out=ws.proj)
             else:
-                G.mm_nt(ws.xn2[l], ar.gu_w(l), out=ws.gu[l])
-                K.swiglu_fwd(ws.gu[l], out=ws.act[l])
-            G.mm_nt(ws.act[l], ar.w(p + "mlp.down_proj.weight"), out=ws.proj)
+                if cfg.intermediate_size % 64 == 0 and TC.usable(ws.xn2[l], ar.gu_w(l)):
+                    TC.linear_swiglu(ws.xn2[l], ar.gu_w(l), ws.gu[l], ws.act[l])     # SwiGLU is the GEMM epilogue
+                else:
+                    G.mm_nt(ws.xn2[l], ar.gu_w(l), out=ws.gu[l])
+                    K.swiglu_fwd(ws.gu[l], out=ws.act[l])
+                G.mm_nt(ws.act[l], ar.w(p + "mlp.down_proj.weight"), out=ws.proj)
             delta = ws.proj
         K.rmsnorm_fwd(ws.xm[L - 1], ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=ws.xnf, rstd=ws.rstdf,
                       x_out=ws.xf)
@@ -291,25 +383,42 @@ class LlamaEngine:
         cfg, ar = self.cfg, self.arena
         B, S, L = ws.B, ws.S, cfg.num_hidden_layers
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+        f8 = ws.fp8
         K.rmsnorm_bwd(ws.dxnf, ws.xf, ar.w("model.norm.weight"), ws.rstdf, None, ws.dx, ar.g("model.norm.weight"))
         for l in reversed(range(L)):
             p = f"model.layers.{l}."
             # ---- MLP block (ws.dx is the gradient of x_out = xm + down(act))
-            G.mm_tn_acc(ws.dx, ws.act[l], ar.g(p + "mlp.down_proj.weight"))
             w_down = ar.w(p + "mlp.down_proj.weight")
-            if TC.swiglu_bwd_usable(ws.dx, w_down, ws.gu[l]):
-                TC.linear_swiglu_bwd(ws.dx, w_down, ws.gu[l])              # dgrad GEMM with the SwiGLU backward as epilogue
+            if f8 is not None:
+                gq, gt, ig = f8.grad(l, _F8_DOWN, ws.dx)
+                F.wgrad(gt, f8.act_t[l], ig, f8.act_inv(l, _F8_DOWN), ar.g(p + "mlp.down_proj.weight"))
+                wt, iw = f8.weight_t(l, _F8_DOWN, w_down)
+                F.linear_swiglu_bwd(gq, wt, ig, iw, ws.gu[l])
+                gq, gt, ig = f8.grad(l, _F8_GU, ws.gu[l])
+                F.wgrad(gt, f8.xn2_t[l], ig, f8.act_inv(l, _F8_GU), ar.gu_g(l))
+                wt, iw = f8.weight_t(l, _F8_GU, ar.gu_w(l))
+                F.linear(gq, wt, ig, iw, out=ws.dn)
             else:
-                G.mm_nn(ws.dx, w_down, out=ws.dact)
-                K.swiglu_bwd(ws.dact, ws.gu[l], ws.gu[l])                  # in place: gu <- d(gu)
-            G.mm_tn_acc(ws.gu[l], ws.xn2[l], ar.gu_g(l))
-            G.mm_nn(ws.gu[l], ar.gu_w(l), out=ws.dn)
+                G.mm_tn_acc(ws.dx, ws.act[l], ar.g(p + "mlp.down_proj.weight"))
+                if TC.swiglu_bwd_usable(ws.dx, w_down, ws.gu[l]):
+                    TC.linear_swiglu_bwd(ws.dx, w_down, ws.gu[l])              # dgrad GEMM with the SwiGLU backward as epilogue
+                else:
+                    G.mm_nn(ws.dx, w_down, out=ws.dact)
+                    K.swiglu_bwd(ws.dact, ws.gu[l], ws.gu[l])                  # in place: gu <- d(gu)
+                G.mm_tn_acc(ws.gu[l], ws.xn2[l], ar.gu_g(l))
+                G.mm_nn(ws.gu[l], ar.gu_w(l), out=ws.dn)
             K.rmsnorm_bwd(ws.dn, ws.xm[l], ar.w(p + "post_attention_layernorm.weight"), ws.rstd2[l], ws.dx, ws.dx,
                           ar.g(p + "post_attention_layernorm.weight"))
             # ---- attention block (ws.dx is now the gradient of xm = xa + o(att))
-            G.mm_tn_acc(ws.dx, ws.att[l], ar.g(p + "self_attn.o_proj.weight"))
-            G.mm_nn(ws.dx, ar.w(p + "self_attn.o_proj.weight"), out=ws.datt)
-            parts_ok = (attention_mask is None and cfg.q_dim % 64 == 0 and cfg.kv_dim % 64 == 0
+            if f8 is not None:
+                gq, gt, ig = f8.grad(l, _F8_O, ws.dx)
+                F.wgrad(gt, f8.att_t[l], ig, f8.act_inv(l, _F8_O), ar.g(p + "self_attn.o_proj.weight"))
+                wt, iw = f8.weight_t(l, _F8_O, ar.w(p + "self_attn.o_proj.weight"))
+                F.linear(gq, wt, ig, iw, out=ws.datt)
+            else:
+                G.mm_tn_acc(ws.dx, ws.att[l], ar.g(p + "self_attn.o_proj.weight"))
+                G.mm_nn(ws.dx, ar.w(p + "self_attn.o_proj.weight"), out=ws.datt)
+            parts_ok = (f8 is None and attention_mask is None and cfg.q_dim % 64 == 0 and cfg.kv_dim % 64 == 0
                         and TC.nn_usable(ws.datt, ar.qkv_w(l)))
             if attention_mask is None:
                 res = A.attention_bwd(ws.datt, ws.qkv[l], ws.att[l], ws.aux[l], ws.dqkv, B, S, Hq, Hkv, D, want_parts=parts_ok,
@@ -334,8 +443,14 @@ class LlamaEngine:
             else:
                 if attention_mask is not None or not A.bwd_applies_rope(ws.aux[l]):
                     K.rope_(ws.dqkv, ws.cos, ws.sin, S, Hq + Hkv, D, backward=True)
-                G.mm_tn_acc(ws.dqkv, ws.xn1[l], ar.qkv_g(l))
-                G.mm_nn(ws.dqkv, ar.qkv_w(l), out=ws.dn)
+                if f8 is not None:
+                    gq, gt, ig = f8.grad(l, _F8_QKV, ws.dqkv)
+                    F.wgrad(gt, f8.xn1_t[l], ig, f8.act_inv(l, _F8_QKV), ar.qkv_g(l))
+                    wt, iw = f8.weight_t(l, _F8_QKV, ar.qkv_w(l))
+                    F.linear(gq, wt, ig, iw, out=ws.dn)
+                else:
+                    G.mm_tn_acc(ws.dqkv, ws.xn1[l], ar.qkv_g(l))
+                    G.mm_nn(ws.dqkv, ar.qkv_w(l), out=ws.dn)
             K.rmsnorm_bwd(ws.dn, ws.xa[l], ar.w(p + "input_layernorm.weight"), ws.rstd1[l], ws.dx, ws.dx,
                           ar.g(p + "input_layernorm.weight"))
             ws.att[l] = None
@@ -500,13 +615,20 @@ class LlamaForCausalLM(nn.Module):
 
     def __init__(self, config: LlamaConfig, device=None, precision: str = "bf16-mixed", seed: int | None = None,
                  init: bool = True, lce_chunk: int = 32768):
+        """``precision``: "bf16-mixed", "fp16-mixed", "32-true" (compute weights and activations in that dtype, fp32 master
+        weights and gradients), or "fp8-mixed": bf16-mixed with the q|k|v, o, gate|up and down projections of every decoder
+        layer run as FP8 GEMMs in forward, dgrad and wgrad (e4m3 activations and weights, e5m2 gradients, per-tensor
+        current scaling; see ops/fp8.py).  On CUDA, fp8-mixed raises ValueError for shapes the FP8 kernels do not cover."""
         super().__init__()
         self.config = config
         self.precision = precision
-        compute = {"bf16-mixed": torch.bfloat16, "fp16-mixed": torch.float16, "32-true": torch.float32}[precision]
+        compute = {"bf16-mixed": torch.bfloat16, "fp16-mixed": torch.float16, "32-true": torch.float32,
+                   "fp8-mixed": torch.bfloat16}[precision]
         device = torch.device(device if device is not None else "cpu")
+        if precision == "fp8-mixed" and device.type == "cuda":
+            F.check_config(config)
         self.arena = ParamArena(config, device, compute)
-        self.engine = LlamaEngine(config, self.arena, lce_chunk=lce_chunk)
+        self.engine = LlamaEngine(config, self.arena, lce_chunk=lce_chunk, fp8=precision == "fp8-mixed")
         self._build_tree()
         if init:
             self.arena.init_weights(seed)
@@ -561,6 +683,8 @@ class LlamaForCausalLM(nn.Module):
             if device.type == "cuda" and device.index is None:
                 device = torch.device("cuda", torch.cuda.current_device())
             if device != self.arena.device:
+                if self.engine.fp8 and device.type == "cuda":
+                    F.check_config(self.config)
                 self.arena.migrate(device)
                 self.engine._ws.clear()
                 self.engine._graphs.clear()
@@ -623,7 +747,8 @@ class LlamaForCausalLM(nn.Module):
         ``eos_token_id`` (int or list) defaults to ``config.eos_token_id``; after a row emits it, the row is filled with
         ``pad_token_id`` (default: the first EOS id).  Reads the current compute weights.  bf16-mixed CUDA models run the
         decode kernels (csrc/decode_sm90.cu) with the step replayed from a CUDA graph; other precisions and devices run the
-        PyTorch reference path.  Raises ValueError for a parameter-sharded (FULL_SHARD) model, a prompt plus
+        PyTorch reference path.  fp8-mixed models generate on the bf16 path from their bf16 compute weights (no FP8 GEMMs).
+        Raises ValueError for a parameter-sharded (FULL_SHARD) model, a prompt plus
         ``max_new_tokens`` longer than ``max_position_embeddings``, or a mask that is not left-padded."""
         from .generation import generate
 
@@ -641,7 +766,9 @@ class LlamaForCausalLM(nn.Module):
         Position 0, padded and ignored positions give 0.0 / False.  ``attention_mask`` may hold any one contiguous run of
         ones per row (left, right or no padding); each row is scored like its unpadded tokens alone, positions from 0.
         Reads the current compute weights.  bf16-mixed CUDA models run the scoring LM-head kernels (no logits are written,
-        exact for any logit range); other precisions and devices run the PyTorch reference path.  Raises ValueError for a
+        exact for any logit range); other precisions and devices run the PyTorch reference path.  fp8-mixed models score on
+        the bf16 path from their bf16 compute weights (no FP8 GEMMs), so their log-likelihoods differ slightly from the
+        FP8 eval loss of ``forward``.  Raises ValueError for a
         parameter-sharded (FULL_SHARD) model, a sequence longer than ``max_position_embeddings``, mismatched shapes, a mask
         that is not one run per row, or token / label ids outside the vocabulary."""
         from .scoring import score

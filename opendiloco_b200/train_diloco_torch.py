@@ -49,7 +49,7 @@ class TorchDilocoConfig(BaseConfig):
     checkpoint_path: str = "outputs"
     warmup_steps: int = 1000
     total_steps: int = 88_000
-    precision: Literal["fp16-mixed", "bf16-mixed", "32-true"] = "bf16-mixed"
+    precision: Literal["fp16-mixed", "bf16-mixed", "32-true", "fp8-mixed"] = "bf16-mixed"
     project: str = "hivemind_debug"
     model_name_or_path: str = "PrimeIntellect/llama-150m-fresh"
     lr: float = 4e-4

@@ -94,7 +94,7 @@ class Config(BaseConfig):
     warmup_steps: int = 1000
     total_steps: int = 88_000
     sharding_strategy: str = "NO_SHARD"
-    precision: Literal["fp16-mixed", "bf16-mixed", "32-true"] = "bf16-mixed"
+    precision: Literal["fp16-mixed", "bf16-mixed", "32-true", "fp8-mixed"] = "bf16-mixed"
     # checkpointing / logging
     project: str = "hivemind_debug"
     metric_logger_type: Literal["wandb", "dummy"] = "wandb"
