@@ -5,16 +5,25 @@
 //   dS = P * (dP - D) * scale        D  = rowsum(dO * O)        (pre-pass kernel)
 //   dK = dS^T Q                      dQ = dS K                  (dQ: fp32 reduce-add across key tiles, post-pass -> bf16)
 //
-// One CTA per (64-key tile, kv-head, batch), 160 threads: warp 4 streams Q / dO tiles and the per-query statistics of the
-// CTA's work items (query heads of its GQA group x causal range of 64-query tiles) through a STAGES-deep TMA + mbarrier
-// ring; warps 0-3 are one wgmma warpgroup that keeps dK / dV accumulators in registers.  The score tiles are computed
-// TRANSPOSED (keys on the rows) so that P^T and dS^T are directly the register A operands of the dV / dK products:
+// One CTA per (128-key tile, kv-head, batch), 288 threads: warp 8 streams Q / dO tiles and the per-query statistics of
+// the CTA's work items (query heads of its GQA group x causal range of 64-query tiles) through a STAGES-deep TMA +
+// mbarrier ring; warps 0-3 and 4-7 are two wgmma warpgroups, each owning 64 of the keys with its dK / dV accumulators in
+// registers.  Both consume the same stage (empty barrier count 2), so Q and dO are loaded once per 128 keys.  The MMAs
+// of one warpgroup run in program order, and the other warpgroup's MMAs fill the tensor cores while one does its exp / dS
+// work.  Issuing the next item's S^T / dP^T before this item's dV / dK / dQ keeps 64 more accumulators live: that
+// variant needs 222 registers per thread (0 spills under __maxnreg__(224)), which a 288-thread CTA cannot launch with.
+// Built as a 384-thread CTA with a producer warpgroup (setmaxnreg.dec 24 / 40, consumers .inc 240 / 232), ptxas 12.9
+// still allocated it within 168 registers and spilled 300 bytes, so this layout keeps the in-order form.  The score tiles are computed TRANSPOSED (keys on the rows) so
+// that P^T and dS^T are directly the register A operands of the dV / dK products:
 //     S^T  = K  Q^T     A = K (smem, K-major)      B = Q  (smem, K-major)
 //     dP^T = V  dO^T    A = V (smem, K-major)      B = dO (smem, K-major)
 //     dV  += P^T dO     A = P^T (registers)        B = dO (smem, MN-major)
 //     dK  += dS^T Q     A = dS^T (registers)       B = Q  (smem, MN-major)
-//     dQ   = dS K       A = dS^T tile written to smem (128-byte swizzle), read MN-major    B = K (smem, MN-major)
+//     dQ   = dS K       A = the [128 keys x 64 queries] dS^T tile both warpgroups write to smem, read MN-major;
+//                       B = K (smem, MN-major); warpgroup w computes dQ columns 32w..32w+31 over all 128 keys
 // The same swizzled [64 x 64] TMA tiles serve as K-major and as MN-major operands - only the descriptor changes.
+// dQ leaves through shared memory: each warpgroup stages its fp32 [64 x 32] half with the 128-byte swizzle of the dQ
+// accumulator's tensor map and one thread reduce-adds it into global memory with one bulk tensor reduction.
 #include "common.cuh"
 #include "sm90_ptx.cuh"
 
@@ -23,29 +32,27 @@ using namespace sm90;
 
 namespace attn_bwd {
 
-constexpr int BQ = 64, BKV = 64, D = 64;
-constexpr int STAGES = 2;
-constexpr int THREADS = 160;
-constexpr int TILE = 64 * 128;                   // a [64 x 64] bf16 tile, 128-byte swizzled rows
+constexpr int BQ = 64, BKV = 128, D = 64;        // BKV keys per CTA, 64 per consumer warpgroup
+constexpr int STAGES = 3;
+constexpr int THREADS = 288;
+constexpr int TILE = 64 * 128;                   // a [64 x 64] bf16 tile (or [64 x 32] fp32), 128-byte swizzled rows
 constexpr int STAT_BYTES = 2 * 64 * 4;           // per work item: -lse * log2(e) [64], then -D * scale [64]
-// K, V, dS^T, STAGES x (Q, dO, stats)
-constexpr int SMEM_BYTES = 3 * TILE + STAGES * (2 * TILE + STAT_BYTES) + 1024 /*align*/ + 128 /*barriers*/;
-
-__device__ __forceinline__ void red_add_f2(float* p, float a, float b) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
-}
+// K, V (2 tiles each), 2 x dS^T [128 x 64], 2 x dQ staging [64 x 32] fp32, STAGES x (Q, dO, stats)
+constexpr int SMEM_BYTES = 4 * TILE + 4 * TILE + 2 * TILE + STAGES * (2 * TILE + STAT_BYTES) + 1024 /*align*/ + 128 /*barriers*/;
 
 // stats: per query (b, h, s) the pre-pass layout [B, Hq, S/128, 2, 128]: -lse * log2(e), then -D * scale
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
-                const float* __restrict__ stats, float* __restrict__ dq_acc, __nv_bfloat16* __restrict__ dk,
-                __nv_bfloat16* __restrict__ dv, int S, int Hq, int Hkv, long long ld_dkv, float scale, float scale_log2) {
+                const __grid_constant__ CUtensorMap tmap_dq, const float* __restrict__ stats, __nv_bfloat16* __restrict__ dk,
+                __nv_bfloat16* __restrict__ dv, const float* __restrict__ cos_t, const float* __restrict__ sin_t, int S, int Hq,
+                int Hkv, long long ld_dkv, float scale, float scale_log2) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sK = smem;
-  uint8_t* sV = sK + TILE;
-  uint8_t* sdS = sV + TILE;                      // dS^T [64 keys][64 queries], 128-byte swizzle
-  uint8_t* sQ = sdS + TILE;                      // [stage][Q | dO]
+  uint8_t* sK = smem;                            // [128 keys][64], two TMA tiles
+  uint8_t* sV = sK + 2 * TILE;
+  uint8_t* sdS = sV + 2 * TILE;                  // [2 buffers] dS^T [128 keys][64 queries], 128-byte swizzle
+  uint8_t* sdQ = sdS + 4 * TILE;                 // [warpgroup] fp32 dQ [64 queries][32], 128-byte swizzle
+  uint8_t* sQ = sdQ + 2 * TILE;                  // [stage][Q | dO]
   float* sStat = reinterpret_cast<float*>(sQ + STAGES * 2 * TILE);   // [stage][2][64]
   uint64_t* kv_full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sStat) + STAGES * STAT_BYTES);
   uint64_t* full = kv_full + 1;
@@ -57,28 +64,32 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_const
   const int group = Hq / Hkv;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t0 = b * S;
-  const int per_head = nqb - kb;                 // causal: query tiles kb .. nqb-1
+  const int qb0 = kb * (BKV / BQ);               // causal: query tiles qb0 .. nqb-1
+  const int per_head = nqb - qb0;
   const int n_items = group * per_head;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_do);
+    tma_prefetch_desc(&tmap_dq);
     mbar_init(kv_full, 1);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }
     fence_barrier_init();
   }
   __syncthreads();
   pdl_wait();
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
-      mbar_arrive_expect_tx(kv_full, 2 * TILE);
-      tma_load_2d(sK, &tmap_qkv, kv_full, (Hq + hk) * D, t0 + kb * BKV);
-      tma_load_2d(sV, &tmap_qkv, kv_full, (Hq + Hkv + hk) * D, t0 + kb * BKV);
+      mbar_arrive_expect_tx(kv_full, 4 * TILE);
+      for (int j = 0; j < 2; ++j) {
+        tma_load_2d(sK + j * TILE, &tmap_qkv, kv_full, (Hq + hk) * D, t0 + kb * BKV + 64 * j);
+        tma_load_2d(sV + j * TILE, &tmap_qkv, kv_full, (Hq + Hkv + hk) * D, t0 + kb * BKV + 64 * j);
+      }
       for (int it = 0; it < n_items; ++it) {
         const int s = it % STAGES;
-        const int h = hk * group + it / per_head, qb = kb + it % per_head;
+        const int h = hk * group + it / per_head, qb = qb0 + it % per_head;
         mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
         mbar_arrive_expect_tx(&full[s], 2 * TILE + STAT_BYTES);
         tma_load_2d(sQ + s * 2 * TILE, &tmap_qkv, &full[s], h * D, t0 + qb * BQ);
@@ -92,40 +103,73 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_const
     return;
   }
 
-  // -------------------------------------------------------------------- wgmma warpgroup
-  // accumulator fragment of m64n64: acc[4*i + 2*h + e] is row (16*warp + lane/4 + 8*h), column (8*i + 2*(lane%4) + e)
+  // -------------------------------------------------------------------- wgmma warpgroups
+  // accumulator fragment of m64nN: acc[4*i + 2*h + e] is row (16*warp + lane/4 + 8*h), column (8*i + 2*(lane%4) + e)
+  const int wg = warp >> 2;                      // this warpgroup's keys: kb*BKV + 64*wg ...
+  const int tid = threadIdx.x & 127;
+  const int diag = qb0 + wg;                     // the query tile on this warpgroup's diagonal
   float dvacc[32], dkacc[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) dvacc[i] = dkacc[i] = 0.f;
-  const int krow = warp * 16 + (lane >> 2);      // key row (inside the tile) of acc[.. h = 0 ..]
-  const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV), ds_addr = smem_u32(sdS);
+  const int krow = (warp & 3) * 16 + (lane >> 2);   // key row (inside the warpgroup's 64) of acc[.. h = 0 ..]
+  const uint32_t k_addr = smem_u32(sK + wg * TILE), v_addr = smem_u32(sV + wg * TILE);
   const uint64_t kdesc = make_smem_desc_sw128(k_addr, 16, 1024);
   const uint64_t vdesc = make_smem_desc_sw128(v_addr, 16, 1024);
-  const uint64_t k_mn = make_smem_desc_sw128(k_addr, TILE, 1024);
-  const uint64_t ds_mn = make_smem_desc_sw128(ds_addr, TILE, 1024);
+  const uint64_t k_mn = make_smem_desc_sw128(smem_u32(sK) + 64 * wg, TILE, 1024);   // K columns 32*wg .. 32*wg+31
+  uint8_t* const my_dq = sdQ + wg * TILE;
   mbar_wait(kv_full, 0);
+
+  float st[32], dpt[32], dq[16];
+  uint32_t pf[4][4], dsf[4][4];
+
+  // S^T and dP^T of item `it` into st / dpt (one wgmma group)
+  auto issue_scores = [&](int it) {
+    const int s = it % STAGES;
+    mbar_wait(&full[s], (it / STAGES) & 1);
+    const uint32_t q_addr = smem_u32(sQ + s * 2 * TILE);
+    const uint64_t qdesc = make_smem_desc_sw128(q_addr, 16, 1024), dodesc = make_smem_desc_sw128(q_addr + TILE, 16, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_m64n64k16_ss<0, 0>(st, kdesc + 2 * k, qdesc + 2 * k, k > 0 ? 1u : 0u);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_m64n64k16_ss<0, 0>(dpt, vdesc + 2 * k, dodesc + 2 * k, k > 0 ? 1u : 0u);
+    wgmma_commit();
+  };
+  // dQ rows of item `it` (retired in dq): stage this warpgroup's half in smem, one thread reduce-adds it
+  auto store_dq = [&](int it) {
+    const int h = hk * group + it / per_head, qb = qb0 + it % per_head;
+    if (tid == 0) bulk_wait_read<0>();           // the previous reduction has finished reading the staging tile
+    named_bar_sync(2 + wg, 128);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int r = krow + 8 * hh;
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        *reinterpret_cast<float2*>(my_dq + r * 128 + (((2 * i + ((lane & 3) >> 1)) ^ (r & 7)) << 4) + 8 * (lane & 1)) =
+            make_float2(dq[4 * i + 2 * hh], dq[4 * i + 2 * hh + 1]);
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(2 + wg, 128);
+    if (tid == 0) {
+      tma_reduce_add_2d(my_dq, &tmap_dq, h * D + 32 * wg, t0 + qb * BQ);
+      bulk_commit();
+    }
+  };
 
   for (int it = 0; it < n_items; ++it) {
     const int s = it % STAGES;
-    const int h = hk * group + it / per_head, qb = kb + it % per_head;
-    mbar_wait(&full[s], (it / STAGES) & 1);
-    const uint32_t q_addr = smem_u32(sQ + s * 2 * TILE), do_addr = q_addr + TILE;
+    const int qb = qb0 + it % per_head;
     const float* lse2 = sStat + s * 128;
     const float* dsc = lse2 + 64;
-
-    float st[32], dpt[32];
-    {
-      const uint64_t qdesc = make_smem_desc_sw128(q_addr, 16, 1024), dodesc = make_smem_desc_sw128(do_addr, 16, 1024);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_m64n64k16_ss<0, 0>(st, kdesc + 2 * k, qdesc + 2 * k, k > 0 ? 1u : 0u);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_m64n64k16_ss<0, 0>(dpt, vdesc + 2 * k, dodesc + 2 * k, k > 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-    }
-    // P^T, dS^T as register A operands (k = queries), dS^T also into the swizzled smem tile for dQ
-    uint32_t pf[4][4], dsf[4][4];
+    issue_scores(it);
+    wgmma_wait<0>();
+    // Causal mask on and before the diagonal tile.  The one query tile before it (the CTA's first tile, for the second
+    // warpgroup) sees none of the keys: it runs the same MMAs with P = dS = 0, which keeps every wgmma out of divergent
+    // code, and the idle warpgroup would otherwise only wait at the barrier below.
+    const bool masked = qb <= diag;
+    const int kq = 64 * (diag - qb) + krow;       // key row relative to the item's first query, for acc[.. h = 0 ..]
+    // P^T, dS^T as register A operands (k = queries), dS^T also into this warpgroup's rows of the swizzled smem tile
+    uint8_t* ds_buf = sdS + (it & 1) * 2 * TILE;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       float pv[4], dsv[4];
@@ -136,7 +180,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_const
           const int x = 4 * i + 2 * hh + e;
           const int qc = 8 * i + 2 * (lane & 3) + e;     // query column inside the tile
           float pe = exp2f(fmaf(st[x], scale_log2, lse2[qc]));
-          if (qb == kb && krow + 8 * hh > qc) pe = 0.f;
+          if (masked && kq + 8 * hh > qc) pe = 0.f;
           pv[2 * hh + e] = pe;
           dsv[2 * hh + e] = pe * fmaf(dpt[x], scale, dsc[qc]);
         }
@@ -148,41 +192,53 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_const
       dsf[i >> 1][(i & 1) * 2 + 1] = d1;
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        const int r = krow + 8 * hh;
-        *reinterpret_cast<uint32_t*>(sdS + r * 128 + ((i ^ (r & 7)) << 4) + 4 * (lane & 3)) = hh ? d1 : d0;
+        const int r = 64 * wg + krow + 8 * hh;
+        *reinterpret_cast<uint32_t*>(ds_buf + r * 128 + ((i ^ (r & 7)) << 4) + 4 * (lane & 3)) = hh ? d1 : d0;
       }
     }
     fence_proxy_async_smem();                    // generic-proxy stores -> visible to wgmma
-    named_bar_sync(1, 128);
-    float dq[32];
+    // Both halves of the dS^T tile written.  The other buffer is free as well: each warpgroup retired the dQ MMAs that
+    // read it (item it-1) before arriving here, so only one barrier per item joins the two warpgroups.
+    named_bar_sync(1, 256);
     {
-      const uint64_t q_mn = make_smem_desc_sw128(q_addr, TILE, 1024), do_mn = make_smem_desc_sw128(do_addr, TILE, 1024);
+      const uint32_t q_addr = smem_u32(sQ + s * 2 * TILE);
+      const uint64_t q_mn = make_smem_desc_sw128(q_addr, TILE, 1024), do_mn = make_smem_desc_sw128(q_addr + TILE, TILE, 1024);
+      const uint64_t ds_mn = make_smem_desc_sw128(smem_u32(ds_buf), TILE, 1024);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs<1>(dvacc, pf[kk], do_mn + 128 * kk, 1u);
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs<1>(dkacc, dsf[kk], q_mn + 128 * kk, 1u);
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_ss<1, 1>(dq, ds_mn + 128 * kk, k_mn + 128 * kk, kk > 0 ? 1u : 0u);
+      for (int kk = 0; kk < 8; ++kk) wgmma_m64n32k16_ss<1, 1>(dq, ds_mn + 128 * kk, k_mn + 128 * kk, kk > 0 ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<0>();
     }
-    named_bar_sync(1, 128);                      // every warp's MMAs retired: stage and dS^T tile may be rewritten
-    if (threadIdx.x == 0) mbar_arrive(&empty[s]);
-    // dQ rows of this item: reduce-add into the fp32 accumulator
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      const long long tq = (long long)t0 + qb * BQ + krow + 8 * hh;
-      float* drow = dq_acc + (tq * Hq + h) * D + 2 * (lane & 3);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) red_add_f2(drow + 8 * i, dq[4 * i + 2 * hh], dq[4 * i + 2 * hh + 1]);
-    }
+    if (tid == 0) mbar_arrive(&empty[s]);
+    store_dq(it);
   }
+  if (tid == 0) bulk_wait<0>();                  // the staging tile stays valid until the last reduction completes
 
-  // dK / dV of this warp's 16 keys
+  // dK / dV of this warp's 16 keys; with cos/sin dK leaves with the RoPE rotation undone (rotation by -theta of the
+  // pairs (j, j+32), which sit in accumulator groups i and i+4 of the same thread)
+  const int key0 = kb * BKV + 64 * wg;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
-    const long long t = (long long)t0 + kb * BKV + krow + 8 * hh;
+    const int pos = key0 + krow + 8 * hh;
+    if (cos_t != nullptr) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * i + 2 * (lane & 3) + e;
+          const float cs = cos_t[(size_t)pos * 32 + c], sn = sin_t[(size_t)pos * 32 + c];
+          const float x = dkacc[4 * i + 2 * hh + e], y = dkacc[4 * (i + 4) + 2 * hh + e];
+          dkacc[4 * i + 2 * hh + e] = x * cs + y * sn;
+          dkacc[4 * (i + 4) + 2 * hh + e] = y * cs - x * sn;
+        }
+      }
+    }
+    const long long t = (long long)t0 + pos;
     __nv_bfloat16* krow_p = dk + t * ld_dkv + hk * D + 2 * (lane & 3);
     __nv_bfloat16* vrow_p = dv + t * ld_dkv + hk * D + 2 * (lane & 3);
 #pragma unroll
@@ -229,35 +285,27 @@ __global__ void __launch_bounds__(256) attn_dsum_kernel(const __nv_bfloat16* __r
 }
 
 // Post-pass: fp32 dQ accumulator -> bf16 into dq_out (row stride ld_out), and - when cos/sin tables are given - the
-// transpose RoPE rotation of dQ (on the way) and of dK (in place), so the packed dq|dk|dv buffer leaves ready for the
-// projection's dgrad / wgrad GEMMs.  One thread per 8 rotation pairs: x[j..j+8) and x[j+32..j+40) of one (token, head).
+// transpose RoPE rotation of dQ on the way (the main kernel already rotated dK), so the packed dq|dk|dv buffer leaves
+// ready for the projection's dgrad / wgrad GEMMs.  One thread per 8 rotation pairs: x[j..j+8) and x[j+32..j+40) of one
+// (token, head).
 __global__ void __launch_bounds__(256) attn_bwd_finish_kernel(const float* __restrict__ dq_acc, __nv_bfloat16* __restrict__ dq_out,
-                                                              __nv_bfloat16* __restrict__ dk, const float* __restrict__ cos_t,
-                                                              const float* __restrict__ sin_t, long long T, int S, int Hq, int Hkv,
-                                                              long long ld_out, long long ld_dk) {
+                                                              const float* __restrict__ cos_t, const float* __restrict__ sin_t,
+                                                              long long T, int S, int Hq, long long ld_out) {
   pdl_launch_dependents();
   pdl_wait();
-  const int H = Hq + (cos_t != nullptr ? Hkv : 0);
-  const long long total = T * H * 4;
+  const long long total = T * Hq * 4;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int jv = (int)(i & 3);
   const long long th = i >> 2;
-  const int head = (int)(th % H);
-  const long long t = th / H;
+  const int head = (int)(th % Hq);
+  const long long t = th / Hq;
   float a[8], b[8];
-  __nv_bfloat16* dst;
-  if (head < Hq) {
-    const float* src = dq_acc + (t * Hq + head) * 64 + jv * 8;
-    const float4 a0 = ld_f4(src), a1 = ld_f4(src + 4), b0 = ld_f4(src + 32), b1 = ld_f4(src + 36);
-    a[0] = a0.x; a[1] = a0.y; a[2] = a0.z; a[3] = a0.w; a[4] = a1.x; a[5] = a1.y; a[6] = a1.z; a[7] = a1.w;
-    b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
-    dst = dq_out + t * ld_out + head * 64 + jv * 8;
-  } else {
-    dst = dk + t * ld_dk + (head - Hq) * 64 + jv * 8;
-    unpack8(ld_v4(dst), a);
-    unpack8(ld_v4(dst + 32), b);
-  }
+  const float* src = dq_acc + (t * Hq + head) * 64 + jv * 8;
+  const float4 a0 = ld_f4(src), a1 = ld_f4(src + 4), b0 = ld_f4(src + 32), b1 = ld_f4(src + 36);
+  a[0] = a0.x; a[1] = a0.y; a[2] = a0.z; a[3] = a0.w; a[4] = a1.x; a[5] = a1.y; a[6] = a1.z; a[7] = a1.w;
+  b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
+  __nv_bfloat16* dst = dq_out + t * ld_out + head * 64 + jv * 8;
   if (cos_t != nullptr) {
     const int pos = (int)(t % S);
     const float4 c0 = ld_f4(cos_t + (size_t)pos * 32 + jv * 8), c1 = ld_f4(cos_t + (size_t)pos * 32 + jv * 8 + 4);
@@ -299,16 +347,18 @@ ODB_EXPORT int odb_attn_bwd(const void* qkv, const void* out, const void* dout, 
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
-  CUtensorMap tq, tdo;
+  CUtensorMap tq, tdo, tdq;
   int rc;
   if ((rc = make_tmap_2d(&tq, qkv, T, (Hq + 2 * Hkv) * D, ld_qkv * 2, 64, 64, 2))) return rc;
   if ((rc = make_tmap_2d(&tdo, dout, T, Hq * D, ld_out * 2, 64, 64, 2))) return rc;
-  launch_pdl(attn_bwd_kernel, dim3(S / BKV, Hkv, B), dim3(THREADS), SMEM_BYTES, st, tq, tdo, (const float*)stats, (float*)dq_acc,
-             (__nv_bfloat16*)dk, (__nv_bfloat16*)dv, S, Hq, Hkv, ld_dkv, softmax_scale, softmax_scale * 1.4426950408889634f);
+  if ((rc = make_tmap_2d(&tdq, dq_acc, T, Hq * D, (long long)Hq * D * 4, 64, 32, 4))) return rc;
+  launch_pdl(attn_bwd_kernel, dim3(S / BKV, Hkv, B), dim3(THREADS), SMEM_BYTES, st, tq, tdo, tdq, (const float*)stats,
+             (__nv_bfloat16*)dk, (__nv_bfloat16*)dv, (const float*)cos_t, (const float*)sin_t, S, Hq, Hkv, ld_dkv, softmax_scale,
+             softmax_scale * 1.4426950408889634f);
   {
-    const long long threads = T * (Hq + (cos_t ? Hkv : 0)) * 4;
+    const long long threads = T * Hq * 4;
     launch_pdl(attn_bwd_finish_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, (const float*)dq_acc,
-               (__nv_bfloat16*)dq, (__nv_bfloat16*)dk, (const float*)cos_t, (const float*)sin_t, T, S, Hq, Hkv, ld_dq, ld_dkv);
+               (__nv_bfloat16*)dq, (const float*)cos_t, (const float*)sin_t, T, S, Hq, ld_dq);
   }
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : (int)e;

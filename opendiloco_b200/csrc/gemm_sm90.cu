@@ -38,8 +38,8 @@
 // (odb_gemm_fp8_*, odb_wgrad_fp8).  An FP8 k-block is 128 elements deep: the same 128-byte swizzle rows as bf16.  The
 // tensor core's FP8 accumulation is narrower than fp32, so each consumer warpgroup issues every k-block as 4 x m64n128k32
 // into a fresh 64-register scratch accumulator, waits, and adds it into its fp32 accumulator: partial sums are promoted to
-// fp32 once per 128 products.  Scratch plus accumulator must fit the 168 registers ptxas allots each thread of a
-// 384-thread CTA (setmaxnreg does not raise that limit at compile time), so the FP8 tile is 128 x 128 (64 + 64 registers)
+// fp32 once per 128 products.  Scratch plus accumulator are kept within the 168 registers a thread of a 384-thread CTA
+// is launched with (a tile relying on the setmaxnreg budget was not tried), so the FP8 tile is 128 x 128 (64 + 64 registers)
 // instead of 128 x 256; the epilogues take the tile width as a constant.  They first multiply the accumulator by the two
 // dequantisation factors (device scalars inv_a * inv_b, powers of two), then run as for bf16.
 #include <limits.h>

@@ -34,7 +34,7 @@ def _tc_usable(qkv: torch.Tensor, S: int, Hq: int, Hkv: int, D: int) -> bool:
 
 
 def bwd_applies_rope(aux) -> bool:
-    """True when ``attention_bwd`` given ``rope=`` already undid the RoPE rotation of dq / dk (our kernels' post-pass)."""
+    """True when ``attention_bwd`` given ``rope=`` already undid the RoPE rotation of dq / dk (our kernels)."""
     return isinstance(aux[0], str) and aux[0] == "tc"
 
 _lib.register_optional("odb_attn_fwd", [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
@@ -60,8 +60,9 @@ def tc_attention_bwd(dout: torch.Tensor, qkv: torch.Tensor, out: torch.Tensor, l
                      D: int = 64, dqkv: torch.Tensor | None = None, cos: torch.Tensor | None = None, sin: torch.Tensor | None = None):
     """Our attention backward (csrc/attn_bwd_sm90.cu): pre-pass (row statistics, zero dQ accumulator), main
     kernel, post-pass (dQ fp32 -> bf16).  With ``dqkv`` the three gradients land in the column blocks of that packed
-    [T, (Hq+2*Hkv)*D] buffer (returned); otherwise returns dense (dq, dk, dv).  With ``cos``/``sin`` the post-pass also
-    undoes the RoPE rotation of dq and dk (the backward of the fused QKV+RoPE projection epilogue)."""
+    [T, (Hq+2*Hkv)*D] buffer (returned); otherwise returns dense (dq, dk, dv).  With ``cos``/``sin`` the main kernel's dk
+    store and the post-pass also undo the RoPE rotation of dk and dq (the backward of the fused QKV+RoPE projection
+    epilogue)."""
     assert D == 64 and S % 128 == 0 and dout.is_contiguous() and out.is_contiguous()
     T = B * S
     dev = qkv.device
