@@ -5,6 +5,7 @@
 from .models.config import LlamaConfig  # noqa: F401
 from .models.llama import LlamaForCausalLM  # noqa: F401
 from .optim.fused import FusedAdamW, clip_grad_norm_  # noqa: F401
+from .optim.muon import FusedMuon  # noqa: F401
 from .parallel.diloco import (AllReduceStrategy, DiLoCoGradAverager, DiLoCoOptimizer, DiLoCoStateAverager,  # noqa: F401
                               DiloCoProgressTracker)
 from .parallel.swarm import DHT  # noqa: F401

@@ -33,6 +33,10 @@
 //              column, s = sum exp(z - m) (every exponent <= 0: exact for any logit range, no clamp) and the label logit z_y
 //              taken from the same accumulator.  Nothing of size [M, N] is written.
 //   kWgradAcc: fp32 reduce-add of the tile into dW (gradient accumulation across micro-batches + split-K over tokens)
+//   kAxpby   : C[b] = alpha * acc + beta * D[b] (D bf16 in C's layout, may be null), for a batch of equal-shaped problems
+//              stacked along rows: grid.y is the batch index and problem b reads A rows from b * a_rows and B rows from
+//              b * b_rows of the stacked tensors (Newton-Schulz of the Muon optimizer, csrc/muon.cu).  The stacking is
+//              exact when K % 64 == 0: a tile then never reads another problem's rows into a valid output element.
 //
 // Element type (ELEM): 0 = bf16 operands (everything above).  1 / 2 = FP8 operands, A e4m3 / e5m2, B e4m3, both K-major
 // (odb_gemm_fp8_*, odb_wgrad_fp8).  An FP8 k-block is 128 elements deep: the same 128-byte swizzle rows as bf16.  The
@@ -63,7 +67,7 @@ constexpr int THREADS = 384;
 constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 1024 /*align*/ + 256 /*barriers*/;
 constexpr int GROUP_M = 8;                 // rasterisation: 8 m-blocks x all n-blocks per super-block (L2 reuse of A and B)
 
-enum Epi { kStore = 0, kSwiGLU = 1, kRoPE = 2, kSwiGLUBwd = 3, kLCEFwd = 4, kLCEdX = 5, kWgradAcc = 6, kLCEScore = 7 };
+enum Epi { kStore = 0, kSwiGLU = 1, kRoPE = 2, kSwiGLUBwd = 3, kLCEFwd = 4, kLCEdX = 5, kWgradAcc = 6, kLCEScore = 7, kAxpby = 8 };
 
 // group_m > 0: groups of group_m m-blocks x all n-blocks, m fastest inside a group (A and B tiles of a group stay in L2).
 // group_m == 0: n fastest over the whole problem - for a few n-blocks and a very deep K (the LM-head dX: 4 n-blocks,
@@ -111,6 +115,9 @@ struct Params {
   float* sc_zlab;            // kLCEScore: [M] the label logit
   const float* inv_a;        // FP8: device scalars 1 / scale of A and of B (dequantisation in the epilogue)
   const float* inv_b;
+  int a_rows, b_rows;        // kAxpby: row offset of problem b in the stacked A / B tensors is b * a_rows / b * b_rows
+  long long c_bstride;       // kAxpby: elements between consecutive problems of C and D (D = aux, row stride ldc)
+  float alpha, beta;         // kAxpby
 };
 
 __device__ __forceinline__ void red_add_f2(float* p, float a, float b) {
@@ -168,6 +175,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       // which A tensor this tile reads (A_MN: the split is along M, so it is fixed per tile)
       const CUtensorMap* ta_m = &tmap_a;
       int am0 = m0;
+      int bk0 = 0, bn0 = n0;                    // kAxpby: this problem's first B row (MN-major: along K; K-major: along N)
+      if constexpr (EPI == kAxpby) {
+        am0 += (int)blockIdx.y * p.a_rows;
+        if constexpr (B_MN) bk0 = (int)blockIdx.y * p.b_rows;
+        else bn0 += (int)blockIdx.y * p.b_rows;
+      }
       if constexpr (A_MN) {
         if (p.ks1 && m_blk >= p.ks2) { ta_m = &tmap_a2; am0 = m0 - p.ks2 * BM; }
         else if (p.ks1 && m_blk >= p.ks1) { ta_m = &tmap_a1; am0 = m0 - p.ks1 * BM; }
@@ -183,13 +196,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           tma_load_2d(sa, ta_m, &full_bar[stage], am0, kb * BK);
           tma_load_2d(sa + BOX_BYTES, ta_m, &full_bar[stage], am0 + 64, kb * BK);
         } else {
-          if (p.ks1 == 0 || kb < p.ks1) tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * KB, m0);
+          if (p.ks1 == 0 || kb < p.ks1) tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * KB, am0);
           else if (kb < p.ks2) tma_load_2d(sa, &tmap_a1, &full_bar[stage], (kb - p.ks1) * BK, m0);
           else tma_load_2d(sa, &tmap_a2, &full_bar[stage], (kb - p.ks2) * BK, m0);
         }
         if constexpr (B_MN) {       // [K rows, N cols]: four 64(n) x 64(k) boxes
 #pragma unroll
-          for (int j = 0; j < 4; ++j) tma_load_2d(sb + j * BOX_BYTES, &tmap_b, &full_bar[stage], n0 + 64 * j, kb * BK);
+          for (int j = 0; j < 4; ++j) tma_load_2d(sb + j * BOX_BYTES, &tmap_b, &full_bar[stage], n0 + 64 * j, bk0 + kb * BK);
         } else if constexpr (CL == 2) {   // this CTA's half of B (gate | up for kSwiGLU) into both CTAs
           const int b_row = EPI == kSwiGLU ? (rank == 0 ? n_blk * (BN / 2) : p.I + n_blk * (BN / 2)) : n0 + (int)rank * (BN / 2);
           tma_load_2d_multicast(sb + rank * (B_BYTES / 2), &tmap_b, &full_bar[stage], kb * KB, b_row, (uint16_t)0x3);
@@ -198,7 +211,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, g0);
           tma_load_2d(sb + BNE / 2 * 128, &tmap_b, &full_bar[stage], kb * KB, p.I + g0);
         } else {
-          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, n0);
+          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, bn0);
         }
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
@@ -477,6 +490,27 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
       }
       if (row_ok && lab >= 0 && (lab & 6) == 0) p.sc_zlab[row] = zl;     // this thread owns the label column
     }
+  } else if constexpr (EPI == kAxpby) {
+    const size_t boff = (size_t)blockIdx.y * p.c_bstride;
+    __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C) + boff;
+    const __nv_bfloat16* D = p.aux ? reinterpret_cast<const __nv_bfloat16*>(p.aux) + boff : nullptr;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rbase + 8 * h;
+      if (row >= p.M) continue;
+#pragma unroll
+      for (int i = 0; i < NI; ++i) {
+        const int col = n0 + 8 * i + cq;
+        if (col >= p.N) continue;                // N % 64 == 0
+        float v0 = p.alpha * acc[4 * i + 2 * h], v1 = p.alpha * acc[4 * i + 2 * h + 1];
+        if (D) {
+          const float2 d = ld_bf2(D + (size_t)row * p.ldc + col);
+          v0 = fmaf(p.beta, d.x, v0);
+          v1 = fmaf(p.beta, d.y, v1);
+        }
+        st_bf2(C + (size_t)row * p.ldc + col, v0, v1);
+      }
+    }
   } else if constexpr (EPI == kWgradAcc) {
     float* dW = reinterpret_cast<float*>(p.C);
 #pragma unroll
@@ -500,6 +534,10 @@ struct ASplit {
   int K0 = 0, K1 = 0, K2 = 0;      // extents of the three A tensors along the split dimension; K0 == 0 => no split
 };
 
+struct BatchArgs {
+  int batch = 1; int a_rows = 0, b_rows = 0; long long c_bstride = 0; float alpha = 1.f, beta = 0.f;
+};
+
 struct LceArgs {
   const float* row_shift = nullptr; float* partials = nullptr; int want_sumsq = 0; int store = 1;
   const float* rowscale = nullptr; const long long* labels = nullptr; const float* gscale = nullptr;
@@ -511,7 +549,10 @@ template <int EPI, bool A_MN, bool B_MN, int CL = 1, int ELEM = 0>
 static int launch(const void* A, const void* B, void* C, void* aux, int M, int N, int K, long long lda, long long ldb,
                   long long ldc, long long ldaux, int I, int S, int rope_cols, const float* cos_t, const float* sin_t,
                   cudaStream_t st, const ASplit& sp = ASplit(), const LceArgs& lce = LceArgs(), const float* inv_a = nullptr,
-                  const float* inv_b = nullptr) {
+                  const float* inv_b = nullptr, const BatchArgs& ba = BatchArgs()) {
+  // kAxpby: the tensor maps span the whole stacked batch; problem b starts ba.a_rows * b / ba.b_rows * b rows in
+  const int a_rows_all = EPI == kAxpby ? ba.batch * ba.a_rows : (A_MN ? K : M);
+  const int b_rows_all = EPI == kAxpby ? ba.batch * ba.b_rows : (B_MN ? K : N);
   constexpr int EB = ELEM ? 1 : 2;               // operand bytes per element
   constexpr int KB = ELEM ? BK8 : BK;
   constexpr int BNE = ELEM ? BN / 2 : BN;        // tile columns
@@ -522,7 +563,7 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
   } else if (A_MN) {          // A given as [K rows, M cols] (possibly three tensors side by side along M)
     if ((rc = make_tmap_2d(&ta, A, K, sp.K0 ? sp.K0 : M, lda * 2, 64, 64, 2))) return rc;
   } else {
-    if ((rc = make_tmap_2d(&ta, A, M, sp.K0 ? sp.K0 : K, lda * 2, BM, BK, 2))) return rc;
+    if ((rc = make_tmap_2d(&ta, A, a_rows_all, sp.K0 ? sp.K0 : K, lda * 2, BM, BK, 2))) return rc;
   }
   ta1 = ta; ta2 = ta;
   if (sp.K0) {
@@ -535,13 +576,13 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
     }
   }
   if (B_MN) {
-    if ((rc = make_tmap_2d(&tb, B, K, N, ldb * 2, 64, 64, 2))) return rc;            // [K rows, N cols], 64 x 64 boxes
+    if ((rc = make_tmap_2d(&tb, B, b_rows_all, N, ldb * 2, 64, 64, 2))) return rc;   // [K rows, N cols], 64 x 64 boxes
   } else if (EPI == kSwiGLU) {
     if ((rc = make_tmap_2d(&tb, B, 2 * I, K, ldb * EB, BNE / 2, KB, EB))) return rc;
   } else if (CL == 2) {
     if ((rc = make_tmap_2d(&tb, B, N, K, ldb * 2, BN / 2, BK, 2))) return rc;      // each CTA of the pair loads one half
   } else {
-    if ((rc = make_tmap_2d(&tb, B, N, K, ldb * EB, BNE, KB, EB))) return rc;
+    if ((rc = make_tmap_2d(&tb, B, b_rows_all, K, ldb * EB, BNE, KB, EB))) return rc;
   }
   Params p{};
   p.M = M; p.N = N; p.K = K;
@@ -558,6 +599,7 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
   p.wlab = (const __nv_bfloat16*)lce.wlab; p.ldwlab = lce.ldwlab;
   p.sc_max = lce.sc_max; p.sc_sum = lce.sc_sum; p.sc_idx = lce.sc_idx; p.sc_zlab = lce.sc_zlab;
   p.inv_a = inv_a; p.inv_b = inv_b;
+  p.a_rows = ba.a_rows; p.b_rows = ba.b_rows; p.c_bstride = ba.c_bstride; p.alpha = ba.alpha; p.beta = ba.beta;
   const int tiles = p.num_m * p.num_n;
   const int kb_total = ceil_div(K, KB);
   p.splits = 1;
@@ -583,7 +625,7 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
     attr_set = true;
   }
   const int cluster_tiles = ceil_div(p.num_m, CL) * p.num_n;
-  launch_pdl_cluster(gemm_kernel<EPI, A_MN, B_MN, CL, ELEM>, dim3(cluster_tiles * CL * p.splits), dim3(THREADS), SMEM_BYTES, st, CL,
+  launch_pdl_cluster(gemm_kernel<EPI, A_MN, B_MN, CL, ELEM>, dim3(cluster_tiles * CL * p.splits, ba.batch), dim3(THREADS), SMEM_BYTES, st, CL,
                      ta, ta1, ta2, tb, p);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : (int)e;
@@ -782,4 +824,26 @@ ODB_EXPORT int odb_wgrad_fp8(const void* dYt, const void* Xt, void* dW, int N_ou
   return gemm::launch<gemm::kWgradAcc, false, false, 1, 2>(dYt, Xt, dW, nullptr, N_out, K_out, T, ld_dyt, ld_xt, ldw, 0, 0, 0, 0,
                                                            nullptr, nullptr, st, gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a,
                                                            (const float*)inv_b);
+}
+
+// Batched C[b] = alpha * A[b] * B[b]^T + beta * D[b] over `batch` problems stacked along rows: A[b] is [M, K] at row b * M
+// of A, B[b] is [N, K] at row b * N of B, C[b] and D[b] are [M, N] with row stride ldc, consecutive problems M * ldc
+// elements apart.  D may be null (beta unused); it may be A or B, never C.  M, N, K % 64 == 0.
+ODB_EXPORT int odb_gemm_batched_axpby_tn(const void* A, const void* B, void* C, const void* D, int batch, int M, int N, int K,
+                                         long long ldc, float alpha, float beta, cudaStream_t st) {
+  if (batch <= 0 || M % 64 || N % 64 || K % 64 || ldc % 8 || ldc < N) return -1;
+  gemm::BatchArgs ba;
+  ba.batch = batch; ba.a_rows = M; ba.b_rows = N; ba.c_bstride = (long long)M * ldc; ba.alpha = alpha; ba.beta = beta;
+  return gemm::launch<gemm::kAxpby, false, false>(A, B, C, const_cast<void*>(D), M, N, K, K, K, ldc, ldc, 0, 0, 0, nullptr,
+                                                  nullptr, st, gemm::ASplit(), gemm::LceArgs(), nullptr, nullptr, ba);
+}
+
+// as odb_gemm_batched_axpby_tn with B[b] = [K, N] row-major at row b * K of B (MN-major operand): C[b] = alpha A[b] B[b] + beta D[b]
+ODB_EXPORT int odb_gemm_batched_axpby_nn(const void* A, const void* B, void* C, const void* D, int batch, int M, int N, int K,
+                                         long long ldc, float alpha, float beta, cudaStream_t st) {
+  if (batch <= 0 || M % 64 || N % 64 || K % 64 || ldc % 8 || ldc < N) return -1;
+  gemm::BatchArgs ba;
+  ba.batch = batch; ba.a_rows = M; ba.b_rows = K; ba.c_bstride = (long long)M * ldc; ba.alpha = alpha; ba.beta = beta;
+  return gemm::launch<gemm::kAxpby, false, true>(A, B, C, const_cast<void*>(D), M, N, K, K, N, ldc, ldc, 0, 0, 0, nullptr,
+                                                 nullptr, st, gemm::ASplit(), gemm::LceArgs(), nullptr, nullptr, ba);
 }

@@ -27,10 +27,12 @@ import torch.distributed as dist
 
 from .models.llama import LlamaForCausalLM
 from .optim.fused import FusedAdamW
+from .optim.muon import FusedMuon
 from .parallel import comm
 from .parallel.compression import get_compression
 from .parallel.diloco import DiLoCoOptimizer
 from .parallel.swarm import DHT
+from .utils.ckpt import check_inner_kind, inner_kind
 from .utils.config import BaseConfig, parse_argv
 from .utils.data import TEST_VOCAB_SIZE, TokenFileLoader, get_fake_dataloader, get_text_dataloader
 from .utils.logger import get_logger, make_metric_logger
@@ -50,6 +52,8 @@ class TorchDilocoConfig(BaseConfig):
     warmup_steps: int = 1000
     total_steps: int = 88_000
     precision: Literal["fp16-mixed", "bf16-mixed", "32-true", "fp8-mixed"] = "bf16-mixed"
+    inner_optimizer: Literal["adamw", "muon"] = "adamw"   # muon: FusedMuon, AdamW for the non-matrix weights
+    muon_momentum: float = 0.95
     project: str = "hivemind_debug"
     model_name_or_path: str = "PrimeIntellect/llama-150m-fresh"
     lr: float = 4e-4
@@ -83,6 +87,8 @@ def save_checkpoint(path: str, real_step: int, model, optimizer: DiLoCoOptimizer
             "scheduler_state_dict": scheduler.state_dict(), "loss": loss, "step": real_step,
             "theta_outer": optimizer.state_averager.theta_outer.detach().cpu(), "local_epoch": optimizer.local_epoch,
             "samples_accumulated": optimizer.tracker.local_progress.samples_accumulated}
+    if inner_kind(optimizer.inner_optimizer) != "adamw":
+        data["inner_optimizer"] = inner_kind(optimizer.inner_optimizer)
     buf = io.BytesIO()
     torch.save(data, buf)
     with fsspec.open(path, "wb", auto_mkdir=True) as f:
@@ -99,6 +105,7 @@ def load_checkpoint(model, optimizer: DiLoCoOptimizer, scheduler, filename: str,
     if resume_only_model:
         sa.theta_outer.copy_(sa.theta_local)
         return 0, ckpt["loss"]
+    check_inner_kind(ckpt.get("inner_optimizer", "adamw"), optimizer.inner_optimizer)
     optimizer.inner_optimizer.load_state_dict(ckpt["inner_optimizer_state_dict"])
     scheduler.load_state_dict(ckpt["scheduler_state_dict"])
     sa.optimizer.load_state_dict(ckpt["outer_optimizer_state_dict"])
@@ -152,7 +159,9 @@ def main(cfg: TorchDilocoConfig) -> None:
     optimizer = DiLoCoOptimizer(
         dht=dht, run_id=cfg.project, batch_size=cfg.batch_size, num_inner_steps=cfg.local_steps, params=model.parameters(),
         outer_optimizer=partial(torch.optim.SGD, lr=cfg.outer_lr, momentum=0.9, nesterov=True),
-        inner_optimizer=partial(FusedAdamW, lr=cfg.lr, weight_decay=0.1, betas=(0.9, 0.95)),
+        inner_optimizer=partial(FusedAdamW, lr=cfg.lr, weight_decay=0.1, betas=(0.9, 0.95)) if cfg.inner_optimizer == "adamw"
+        else partial(FusedMuon, lr=cfg.lr, weight_decay=0.1, momentum=cfg.muon_momentum, adjust_lr_fn="match_rms_adamw",
+                     adamw_betas=(0.9, 0.95)),
         grad_compression=get_compression(cfg.compression))
     inner = optimizer.inner_optimizer
     scheduler = get_cosine_schedule_with_warmup(inner, cfg.warmup_steps, cfg.total_steps)

@@ -31,6 +31,7 @@ from pydantic import model_validator
 
 from .models.llama import LlamaForCausalLM
 from .optim.fused import FusedAdamW
+from .optim.muon import FusedMuon
 from .parallel import comm
 from .parallel.compression import get_compression_kwargs
 from .parallel.diloco import AllReduceStrategy, DiLoCoOptimizer
@@ -95,6 +96,8 @@ class Config(BaseConfig):
     total_steps: int = 88_000
     sharding_strategy: str = "NO_SHARD"
     precision: Literal["fp16-mixed", "bf16-mixed", "32-true", "fp8-mixed"] = "bf16-mixed"
+    inner_optimizer: Literal["adamw", "muon"] = "adamw"   # muon: FusedMuon (NO_SHARD only), AdamW for the non-matrix weights
+    muon_momentum: float = 0.95
     # checkpointing / logging
     project: str = "hivemind_debug"
     metric_logger_type: Literal["wandb", "dummy"] = "wandb"
@@ -143,6 +146,8 @@ def get_dataloader(config: Config, topo: comm.Topology, vocab_size: int):
 def train(config: Config) -> None:
     if config.sharding_strategy not in SHARDING:
         raise ValueError(f"Invalid sharding_strategy: {config.sharding_strategy}. Choose one of {sorted(SHARDING)}")
+    if config.inner_optimizer == "muon" and config.sharding_strategy != "NO_SHARD":
+        raise ValueError(f"--inner_optimizer muon needs whole matrices: it supports NO_SHARD only, not {config.sharding_strategy}")
     topo = _setup_world(config)
     hv = config.hv
     rank, local_rank = topo.rank, topo.local_rank
@@ -173,6 +178,10 @@ def train(config: Config) -> None:
     shard = config.sharding_strategy != "NO_SHARD"
     inner_factory = partial(FusedAdamW, lr=config.lr, weight_decay=0.1, betas=(0.9, 0.95), dp_group=topo.inner_group, shard=shard,
                             shard_params=config.sharding_strategy in ("FULL_SHARD", "HYBRID_SHARD"))
+    if config.inner_optimizer == "muon":
+        # match_rms_adamw keeps --lr and the 0.1 weight decay meaningful for the Muon matrices
+        inner_factory = partial(FusedMuon, lr=config.lr, weight_decay=0.1, momentum=config.muon_momentum,
+                                adjust_lr_fn="match_rms_adamw", adamw_betas=(0.9, 0.95), dp_group=topo.inner_group)
     scheduler_fn = partial(get_cosine_schedule_with_warmup, num_warmup_steps=config.warmup_steps,
                            num_training_steps=config.total_steps)
     ckpt_rank_dir = get_diloco_rank_dir_name(topo.world_rank) if hv is not None else ""

@@ -20,6 +20,7 @@ import torch
 
 from .models.llama import LlamaForCausalLM
 from .optim.fused import FusedAdamW
+from .optim.muon import FusedMuon
 from .parallel import comm
 from .parallel.diloco import AllReduceStrategy, DiLoCoOptimizer
 from .parallel.swarm import DHT
@@ -51,6 +52,9 @@ class TrainerConfig:
     compression: object | None = None
     fused_collective: bool | None = None
     offload_device: str | None = None
+    inner_optimizer: str = "adamw"       # "adamw" | "muon" (FusedMuon: Muon on the projection matrices, NO_SHARD only)
+    muon_momentum: float = 0.95
+    muon_adjust_lr_fn: str | None = "match_rms_adamw"
 
 
 SHARDED = {"SHARD_GRAD_OP", "_HYBRID_SHARD_ZERO2", "FULL_SHARD", "HYBRID_SHARD"}
@@ -59,11 +63,19 @@ SHARDED = {"SHARD_GRAD_OP", "_HYBRID_SHARD_ZERO2", "FULL_SHARD", "HYBRID_SHARD"}
 class DiLoCoTrainer:
     def __init__(self, model: LlamaForCausalLM, cfg: TrainerConfig, topo: comm.Topology | None = None):
         self.model, self.cfg = model, cfg
+        if cfg.inner_optimizer not in ("adamw", "muon"):
+            raise ValueError(f"unknown inner_optimizer {cfg.inner_optimizer!r}: choose 'adamw' or 'muon'")
+        if cfg.inner_optimizer == "muon" and cfg.sharding_strategy in SHARDED:
+            raise ValueError(f"inner_optimizer='muon' needs whole matrices: it supports NO_SHARD only, not {cfg.sharding_strategy}")
         self.topo = topo if topo is not None else comm.build_topology()
         shard = cfg.sharding_strategy in SHARDED
         inner_factory = partial(FusedAdamW, lr=cfg.lr, weight_decay=cfg.weight_decay, betas=cfg.betas, eps=cfg.eps,
                                 max_grad_norm=cfg.max_grad_norm, zero_grad_in_step=True, dp_group=self.topo.inner_group,
                                 shard=shard, shard_params=cfg.sharding_strategy in ("FULL_SHARD", "HYBRID_SHARD"))
+        if cfg.inner_optimizer == "muon":
+            inner_factory = partial(FusedMuon, lr=cfg.lr, weight_decay=cfg.weight_decay, momentum=cfg.muon_momentum,
+                                    adjust_lr_fn=cfg.muon_adjust_lr_fn, adamw_betas=cfg.betas, adamw_eps=cfg.eps,
+                                    max_grad_norm=cfg.max_grad_norm, zero_grad_in_step=True, dp_group=self.topo.inner_group)
         sched_factory = partial(get_cosine_schedule_with_warmup, num_warmup_steps=cfg.warmup_steps,
                                 num_training_steps=cfg.total_steps)
         params = list(model.parameters())

@@ -120,6 +120,18 @@ def _flat_view(optimizer):
     return getattr(_inner_of(optimizer), "fv", None)
 
 
+def inner_kind(optimizer) -> str:
+    """``"muon"`` for FusedMuon, ``"adamw"`` otherwise.  Flat shards of both look alike (exp_avg holds Muon's momentum on
+    the matrix slots), so Muon checkpoints carry the tag and a resume under the other optimizer is refused."""
+    return getattr(_inner_of(optimizer), "CHECKPOINT_KIND", "adamw")
+
+
+def check_inner_kind(saved: str, optimizer) -> None:
+    ours = inner_kind(optimizer)
+    if saved != ours:
+        raise ValueError(f"checkpoint was written by the {saved!r} inner optimizer; it cannot be resumed with {ours!r}")
+
+
 # ------------------------------------------------------------------------------------------------ save
 def save_checkpoint(checkpoint_path: str, model: torch.nn.Module, optimizer: torch.optim.Optimizer, scheduler=None,
                     outer_optimizer: torch.optim.Optimizer | None = None, scaler=None, loss: float | None = None,
@@ -131,6 +143,9 @@ def save_checkpoint(checkpoint_path: str, model: torch.nn.Module, optimizer: tor
     fv = _flat_view(optimizer)
     inner = _inner_of(optimizer)
     shard: dict = {"format": "opendiloco_b200.flat.v1"}
+    kind = inner_kind(optimizer)
+    if kind != "adamw":
+        shard["inner_optimizer"] = kind
     if fv is not None:
         lo, hi = fv.lo, fv.hi
         writes = fv.sharded or rank == 0
@@ -150,6 +165,8 @@ def save_checkpoint(checkpoint_path: str, model: torch.nn.Module, optimizer: tor
             arena = getattr(model, "arena", None)
             meta = {"format": shard["format"], "numel": fv.numel, "sharded": bool(fv.sharded),
                     "slots": {n: [s.offset, list(s.shape)] for n, s in arena.slots.items()} if arena is not None else None}
+            if kind != "adamw":
+                meta["inner_optimizer"] = kind
             with fsspec.open(os.path.join(checkpoint_path, METADATA_FILE), "w", auto_mkdir=True) as f:
                 json.dump(meta, f)
     elif rank == 0:   # generic torch model/optimizer
@@ -214,13 +231,14 @@ def load_checkpoint(checkpoint_path: str, model: torch.nn.Module, optimizer: tor
     inner = _inner_of(optimizer)
     _SHARD_CACHE.clear()
     if fv is not None:
+        first = _load_shard(sorted(f for f in GenericFileSystem().ls(checkpoint_path, detail=False) if f.endswith(".distcp"))[0])
+        check_inner_kind(first.get("inner_optimizer", "adamw"), optimizer)
         dev = fv.flat.device
         fv.flat[fv.lo:fv.hi].copy_(_assemble(checkpoint_path, "model", fv.lo, fv.hi, dev))
         m, v = _assemble(checkpoint_path, "exp_avg", fv.lo, fv.hi, dev), _assemble(checkpoint_path, "exp_avg_sq", fv.lo, fv.hi, dev)
         if m is not None:
             inner.exp_avg.copy_(m)
             inner.exp_avg_sq.copy_(v)
-        first = _load_shard(sorted(f for f in GenericFileSystem().ls(checkpoint_path, detail=False) if f.endswith(".distcp"))[0])
         inner._step = int(first.get("step", 0))
         # publish the restored weights to the compute copy (and to the worker's other GPUs when sharded)
         arena = getattr(model, "arena", None)
@@ -239,6 +257,7 @@ def load_checkpoint(checkpoint_path: str, model: torch.nn.Module, optimizer: tor
                 sa.momentum_buffer.copy_(mom)
     else:
         sh = _load(os.path.join(checkpoint_path, "__0_0.distcp"))
+        check_inner_kind(sh.get("inner_optimizer", "adamw"), optimizer)
         model.load_state_dict(sh["model_state_dict"])
         inner.load_state_dict(sh["optimizer_state_dict"])
     if data_loader is not None and hasattr(data_loader, "load_state_dict"):
@@ -246,7 +265,8 @@ def load_checkpoint(checkpoint_path: str, model: torch.nn.Module, optimizer: tor
     g = _load(os.path.join(checkpoint_path, GLOBAL_STATE_FILE))
     if scheduler is not None and g.get("scheduler") is not None:
         scheduler.load_state_dict(g["scheduler"])
-        inner.param_groups[0]["lr"] = scheduler.get_last_lr()[0]          # reference ckpt_utils.py:149-151
+        for grp, lr in zip(inner.param_groups, scheduler.get_last_lr()):  # reference ckpt_utils.py:149-151, every group
+            grp["lr"] = lr
     if outer_optimizer is not None and "outer_optimizer" in g:
         for grp, saved in zip(outer_optimizer.param_groups, g["outer_optimizer"]["param_groups"]):
             grp.update({k: v for k, v in saved.items() if k != "params"})

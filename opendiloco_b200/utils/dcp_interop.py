@@ -46,6 +46,9 @@ def _gather_flat(ckpt_dir: str) -> tuple[dict, dict[str, torch.Tensor]]:
     """Assemble the full flat vectors of a flat-shard checkpoint directory -> (metadata, {key: flat fp32 tensor})."""
     with open(os.path.join(ckpt_dir, METADATA_FILE)) as f:
         meta = json.load(f)
+    if meta.get("inner_optimizer", "adamw") != "adamw":
+        # the reference's layout holds AdamW moments only: Muon's momentum would be read back as exp_avg
+        raise ValueError(f"{ckpt_dir} was written by the {meta['inner_optimizer']!r} inner optimizer; only AdamW checkpoints convert")
     n = int(meta["numel"])
     flat: dict[str, torch.Tensor] = {}
     step, groups = 0, None
