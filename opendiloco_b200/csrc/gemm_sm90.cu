@@ -2,15 +2,24 @@
 //
 //   C[M,N] = A[M,K] * B[N,K]^T      bf16 operands, fp32 accumulation in registers
 //
-// One CTA per 128 x 256 output tile, 384 threads in three warpgroups:
+// 128 x 256 output tiles, 384 threads in three warpgroups, persistent: the grid has min(work items, SMs) CTAs and CTA c
+// computes work items c, c + gridDim.x, c + 2 gridDim.x, ...  (the items running at any moment are consecutive, so the
+// rasterisation of tile_coords holds).
 //   warpgroup 0    TMA producer (one thread): A tile 128x64, B tile 256x64 per stage (128-byte swizzle), mbarrier
-//                  full/empty ring of STAGES stages; gives its registers to the MMA warpgroups (setmaxnreg)
+//                  full/empty ring of STAGES stages that runs on across all of the CTA's tiles (stage and phase carry
+//                  over), so the next tile's first stages load while the MMA warpgroups run an epilogue; gives its
+//                  registers to the MMA warpgroups (setmaxnreg)
 //   warpgroups 1-2 MMA + epilogue: each issues wgmma m64n256k16 for its 64 rows of the tile (4 per 64-deep k-block),
-//                  keeps one wgmma group in flight, then runs the fused epilogue straight from the accumulator registers
+//                  keeps one wgmma group in flight, releases the tile's last stage as soon as its MMAs retire, then runs
+//                  the fused epilogue from the accumulator registers.  Stored outputs go through a 16 KB staging buffer per
+//                  warpgroup (two 64-row x 128-byte boxes, 128-byte swizzle, the layout TMA writes for a load) and leave by
+//                  TMA (cp.async.bulk.tensor stores, fp32 reduce-add for the weight gradient); the tensor map of the
+//                  output clips partial tiles.  A box is rewritten only after the store that read it has (bulk_wait_read).
 //
 // CL = 2 (odb_gemm2_*: forward projections with at least one wave of 256 x 256 tiles): a cluster of two CTAs computes a 256 x 256 tile,
 // the two m-halves of the same B tile.  Each CTA loads its own A and ONE half of B, multicast into both CTAs, so the B
-// traffic from L2 per CTA halves; a stage is refilled only when the MMA warpgroups of both CTAs have released it.
+// traffic from L2 per CTA halves; a stage is refilled only when the MMA warpgroups of both CTAs have released it.  Both
+// CTAs of a cluster walk the same sequence of cluster tiles.
 //
 // Operand layouts (template flags, the shared-memory descriptor expresses both - no transposed copies are made):
 //   A_MN = false : A is [M, K] row-major (K-major)          A_MN = true : A is [K, M] row-major (MN-major, wgrad)
@@ -34,7 +43,7 @@
 //              taken from the same accumulator.  Nothing of size [M, N] is written.
 //   kWgradAcc: fp32 reduce-add of the tile into dW (gradient accumulation across micro-batches + split-K over tokens)
 //   kAxpby   : C[b] = alpha * acc + beta * D[b] (D bf16 in C's layout, may be null), for a batch of equal-shaped problems
-//              stacked along rows: grid.y is the batch index and problem b reads A rows from b * a_rows and B rows from
+//              stacked along rows: work item w is tile w % tiles of problem b = w / tiles, which reads A rows from b * a_rows and B rows from
 //              b * b_rows of the stacked tensors (Newton-Schulz of the Muon optimizer, csrc/muon.cu).  The stacking is
 //              exact when K % 64 == 0: a tile then never reads another problem's rows into a valid output element.
 //
@@ -64,7 +73,10 @@ constexpr int B_BYTES = BN * BK * 2;       // 32 KB
 constexpr int BOX_BYTES = 64 * 64 * 2;     // one 64 x 64 box of an MN-major operand
 constexpr int STAGES = 4;
 constexpr int THREADS = 384;
-constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 1024 /*align*/ + 256 /*barriers*/;
+constexpr int OUT_BOX = 64 * 128;          // one output box: 64 rows x 128 bytes (64 bf16 or 32 fp32 columns)
+constexpr int STG_BYTES = 2 * OUT_BOX;     // output staging of one MMA warpgroup
+constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 2 * STG_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+static_assert(SMEM_BYTES <= 232448, "sm_90 opt-in shared memory per block");
 constexpr int GROUP_M = 8;                 // rasterisation: 8 m-blocks x all n-blocks per super-block (L2 reuse of A and B)
 
 enum Epi { kStore = 0, kSwiGLU = 1, kRoPE = 2, kSwiGLUBwd = 3, kLCEFwd = 4, kLCEdX = 5, kWgradAcc = 6, kLCEScore = 7, kAxpby = 8 };
@@ -118,27 +130,59 @@ struct Params {
   int a_rows, b_rows;        // kAxpby: row offset of problem b in the stacked A / B tensors is b * a_rows / b * b_rows
   long long c_bstride;       // kAxpby: elements between consecutive problems of C and D (D = aux, row stride ldc)
   float alpha, beta;         // kAxpby
+  int batch;                 // kAxpby: number of problems (1 otherwise)
 };
 
-__device__ __forceinline__ void red_add_f2(float* p, float a, float b) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
-}
 __device__ __forceinline__ void st_bf2(void* p, float a, float b) { *reinterpret_cast<uint32_t*>(p) = f2_to_bf2(a, b); }
 __device__ __forceinline__ float2 ld_bf2(const void* p) { return bf2_to_f2(*reinterpret_cast<const uint32_t*>(p)); }
+__device__ __forceinline__ void sts_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void sts_f2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+
+// One work item: a tile of the output (a K-slice of it for split-K) of problem b (kAxpby)
+struct Tile {
+  int m_blk, n_blk, m0, n0, kb0, kb1, b;
+};
+
+template <int CL, int ELEM>
+__device__ __forceinline__ Tile tile_of(const Params& p, int work, uint32_t rank) {
+  constexpr int KB = ELEM ? BK8 : BK;            // elements per k-block
+  constexpr int BNE = ELEM ? BN / 2 : BN;        // tile columns
+  const int num_mc = (p.num_m + CL - 1) / CL;
+  const int per_batch = num_mc * p.num_n * p.splits;
+  Tile t;
+  t.b = work / per_batch;
+  work -= t.b * per_batch;
+  const int tile = work / p.splits, split = work - tile * p.splits;
+  tile_coords(tile, num_mc, p.num_n, p.group_m, t.m_blk, t.n_blk);
+  t.m_blk = t.m_blk * CL + (int)rank;            // CL = 2: this CTA's m-half of the cluster tile (may lie beyond M)
+  t.m0 = t.m_blk * BM;
+  t.n0 = t.n_blk * BNE;
+  t.kb0 = split * p.kb_per_split;
+  t.kb1 = min((p.K + KB - 1) / KB, t.kb0 + p.kb_per_split);
+  return t;
+}
 
 template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM>
-__device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_a, uint8_t* smem_b, uint64_t* full_bar,
-                                                 uint64_t* empty_bar, int wg, int m0, int n0, int n_blk, int kb0, int kb1);
+__device__ __forceinline__ void mma_and_epilogue(const Params& p, const CUtensorMap* tmap_c, const CUtensorMap* tmap_c2,
+                                                 uint8_t* smem_a, uint8_t* smem_b, uint8_t* smem_c, uint64_t* full_bar,
+                                                 uint64_t* empty_bar, int cw, const Tile& tl, int& stage, uint32_t& phase);
 
+// Output maps (tmap_c, tmap_c2): C (gu for kSwiGLU, fp32 dW for kWgradAcc) and act (kSwiGLU); see launch().
 template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM = 0>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a1,
-            const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_b, Params p) {
+            const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_b,
+            const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_c2, Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + STAGES * B_BYTES);
+  uint8_t* smem_c = smem_b + STAGES * B_BYTES;   // output staging, STG_BYTES per MMA warpgroup
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_c + 2 * STG_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   pdl_launch_dependents();
@@ -146,21 +190,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   static_assert(ELEM == 0 || (CL == 1 && !A_MN && !B_MN), "FP8 wgmma takes K-major operands only");
   constexpr int KB = ELEM ? BK8 : BK;            // elements per k-block
   constexpr int BNE = ELEM ? BN / 2 : BN;        // tile columns
+  constexpr bool TMA_OUT = EPI == kStore || EPI == kRoPE || EPI == kSwiGLU || EPI == kLCEFwd || EPI == kWgradAcc;
   const int wg = threadIdx.x >> 7;
   const uint32_t rank = CL == 2 ? cluster_ctarank() : 0;
-  const int work = blockIdx.x / CL;
-  const int tile = work / p.splits, split = work - tile * p.splits;
-  int m_blk, n_blk;
-  tile_coords(tile, (p.num_m + CL - 1) / CL, p.num_n, p.group_m, m_blk, n_blk);
-  m_blk = m_blk * CL + (int)rank;                // CL = 2: this CTA's m-half of the cluster tile (may lie beyond M)
-  const int m0 = m_blk * BM, n0 = n_blk * BNE;
-  const int num_k_total = (p.K + KB - 1) / KB;
-  const int kb0 = split * p.kb_per_split;
-  const int kb1 = min(num_k_total, kb0 + p.kb_per_split);
+  const int work_total = (p.num_m + CL - 1) / CL * p.num_n * p.splits * p.batch;
+  const int work_first = blockIdx.x / CL, work_step = gridDim.x / CL;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if constexpr (TMA_OUT) tma_prefetch_desc(&tmap_c);
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2 * CL); }
     fence_barrier_init();
   }
@@ -172,71 +211,121 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     // ------------------------------------------------------------------ TMA producer
     reg_dealloc<40>();
     if (threadIdx.x == 0) {
-      // which A tensor this tile reads (A_MN: the split is along M, so it is fixed per tile)
-      const CUtensorMap* ta_m = &tmap_a;
-      int am0 = m0;
-      int bk0 = 0, bn0 = n0;                    // kAxpby: this problem's first B row (MN-major: along K; K-major: along N)
-      if constexpr (EPI == kAxpby) {
-        am0 += (int)blockIdx.y * p.a_rows;
-        if constexpr (B_MN) bk0 = (int)blockIdx.y * p.b_rows;
-        else bn0 += (int)blockIdx.y * p.b_rows;
-      }
-      if constexpr (A_MN) {
-        if (p.ks1 && m_blk >= p.ks2) { ta_m = &tmap_a2; am0 = m0 - p.ks2 * BM; }
-        else if (p.ks1 && m_blk >= p.ks1) { ta_m = &tmap_a1; am0 = m0 - p.ks1 * BM; }
-      }
       int stage = 0;
       uint32_t phase = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + BNE * 128);
-        uint8_t* sa = smem_a + stage * A_BYTES;
-        uint8_t* sb = smem_b + stage * B_BYTES;
-        if constexpr (A_MN) {       // [K rows, M cols]: two 64(m) x 64(k) boxes
-          tma_load_2d(sa, ta_m, &full_bar[stage], am0, kb * BK);
-          tma_load_2d(sa + BOX_BYTES, ta_m, &full_bar[stage], am0 + 64, kb * BK);
-        } else {
-          if (p.ks1 == 0 || kb < p.ks1) tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * KB, am0);
-          else if (kb < p.ks2) tma_load_2d(sa, &tmap_a1, &full_bar[stage], (kb - p.ks1) * BK, m0);
-          else tma_load_2d(sa, &tmap_a2, &full_bar[stage], (kb - p.ks2) * BK, m0);
+      for (int work = work_first; work < work_total; work += work_step) {
+        const Tile t = tile_of<CL, ELEM>(p, work, rank);
+        // which A tensor this tile reads (A_MN: the split is along M, so it is fixed per tile)
+        const CUtensorMap* ta_m = &tmap_a;
+        int am0 = t.m0;
+        int bk0 = 0, bn0 = t.n0;                // kAxpby: this problem's first B row (MN-major: along K; K-major: along N)
+        if constexpr (EPI == kAxpby) {
+          am0 += t.b * p.a_rows;
+          if constexpr (B_MN) bk0 = t.b * p.b_rows;
+          else bn0 += t.b * p.b_rows;
         }
-        if constexpr (B_MN) {       // [K rows, N cols]: four 64(n) x 64(k) boxes
+        if constexpr (A_MN) {
+          if (p.ks1 && t.m_blk >= p.ks2) { ta_m = &tmap_a2; am0 = t.m0 - p.ks2 * BM; }
+          else if (p.ks1 && t.m_blk >= p.ks1) { ta_m = &tmap_a1; am0 = t.m0 - p.ks1 * BM; }
+        }
+        for (int kb = t.kb0; kb < t.kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + BNE * 128);
+          uint8_t* sa = smem_a + stage * A_BYTES;
+          uint8_t* sb = smem_b + stage * B_BYTES;
+          if constexpr (A_MN) {     // [K rows, M cols]: two 64(m) x 64(k) boxes
+            tma_load_2d(sa, ta_m, &full_bar[stage], am0, kb * BK);
+            tma_load_2d(sa + BOX_BYTES, ta_m, &full_bar[stage], am0 + 64, kb * BK);
+          } else {
+            if (p.ks1 == 0 || kb < p.ks1) tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * KB, am0);
+            else if (kb < p.ks2) tma_load_2d(sa, &tmap_a1, &full_bar[stage], (kb - p.ks1) * BK, t.m0);
+            else tma_load_2d(sa, &tmap_a2, &full_bar[stage], (kb - p.ks2) * BK, t.m0);
+          }
+          if constexpr (B_MN) {     // [K rows, N cols]: four 64(n) x 64(k) boxes
 #pragma unroll
-          for (int j = 0; j < 4; ++j) tma_load_2d(sb + j * BOX_BYTES, &tmap_b, &full_bar[stage], n0 + 64 * j, bk0 + kb * BK);
-        } else if constexpr (CL == 2) {   // this CTA's half of B (gate | up for kSwiGLU) into both CTAs
-          const int b_row = EPI == kSwiGLU ? (rank == 0 ? n_blk * (BN / 2) : p.I + n_blk * (BN / 2)) : n0 + (int)rank * (BN / 2);
-          tma_load_2d_multicast(sb + rank * (B_BYTES / 2), &tmap_b, &full_bar[stage], kb * KB, b_row, (uint16_t)0x3);
-        } else if constexpr (EPI == kSwiGLU) {
-          const int g0 = n_blk * (BNE / 2);
-          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, g0);
-          tma_load_2d(sb + BNE / 2 * 128, &tmap_b, &full_bar[stage], kb * KB, p.I + g0);
-        } else {
-          tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, bn0);
+            for (int j = 0; j < 4; ++j) tma_load_2d(sb + j * BOX_BYTES, &tmap_b, &full_bar[stage], t.n0 + 64 * j, bk0 + kb * BK);
+          } else if constexpr (CL == 2) {   // this CTA's half of B (gate | up for kSwiGLU) into both CTAs
+            const int b_row = EPI == kSwiGLU ? (rank == 0 ? t.n_blk * (BN / 2) : p.I + t.n_blk * (BN / 2)) : t.n0 + (int)rank * (BN / 2);
+            tma_load_2d_multicast(sb + rank * (B_BYTES / 2), &tmap_b, &full_bar[stage], kb * KB, b_row, (uint16_t)0x3);
+          } else if constexpr (EPI == kSwiGLU) {
+            const int g0 = t.n_blk * (BNE / 2);
+            tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, g0);
+            tma_load_2d(sb + BNE / 2 * 128, &tmap_b, &full_bar[stage], kb * KB, p.I + g0);
+          } else {
+            tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, bn0);
+          }
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
   } else {
-    mma_and_epilogue<EPI, A_MN, B_MN, CL, ELEM>(p, smem_a, smem_b, full_bar, empty_bar, wg, m0, n0, n_blk, kb0, kb1);
+    reg_alloc<232>();
+    const int cw = wg - 1;                       // this warpgroup's 64 rows of each tile
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int work = work_first; work < work_total; work += work_step) {
+      const Tile t = tile_of<CL, ELEM>(p, work, rank);
+      mma_and_epilogue<EPI, A_MN, B_MN, CL, ELEM>(p, &tmap_c, &tmap_c2, smem_a, smem_b, smem_c, full_bar, empty_bar, cw, t,
+                                                  stage, phase);
+    }
+    if constexpr (TMA_OUT) {
+      if ((threadIdx.x & 127) == 0) bulk_wait<0>();   // the last stores have read the staging and reached memory
+    }
   }
   if constexpr (CL == 2) cluster_sync();         // no CTA leaves while its peer may still arrive on its barriers
 }
 
+// ---------------------------------------------------------------------------------------- output staging (TMA epilogues)
+// A box is 64 rows x 128 bytes, 1024-byte aligned, in the 128-byte swizzle: the 16-byte chunk j of row r is stored at
+// chunk j ^ (r % 8).  In the accumulator fragment a warp's lanes hold rows lane / 4 (+ 8) and 4-byte column pairs
+// lane % 4 of each 8-column group, so the eight rows of one bf16 store land in eight different chunks: no bank conflicts.
+// `at` is the address of this thread's first element in chunk 0 of its row r0 (box + r0 * 128 + byte offset in the chunk,
+// XOR (r0 % 8) << 4): chunk j of rows r0 and r0 + 8 is then at (at ^ j << 4) and 1024 bytes further.
+__device__ __forceinline__ uint32_t stage_addr(uint32_t box, int r0, int byte_in_chunk) {
+  return (box + r0 * 128 + byte_in_chunk) ^ ((r0 & 7) << 4);
+}
+// bf16: the 8-column groups i0 .. i0+7 of v (fragment layout) become one 64 x 64 box; `at` = stage_addr(box, r0, 2 * cq)
+template <int N>
+__device__ __forceinline__ void stage_bf16(uint32_t at, const float (&v)[N], int i0) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      sts_b32((at ^ (j << 4)) + 1024 * h, f2_to_bf2(v[4 * (i0 + j) + 2 * h], v[4 * (i0 + j) + 2 * h + 1]));
+}
+// fp32: the 8-column groups i0 .. i0+3 of v become one 64 x 32 box: columns 8j + cq, 8j + cq + 1 are 8 bytes of chunk
+// 2j + cq / 4; `at` = stage_addr(box, r0, 4 * (cq & 2))
+__device__ __forceinline__ void stage_f32(uint32_t at, const float (&v)[128], int i0, int cq) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      sts_f2((at ^ ((2 * j + cq / 4) << 4)) + 1024 * h, v[4 * (i0 + j) + 2 * h], v[4 * (i0 + j) + 2 * h + 1]);
+}
+// Round of the staging protocol of one MMA warpgroup (named barrier 1 + cw): the leader's earlier stores have finished
+// reading the staging before anyone writes it; the writes are visible to the async proxy before the leader stores them.
+__device__ __forceinline__ void staging_acquire(int cw, bool leader) {
+  if (leader) bulk_wait_read<0>();
+  named_bar_sync(1 + cw, 128);
+}
+__device__ __forceinline__ void staging_publish(int cw) {
+  fence_proxy_async_smem();
+  named_bar_sync(1 + cw, 128);
+}
+
 template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM>
-__device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_a, uint8_t* smem_b, uint64_t* full_bar,
-                                                 uint64_t* empty_bar, int wg, int m0, int n0, int n_blk, int kb0, int kb1) {
-  reg_alloc<232>();
-  const int cw = wg - 1;                         // this warpgroup's 64 rows of the tile
+__device__ __forceinline__ void mma_and_epilogue(const Params& p, const CUtensorMap* tmap_c, const CUtensorMap* tmap_c2,
+                                                 uint8_t* smem_a, uint8_t* smem_b, uint8_t* smem_c, uint64_t* full_bar,
+                                                 uint64_t* empty_bar, int cw, const Tile& tl, int& stage, uint32_t& phase) {
   constexpr int NI = ELEM ? 16 : 32;             // 8-column groups of the tile: acc[4*i + 2*h + e], i < NI
   constexpr int BNE = 8 * NI;
+  const int m0 = tl.m0, n0 = tl.n0, n_blk = tl.n_blk, kb0 = tl.kb0, kb1 = tl.kb1;
   float acc[128];
   if constexpr (ELEM != 0) {
     // FP8: per k-block 4 x k32 into `part` (same fragment layout as acc[0..63]), then acc += part in fp32 (promotion)
     float part[64];
 #pragma unroll
     for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
     for (int kb = kb0; kb < kb1; ++kb) {
       mbar_wait(&full_bar[stage], phase);
       const uint64_t adesc = make_smem_desc_sw128(smem_u32(smem_a + stage * A_BYTES) + cw * 64 * 128, 16, 1024);
@@ -256,8 +345,18 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
 #pragma unroll
     for (int j = 0; j < 64; ++j) acc[j] *= dq;
   } else {
-    int stage = 0, prev_stage = 0;
-    uint32_t phase = 0;
+    // release a stage to the producer (both CTAs' producers for CL = 2: the stage holds the peer's multicast half of B)
+    auto release = [&](int s) {
+      if ((threadIdx.x & 127) == 0) {
+        mbar_arrive(&empty_bar[s]);
+        if constexpr (CL == 2) mbar_arrive_cluster(&empty_bar[s], cluster_ctarank() ^ 1);
+      }
+    };
+    // scale_d = 0 on the tile's first k-block discards acc, but the wgmma operands read it: zeroing it here ends the
+    // previous tile's values (which would otherwise stay live through its epilogue and spill)
+#pragma unroll
+    for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+    int prev_stage = stage;
     for (int kb = kb0; kb < kb1; ++kb) {
       mbar_wait(&full_bar[stage], phase);
       const uint32_t a_base = smem_u32(smem_a + stage * A_BYTES) + (A_MN ? cw * BOX_BYTES : cw * 64 * 128);
@@ -274,31 +373,47 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
       }
       wgmma_commit();
       wgmma_wait<1>();                           // the previous k-block's MMAs have retired: release its stage
-      if (kb > kb0 && (threadIdx.x & 127) == 0) {
-        mbar_arrive(&empty_bar[prev_stage]);
-        if constexpr (CL == 2) mbar_arrive_cluster(&empty_bar[prev_stage], cluster_ctarank() ^ 1);
-      }
+      if (kb > kb0) release(prev_stage);
       prev_stage = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
     wgmma_wait<0>();
+    if (kb1 > kb0) release(prev_stage);          // before the epilogue: the producer refills it for the next tile meanwhile
   }
 
   // -------------------------------------------------------------------- epilogue from the accumulator registers
   // Fragment of m64n256: acc[4*i + 2*h + e] is row (16*warp + lane/4 + 8*h), column (8*i + 2*(lane%4) + e).
   const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
-  const int rbase = m0 + cw * 64 + warp * 16 + (lane >> 2);
+  const int r0 = warp * 16 + (lane >> 2);        // rows r0 and r0 + 8 of this warpgroup's 64
+  const int rbase = m0 + cw * 64 + r0;
   const int cq = 2 * (lane & 3);
+  // TMA epilogues: this warpgroup's boxes start at row `row0`; two staging boxes s0, s1; thread 0 of the warpgroup stores
+  const int row0 = m0 + cw * 64;
+  const bool leader = t == 0, rows_ok = row0 < p.M;
+  uint8_t* stg0 = smem_c + cw * STG_BYTES;
+  uint8_t* stg1 = stg0 + OUT_BOX;
+  const uint32_t s0 = stage_addr(smem_u32(stg0), r0, 2 * cq), s1 = s0 + OUT_BOX;   // bf16 boxes
+  // the bf16 tile in acc to C columns n0.. (boxes wholly right of N are skipped, the others clipped by the map)
+  auto store_tile = [&]() {
+#pragma unroll
+    for (int c = 0; c < NI / 8; c += 2) {
+      staging_acquire(cw, leader);
+      stage_bf16(s0, acc, 8 * c);
+      stage_bf16(s1, acc, 8 * c + 8);
+      staging_publish(cw);
+      if (leader && rows_ok) {
+        if (n0 + 64 * c < p.N) tma_store_2d(stg0, tmap_c, n0 + 64 * c, row0);
+        if (n0 + 64 * c + 64 < p.N) tma_store_2d(stg1, tmap_c, n0 + 64 * c + 64, row0);
+        bulk_commit();
+      }
+    }
+  };
 
   if constexpr (EPI == kStore || EPI == kRoPE) {
-    __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C);
-    const bool rope_tile = EPI == kRoPE && n0 < p.rope_cols;
+    if (EPI == kRoPE && n0 < p.rope_cols) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = rbase + 8 * h;
-      if (row >= p.M) continue;
-      if (EPI == kRoPE && rope_tile) {
-        const int pos = row % p.S;
+      for (int h = 0; h < 2; ++h) {
+        const int pos = (rbase + 8 * h) % p.S;   // rows beyond M are computed too (in-range table rows) and clipped
 #pragma unroll
         for (int c = 0; c < NI / 8; ++c) {
           if (n0 + c * 64 >= p.rope_cols) continue;
@@ -317,37 +432,46 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
           }
         }
       }
-      __nv_bfloat16* crow = C + (size_t)row * p.ldc;
-#pragma unroll
-      for (int i = 0; i < NI; ++i) {
-        const int col = n0 + 8 * i + cq;
-        if (col + 1 < p.N) st_bf2(crow + col, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-        else if (col < p.N) crow[col] = __float2bfloat16_rn(acc[4 * i + 2 * h]);
-      }
     }
+    store_tile();
   } else if constexpr (EPI == kSwiGLU) {
-    // tile columns [0,BNE/2) are gate columns g0.., [BNE/2,BNE) the matching up columns
-    __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.C);
-    __nv_bfloat16* act = reinterpret_cast<__nv_bfloat16*>(p.aux);
+    // tile columns [0,BNE/2) are gate columns g0.., [BNE/2,BNE) the matching up columns; C = gu [M, 2I] (tmap_c),
+    // aux = act [M, I] (tmap_c2).  I % 64 == 0: a 64-column box is either all gate (up) columns or wholly beyond I.
+    constexpr int NB = NI / 16;                  // 64-column boxes of gate (of up, of act) per tile
     const int g0 = n_blk * (BNE / 2);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = rbase + 8 * h;
-      if (row >= p.M) continue;
+    for (int c = 0; c < NB; ++c) {
+      staging_acquire(cw, leader);
+      stage_bf16(s0, acc, 8 * c);
+      stage_bf16(s1, acc, NI / 2 + 8 * c);
+      staging_publish(cw);
+      if (leader && rows_ok && g0 + 64 * c < p.I) {
+        tma_store_2d(stg0, tmap_c, g0 + 64 * c, row0);
+        tma_store_2d(stg1, tmap_c, p.I + g0 + 64 * c, row0);
+        bulk_commit();
+      }
+    }
+    // the activation, from the bf16 values the backward will see, replaces the gate half of acc
 #pragma unroll
-      for (int i = 0; i < NI / 2; ++i) {
-        const int col = g0 + 8 * i + cq;
-        if (col >= p.I) continue;                // I % 64 == 0: pairs never straddle the end
-        const float ga = acc[4 * i + 2 * h], gb = acc[4 * i + 2 * h + 1];
-        const float ua = acc[4 * (i + NI / 2) + 2 * h], ub = acc[4 * (i + NI / 2) + 2 * h + 1];
-        st_bf2(gu + (size_t)row * p.ldc + col, ga, gb);
-        st_bf2(gu + (size_t)row * p.ldc + p.I + col, ua, ub);
-        // the activation is computed from the bf16 values the backward will see
-        const float ga_r = bf16_round(ga), gb_r = bf16_round(gb), ua_r = bf16_round(ua), ub_r = bf16_round(ub);
-        st_bf2(act + (size_t)row * p.ldaux + col, ga_r * fast_sigmoid(ga_r) * ua_r, gb_r * fast_sigmoid(gb_r) * ub_r);
+    for (int j = 0; j < 2 * NI; ++j) {
+      const float g = bf16_round(acc[j]), u = bf16_round(acc[j + 2 * NI]);
+      acc[j] = g * fast_sigmoid(g) * u;
+    }
+#pragma unroll
+    for (int c = 0; c < NB; c += 2) {
+      staging_acquire(cw, leader);
+      stage_bf16(s0, acc, 8 * c);
+      if (c + 1 < NB) stage_bf16(s1, acc, 8 * c + 8);
+      staging_publish(cw);
+      if (leader && rows_ok) {
+        if (g0 + 64 * c < p.I) tma_store_2d(stg0, tmap_c2, g0 + 64 * c, row0);
+        if (c + 1 < NB && g0 + 64 * c + 64 < p.I) tma_store_2d(stg1, tmap_c2, g0 + 64 * c + 64, row0);
+        bulk_commit();
       }
     }
   } else if constexpr (EPI == kSwiGLUBwd) {
+    // register epilogue: staging d(gate) / d(up) needs the gate / up loads in registers next to the accumulator, which
+    // does not fit the 168 registers a thread has
     __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.C);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -375,41 +499,53 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
   } else if constexpr (EPI == kLCEFwd) {
     static_assert(ELEM == 0, "bf16 only");
     constexpr float L2E = 1.4426950408889634f;
-    __nv_bfloat16* E = reinterpret_cast<__nv_bfloat16*>(p.C);
+    float shift[2], psum[2] = {0.f, 0.f}, psq[2] = {0.f, 0.f};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) shift[h] = rbase + 8 * h < p.M ? p.row_shift[rbase + 8 * h] * L2E : 0.f;
+    // 128 columns (two boxes) at a time: e replaces the logits in acc and is stored right away (training)
+#pragma unroll
+    for (int c = 0; c < 4; c += 2) {
+#pragma unroll
+      for (int i = 8 * c; i < 8 * c + 16; ++i) {
+        const int col = n0 + 8 * i + cq;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float& v = acc[4 * i + 2 * h + e];
+            const bool ok = col + e < p.N;
+            // clamp: a row whose label is > 69 nats below its best logit would overflow the fp32 row sum otherwise
+            float x;
+            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(x) : "f"(fminf(fmaf(v, L2E, -shift[h]), 100.f)));
+            psq[h] += ok ? v * v : 0.f;
+            v = ok ? x : 0.f;
+            psum[h] += v;
+          }
+        }
+      }
+      if (p.store) {
+        staging_acquire(cw, leader);
+        stage_bf16(s0, acc, 8 * c);
+        stage_bf16(s1, acc, 8 * c + 8);
+        staging_publish(cw);
+        if (leader && rows_ok) {
+          if (n0 + 64 * c < p.N) tma_store_2d(stg0, tmap_c, n0 + 64 * c, row0);
+          if (n0 + 64 * c + 64 < p.N) tma_store_2d(stg1, tmap_c, n0 + 64 * c + 64, row0);
+          bulk_commit();
+        }
+      }
+    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = rbase + 8 * h;
-      const bool row_ok = row < p.M;
-      const float shift = row_ok ? p.row_shift[row] * L2E : 0.f;
-      float psum = 0.f, psq = 0.f;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int col = n0 + 8 * i + cq;
-        float ev[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float v = acc[4 * i + 2 * h + e];
-          const bool ok = col + e < p.N;
-          // clamp: a row whose label is > 69 nats below its best logit would overflow the fp32 row sum otherwise
-          float x;
-          asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(x) : "f"(fminf(fmaf(v, L2E, -shift), 100.f)));
-          ev[e] = ok ? x : 0.f;
-          psum += ev[e];
-          psq += ok ? v * v : 0.f;
-        }
-        if (p.store && row_ok) {
-          __nv_bfloat16* erow = E + (size_t)row * p.ldc;
-          if (col + 1 < p.N) st_bf2(erow + col, ev[0], ev[1]);
-          else if (col < p.N) erow[col] = __float2bfloat16_rn(ev[0]);
-        }
-      }
-      psum += __shfl_xor_sync(0xffffffffu, psum, 1);
-      psum += __shfl_xor_sync(0xffffffffu, psum, 2);
-      psq += __shfl_xor_sync(0xffffffffu, psq, 1);
-      psq += __shfl_xor_sync(0xffffffffu, psq, 2);
-      if (row_ok && (lane & 3) == 0) {
-        p.partials[(size_t)n_blk * p.M + row] = psum;
-        if (p.want_sumsq) p.partials[((size_t)p.num_n + n_blk) * p.M + row] = psq;
+      float ps = psum[h], pq = psq[h];
+      ps += __shfl_xor_sync(0xffffffffu, ps, 1);
+      ps += __shfl_xor_sync(0xffffffffu, ps, 2);
+      pq += __shfl_xor_sync(0xffffffffu, pq, 1);
+      pq += __shfl_xor_sync(0xffffffffu, pq, 2);
+      if (row < p.M && (lane & 3) == 0) {
+        p.partials[(size_t)n_blk * p.M + row] = ps;
+        if (p.want_sumsq) p.partials[((size_t)p.num_n + n_blk) * p.M + row] = pq;
       }
     }
   } else if constexpr (EPI == kLCEdX) {
@@ -491,7 +627,7 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
       if (row_ok && lab >= 0 && (lab & 6) == 0) p.sc_zlab[row] = zl;     // this thread owns the label column
     }
   } else if constexpr (EPI == kAxpby) {
-    const size_t boff = (size_t)blockIdx.y * p.c_bstride;
+    const size_t boff = (size_t)tl.b * p.c_bstride;
     __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C) + boff;
     const __nv_bfloat16* D = p.aux ? reinterpret_cast<const __nv_bfloat16*>(p.aux) + boff : nullptr;
 #pragma unroll
@@ -512,17 +648,18 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, uint8_t* smem_
       }
     }
   } else if constexpr (EPI == kWgradAcc) {
-    float* dW = reinterpret_cast<float*>(p.C);
+    // fp32 reduce-add into dW (tmap_c) in 64 x 32 boxes: the split-K items of a tile and later micro-batches add into it
+    const uint32_t f0 = stage_addr(smem_u32(stg0), r0, 4 * (cq & 2));
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = rbase + 8 * h;
-      if (row >= p.M) continue;
-      float* drow = dW + (size_t)row * p.ldc;
-#pragma unroll
-      for (int i = 0; i < NI; ++i) {
-        const int col = n0 + 8 * i + cq;
-        if (col + 1 < p.N) red_add_f2(drow + col, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-        else if (col < p.N) atomicAdd(drow + col, acc[4 * i + 2 * h]);
+    for (int c = 0; c < NI / 4; c += 2) {
+      staging_acquire(cw, leader);
+      stage_f32(f0, acc, 4 * c, cq);
+      stage_f32(f0 + OUT_BOX, acc, 4 * c + 4, cq);
+      staging_publish(cw);
+      if (leader && rows_ok) {
+        if (n0 + 32 * c < p.N) tma_reduce_add_2d(stg0, tmap_c, n0 + 32 * c, row0);
+        if (n0 + 32 * c + 32 < p.N) tma_reduce_add_2d(stg1, tmap_c, n0 + 32 * c + 32, row0);
+        bulk_commit();
       }
     }
   }
@@ -584,6 +721,20 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
   } else {
     if ((rc = make_tmap_2d(&tb, B, b_rows_all, K, ldb * EB, BNE, KB, EB))) return rc;
   }
+  // outputs stored by TMA: 64-row boxes of 128 bytes on the caller's view (base, [rows, cols], row stride), so partial
+  // tiles are clipped to it.  TMA needs a 16-byte aligned base: a misaligned output is refused (-1).
+  CUtensorMap tc = tb, tc2 = tb;                 // unused maps stay valid copies
+  auto out_map = [](CUtensorMap* m, void* base, int rows, int cols, long long ld, int eb) {
+    if (reinterpret_cast<uintptr_t>(base) % 16) return -1;
+    return make_tmap_2d(m, base, rows, cols, ld * eb, 64, 128 / eb, eb);
+  };
+  if (EPI == kStore || EPI == kRoPE || (EPI == kLCEFwd && lce.store)) {
+    if ((rc = out_map(&tc, C, M, N, ldc, 2))) return rc;
+  } else if (EPI == kSwiGLU) {
+    if ((rc = out_map(&tc, C, M, 2 * I, ldc, 2)) || (rc = out_map(&tc2, aux, M, I, ldaux, 2))) return rc;
+  } else if (EPI == kWgradAcc) {
+    if ((rc = out_map(&tc, C, M, N, ldc, 4))) return rc;
+  }
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.num_m = ceil_div(M, BM);
@@ -600,12 +751,14 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
   p.sc_max = lce.sc_max; p.sc_sum = lce.sc_sum; p.sc_idx = lce.sc_idx; p.sc_zlab = lce.sc_zlab;
   p.inv_a = inv_a; p.inv_b = inv_b;
   p.a_rows = ba.a_rows; p.b_rows = ba.b_rows; p.c_bstride = ba.c_bstride; p.alpha = ba.alpha; p.beta = ba.beta;
+  p.batch = ba.batch;
   const int tiles = p.num_m * p.num_n;
   const int kb_total = ceil_div(K, KB);
   p.splits = 1;
   p.kb_per_split = kb_total;
   if (EPI == kWgradAcc) {
-    // split-K over the tokens so that tiles * splits is close to a whole number of waves, >= 16 k-blocks per work item
+    // split-K over the tokens so that tiles * splits is close to a whole multiple of the grid (one CTA per SM), so every
+    // persistent CTA gets the same number of work items; >= 16 k-blocks per work item
     int best = 1;
     double best_eff = 0.0;
     for (int s = 1; s <= 64 && kb_total / s >= 16; ++s) {
@@ -624,9 +777,11 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
-  const int cluster_tiles = ceil_div(p.num_m, CL) * p.num_n;
-  launch_pdl_cluster(gemm_kernel<EPI, A_MN, B_MN, CL, ELEM>, dim3(cluster_tiles * CL * p.splits, ba.batch), dim3(THREADS), SMEM_BYTES, st, CL,
-                     ta, ta1, ta2, tb, p);
+  // persistent grid: one CTA (CL = 2: one cluster per two SMs) per SM, or fewer when there are fewer work items
+  const int work = ceil_div(p.num_m, CL) * p.num_n * p.splits * ba.batch;
+  const int clusters = work < sm_count() / CL ? work : sm_count() / CL;
+  launch_pdl_cluster(gemm_kernel<EPI, A_MN, B_MN, CL, ELEM>, dim3(clusters * CL), dim3(THREADS), SMEM_BYTES, st, CL,
+                     ta, ta1, ta2, tb, tc, tc2, p);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : (int)e;
 }

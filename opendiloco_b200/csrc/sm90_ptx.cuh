@@ -70,6 +70,13 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
                : "memory");
 }
 
+// shared -> global store of one tensor-map box (elements outside the map's extent are not written), tracked by the issuing
+// thread's bulk group.  The shared-memory source follows the map's swizzle and is 128-byte aligned.
+__device__ __forceinline__ void tma_store_2d(const void* smem_src, const CUtensorMap* m, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
 // shared -> global reduce-add of one tensor-map box (fp32 add for a FLOAT32 map), tracked by the issuing thread's bulk
 // group.  The shared-memory source follows the map's swizzle and is 128-byte aligned.
 __device__ __forceinline__ void tma_reduce_add_2d(const void* smem_src, const CUtensorMap* m, int c0, int c1) {

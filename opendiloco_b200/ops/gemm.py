@@ -42,7 +42,8 @@ def mm_nn(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor | None = None) -> 
 def mm_tn_acc(a: torch.Tensor, b: torch.Tensor, acc: torch.Tensor, alpha: float = 1.0) -> None:
     """acc (fp32 [N,K]) += alpha * a^T @ b with low-precision a [T,N], b [T,K] and fp32 accumulation/output."""
     global _ADDMM_DTYPE_OK
-    if alpha == 1.0 and acc.dtype == torch.float32 and acc.stride(-1) == 1 and TC.wgrad_usable(a, b):
+    if (alpha == 1.0 and acc.dtype == torch.float32 and acc.stride(-1) == 1 and acc.data_ptr() % 16 == 0
+            and TC.wgrad_usable(a, b)):
         TC.wgrad_acc(a, b, acc)          # wgmma, MN-major operands, split-K, fp32 reduce-add into the grad arena
         return
     if a.dtype == acc.dtype:

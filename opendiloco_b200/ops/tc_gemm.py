@@ -73,9 +73,10 @@ def _fn(name: str, M: int = 1 << 30, N: int = 1 << 30):
 
 
 def usable(*tensors: torch.Tensor) -> bool:
-    """CUDA bf16 matrices with contiguous rows whose row stride and width are multiples of 8 elements (16-byte TMA rows);
-    anything else (e.g. an odd vocabulary size) takes the library GEMM."""
-    return ENABLED and all(t.is_cuda and t.dtype == torch.bfloat16 and t.stride(-1) == 1 and
+    """CUDA bf16 matrices with contiguous rows whose row stride and width are multiples of 8 elements (16-byte TMA rows)
+    and whose base is 16-byte aligned (TMA reads the operands and stores the output); anything else (e.g. an odd
+    vocabulary size, a view starting at an odd column) takes the library GEMM."""
+    return ENABLED and all(t.is_cuda and t.dtype == torch.bfloat16 and t.stride(-1) == 1 and t.data_ptr() % 16 == 0 and
                            (t.dim() < 2 or (t.stride(0) % 8 == 0 and t.shape[-1] % 8 == 0)) for t in tensors) and \
         _lib.has_symbol("odb_gemm_bf16_tn")
 

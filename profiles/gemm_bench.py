@@ -1,6 +1,15 @@
-"""wgmma GEMM family vs cuBLAS (torch.mm): numerics + CUDA-event timing at the Llama-150M / 1B shapes."""
-import os, sys, torch
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+"""wgmma GEMM family vs cuBLAS (torch.mm): numerics + CUDA-event timing at the Llama-150M / 1B shapes.
+
+    python profiles/gemm_bench.py [--root DIR] [--step-only]
+
+--root DIR imports opendiloco_b200 from another built tree (e.g. an older commit, to compare two versions in one run);
+--step-only times just the GEMMs of a Llama-150M micro-step (T = 32768) and prints one line per shape."""
+import argparse, os, sys, torch
+_ap = argparse.ArgumentParser()
+_ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+_ap.add_argument("--step-only", action="store_true")
+ARGS = _ap.parse_args()
+sys.path.insert(0, os.path.abspath(ARGS.root))
 from opendiloco_b200.ops import tc_gemm as T, kernels as K
 dev = "cuda"; BF = torch.bfloat16
 torch.manual_seed(0)
@@ -15,6 +24,50 @@ def timeit(fn, n=20):
     return e0.elapsed_time(e1) / n
 
 def rel(a, b): return ((a.float() - b.float()).norm() / b.float().norm()).item()
+
+
+def step_shapes(Tn=32768, h=1024, I=2688, V=32000, S=1024):
+    """Every GEMM of a Llama-150M micro-step at Tn tokens: microseconds (median of 5 timings of 20 calls) and TFLOP/s."""
+    x = torch.randn(Tn, h, device=dev).to(BF)
+    rows = []
+    def run(name, fn, flops):
+        fn(); torch.cuda.synchronize()
+        ts = sorted(timeit(fn) for _ in range(5))
+        rows.append((name, ts[2] * 1e3, flops / (ts[2] * 1e-3) / 1e12, (ts[-1] - ts[0]) * 1e3))
+    w_qkv = (torch.randn(3 * h, h, device=dev) * 0.05).to(BF); qkv = torch.empty(Tn, 3 * h, device=dev, dtype=BF)
+    cos, sin = K.rope_tables(S, 64, 10000.0, dev)
+    run("qkv_rope fwd K1024", lambda: T.linear_qkv_rope(x, w_qkv, qkv, cos, sin, S, 2 * h), 2 * Tn * 3 * h * h)
+    w_o = (torch.randn(h, h, device=dev) * 0.05).to(BF); o = torch.empty(Tn, h, device=dev, dtype=BF)
+    run("o fwd K1024", lambda: T.linear(x, w_o, o), 2 * Tn * h * h)
+    w_gu = (torch.randn(2 * I, h, device=dev) * 0.05).to(BF)
+    gu = torch.empty(Tn, 2 * I, device=dev, dtype=BF); act = torch.empty(Tn, I, device=dev, dtype=BF)
+    run("gate|up swiglu fwd K1024", lambda: T.linear_swiglu(x, w_gu, gu, act), 2 * Tn * 2 * I * h)
+    w_d = (torch.randn(h, I, device=dev) * 0.05).to(BF)
+    run("down fwd K2688", lambda: T.linear(act, w_d, o), 2 * Tn * h * I)
+    dy = torch.randn(Tn, h, device=dev).to(BF); gu0 = torch.randn(Tn, 2 * I, device=dev).to(BF)
+    run("down dgrad+swiglu bwd K1024", lambda: T.linear_swiglu_bwd(dy, w_d, gu0), 2 * Tn * I * h)
+    run("gate|up dgrad (nn) K5376", lambda: T.linear_nn(gu0, w_gu, o), 2 * Tn * h * 2 * I)
+    run("o dgrad (nn) K1024", lambda: T.linear_nn(dy, w_o, o), 2 * Tn * h * h)
+    dqkv = torch.randn(Tn, 3 * h, device=dev).to(BF)
+    run("qkv dgrad (nn) K3072", lambda: T.linear_nn(dqkv, w_qkv, o), 2 * Tn * h * 3 * h)
+    for (n, k, a) in [(3 * h, h, dqkv), (h, h, dy), (2 * I, h, gu0), (h, I, dy)]:
+        b = x if k == h else act
+        dw = torch.zeros(n, k, device=dev)
+        run(f"wgrad N{n} K{k}", lambda a=a, b=b, dw=dw: T.wgrad_acc(a, b, dw), 2 * Tn * n * k)
+    w_lm = (torch.randn(V, h, device=dev) * 0.02).to(BF)
+    shift = torch.zeros(Tn, device=dev)
+    planes = (V + 255) // 256
+    partials = torch.empty(planes * Tn, device=dev); e = torch.empty(Tn, V, device=dev, dtype=BF)
+    run("lce_fwd store=1 K1024", lambda: T.lce_fwd(x, w_lm, shift, partials, e), 2 * Tn * V * h)
+    rs = torch.full((Tn,), 1e-3, device=dev); lab = torch.randint(0, V, (Tn,), device=dev); gs = torch.ones((), device=dev)
+    run("lce_dx K32000", lambda: T.lce_dx(e, w_lm, rs, lab, gs, o), 2 * Tn * V * h)
+    for name, us, tf, spread in rows:
+        print(f"STEP {name:32s} {us:9.1f} us {tf:6.1f} TF/s  (spread {spread:.1f} us)")
+
+
+if ARGS.step_only:
+    step_shapes()
+    sys.exit(0)
 
 print("== plain TN GEMM")
 for (M, N, Kd) in [(300, 520, 200), (128, 256, 64), (4096, 1024, 1024), (32768, 1024, 1024), (32768, 3072, 1024), (32768, 5376, 1024),
