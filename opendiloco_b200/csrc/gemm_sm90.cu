@@ -30,7 +30,9 @@
 //   kSwiGLU  : B rows are [gate rows n0..n0+127 | up rows I+n0..I+n0+127]; writes gate|up (needed by backward) AND
 //              act = silu(gate) * up, so the SwiGLU kernel and its re-read of the 2I-wide tensor disappear
 //   kSwiGLUBwd: the GEMM result is d(act) of the down projection; the epilogue reads the matching gate / up values of
-//              C = gu [M, 2I] and turns them IN PLACE into d(gate) / d(up) - d(act) never reaches memory
+//              C = gu [M, 2I] and turns them IN PLACE into d(gate) / d(up) - d(act) never reaches memory.  The producer
+//              carries the gate / up values through the operand ring behind the tile's last k-block (one ring entry per
+//              64-column round), so they arrive while the last MMAs run; d(gate) / d(up) leave by TMA like the other outputs
 //   kRoPE    : C is the packed qkv buffer; 64-column chunks are heads; chunks below `rope_cols` are rotated with the
 //              HF rotate-half convention using fp32 cos/sin tables (position = row % S)
 //   kLCEFwd  : fused linear-cross-entropy forward.  The accumulator holds a tile of LM-head logits z; the epilogue turns
@@ -138,6 +140,11 @@ __device__ __forceinline__ float2 ld_bf2(const void* p) { return bf2_to_f2(*rein
 __device__ __forceinline__ void sts_b32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
+__device__ __forceinline__ uint32_t lds_b32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
 __device__ __forceinline__ void sts_f2(uint32_t addr, float a, float b) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
@@ -166,12 +173,21 @@ __device__ __forceinline__ Tile tile_of(const Params& p, int work, uint32_t rank
   return t;
 }
 
+// kSwiGLUBwd: ring entries that carry a tile's gate / up values, one per 64-column round of the tile's d(act) columns
+// n0.. below I (I % 64 == 0: a round is wholly inside I or wholly beyond it).  The producer and the consumers both count
+// with this function: a disagreement would desynchronise the ring's phases.
+template <int BNE>
+__device__ __forceinline__ int swiglu_bwd_rounds(const Params& p, int n0) {
+  return min(BNE / 64, (p.I - n0) / 64);
+}
+
 template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM>
 __device__ __forceinline__ void mma_and_epilogue(const Params& p, const CUtensorMap* tmap_c, const CUtensorMap* tmap_c2,
                                                  uint8_t* smem_a, uint8_t* smem_b, uint8_t* smem_c, uint64_t* full_bar,
                                                  uint64_t* empty_bar, int cw, const Tile& tl, int& stage, uint32_t& phase);
 
-// Output maps (tmap_c, tmap_c2): C (gu for kSwiGLU, fp32 dW for kWgradAcc) and act (kSwiGLU); see launch().
+// Output maps (tmap_c, tmap_c2): C (gu for kSwiGLU and kSwiGLUBwd, which also loads from it; fp32 dW for kWgradAcc) and
+// act (kSwiGLU); see launch().
 template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM = 0>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a1,
@@ -190,7 +206,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   static_assert(ELEM == 0 || (CL == 1 && !A_MN && !B_MN), "FP8 wgmma takes K-major operands only");
   constexpr int KB = ELEM ? BK8 : BK;            // elements per k-block
   constexpr int BNE = ELEM ? BN / 2 : BN;        // tile columns
-  constexpr bool TMA_OUT = EPI == kStore || EPI == kRoPE || EPI == kSwiGLU || EPI == kLCEFwd || EPI == kWgradAcc;
+  constexpr bool TMA_OUT =
+      EPI == kStore || EPI == kRoPE || EPI == kSwiGLU || EPI == kSwiGLUBwd || EPI == kLCEFwd || EPI == kWgradAcc;
   const int wg = threadIdx.x >> 7;
   const uint32_t rank = CL == 2 ? cluster_ctarank() : 0;
   const int work_total = (p.num_m + CL - 1) / CL * p.num_n * p.splits * p.batch;
@@ -255,6 +272,23 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, bn0);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        if constexpr (EPI == kSwiGLUBwd) {
+          // the epilogue's gate / up values, 64 columns per entry: the gate boxes of rows m0 and m0 + 64 in the A slot, the
+          // up boxes in the B slot (rows beyond M arrive as zeros and count towards the transaction bytes)
+          const int rounds = swiglu_bwd_rounds<BNE>(p, t.n0);
+          for (int c = 0; c < rounds; ++c) {
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_arrive_expect_tx(&full_bar[stage], 4 * OUT_BOX);
+            uint8_t* sa = smem_a + stage * A_BYTES;
+            uint8_t* sb = smem_b + stage * B_BYTES;
+            const int col = t.n0 + 64 * c;
+            tma_load_2d(sa, &tmap_c, &full_bar[stage], col, t.m0);
+            tma_load_2d(sa + OUT_BOX, &tmap_c, &full_bar[stage], col, t.m0 + 64);
+            tma_load_2d(sb, &tmap_c, &full_bar[stage], p.I + col, t.m0);
+            tma_load_2d(sb + OUT_BOX, &tmap_c, &full_bar[stage], p.I + col, t.m0 + 64);
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
         }
       }
     }
@@ -470,31 +504,52 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, const CUtensor
       }
     }
   } else if constexpr (EPI == kSwiGLUBwd) {
-    // register epilogue: staging d(gate) / d(up) needs the gate / up loads in registers next to the accumulator, which
-    // does not fit the 168 registers a thread has
-    __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.C);
+    // Round c takes the ring entry the producer filled with the gate / up boxes of gate columns n0 + 64c.. (this
+    // warpgroup's box at cw * OUT_BOX of the A / B slot, the staging layout) and the accumulator's 8-column groups
+    // 8c .. 8c+7; d(gate) / d(up) go to the staging and are stored in place into gu (tmap_c).  The ring entry is released
+    // once every thread has passed the staging barrier, so the producer refills it without waiting for the stores.
+    const int rounds = swiglu_bwd_rounds<BNE>(p, n0);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = rbase + 8 * h;
-      if (row >= p.M) continue;
-      __nv_bfloat16* grow = gu + (size_t)row * p.ldc;
+    for (int c = 0; c < NI / 8; ++c) {
+      if (c >= rounds) break;
+      mbar_wait(&full_bar[stage], phase);
+      staging_acquire(cw, leader);
+      const uint32_t g_at = stage_addr(smem_u32(smem_a + stage * A_BYTES) + cw * OUT_BOX, r0, 2 * cq);
+      const uint32_t u_at = stage_addr(smem_u32(smem_b + stage * B_BYTES) + cw * OUT_BOX, r0, 2 * cq);
 #pragma unroll
-      for (int i = 0; i < NI; ++i) {
-        const int col = n0 + 8 * i + cq;
-        if (col >= p.I) continue;
-        const float2 g = ld_bf2(grow + col), u = ld_bf2(grow + p.I + col);
-        float og[2], ou[2];
-        const float gg[2] = {g.x, g.y}, uu[2] = {u.x, u.y};
+      for (int h = 0; h < 2; ++h) {
+        uint32_t gv[8], uv[8];
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float dj = bf16_round(acc[4 * i + 2 * h + e]);   // the un-fused path rounds d(act) to bf16 first
-          const float sg = fast_sigmoid(gg[e]);
-          og[e] = dj * uu[e] * sg * (1.f + gg[e] * (1.f - sg));
-          ou[e] = dj * gg[e] * sg;
+        for (int j = 0; j < 8; ++j) {
+          gv[j] = lds_b32((g_at ^ (j << 4)) + 1024 * h);
+          uv[j] = lds_b32((u_at ^ (j << 4)) + 1024 * h);
         }
-        st_bf2(grow + col, og[0], og[1]);
-        st_bf2(grow + p.I + col, ou[0], ou[1]);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float2 g = bf2_to_f2(gv[j]), u = bf2_to_f2(uv[j]);
+          float og[2], ou[2];
+          const float gg[2] = {g.x, g.y}, uu[2] = {u.x, u.y};
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float dj = bf16_round(acc[4 * (8 * c + j) + 2 * h + e]);   // the un-fused path rounds d(act) to bf16 first
+            const float sg = fast_sigmoid(gg[e]);
+            og[e] = dj * uu[e] * sg * (1.f + gg[e] * (1.f - sg));
+            ou[e] = dj * gg[e] * sg;
+          }
+          sts_b32((s0 ^ (j << 4)) + 1024 * h, f2_to_bf2(og[0], og[1]));
+          sts_b32((s1 ^ (j << 4)) + 1024 * h, f2_to_bf2(ou[0], ou[1]));
+        }
       }
+      staging_publish(cw);
+      if (leader) {
+        mbar_arrive(&empty_bar[stage]);
+        if (rows_ok) {
+          tma_store_2d(stg0, tmap_c, n0 + 64 * c, row0);
+          tma_store_2d(stg1, tmap_c, p.I + n0 + 64 * c, row0);
+          bulk_commit();
+        }
+      }
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
   } else if constexpr (EPI == kLCEFwd) {
     static_assert(ELEM == 0, "bf16 only");
@@ -732,6 +787,8 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
     if ((rc = out_map(&tc, C, M, N, ldc, 2))) return rc;
   } else if (EPI == kSwiGLU) {
     if ((rc = out_map(&tc, C, M, 2 * I, ldc, 2)) || (rc = out_map(&tc2, aux, M, I, ldaux, 2))) return rc;
+  } else if (EPI == kSwiGLUBwd) {
+    if ((rc = out_map(&tc, C, M, 2 * I, ldc, 2))) return rc;      // gu: the epilogue's gate / up loads and its stores
   } else if (EPI == kWgradAcc) {
     if ((rc = out_map(&tc, C, M, N, ldc, 4))) return rc;
   }
@@ -815,7 +872,8 @@ ODB_EXPORT int odb_gemm2_swiglu(const void* X, const void* Wgu, void* gu, void* 
 }
 
 // Backward of the SwiGLU MLP's middle: gu[M,2I] (gate|up, bf16) is replaced IN PLACE by d(gate)|d(up), where
-// d(act)[M,I] = dY[M,K] * WdT[I,K]^T is formed in registers only (I % 64 == 0).
+// d(act)[M,I] = dY[M,K] * WdT[I,K]^T is formed in registers only (I % 64 == 0; gu is read and written by TMA, so a base
+// that is not 16-byte aligned is refused with -1).
 ODB_EXPORT int odb_gemm_swiglu_bwd(const void* dY, const void* WdT, void* gu, int M, int I, int K, long long lda, long long ldb,
                                    cudaStream_t st) {
   if (K % 8 || I % 64 || lda % 8 || ldb % 8) return -1;
