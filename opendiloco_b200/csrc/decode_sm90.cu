@@ -11,6 +11,8 @@
 // chunk of them is ONE bulk copy.
 #include <curand_kernel.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 #include "sm90_ptx.cuh"
 
@@ -24,17 +26,12 @@ constexpr int CH = 128;             // keys per attention CTA
 constexpr int ATT_THREADS = 128;    // one thread per key in the score phase, four warps in P V
 
 // ------------------------------------------------------------------------------------------------ RoPE + append
-// grid B, block 256.  qkv [B, ld] (q heads, k heads, v heads; unrotated GEMM output).  q is rotated in place; rotated k and
-// v go to the cache.  Rounding: fp32 rotation of the bf16 inputs, one rounding to bf16 (as ops.kernels.rope_).
-__global__ void __launch_bounds__(256)
-rope_append_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const float* __restrict__ cos_t, const float* __restrict__ sin_t,
-                   const int* __restrict__ pos, __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc, int Hq, int Hkv,
-                   int Smax) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int b = blockIdx.x;
-  const int p = pos[b];
-  __nv_bfloat16* row = qkv + (long long)b * ld;
+// One block per token.  row: the token's qkv row (q heads, k heads, v heads; unrotated GEMM output); p its position; b its
+// sequence.  q is rotated in place; rotated k and v go to the cache at (b, p).  Rounding: fp32 rotation of the bf16 inputs,
+// one rounding to bf16 (as ops.kernels.rope_).
+__device__ __forceinline__ void rope_append_token(__nv_bfloat16* __restrict__ row, int p, int b, const float* __restrict__ cos_t,
+                                                  const float* __restrict__ sin_t, __nv_bfloat16* __restrict__ kc,
+                                                  __nv_bfloat16* __restrict__ vc, int Hq, int Hkv, int Smax) {
   const float* cr = cos_t + (long long)p * (D / 2);
   const float* sr = sin_t + (long long)p * (D / 2);
   const int n_rot = (Hq + Hkv) * (D / 2);
@@ -59,6 +56,29 @@ rope_append_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const float* _
       reinterpret_cast<uint32_t*>(vc + (((long long)b * Hkv + hk) * Smax + p) * D)[e] = v;
     }
   }
+}
+
+// grid B, block 256: one new token per row at the row's own position pos[b] (read from device memory, so a captured graph
+// stays valid at every step).
+__global__ void __launch_bounds__(256)
+rope_append_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const float* __restrict__ cos_t, const float* __restrict__ sin_t,
+                   const int* __restrict__ pos, __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc, int Hq, int Hkv,
+                   int Smax) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x;
+  rope_append_token(qkv + (long long)b * ld, pos[b], b, cos_t, sin_t, kc, vc, Hq, Hkv, Smax);
+}
+
+// grid (B, n), block 256: n tokens per row, slot-major rows (row j*B + b is token j of sequence b, at position pos[b] + j).
+__global__ void __launch_bounds__(256)
+rope_append_multi_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const float* __restrict__ cos_t,
+                         const float* __restrict__ sin_t, const int* __restrict__ pos, __nv_bfloat16* __restrict__ kc,
+                         __nv_bfloat16* __restrict__ vc, int Hq, int Hkv, int Smax) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x, j = blockIdx.y, B = gridDim.x;
+  rope_append_token(qkv + ((long long)j * B + b) * ld, pos[b] + j, b, cos_t, sin_t, kc, vc, Hq, Hkv, Smax);
 }
 
 // ------------------------------------------------------------------------------------------------ prefill cache fill
@@ -271,27 +291,17 @@ __device__ uint32_t bisect_threshold(const float* e, int V, float target, float*
   return lo;
 }
 
-__global__ void __launch_bounds__(SAMPLE_THREADS)
-sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const long long* __restrict__ ictl,
-              const float* __restrict__ fctl, int* __restrict__ pos, int* __restrict__ gen, int* __restrict__ finished,
-              long long* __restrict__ out, int max_new, long long* __restrict__ ids_next) {
-  extern __shared__ __align__(16) float e[];     // [V] exp(x - max) of the kept tokens, 0 elsewhere
-  __shared__ float red[33];
-  __shared__ ArgMax am[32];
-  __shared__ int tok_sm;
-  pdl_launch_dependents();
-  pdl_wait();
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const __nv_bfloat16* row = logits + (long long)b * ld;
-
-  // ---- argmax (greedy, and the reference point of the exponentials)
+// Block-wide argmax of a bf16 row (ties to the lowest index); am: 32 shared slots.  Every thread gets the result.
+__device__ ArgMax block_argmax(const __nv_bfloat16* __restrict__ row, int V, ArgMax* am) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   ArgMax best = {-INFINITY, V};
-  for (int i = tid; i < V; i += SAMPLE_THREADS) best = argmax_merge(best, ArgMax{__bfloat162float(row[i]), i});
+  for (int i = tid; i < V; i += blockDim.x) best = argmax_merge(best, ArgMax{__bfloat162float(row[i]), i});
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     ArgMax other{__shfl_xor_sync(0xffffffffu, best.v, o), __shfl_xor_sync(0xffffffffu, best.i, o)};
     best = argmax_merge(best, other);
   }
+  __syncthreads();                               // am may still be read by a previous call
   if (lane == 0) am[warp] = best;
   __syncthreads();
   if (warp == 0) {
@@ -305,88 +315,424 @@ sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, con
   }
   __syncthreads();
   best = am[0];
-  if (best.i >= V) best.i = 0;                   // all-NaN row: emit token 0 rather than an out-of-range id
+  if (best.i >= V) best.i = 0;                   // all-NaN row: token 0 rather than an out-of-range id
+  return best;
+}
 
-  const bool do_sample = ictl[0] != 0;
-  const int top_k = (int)ictl[1];
-  if (tid == 0) tok_sm = best.i;
-  if (do_sample && top_k != 1) {
-    const float temp = fctl[0], top_p = fctl[1];
-    const float mx = best.v / temp;
-    // HF warper order: temperature, then top-k, then top-p; probabilities are exp(x - max) up to the normaliser
-    for (int i = tid; i < V; i += SAMPLE_THREADS) e[i] = exp2f((__bfloat162float(row[i]) / temp - mx) * 1.4426950408889634f);
+// The unnormalised warped probability of logit x: exp(x / temp - mx).  Every user goes through this one expression, so
+// a weight recomputed from the logits is bit-identical to the one the thresholds were found on.
+__device__ __forceinline__ float warped_weight(float x, float temp, float mx) {
+  return exp2f((x / temp - mx) * 1.4426950408889634f);
+}
+
+// HF warper order: temperature, then top-k, then top-p.  Fills e[i] with the kept weights (0 elsewhere) and returns the
+// threshold T on the weight's bit pattern: token i is kept iff bits(warped_weight(x_i)) >= T.  mx = max logit / temp.
+__device__ uint32_t warp_weights(const __nv_bfloat16* __restrict__ row, int V, float temp, int top_k, float top_p, float mx, float* e,
+                                 float* red) {
+  const int tid = threadIdx.x;
+  uint32_t T = 0;
+  for (int i = tid; i < V; i += blockDim.x) e[i] = warped_weight(__bfloat162float(row[i]), temp, mx);
+  __syncthreads();
+  if (top_k > 0 && top_k < V) {
+    T = bisect_threshold<false>(e, V, (float)top_k, red);
+    for (int i = tid; i < V; i += blockDim.x)
+      if (__float_as_uint(e[i]) < T) e[i] = 0.f;
     __syncthreads();
-    if (top_k > 0 && top_k < V) {
-      const uint32_t t = bisect_threshold<false>(e, V, (float)top_k, red);
-      for (int i = tid; i < V; i += SAMPLE_THREADS)
-        if (__float_as_uint(e[i]) < t) e[i] = 0.f;
-      __syncthreads();
-    }
-    if (top_p < 1.f) {
-      float z = 0.f;
-      for (int i = tid; i < V; i += SAMPLE_THREADS) z += e[i];
-      z = block_sum(z, red);
-      const uint32_t t = bisect_threshold<true>(e, V, top_p * z, red);
-      for (int i = tid; i < V; i += SAMPLE_THREADS)
-        if (__float_as_uint(e[i]) < t) e[i] = 0.f;
-      __syncthreads();
-    }
-    // inverse CDF in index order: thread t owns a contiguous segment; exclusive scan of the segment sums
-    const int per = ceil_div(V, SAMPLE_THREADS);
-    const int s0 = min(V, tid * per), s1 = min(V, s0 + per);
-    float local = 0.f;
-    for (int i = s0; i < s1; ++i) local += e[i];
-    float incl = local;
+  }
+  if (top_p < 1.f) {
+    float z = 0.f;
+    for (int i = tid; i < V; i += blockDim.x) z += e[i];
+    z = block_sum(z, red);
+    const uint32_t t = bisect_threshold<true>(e, V, top_p * z, red);
+    for (int i = tid; i < V; i += blockDim.x)
+      if (__float_as_uint(e[i]) < t) e[i] = 0.f;
+    __syncthreads();
+    T = max(T, t);
+  }
+  return T;
+}
+
+// Inverse CDF in index order over the weights e[0, V): u in (0, 1] picks the token; `fallback` when rounding leaves r
+// outside every segment.  Thread t owns a contiguous segment; exclusive scan of the segment sums.  red: 33 floats.
+__device__ int draw_index(const float* e, int V, float u, int fallback, float* red, int* tok_sm) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int per = ceil_div(V, (int)blockDim.x);
+  const int s0 = min(V, tid * per), s1 = min(V, s0 + per);
+  float local = 0.f;
+  for (int i = s0; i < s1; ++i) local += e[i];
+  float incl = local;
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const float y = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    __syncthreads();
-    if (lane == 31) red[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      float w = red[lane], wi = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const float y = __shfl_up_sync(0xffffffffu, wi, o);
-        if (lane >= o) wi += y;
-      }
-      red[lane] = wi - w;                        // exclusive prefix of the warp totals
-      if (lane == 31) red[32] = wi;              // total kept mass
-    }
-    __syncthreads();
-    const float pre = red[warp] + incl - local, total = red[32];
-    curandStatePhilox4_32_10_t rng;
-    curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)gen[b], &rng);
-    const float r = curand_uniform(&rng) * total;   // u in (0, 1]
-    if (local > 0.f && pre <= r && r < pre + local) {
-      float acc = pre;
-      int pick = -1;
-      for (int i = s0; i < s1; ++i) {
-        if (e[i] > 0.f) {
-          pick = i;
-          acc += e[i];
-          if (r < acc) break;
-        }
-      }
-      tok_sm = pick;                             // at most one thread's segment brackets r
-    }
+  for (int o = 1; o < 32; o <<= 1) {
+    const float y = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += y;
   }
   __syncthreads();
+  if (lane == 31) red[warp] = incl;
+  if (tid == 0) *tok_sm = fallback;
+  __syncthreads();
+  if (warp == 0) {
+    float w = red[lane], wi = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const float y = __shfl_up_sync(0xffffffffu, wi, o);
+      if (lane >= o) wi += y;
+    }
+    red[lane] = wi - w;                          // exclusive prefix of the warp totals
+    if (lane == 31) red[32] = wi;                // total kept mass
+  }
+  __syncthreads();
+  const float pre = red[warp] + incl - local, total = red[32];
+  const float r = u * total;
+  if (local > 0.f && pre <= r && r < pre + local) {
+    float acc = pre;
+    int pick = -1;
+    for (int i = s0; i < s1; ++i) {
+      if (e[i] > 0.f) {
+        pick = i;
+        acc += e[i];
+        if (r < acc) break;
+      }
+    }
+    *tok_sm = pick;                              // at most one thread's segment brackets r
+  }
+  __syncthreads();
+  return *tok_sm;
+}
+
+__global__ void __launch_bounds__(SAMPLE_THREADS)
+sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const long long* __restrict__ ictl,
+              const float* __restrict__ fctl, int* __restrict__ pos, int* __restrict__ gen, int* __restrict__ finished,
+              long long* __restrict__ out, int max_new, long long* __restrict__ ids_next) {
+  extern __shared__ __align__(16) float e[];     // [V] exp(x - max) of the kept tokens, 0 elsewhere
+  __shared__ float red[33];
+  __shared__ ArgMax am[32];
+  __shared__ int tok_sm;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const __nv_bfloat16* row = logits + (long long)b * ld;
+
+  // ---- argmax (greedy, and the reference point of the exponentials)
+  const ArgMax best = block_argmax(row, V, am);
+  const bool do_sample = ictl[0] != 0;
+  const int top_k = (int)ictl[1];
+  int tok = best.i;
+  if (do_sample && top_k != 1) {
+    const float temp = fctl[0], top_p = fctl[1];
+    warp_weights(row, V, temp, top_k, top_p, best.v / temp, e, red);
+    curandStatePhilox4_32_10_t rng;
+    curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)gen[b], &rng);
+    tok = draw_index(e, V, curand_uniform(&rng), best.i, red, &tok_sm);   // u in (0, 1]
+  }
   if (tid == 0) {
     const int g = gen[b];
     const bool fin = finished[b] != 0;
-    const long long tok = fin ? ictl[3] : (long long)tok_sm;
-    if (g < max_new) out[(long long)b * max_new + g] = tok;
-    ids_next[b] = tok;
+    const long long t = fin ? ictl[3] : (long long)tok;
+    if (g < max_new) out[(long long)b * max_new + g] = t;
+    ids_next[b] = t;
     gen[b] = g + 1;
     pos[b] = pos[b] + 1;
     if (!fin) {
       const int n_eos = (int)min(ictl[4], (long long)MAX_EOS);
       for (int k = 0; k < n_eos; ++k)
-        if (tok == ictl[5 + k]) finished[b] = 1;
+        if (t == ictl[5 + k]) finished[b] = 1;
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ verify attention
+// Assisted generation scores n <= 8 tokens per row in one pass.  Rows are slot-major: row j*B + b is token j of sequence b,
+// at position pos[b] + j, and it attends keys 0 .. pos[b] + j (causal inside the block).
+//
+// grid (splits, Hkv, B), 160 threads.  CTA (s, hk, b) takes the G*n <= 64 queries of kv head hk as ONE m64 tile (query
+// qi = j*G + g is tile row qi; rows >= G*n are zero and masked) against the 64-key tiles [s*tps, (s+1)*tps) of the row's
+// keys, stopping at the tile holding pos[b] + n - 1:
+//   warp 4      TMA: the K and V tiles [64 keys x 64] of the [B*Hkv*Smax, 64] caches, 128-byte swizzle, through a
+//               VSTAGES-deep full / empty mbarrier ring
+//   warps 0-3   one warpgroup: Q gathered into shared memory in the same swizzled layout, S = Q K^T on wgmma m64n64k16,
+//               causal mask + online softmax (exp2 domain) on the accumulators, O += P V with P as the register operand
+// Writes the unnormalised partial output and its (max, sum) per query row; verify_combine_kernel merges the splits.
+constexpr int VB = 64;                           // keys per tile
+constexpr int VSTAGES = 2;
+constexpr int VTHREADS = 160;
+constexpr int VTILE = 64 * 128;                  // a [64 x 64] bf16 tile, 128-byte swizzled rows
+constexpr int VSMEM = VTILE + VSTAGES * 2 * VTILE + 1024 /*align*/ + 128 /*barriers*/;
+
+__global__ void __launch_bounds__(VTHREADS)
+verify_attn_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
+                   const __nv_bfloat16* __restrict__ q, long long ldq, const int* __restrict__ pos, float* __restrict__ part_o,
+                   float* __restrict__ part_ml, int Hkv, int Smax, int cap, int tps, float scale_log2, int lg, int n) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;
+  uint8_t* sKV = smem + VTILE;                   // [stage][K | V]
+  uint64_t* full = reinterpret_cast<uint64_t*>(sKV + VSTAGES * 2 * VTILE);
+  uint64_t* empty = full + VSTAGES;
+
+  pdl_launch_dependents();
+  const int s = blockIdx.x, hk = blockIdx.y, b = blockIdx.z, B = gridDim.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int G = 1 << lg, nq = G * n, Hq = Hkv * G;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_k);
+    tma_prefetch_desc(&tmap_v);
+    for (int i = 0; i < VSTAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  const int p0 = pos[b];
+  const int t_begin = s * tps, t_end = min((s + 1) * tps, ceil_div(p0 + n, VB));
+  if (t_begin >= t_end) return;                  // uniform over the CTA
+  const int row0 = (b * Hkv + hk) * Smax;
+
+  if (warp == 4) {
+    // ------------------------------------------------------------------ TMA producer
+    if (lane == 0) {
+      for (int t = t_begin; t < t_end; ++t) {
+        const int i = t - t_begin, st = i % VSTAGES;
+        mbar_wait(&empty[st], ((i / VSTAGES) & 1) ^ 1);
+        mbar_arrive_expect_tx(&full[st], 2 * VTILE);
+        tma_load_2d(sKV + st * 2 * VTILE, &tmap_k, &full[st], 0, row0 + t * VB);
+        tma_load_2d(sKV + st * 2 * VTILE + VTILE, &tmap_v, &full[st], 0, row0 + t * VB);
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- Q tile: row qi, 16-byte chunk c at c ^ (qi & 7)
+  for (int i = threadIdx.x; i < 64 * 8; i += 128) {
+    const int qi = i >> 3, c = i & 7;
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (qi < nq)
+      v = ld_nc_v4(q + ((long long)(qi >> lg) * B + b) * ldq + (long long)(hk * G + (qi & (G - 1))) * D + c * 8);
+    *reinterpret_cast<uint4*>(sQ + qi * 128 + ((c ^ (qi & 7)) << 4)) = v;
+  }
+  fence_proxy_async_smem();                      // generic-proxy writes -> visible to wgmma
+  named_bar_sync(1, 128);
+
+  // accumulator fragment of m64n64: acc[4*i + 2*h + e] is row (16*warp + lane/4 + 8*h), column (8*i + 2*(lane%4) + e)
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  int last[2];                                   // the last key each of the thread's two rows may see (-1: padding row)
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int qi = 16 * warp + (lane >> 2) + 8 * hh;
+    last[hh] = qi < nq ? p0 + (qi >> lg) : -1;
+  }
+  const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ), 16, 1024);
+
+  for (int t = t_begin; t < t_end; ++t) {
+    const int i = t - t_begin, st = i % VSTAGES;
+    mbar_wait(&full[st], (i / VSTAGES) & 1);
+    const uint32_t k_addr = smem_u32(sKV + st * 2 * VTILE);
+    const uint64_t kdesc = make_smem_desc_sw128(k_addr, 16, 1024);
+    const uint64_t vdesc = make_smem_desc_sw128(k_addr + VTILE, VTILE, 1024);   // V: [keys x 64] read MN-major
+
+    float sc[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_m64n64k16_ss<0, 0>(sc, qdesc + 2 * k, kdesc + 2 * k, k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int ii = 0; ii < 8; ++ii) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float v = sc[4 * ii + 2 * hh + e] * scale_log2;
+          if (t * VB + 8 * ii + 2 * (lane & 3) + e > last[hh]) v = -INFINITY;
+          sc[4 * ii + 2 * hh + e] = v;
+          mx[hh] = fmaxf(mx[hh], v);
+        }
+      }
+    }
+    float alpha[2], mref[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float mn = fmaxf(m[r], mx[r]);
+      // a row that has seen no key yet keeps (max, sum, O) = (-inf, 0, 0): no -inf - -inf
+      alpha[r] = mn == -INFINITY ? 1.f : exp2f(m[r] - mn);
+      mref[r] = mn == -INFINITY ? 0.f : mn;
+      m[r] = mn;
+      l[r] *= alpha[r];
+    }
+    uint32_t pf[4][4];                           // P as the register A operand of P V (k = keys)
+#pragma unroll
+    for (int ii = 0; ii < 8; ++ii) {
+      float pv[4];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          pv[2 * hh + e] = exp2f(sc[4 * ii + 2 * hh + e] - mref[hh]);
+          l[hh] += pv[2 * hh + e];
+        }
+      }
+      pf[ii >> 1][(ii & 1) * 2 + 0] = f2_to_bf2(pv[0], pv[1]);
+      pf[ii >> 1][(ii & 1) * 2 + 1] = f2_to_bf2(pv[2], pv[3]);
+    }
+#pragma unroll
+    for (int ii = 0; ii < 8; ++ii) {
+      o[4 * ii + 0] *= alpha[0]; o[4 * ii + 1] *= alpha[0];
+      o[4 * ii + 2] *= alpha[1]; o[4 * ii + 3] *= alpha[1];
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs<1>(o, pf[kk], vdesc + 128 * kk, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (threadIdx.x == 0) mbar_arrive(&empty[st]);   // this warpgroup's MMAs on the stage have retired
+  }
+
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int qi = 16 * warp + (lane >> 2) + 8 * r;
+    if (qi >= nq) continue;
+    const long long orow = (long long)(qi >> lg) * B + b;
+    const long long base = (orow * Hq + hk * G + (qi & (G - 1))) * cap + s;
+    float* po = part_o + base * D + 2 * (lane & 3);
+#pragma unroll
+    for (int ii = 0; ii < 8; ++ii) *reinterpret_cast<float2*>(po + 8 * ii) = make_float2(o[4 * ii + 2 * r], o[4 * ii + 2 * r + 1]);
+    if ((lane & 3) == 0) {
+      part_ml[base * 2] = m[r];
+      part_ml[base * 2 + 1] = l[r];
+    }
+  }
+}
+
+// grid (Hq, n*B), block 64: merge the splits of query row r = j*B + b, head h (splits holding keys <= pos[b] + j; each
+// of them holds key s*span, so its max is finite).
+__global__ void __launch_bounds__(64)
+verify_combine_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml, const int* __restrict__ pos,
+                      __nv_bfloat16* __restrict__ out, long long ldo, int cap, int span, int B) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int h = blockIdx.x, r = blockIdx.y, Hq = gridDim.x, d = threadIdx.x;
+  const int b = r % B, j = r / B;
+  const int used = ceil_div(pos[b] + j + 1, span);
+  const long long base = ((long long)r * Hq + h) * cap;
+  float M = -INFINITY;
+  for (int c = 0; c < used; ++c) M = fmaxf(M, part_ml[(base + c) * 2]);
+  float L = 0.f, acc = 0.f;
+  for (int c = 0; c < used; ++c) {
+    const float w = exp2f(part_ml[(base + c) * 2] - M);
+    L = fmaf(part_ml[(base + c) * 2 + 1], w, L);
+    acc = fmaf(part_o[(base + c) * D + d], w, acc);
+  }
+  out[(long long)r * ldo + h * D + d] = __float2bfloat16_rn(acc / L);
+}
+
+// ------------------------------------------------------------------------------------------------ acceptance
+// One CTA per row: the speculative-sampling decision of one assisted round (Leviathan et al. 2023, Chen et al. 2023).
+//   plog [(K+1)*B, ldp] target logits, slot-major: slot i predicts the token at pos[b] + i + 1
+//   qlog [K*B, ldq] draft logits of the proposals; tok [(K+1)*B]: slot 0 the row's last token, slots 1..K the proposals
+// Greedy (do_sample = 0 or top_k = 1): accept while the proposal equals the target argmax, then emit the argmax.
+// Sampling: p, q = the warped distributions (warp_weights: the sampler's rules); accept d_i with probability
+// min(1, p(d_i) / q(d_i)); at the first rejection draw from normalise(max(0, p - q)); after K acceptances draw the bonus
+// token from p_{K+1}.  Uniforms: Philox keyed by (seed, row, gen[b]*16 + 2*slot + {0, 1}).
+// Then the emitted tokens go to out[b, gen..] (stopping after an EOS id or at max_new), pos / gen / finished advance, the
+// new last token goes to tok slot 0 and the draft's position is set to the target's.  A row that finishes keeps its pos
+// (every later round rewrites the same in-range cache positions); finished rows are left alone.
+// stats [B, 2] int64: rounds the row took part in, proposals accepted.
+__global__ void __launch_bounds__(SAMPLE_THREADS)
+accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_bfloat16* __restrict__ qlog, long long ldq, int V,
+              int K, const long long* __restrict__ ictl, const float* __restrict__ fctl, long long* __restrict__ tok,
+              int* __restrict__ pos, int* __restrict__ gen, int* __restrict__ finished, long long* __restrict__ out, int ld_out,
+              int max_new, int* __restrict__ draft_pos, long long* __restrict__ stats) {
+  extern __shared__ __align__(16) float e[];
+  __shared__ float red[33];
+  __shared__ ArgMax am[32];
+  __shared__ int tok_sm;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x, B = gridDim.x, tid = threadIdx.x;
+  if (finished[b]) {
+    if (tid == 0) draft_pos[b] = pos[b];
+    return;
+  }
+  const bool greedy = !(ictl[0] != 0 && ictl[1] != 1);
+  const int top_k = (int)ictl[1];
+  const float temp = fctl[0], top_p = fctl[1];
+  const int g0 = gen[b];
+  int n_acc = 0, t_new = 0;
+  for (int i = 0; i <= K; ++i) {
+    const __nv_bfloat16* prow = plog + ((long long)i * B + b) * ldp;
+    const ArgMax pm = block_argmax(prow, V, am);
+    const long long d = i < K ? tok[(long long)(i + 1) * B + b] : -1;
+    if (greedy) {
+      if (d == pm.i) {
+        ++n_acc;
+        continue;
+      }
+      t_new = pm.i;
+      break;
+    }
+    const float mxp = pm.v / temp;
+    const uint32_t Tp = warp_weights(prow, V, temp, top_k, top_p, mxp, e, red);
+    curandStatePhilox4_32_10_t rng;
+    curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)g0 * 16ull + 2ull * i, &rng);
+    const float u_acc = curand_uniform(&rng), u_draw = curand_uniform(&rng);    // (0, 1]
+    if (i == K) {                                // every proposal accepted: the bonus token from p_{K+1}
+      t_new = draw_index(e, V, u_acc, pm.i, red, &tok_sm);
+      break;
+    }
+    float zp = 0.f;
+    for (int v = tid; v < V; v += blockDim.x) zp += e[v];
+    zp = block_sum(zp, red);
+    const float pd = e[d] / zp;
+    const __nv_bfloat16* qrow = qlog + ((long long)i * B + b) * ldq;
+    const ArgMax qm = block_argmax(qrow, V, am);   // starts with a barrier: every thread has read e[d]
+    warp_weights(qrow, V, temp, top_k, top_p, qm.v / temp, e, red);
+    float zq = 0.f;
+    for (int v = tid; v < V; v += blockDim.x) zq += e[v];
+    zq = block_sum(zq, red);
+    const float qd = e[d] / zq;
+    if (pd > 0.f && u_acc * qd <= pd) {
+      ++n_acc;
+      continue;
+    }
+    // rejected: residual max(0, p - q), p recomputed from the logits with the same expression and threshold
+    for (int v = tid; v < V; v += blockDim.x) {
+      const float w = warped_weight(__bfloat162float(prow[v]), temp, mxp);
+      const float pv = __float_as_uint(w) >= Tp ? w / zp : 0.f;
+      e[v] = fmaxf(pv - e[v] / zq, 0.f);
+    }
+    __syncthreads();
+    t_new = draw_index(e, V, u_draw, pm.i, red, &tok_sm);
+    break;
+  }
+  if (tid == 0) {
+    const int n_eos = (int)min(ictl[4], (long long)MAX_EOS);
+    int g = g0;
+    bool fin = false;
+    for (int t = 0; t <= n_acc && !fin && g < max_new; ++t) {
+      const long long x = t < n_acc ? tok[(long long)(t + 1) * B + b] : (long long)t_new;
+      out[(long long)b * ld_out + g] = x;
+      ++g;
+      for (int k = 0; k < n_eos; ++k)
+        if (x == ictl[5 + k]) fin = true;
+    }
+    fin = fin || g >= max_new;
+    stats[2 * b] += 1;
+    stats[2 * b + 1] += n_acc;
+    if (fin) finished[b] = 1;
+    else pos[b] += n_acc + 1;
+    gen[b] = g;
+    tok[b] = t_new;
+    draft_pos[b] = pos[b];
   }
 }
 
@@ -465,6 +811,72 @@ ODB_EXPORT int odb_dec_sample(const void* logits, long long ld, int V, const voi
   launch_pdl(dec::sample_kernel, dim3(B), dim3(dec::SAMPLE_THREADS), smem, st, (const __nv_bfloat16*)logits, ld, V,
              (const long long*)ictl, (const float*)fctl, (int*)pos, (int*)gen, (int*)finished, (long long*)out, max_new,
              (long long*)ids_next);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+// qkv [n*B, ld] bf16, slot-major (row j*B + b: token j of sequence b, at position pos[b] + j); cos/sin fp32 [max_pos, 32];
+// pos int32 [B]; kc/vc [B, Hkv, Smax, 64] bf16
+ODB_EXPORT int odb_dec_rope_append_multi(void* qkv, long long ld, const void* cos_t, const void* sin_t, const void* pos, void* kc,
+                                         void* vc, int B, int n, int Hq, int Hkv, int Smax, cudaStream_t st) {
+  if (ld % 2 || n < 1) return -1;
+  launch_pdl(dec::rope_append_multi_kernel, dim3(B, n), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t,
+             (const float*)sin_t, (const int*)pos, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, Hq, Hkv, Smax);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+// q [n*B, ldq] bf16 slot-major (the q heads first); query row j*B + b attends keys 0..pos[b]+j; kc/vc [B, Hkv, Smax, 64]
+// (Smax a multiple of 64); part_o fp32 [n*B, Hq, cap, 64]; part_ml fp32 [n*B, Hq, cap, 2] with cap = Smax / 64;
+// out [n*B, ldo] bf16.  G = Hq / Hkv in {1, 2, 4, 8}, n <= 8 (G*n <= 64 queries: one m64 tile), pos[b] + n <= Smax.
+// The keys are split so that about two CTAs per SM run: splits = min(tiles, ceil(264 / (Hkv*B))).
+ODB_EXPORT int odb_dec_verify_attn(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o,
+                                   void* part_ml, void* out, long long ldo, int B, int n, int Hq, int Hkv, int Smax, float softmax_scale,
+                                   cudaStream_t st) {
+  if (Hq % Hkv || ldq % 8 || n < 1 || n > 8 || Smax % dec::VB) return -1;
+  const int G = Hq / Hkv;
+  const int lg = G == 1 ? 0 : G == 2 ? 1 : G == 4 ? 2 : G == 8 ? 3 : -1;
+  if (lg < 0) return -2;                         // GQA groups of 1, 2, 4 or 8 query heads
+  CUtensorMap tk, tv;
+  int rc;
+  const long long rows = (long long)B * Hkv * Smax;
+  if ((rc = make_tmap_2d(&tk, kc, rows, dec::D, dec::D * 2, dec::VB, dec::D, 2))) return rc;
+  if ((rc = make_tmap_2d(&tv, vc, rows, dec::D, dec::D * 2, dec::VB, dec::D, 2))) return rc;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(dec::verify_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dec::VSMEM);
+    if (e != cudaSuccess) return (int)e;
+    attr_set = true;
+  }
+  const int cap = Smax / dec::VB;
+  int splits = std::min(cap, std::max(1, odb::ceil_div(264, Hkv * B)));
+  const int tps = odb::ceil_div(cap, splits);
+  splits = odb::ceil_div(cap, tps);
+  launch_pdl(dec::verify_attn_kernel, dim3(splits, Hkv, B), dim3(dec::VTHREADS), dec::VSMEM, st, tk, tv, (const __nv_bfloat16*)q, ldq,
+             (const int*)pos, (float*)part_o, (float*)part_ml, Hkv, Smax, cap, tps, softmax_scale * 1.4426950408889634f, lg, n);
+  ODB_CHECK_LAST();
+  launch_pdl(dec::verify_combine_kernel, dim3(Hq, n * B), dim3(dec::D), 0, st, (const float*)part_o, (const float*)part_ml,
+             (const int*)pos, (__nv_bfloat16*)out, ldo, cap, tps * dec::VB, B);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+// plog [(K+1)*B, ldp] / qlog [K*B, ldq] bf16 slot-major; tok int64 [(K+1)*B]; ictl / fctl: see dec::sample_kernel; pos / gen /
+// finished / draft_pos int32 [B]; out int64 [B, ld_out]; stats int64 [B, 2].  V <= 56000 (fp32 vocabulary in shared memory).
+ODB_EXPORT int odb_dec_accept(const void* plog, long long ldp, const void* qlog, long long ldq, int V, int K, const void* ictl,
+                              const void* fctl, void* tok, void* pos, void* gen, void* finished, void* out, int ld_out, int max_new,
+                              void* draft_pos, void* stats, int B, cudaStream_t st) {
+  const int smem = V * 4;
+  if (smem > 224000 || K < 1 || K > 7) return -1;
+  static int attr = 0;
+  if (smem > 48 * 1024 && smem > attr) {
+    cudaError_t e = cudaFuncSetAttribute(dec::accept_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return (int)e;
+    attr = smem;
+  }
+  launch_pdl(dec::accept_kernel, dim3(B), dim3(dec::SAMPLE_THREADS), smem, st, (const __nv_bfloat16*)plog, ldp,
+             (const __nv_bfloat16*)qlog, ldq, V, K, (const long long*)ictl, (const float*)fctl, (long long*)tok, (int*)pos, (int*)gen,
+             (int*)finished, (long long*)out, ld_out, max_new, (int*)draft_pos, (long long*)stats);
   ODB_CHECK_LAST();
   return 0;
 }

@@ -12,6 +12,12 @@ is captured once into a CUDA graph and replayed (``ODB_CUDA_GRAPH=0``: eager lau
 kernels of ``csrc/decode_sm90.cu`` and the training GEMMs; other precisions and devices run the same program on the
 PyTorch references of :mod:`opendiloco_b200.ops`.
 
+Assisted (speculative) generation, ``generate(assistant_model=...)``: every round the draft proposes K tokens with K
+one-token decode steps (plus one more that only writes d_K into its cache), the target scores ``[last, d_1..d_K]`` in one
+multi-token pass (verify attention over its cache), and one acceptance kernel keeps the longest acceptable prefix plus
+one target token per row.  The whole round is one CUDA graph.  Rejected cache entries are left in place: attention reads
+only up to each row's position, so moving ``pos`` back is the whole rollback.
+
 Nothing here goes through ``LlamaEngine.workspace`` or its captured training graphs: generating between training steps
 leaves the training buffers and graph untouched.
 """
@@ -28,6 +34,9 @@ from ..ops import kernels as K
 from ..ops import tc_gemm as TC
 
 FINISHED_CHECK_EVERY = 16           # decode steps between host checks of "every row has finished"
+ASSISTED_CHECK_EVERY = 4            # assisted rounds between host checks (a round emits 1 .. K+1 tokens per row)
+MAX_ASSISTANT_TOKENS = 7            # verify attention: K+1 <= 8 queries per row and GQA group
+DRAFT_SEED_XOR = 0x5DEECE66D        # the draft's proposals draw from a Philox stream apart from the acceptance draws
 
 
 def _round_up(x: int, m: int) -> int:
@@ -102,6 +111,8 @@ def decode_state(model, B: int, Smax: int) -> DecodeState:
     key = (B, Smax, str(ar.device), ar.compute_dtype)
     st = eng.decode_state
     if st is None or st.key != key:
+        if eng.assisted_state is not None:           # its round graph reads the old caches: let them go
+            eng.assisted_state.drop_graph()
         eng.decode_state = None                       # free the old caches before allocating the new ones
         st = eng.decode_state = DecodeState(model.config, B, Smax, ar.device, ar.compute_dtype)
     return st
@@ -175,24 +186,42 @@ def _head_and_sample(cfg, ar, st: DecodeState, delta) -> None:
 
 
 # ------------------------------------------------------------------------------------------------ decode step
-def _step_eager(model, st: DecodeState) -> None:
+def _layers(model, buf, ids: torch.Tensor, attend):
+    """The decode layer program over the rows of ``buf`` (a DecodeState or AssistedState): embedding of ids, then per layer
+    rmsnorm -> QKV GEMM -> ``attend(l, qkv, att)`` (RoPE, cache append, attention) -> o-proj -> rmsnorm(+residual) ->
+    SwiGLU GEMM -> down.  Returns the last layer's output delta; the residual before it is in buf.res."""
     cfg, ar = model.config, model.arena
-    L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     eps = cfg.rms_norm_eps
-    K.embedding_fwd(st.ids, ar.w("model.embed_tokens.weight"), out=st.res)
+    K.embedding_fwd(ids, ar.w("model.embed_tokens.weight"), out=buf.res)
     delta = None
-    for l in range(L):
+    for l in range(cfg.num_hidden_layers):
         p = f"model.layers.{l}."
-        K.rmsnorm_fwd(st.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=st.xn, rstd=st.rstd, x_out=st.res)
-        G.mm_nt(st.xn, ar.qkv_w(l), out=st.qkv)
-        DK.rope_append(st.qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D)
-        DK.attention(st.qkv, st.kc[l], st.vc[l], st.pos, st.att, Hq, Hkv, D, st.part_o, st.part_ml)
-        G.mm_nt(st.att, ar.w(p + "self_attn.o_proj.weight"), out=st.proj)
-        K.rmsnorm_fwd(st.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=st.proj, out=st.xn, rstd=st.rstd, x_out=st.res)
-        _mlp(cfg, ar, l, st.xn, st.gu, st.act)
-        G.mm_nt(st.act, ar.w(p + "mlp.down_proj.weight"), out=st.proj)
-        delta = st.proj
-    _head_and_sample(cfg, ar, st, delta)
+        K.rmsnorm_fwd(buf.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=buf.xn, rstd=buf.rstd, x_out=buf.res)
+        G.mm_nt(buf.xn, ar.qkv_w(l), out=buf.qkv)
+        attend(l, buf.qkv, buf.att)
+        G.mm_nt(buf.att, ar.w(p + "self_attn.o_proj.weight"), out=buf.proj)
+        K.rmsnorm_fwd(buf.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=buf.proj, out=buf.xn, rstd=buf.rstd, x_out=buf.res)
+        _mlp(cfg, ar, l, buf.xn, buf.gu, buf.act)
+        G.mm_nt(buf.act, ar.w(p + "mlp.down_proj.weight"), out=buf.proj)
+        delta = buf.proj
+    return delta
+
+
+def _one_token_layers(model, st: DecodeState, ids: torch.Tensor):
+    """One token per row at st.pos: the decode layers with single-query RoPE+append and split-KV attention."""
+    cfg = model.config
+    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+
+    def attend(l, qkv, att):
+        DK.rope_append(qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D)
+        DK.attention(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.part_o, st.part_ml)
+
+    return _layers(model, st, ids, attend)
+
+
+def _step_eager(model, st: DecodeState) -> None:
+    delta = _one_token_layers(model, st, st.ids)
+    _head_and_sample(model.config, model.arena, st, delta)
 
 
 @torch.no_grad()
@@ -219,6 +248,168 @@ def step(model, st: DecodeState, graph: bool | None = None) -> None:
     st.graph.replay()
 
 
+# ------------------------------------------------------------------------------------------------ assisted generation
+class AssistedState:
+    """The target's buffers of assisted generation over B rows with K proposals: the multi-token verify pass over
+    (K+1)*B slot-major rows (row j*B + b is slot j of row b), the draft's proposal logits, the draft's own DecodeState
+    (so a model can draft for itself, and the assistant's ``decode_state`` is left alone) and the round graph.  The
+    target's caches, positions and outputs stay in its DecodeState."""
+
+    def __init__(self, cfg, dcfg, B: int, K: int, Smax: int, device, dtype):
+        h, i, V, D = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size, cfg.head_dim
+        T = (K + 1) * B
+        e = lambda *shape: torch.empty(*shape, dtype=dtype, device=device)  # noqa: E731
+        self.B, self.K, self.key = B, K, (B, K, Smax, str(device), dtype, _shape(dcfg))
+        self.draft = DecodeState(dcfg, B, Smax, device, dtype)
+        self.tok = torch.zeros(T, dtype=torch.int64, device=device)          # slot 0: last token; 1..K: proposals
+        self.res, self.xn, self.proj = e(T, h), e(T, h), e(T, h)
+        self.rstd = torch.empty(T, dtype=torch.float32, device=device)
+        self.qkv, self.att, self.gu, self.act = e(T, cfg.qkv_dim), e(T, cfg.q_dim), e(T, 2 * i), e(T, i)
+        self.plog, self.qlog = e(T, V), e(K * B, V)
+        self.stats = torch.zeros(B, 2, dtype=torch.int64, device=device)     # per row: rounds taken part in, accepted
+        # the verify kernels follow the target's shapes alone; the round graph needs the draft's decode kernels too
+        self.kernels = DK.usable_verify(self.res, D, cfg.num_attention_heads, cfg.num_key_value_heads)
+        self.graphable = self.kernels and self.draft.kernels
+        self.part_o = self.part_ml = None
+        if self.kernels:
+            nsp = DK.verify_splits(Smax)
+            self.part_o = torch.empty(T, cfg.num_attention_heads, nsp, D, dtype=torch.float32, device=device)
+            self.part_ml = torch.empty(T, cfg.num_attention_heads, nsp, 2, dtype=torch.float32, device=device)
+        self.graph = None
+        self.graph_key = None
+        self.graph_target = None                      # the target DecodeState the graph reads (kept alive with it)
+
+    def drop_graph(self) -> None:
+        self.graph = self.graph_key = self.graph_target = None
+
+    def verify_passes(self) -> int:
+        """Verify passes of the last generate call (rounds in which some row was still generating)."""
+        return int(self.stats[:, 0].max())
+
+    def acceptance_rate(self) -> float:
+        """Accepted proposals over proposals made, over the rows and rounds of the last generate call."""
+        rounds = int(self.stats[:, 0].sum())
+        return int(self.stats[:, 1].sum()) / (self.K * rounds) if rounds else float("nan")
+
+
+def _shape(cfg) -> tuple:
+    return (cfg.num_hidden_layers, cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, cfg.num_key_value_heads,
+            cfg.head_dim, cfg.vocab_size, cfg.max_position_embeddings, cfg.rope_theta)
+
+
+def assisted_state(model, assistant, B: int, K: int, Smax: int) -> AssistedState:
+    """The model's assisted-generation state for (assistant shapes, B, K, Smax), allocated on first use; at most one is
+    resident, on the target's engine."""
+    eng, ar = model.engine, model.arena
+    key = (B, K, Smax, str(ar.device), ar.compute_dtype, _shape(assistant.config))
+    st = eng.assisted_state
+    if st is None or st.key != key:
+        eng.assisted_state = None                     # free the old buffers before allocating the new ones
+        st = eng.assisted_state = AssistedState(model.config, assistant.config, B, K, Smax, ar.device, ar.compute_dtype)
+    return st
+
+
+def _verify(model, tst: DecodeState, ast: AssistedState) -> None:
+    """The target scores ast.tok (slot j at tst.pos + j) in one pass: logits of every slot -> ast.plog."""
+    cfg, ar = model.config, model.arena
+    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    n = ast.K + 1
+
+    def attend(l, qkv, att):
+        DK.rope_append_multi(qkv, tst.cos, tst.sin, tst.pos, tst.kc[l], tst.vc[l], Hq, Hkv, D, n)
+        DK.verify_attention(qkv, tst.kc[l], tst.vc[l], tst.pos, att, Hq, Hkv, D, n, ast.part_o, ast.part_ml)
+
+    delta = _layers(model, ast, ast.tok, attend)
+    K.rmsnorm_fwd(ast.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=ast.xn, rstd=ast.rstd, x_out=ast.res)
+    G.mm_nt(ast.xn, ar.w("lm_head.weight"), out=ast.plog)
+
+
+def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: int) -> None:
+    B, Kp, dst = ast.B, ast.K, ast.draft
+    dcfg, dar = draft.config, draft.arena
+    for i in range(Kp + 1):
+        # draft step i consumes slot i at dst.pos; steps 0..K-1 propose slot i+1, step K only writes d_K into the cache
+        delta = _one_token_layers(draft, dst, ast.tok[i * B:(i + 1) * B])
+        if i == Kp:
+            break
+        q = ast.qlog[i * B:(i + 1) * B]
+        K.rmsnorm_fwd(dst.res, dar.w("model.norm.weight"), dcfg.rms_norm_eps, delta=delta, out=dst.xn, rstd=dst.rstd, x_out=dst.res)
+        G.mm_nt(dst.xn, dar.w("lm_head.weight"), out=q)
+        DK.sample(q, dst.ictl, dst.fctl, dst.pos, dst.gen, dst.finished, dst.out, ast.tok[(i + 1) * B:(i + 2) * B])
+    _verify(target, tst, ast)
+    DK.accept(ast.plog, ast.qlog, tst.ictl, tst.fctl, ast.tok, tst.pos, tst.gen, tst.finished, tst.out, max_new, dst.pos, ast.stats)
+
+
+@torch.no_grad()
+def assisted_round(target, draft, tst: DecodeState, ast: AssistedState, max_new: int, graph: bool | None = None) -> None:
+    """One assisted round: K draft proposals, one verify pass of the target, acceptance.  With the kernels and ``graph``
+    (default: ``ODB_CUDA_GRAPH`` != 0) the first call runs eagerly (warm-up), the second captures the round and every
+    call replays it."""
+    if graph is None:
+        graph = _use_graph()
+    if not (graph and ast.graphable and tst.kernels):
+        _round_eager(target, draft, tst, ast, max_new)
+        return
+    key = (target.arena.version, target.arena.shadow.data_ptr(), draft.arena.version, draft.arena.shadow.data_ptr(), id(tst),
+           max_new)
+    if ast.graph is None or ast.graph_key != key:
+        if ast.graph_key != ("warm",) + key:
+            ast.graph, ast.graph_key, ast.graph_target = None, ("warm",) + key, tst
+            _round_eager(target, draft, tst, ast, max_new)
+            return
+        torch.cuda.synchronize(tst.device)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, capture_error_mode="thread_local"):
+            _round_eager(target, draft, tst, ast, max_new)
+        ast.graph, ast.graph_key = g, key
+    ast.graph.replay()
+
+
+def _check_assistant(model, assistant, P: int, max_new_tokens: int, num_assistant_tokens) -> None:
+    cfg, ar = model.config, model.arena
+    acfg, aar = assistant.config, assistant.arena
+    if acfg.vocab_size != cfg.vocab_size:
+        raise ValueError(f"assistant_model vocab_size {acfg.vocab_size} differs from the model's {cfg.vocab_size}")
+    if aar.device != ar.device:
+        raise ValueError(f"assistant_model is on {aar.device}, the model on {ar.device}")
+    if aar.compute_dtype != ar.compute_dtype:
+        raise ValueError(f"assistant_model computes in {aar.compute_dtype}, the model in {ar.compute_dtype}")
+    if aar.param_sharded:
+        raise ValueError("assisted generate() needs the assistant's full compute weights; its arena is parameter-sharded (FULL_SHARD)")
+    if isinstance(num_assistant_tokens, bool) or not isinstance(num_assistant_tokens, int) \
+            or not 1 <= num_assistant_tokens <= MAX_ASSISTANT_TOKENS:
+        raise ValueError(f"num_assistant_tokens must be an integer in [1, {MAX_ASSISTANT_TOKENS}], got {num_assistant_tokens!r}")
+    need = P + max_new_tokens + num_assistant_tokens
+    for who, c in (("the model", cfg), ("assistant_model", acfg)):
+        if need > c.max_position_embeddings:
+            raise ValueError(f"prompt length {P} + max_new_tokens {max_new_tokens} + num_assistant_tokens {num_assistant_tokens} "
+                             f"exceeds max_position_embeddings {c.max_position_embeddings} of {who}")
+
+
+def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int, Kp: int, controls: tuple, pad: int,
+                       eos: list[int]) -> torch.Tensor:
+    B = comp.shape[0]
+    Smax = _round_up(P + max_new_tokens + Kp, 128)
+    tst = decode_state(model, B, Smax)
+    ast = assisted_state(model, assistant, B, Kp, Smax)
+    dst = ast.draft
+    do_sample, temperature, top_k, top_p, seed = controls
+    tst.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos)
+    dst.set_controls(do_sample, temperature, top_k, top_p, seed ^ DRAFT_SEED_XOR, 0, [])
+    tst.out.fill_(pad)
+    prefill(model, tst, comp, lens)
+    prefill(assistant, dst, comp, lens)
+    dst.finished.zero_()                              # the draft never stops by itself; its position follows the target's
+    dst.pos.copy_(tst.pos)
+    ast.tok[:B].copy_(tst.ids)
+    ast.stats.zero_()
+    for r in range(max_new_tokens - 1):               # every round emits >= 1 token per unfinished row
+        if r % ASSISTED_CHECK_EVERY == 0 and bool(tst.finished.all()):
+            break
+        assisted_round(model, assistant, tst, ast, max_new_tokens)
+    return tst.out[:, :max_new_tokens].clone()
+
+
 # ------------------------------------------------------------------------------------------------ generate
 def _eos_list(eos) -> list[int]:
     if eos is None:
@@ -231,7 +422,7 @@ def _eos_list(eos) -> list[int]:
 @torch.no_grad()
 def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, max_new_tokens: int = 20,
              do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
-             pad_token_id: int | None = None, seed: int = 0) -> torch.Tensor:
+             pad_token_id: int | None = None, seed: int = 0, assistant_model=None, num_assistant_tokens: int = 4) -> torch.Tensor:
     """See :meth:`LlamaForCausalLM.generate`."""
     cfg, ar = model.config, model.arena
     if ar.param_sharded:
@@ -248,6 +439,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
         raise ValueError(f"temperature must be > 0 when sampling, got {temperature}")
     if do_sample and not 0 < top_p <= 1:
         raise ValueError(f"top_p must be in (0, 1], got {top_p}")
+    if assistant_model is not None:
+        _check_assistant(model, assistant_model, P, max_new_tokens, num_assistant_tokens)
     dev = ar.device
     ids = input_ids.to(dev)
     if attention_mask is None:
@@ -267,11 +460,15 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
                         cfg.num_key_value_heads)
     max_len = int(lens.max())
     Sp = _round_up(max_len, 128) if kernels else max_len
-    Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))
-    st = decode_state(model, B, Smax)
     col = (P - lens.long())[:, None] + torch.arange(Sp, device=dev)[None, :]
     comp = ids.gather(1, col.clamp(max=P - 1))
     comp = comp.masked_fill(torch.arange(Sp, device=dev)[None, :] >= lens.long()[:, None], 0)
+    if assistant_model is not None:
+        new = _assisted_generate(model, assistant_model, comp, lens, P, max_new_tokens, num_assistant_tokens,
+                                 (do_sample, temperature, top_k, top_p, seed), pad, eos)
+        return torch.cat([ids, new], dim=1)
+    Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))
+    st = decode_state(model, B, Smax)
 
     st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos)
     st.out.fill_(pad)

@@ -192,6 +192,7 @@ class LlamaEngine:
         self.head_grad_tmp: torch.Tensor | None = None
         self._graphs: dict[tuple, dict] = {}       # (B, S, loss_scale, labels-alias) -> captured micro-step
         self.decode_state = None                   # generation's KV caches + decode graph (models/generation.py)
+        self.assisted_state = None                 # assisted generation's verify buffers, draft caches + round graph
         self.score_state = None                    # scoring buffers (models/scoring.py)
 
     def workspace(self, B: int, S: int) -> _Workspace:
@@ -689,6 +690,7 @@ class LlamaForCausalLM(nn.Module):
                 self.engine._ws.clear()
                 self.engine._graphs.clear()
                 self.engine.decode_state = None
+                self.engine.assisted_state = None
                 self.engine.score_state = None
                 self.engine.head_grad_tmp = None
                 self._rebind()
@@ -738,7 +740,8 @@ class LlamaForCausalLM(nn.Module):
     @torch.no_grad()
     def generate(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, max_new_tokens: int = 20,
                  do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
-                 pad_token_id: int | None = None, seed: int = 0) -> torch.Tensor:
+                 pad_token_id: int | None = None, seed: int = 0, assistant_model: "LlamaForCausalLM | None" = None,
+                 num_assistant_tokens: int = 4) -> torch.Tensor:
         """KV-cached text generation with HF ``generate`` keyword names.  Returns LongTensor [B, P + max_new_tokens]: the
         prompt as given, then the new tokens.
 
@@ -749,12 +752,21 @@ class LlamaForCausalLM(nn.Module):
         decode kernels (csrc/decode_sm90.cu) with the step replayed from a CUDA graph; other precisions and devices run the
         PyTorch reference path.  fp8-mixed models generate on the bf16 path from their bf16 compute weights (no FP8 GEMMs).
         Raises ValueError for a parameter-sharded (FULL_SHARD) model, a prompt plus
-        ``max_new_tokens`` longer than ``max_position_embeddings``, or a mask that is not left-padded."""
+        ``max_new_tokens`` longer than ``max_position_embeddings``, or a mask that is not left-padded.
+
+        ``assistant_model`` (a smaller model with the same vocabulary, on the same device and compute dtype; the model
+        itself works too) turns on assisted (speculative) generation: each round the assistant proposes
+        ``num_assistant_tokens`` (1..7) tokens, this model scores them all in one pass, and speculative sampling keeps
+        an exact sample of this model's distribution (greedy: exactly its argmax continuation, up to bf16 near-ties
+        between the one- and multi-token attention).  ``engine.assisted_state`` then reports ``verify_passes()`` and
+        ``acceptance_rate()``.  Raises ValueError for a different vocabulary, device or compute dtype, a parameter-sharded
+        assistant, ``num_assistant_tokens`` outside [1, 7], or a prompt plus ``max_new_tokens`` plus
+        ``num_assistant_tokens`` beyond either model's ``max_position_embeddings``."""
         from .generation import generate
 
         return generate(self, input_ids, attention_mask=attention_mask, max_new_tokens=max_new_tokens, do_sample=do_sample,
                         temperature=temperature, top_k=top_k, top_p=top_p, eos_token_id=eos_token_id, pad_token_id=pad_token_id,
-                        seed=seed)
+                        seed=seed, assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens)
 
     @torch.no_grad()
     def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None):

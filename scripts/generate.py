@@ -4,11 +4,14 @@
     python scripts/generate.py --model 150m --checkpoint outputs/model_step_1000 --weights outer --prompt-ids "1 450 4996"
     python scripts/generate.py --model /models/llama-150m --prompt "The capital of" --tokenizer /models/llama-150m \\
         --max-new-tokens 64 --do-sample --temperature 0.8 --top-p 0.95
+    python scripts/generate.py --model 1b --checkpoint outputs_1b/model_step_1000 --assistant-model 150m \\
+        --assistant-checkpoint outputs_150m/model_step_1000 --num-assistant-tokens 4 --prompt-ids "1 450 4996"
 
 ``--checkpoint`` reads a checkpoint directory written by train_fsdp / utils/ckpt.save_checkpoint (the one holding the
 ``*.distcp`` shards, i.e. ``model_step_N`` or its ``diloco_rank_R`` sub-directory).  ``--weights local`` takes the
 worker's own weights (``model``), ``--weights outer`` the DiLoCo global model (``theta_outer``).  Tokenizers are only
-read from a local directory.
+read from a local directory.  ``--assistant-model`` (with ``--assistant-checkpoint`` / ``--assistant-weights``) loads a
+draft model the same way and turns on assisted (speculative) generation.
 """
 import argparse
 import json
@@ -58,17 +61,20 @@ def add_model_args(ap: argparse.ArgumentParser) -> None:
     ap.add_argument("--precision", default=None, help="bf16-mixed (default on CUDA), 32-true (default on CPU), fp16-mixed")
 
 
-def load_model(a: argparse.Namespace) -> LlamaForCausalLM:
-    """The model chosen by the ``add_model_args`` options, in eval mode."""
+def load_model(a: argparse.Namespace, model: str | None = None, checkpoint: str | None = None,
+               weights: str | None = None) -> LlamaForCausalLM:
+    """The model chosen by the ``add_model_args`` options, or by the given model / checkpoint / weights, in eval mode."""
+    if model is None:
+        model, checkpoint, weights = a.model, a.checkpoint, a.weights
     device = torch.device(a.device)
     precision = a.precision or ("bf16-mixed" if device.type == "cuda" else "32-true")
-    cfg = LlamaConfig.from_pretrained(a.model)
-    if a.checkpoint is not None:
-        model = LlamaForCausalLM(cfg, device=device, precision=precision, init=False)
-        load_checkpoint_weights(model, a.checkpoint, a.weights)
+    cfg = LlamaConfig.from_pretrained(model)
+    if checkpoint is not None:
+        m = LlamaForCausalLM(cfg, device=device, precision=precision, init=False)
+        load_checkpoint_weights(m, checkpoint, weights)
     else:
-        model = LlamaForCausalLM.from_pretrained(a.model, config=cfg, device=device, precision=precision, seed=a.init_seed)
-    return model.eval()
+        m = LlamaForCausalLM.from_pretrained(model, config=cfg, device=device, precision=precision, seed=a.init_seed)
+    return m.eval()
 
 
 def main(argv=None) -> None:
@@ -85,7 +91,14 @@ def main(argv=None) -> None:
     ap.add_argument("--eos-token-id", type=int, default=None)
     ap.add_argument("--pad-token-id", type=int, default=None)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--assistant-model", default=None, help="draft model (HF directory or preset) for assisted generation")
+    ap.add_argument("--assistant-checkpoint", default=None, help="training checkpoint directory of the draft's weights")
+    ap.add_argument("--assistant-weights", choices=["local", "outer"], default="local",
+                    help="with --assistant-checkpoint: local or DiLoCo outer weights")
+    ap.add_argument("--num-assistant-tokens", type=int, default=4, help="draft tokens proposed per round (1..7)")
     a = ap.parse_args(argv)
+    if a.assistant_model is None and a.assistant_checkpoint is not None:
+        ap.error("--assistant-checkpoint needs --assistant-model")
 
     tok = None
     if a.tokenizer is not None:
@@ -103,6 +116,9 @@ def main(argv=None) -> None:
 
     device = torch.device(a.device)
     model = load_model(a)
+    assistant = None
+    if a.assistant_model is not None:
+        assistant = load_model(a, a.assistant_model, a.assistant_checkpoint, a.assistant_weights)
 
     # left-pad the batch to a common length
     P = max(len(p) for p in prompts)
@@ -113,12 +129,16 @@ def main(argv=None) -> None:
         mask[i, P - len(p):] = 1
     out = model.generate(ids.to(device), attention_mask=mask.to(device), max_new_tokens=a.max_new_tokens, do_sample=a.do_sample,
                          temperature=a.temperature, top_k=a.top_k, top_p=a.top_p, eos_token_id=a.eos_token_id,
-                         pad_token_id=a.pad_token_id, seed=a.seed).cpu()
+                         pad_token_id=a.pad_token_id, seed=a.seed, assistant_model=assistant,
+                         num_assistant_tokens=a.num_assistant_tokens).cpu()
     for i, p in enumerate(prompts):
         new = out[i, P:].tolist()
         print("ids:", " ".join(str(t) for t in p + new))
         if tok is not None:
             print("text:", tok.decode(p + new, skip_special_tokens=True))
+    if assistant is not None:
+        st = model.engine.assisted_state
+        print(f"assisted: {st.verify_passes()} verify passes, acceptance {st.acceptance_rate():.3f}")
 
 
 if __name__ == "__main__":
