@@ -16,11 +16,6 @@
 //                  TMA (cp.async.bulk.tensor stores, fp32 reduce-add for the weight gradient); the tensor map of the
 //                  output clips partial tiles.  A box is rewritten only after the store that read it has (bulk_wait_read).
 //
-// CL = 2 (odb_gemm2_*: forward projections with at least one wave of 256 x 256 tiles): a cluster of two CTAs computes a 256 x 256 tile,
-// the two m-halves of the same B tile.  Each CTA loads its own A and ONE half of B, multicast into both CTAs, so the B
-// traffic from L2 per CTA halves; a stage is refilled only when the MMA warpgroups of both CTAs have released it.  Both
-// CTAs of a cluster walk the same sequence of cluster tiles.
-//
 // Operand layouts (template flags, the shared-memory descriptor expresses both - no transposed copies are made):
 //   A_MN = false : A is [M, K] row-major (K-major)          A_MN = true : A is [K, M] row-major (MN-major, wgrad)
 //   B_MN = false : B is [N, K] row-major (K-major)          B_MN = true : B is [K, N] row-major (MN-major, dgrad)
@@ -154,18 +149,16 @@ struct Tile {
   int m_blk, n_blk, m0, n0, kb0, kb1, b;
 };
 
-template <int CL, int ELEM>
-__device__ __forceinline__ Tile tile_of(const Params& p, int work, uint32_t rank) {
+template <int ELEM>
+__device__ __forceinline__ Tile tile_of(const Params& p, int work) {
   constexpr int KB = ELEM ? BK8 : BK;            // elements per k-block
   constexpr int BNE = ELEM ? BN / 2 : BN;        // tile columns
-  const int num_mc = (p.num_m + CL - 1) / CL;
-  const int per_batch = num_mc * p.num_n * p.splits;
+  const int per_batch = p.num_m * p.num_n * p.splits;
   Tile t;
   t.b = work / per_batch;
   work -= t.b * per_batch;
   const int tile = work / p.splits, split = work - tile * p.splits;
-  tile_coords(tile, num_mc, p.num_n, p.group_m, t.m_blk, t.n_blk);
-  t.m_blk = t.m_blk * CL + (int)rank;            // CL = 2: this CTA's m-half of the cluster tile (may lie beyond M)
+  tile_coords(tile, p.num_m, p.num_n, p.group_m, t.m_blk, t.n_blk);
   t.m0 = t.m_blk * BM;
   t.n0 = t.n_blk * BNE;
   t.kb0 = split * p.kb_per_split;
@@ -181,14 +174,14 @@ __device__ __forceinline__ int swiglu_bwd_rounds(const Params& p, int n0) {
   return min(BNE / 64, (p.I - n0) / 64);
 }
 
-template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM>
+template <int EPI, bool A_MN, bool B_MN, int ELEM>
 __device__ __forceinline__ void mma_and_epilogue(const Params& p, const CUtensorMap* tmap_c, const CUtensorMap* tmap_c2,
                                                  uint8_t* smem_a, uint8_t* smem_b, uint8_t* smem_c, uint64_t* full_bar,
                                                  uint64_t* empty_bar, int cw, const Tile& tl, int& stage, uint32_t& phase);
 
 // Output maps (tmap_c, tmap_c2): C (gu for kSwiGLU and kSwiGLUBwd, which also loads from it; fp32 dW for kWgradAcc) and
 // act (kSwiGLU); see launch().
-template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM = 0>
+template <int EPI, bool A_MN, bool B_MN, int ELEM = 0>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a1,
             const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_b,
@@ -202,26 +195,23 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   uint64_t* empty_bar = full_bar + STAGES;
 
   pdl_launch_dependents();
-  static_assert(CL == 1 || (CL == 2 && !B_MN && !A_MN), "clusters share a K-major B tile");
-  static_assert(ELEM == 0 || (CL == 1 && !A_MN && !B_MN), "FP8 wgmma takes K-major operands only");
+  static_assert(ELEM == 0 || (!A_MN && !B_MN), "FP8 wgmma takes K-major operands only");
   constexpr int KB = ELEM ? BK8 : BK;            // elements per k-block
   constexpr int BNE = ELEM ? BN / 2 : BN;        // tile columns
   constexpr bool TMA_OUT =
       EPI == kStore || EPI == kRoPE || EPI == kSwiGLU || EPI == kSwiGLUBwd || EPI == kLCEFwd || EPI == kWgradAcc;
   const int wg = threadIdx.x >> 7;
-  const uint32_t rank = CL == 2 ? cluster_ctarank() : 0;
-  const int work_total = (p.num_m + CL - 1) / CL * p.num_n * p.splits * p.batch;
-  const int work_first = blockIdx.x / CL, work_step = gridDim.x / CL;
+  const int work_total = p.num_m * p.num_n * p.splits * p.batch;
+  const int work_first = blockIdx.x, work_step = gridDim.x;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     if constexpr (TMA_OUT) tma_prefetch_desc(&tmap_c);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2 * CL); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
     fence_barrier_init();
   }
-  if constexpr (CL == 2) cluster_sync();         // the peer multicasts into our stages and arrives on our barriers
-  else __syncthreads();
+  __syncthreads();
   pdl_wait();
 
   if (wg == 0) {
@@ -231,7 +221,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       int stage = 0;
       uint32_t phase = 0;
       for (int work = work_first; work < work_total; work += work_step) {
-        const Tile t = tile_of<CL, ELEM>(p, work, rank);
+        const Tile t = tile_of<ELEM>(p, work);
         // which A tensor this tile reads (A_MN: the split is along M, so it is fixed per tile)
         const CUtensorMap* ta_m = &tmap_a;
         int am0 = t.m0;
@@ -261,9 +251,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           if constexpr (B_MN) {     // [K rows, N cols]: four 64(n) x 64(k) boxes
 #pragma unroll
             for (int j = 0; j < 4; ++j) tma_load_2d(sb + j * BOX_BYTES, &tmap_b, &full_bar[stage], t.n0 + 64 * j, bk0 + kb * BK);
-          } else if constexpr (CL == 2) {   // this CTA's half of B (gate | up for kSwiGLU) into both CTAs
-            const int b_row = EPI == kSwiGLU ? (rank == 0 ? t.n_blk * (BN / 2) : p.I + t.n_blk * (BN / 2)) : t.n0 + (int)rank * (BN / 2);
-            tma_load_2d_multicast(sb + rank * (B_BYTES / 2), &tmap_b, &full_bar[stage], kb * KB, b_row, (uint16_t)0x3);
           } else if constexpr (EPI == kSwiGLU) {
             const int g0 = t.n_blk * (BNE / 2);
             tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * KB, g0);
@@ -298,15 +285,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     int stage = 0;
     uint32_t phase = 0;
     for (int work = work_first; work < work_total; work += work_step) {
-      const Tile t = tile_of<CL, ELEM>(p, work, rank);
-      mma_and_epilogue<EPI, A_MN, B_MN, CL, ELEM>(p, &tmap_c, &tmap_c2, smem_a, smem_b, smem_c, full_bar, empty_bar, cw, t,
-                                                  stage, phase);
+      const Tile t = tile_of<ELEM>(p, work);
+      mma_and_epilogue<EPI, A_MN, B_MN, ELEM>(p, &tmap_c, &tmap_c2, smem_a, smem_b, smem_c, full_bar, empty_bar, cw, t, stage,
+                                              phase);
     }
     if constexpr (TMA_OUT) {
       if ((threadIdx.x & 127) == 0) bulk_wait<0>();   // the last stores have read the staging and reached memory
     }
   }
-  if constexpr (CL == 2) cluster_sync();         // no CTA leaves while its peer may still arrive on its barriers
 }
 
 // ---------------------------------------------------------------------------------------- output staging (TMA epilogues)
@@ -347,7 +333,7 @@ __device__ __forceinline__ void staging_publish(int cw) {
   named_bar_sync(1 + cw, 128);
 }
 
-template <int EPI, bool A_MN, bool B_MN, int CL, int ELEM>
+template <int EPI, bool A_MN, bool B_MN, int ELEM>
 __device__ __forceinline__ void mma_and_epilogue(const Params& p, const CUtensorMap* tmap_c, const CUtensorMap* tmap_c2,
                                                  uint8_t* smem_a, uint8_t* smem_b, uint8_t* smem_c, uint64_t* full_bar,
                                                  uint64_t* empty_bar, int cw, const Tile& tl, int& stage, uint32_t& phase) {
@@ -379,12 +365,8 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, const CUtensor
 #pragma unroll
     for (int j = 0; j < 64; ++j) acc[j] *= dq;
   } else {
-    // release a stage to the producer (both CTAs' producers for CL = 2: the stage holds the peer's multicast half of B)
-    auto release = [&](int s) {
-      if ((threadIdx.x & 127) == 0) {
-        mbar_arrive(&empty_bar[s]);
-        if constexpr (CL == 2) mbar_arrive_cluster(&empty_bar[s], cluster_ctarank() ^ 1);
-      }
+    auto release = [&](int s) {                  // hand a stage back to the producer
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[s]);
     };
     // scale_d = 0 on the tile's first k-block discards acc, but the wgmma operands read it: zeroing it here ends the
     // previous tile's values (which would otherwise stay live through its epilogue and spill)
@@ -720,61 +702,55 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, const CUtensor
   }
 }
 
-struct ASplit {
-  const void* A1 = nullptr; const void* A2 = nullptr;
-  long long lda1 = 0, lda2 = 0;
-  int K0 = 0, K1 = 0, K2 = 0;      // extents of the three A tensors along the split dimension; K0 == 0 => no split
+// What launch() needs besides Params: the operands its tensor maps are built from (the kernel sees only the maps).  A
+// three-piece A operand [A | A1 | A2] is read in place, split along K (A_MN = false) or along M (A_MN = true); K0, K1, K2
+// are the extents of the pieces along that dimension, K0 == 0: A is one tensor.
+struct Operands {
+  const void* A = nullptr; long long lda = 0;
+  const void* B = nullptr; long long ldb = 0;
+  const void* A1 = nullptr; long long lda1 = 0;
+  const void* A2 = nullptr; long long lda2 = 0;
+  int K0 = 0, K1 = 0, K2 = 0;
 };
 
-struct BatchArgs {
-  int batch = 1; int a_rows = 0, b_rows = 0; long long c_bstride = 0; float alpha = 1.f, beta = 0.f;
-};
-
-struct LceArgs {
-  const float* row_shift = nullptr; float* partials = nullptr; int want_sumsq = 0; int store = 1;
-  const float* rowscale = nullptr; const long long* labels = nullptr; const float* gscale = nullptr;
-  const void* wlab = nullptr; long long ldwlab = 0;
-  float* sc_max = nullptr; float* sc_sum = nullptr; int* sc_idx = nullptr; float* sc_zlab = nullptr;
-};
-
-template <int EPI, bool A_MN, bool B_MN, int CL = 1, int ELEM = 0>
-static int launch(const void* A, const void* B, void* C, void* aux, int M, int N, int K, long long lda, long long ldb,
-                  long long ldc, long long ldaux, int I, int S, int rope_cols, const float* cos_t, const float* sin_t,
-                  cudaStream_t st, const ASplit& sp = ASplit(), const LceArgs& lce = LceArgs(), const float* inv_a = nullptr,
-                  const float* inv_b = nullptr, const BatchArgs& ba = BatchArgs()) {
-  // kAxpby: the tensor maps span the whole stacked batch; problem b starts ba.a_rows * b / ba.b_rows * b rows in
-  const int a_rows_all = EPI == kAxpby ? ba.batch * ba.a_rows : (A_MN ? K : M);
-  const int b_rows_all = EPI == kAxpby ? ba.batch * ba.b_rows : (B_MN ? K : N);
+// The caller sets the fields of p that its epilogue reads (at least M, N, K; strides in elements); launch() fills in the
+// schedule (num_m, num_n, group_m, splits, kb_per_split, ks1, ks2) and S = 1, batch = 1 when they are left at 0.
+template <int EPI, bool A_MN, bool B_MN, int ELEM = 0>
+static int launch(const Operands& o, Params p, cudaStream_t st) {
+  const int M = p.M, N = p.N, K = p.K, I = p.I;
+  if (p.S <= 0) p.S = 1;
+  if (p.batch <= 0) p.batch = 1;
+  // kAxpby: the tensor maps span the whole stacked batch; problem b starts p.a_rows * b / p.b_rows * b rows in
+  const int a_rows_all = EPI == kAxpby ? p.batch * p.a_rows : (A_MN ? K : M);
+  const int b_rows_all = EPI == kAxpby ? p.batch * p.b_rows : (B_MN ? K : N);
   constexpr int EB = ELEM ? 1 : 2;               // operand bytes per element
   constexpr int KB = ELEM ? BK8 : BK;
   constexpr int BNE = ELEM ? BN / 2 : BN;        // tile columns
   CUtensorMap ta, ta1, ta2, tb;
   int rc;
-  if (ELEM) {          // FP8: K-major A and B, no split, no cluster
-    if ((rc = make_tmap_2d(&ta, A, M, K, lda, BM, KB, EB))) return rc;
+  if (ELEM) {          // FP8: K-major A and B, no split
+    if ((rc = make_tmap_2d(&ta, o.A, M, K, o.lda, BM, KB, EB))) return rc;
   } else if (A_MN) {          // A given as [K rows, M cols] (possibly three tensors side by side along M)
-    if ((rc = make_tmap_2d(&ta, A, K, sp.K0 ? sp.K0 : M, lda * 2, 64, 64, 2))) return rc;
+    if ((rc = make_tmap_2d(&ta, o.A, K, o.K0 ? o.K0 : M, o.lda * 2, 64, 64, 2))) return rc;
   } else {
-    if ((rc = make_tmap_2d(&ta, A, a_rows_all, sp.K0 ? sp.K0 : K, lda * 2, BM, BK, 2))) return rc;
+    if ((rc = make_tmap_2d(&ta, o.A, a_rows_all, o.K0 ? o.K0 : K, o.lda * 2, BM, BK, 2))) return rc;
   }
   ta1 = ta; ta2 = ta;
-  if (sp.K0) {
+  if (o.K0) {
     if (A_MN) {
-      if (sp.K1 && (rc = make_tmap_2d(&ta1, sp.A1, K, sp.K1, sp.lda1 * 2, 64, 64, 2))) return rc;
-      if (sp.K2 && (rc = make_tmap_2d(&ta2, sp.A2, K, sp.K2, sp.lda2 * 2, 64, 64, 2))) return rc;
+      if (o.K1 && (rc = make_tmap_2d(&ta1, o.A1, K, o.K1, o.lda1 * 2, 64, 64, 2))) return rc;
+      if (o.K2 && (rc = make_tmap_2d(&ta2, o.A2, K, o.K2, o.lda2 * 2, 64, 64, 2))) return rc;
     } else {
-      if ((rc = make_tmap_2d(&ta1, sp.A1, M, sp.K1, sp.lda1 * 2, BM, BK, 2))) return rc;
-      if ((rc = make_tmap_2d(&ta2, sp.A2, M, sp.K2, sp.lda2 * 2, BM, BK, 2))) return rc;
+      if ((rc = make_tmap_2d(&ta1, o.A1, M, o.K1, o.lda1 * 2, BM, BK, 2))) return rc;
+      if ((rc = make_tmap_2d(&ta2, o.A2, M, o.K2, o.lda2 * 2, BM, BK, 2))) return rc;
     }
   }
   if (B_MN) {
-    if ((rc = make_tmap_2d(&tb, B, b_rows_all, N, ldb * 2, 64, 64, 2))) return rc;   // [K rows, N cols], 64 x 64 boxes
+    if ((rc = make_tmap_2d(&tb, o.B, b_rows_all, N, o.ldb * 2, 64, 64, 2))) return rc;   // [K rows, N cols], 64 x 64 boxes
   } else if (EPI == kSwiGLU) {
-    if ((rc = make_tmap_2d(&tb, B, 2 * I, K, ldb * EB, BNE / 2, KB, EB))) return rc;
-  } else if (CL == 2) {
-    if ((rc = make_tmap_2d(&tb, B, N, K, ldb * 2, BN / 2, BK, 2))) return rc;      // each CTA of the pair loads one half
+    if ((rc = make_tmap_2d(&tb, o.B, 2 * I, K, o.ldb * EB, BNE / 2, KB, EB))) return rc;
   } else {
-    if ((rc = make_tmap_2d(&tb, B, b_rows_all, K, ldb * EB, BNE, KB, EB))) return rc;
+    if ((rc = make_tmap_2d(&tb, o.B, b_rows_all, K, o.ldb * EB, BNE, KB, EB))) return rc;
   }
   // outputs stored by TMA: 64-row boxes of 128 bytes on the caller's view (base, [rows, cols], row stride), so partial
   // tiles are clipped to it.  TMA needs a 16-byte aligned base: a misaligned output is refused (-1).
@@ -783,32 +759,21 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
     if (reinterpret_cast<uintptr_t>(base) % 16) return -1;
     return make_tmap_2d(m, base, rows, cols, ld * eb, 64, 128 / eb, eb);
   };
-  if (EPI == kStore || EPI == kRoPE || (EPI == kLCEFwd && lce.store)) {
-    if ((rc = out_map(&tc, C, M, N, ldc, 2))) return rc;
+  if (EPI == kStore || EPI == kRoPE || (EPI == kLCEFwd && p.store)) {
+    if ((rc = out_map(&tc, p.C, M, N, p.ldc, 2))) return rc;
   } else if (EPI == kSwiGLU) {
-    if ((rc = out_map(&tc, C, M, 2 * I, ldc, 2)) || (rc = out_map(&tc2, aux, M, I, ldaux, 2))) return rc;
+    if ((rc = out_map(&tc, p.C, M, 2 * I, p.ldc, 2)) || (rc = out_map(&tc2, p.aux, M, I, p.ldaux, 2))) return rc;
   } else if (EPI == kSwiGLUBwd) {
-    if ((rc = out_map(&tc, C, M, 2 * I, ldc, 2))) return rc;      // gu: the epilogue's gate / up loads and its stores
+    if ((rc = out_map(&tc, p.C, M, 2 * I, p.ldc, 2))) return rc;      // gu: the epilogue's gate / up loads and its stores
   } else if (EPI == kWgradAcc) {
-    if ((rc = out_map(&tc, C, M, N, ldc, 4))) return rc;
+    if ((rc = out_map(&tc, p.C, M, N, p.ldc, 4))) return rc;
   }
-  Params p{};
-  p.M = M; p.N = N; p.K = K;
   p.num_m = ceil_div(M, BM);
   p.num_n = (EPI == kSwiGLU) ? ceil_div(I, BNE / 2) : ceil_div(N, BNE);
   p.group_m = EPI == kLCEdX ? 0 : GROUP_M;
-  p.C = C; p.ldc = ldc; p.aux = aux; p.ldaux = ldaux;
-  p.I = I; p.S = S > 0 ? S : 1; p.rope_cols = rope_cols; p.cos_t = cos_t; p.sin_t = sin_t;
   const int split_blk = A_MN ? BM : BK;
-  p.ks1 = sp.K0 ? sp.K0 / split_blk : 0;
-  p.ks2 = sp.K0 ? (sp.K0 + sp.K1) / split_blk : 0;
-  p.row_shift = lce.row_shift; p.partials = lce.partials; p.want_sumsq = lce.want_sumsq; p.store = lce.store;
-  p.rowscale = lce.rowscale; p.labels = lce.labels; p.gscale = lce.gscale;
-  p.wlab = (const __nv_bfloat16*)lce.wlab; p.ldwlab = lce.ldwlab;
-  p.sc_max = lce.sc_max; p.sc_sum = lce.sc_sum; p.sc_idx = lce.sc_idx; p.sc_zlab = lce.sc_zlab;
-  p.inv_a = inv_a; p.inv_b = inv_b;
-  p.a_rows = ba.a_rows; p.b_rows = ba.b_rows; p.c_bstride = ba.c_bstride; p.alpha = ba.alpha; p.beta = ba.beta;
-  p.batch = ba.batch;
+  p.ks1 = o.K0 ? o.K0 / split_blk : 0;
+  p.ks2 = o.K0 ? (o.K0 + o.K1) / split_blk : 0;
   const int tiles = p.num_m * p.num_n;
   const int kb_total = ceil_div(K, KB);
   p.splits = 1;
@@ -829,16 +794,15 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
   }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_kernel<EPI, A_MN, B_MN, CL, ELEM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_kernel<EPI, A_MN, B_MN, ELEM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          SMEM_BYTES);
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
-  // persistent grid: one CTA (CL = 2: one cluster per two SMs) per SM, or fewer when there are fewer work items
-  const int work = ceil_div(p.num_m, CL) * p.num_n * p.splits * ba.batch;
-  const int clusters = work < sm_count() / CL ? work : sm_count() / CL;
-  launch_pdl_cluster(gemm_kernel<EPI, A_MN, B_MN, CL, ELEM>, dim3(clusters * CL), dim3(THREADS), SMEM_BYTES, st, CL,
-                     ta, ta1, ta2, tb, tc, tc2, p);
+  // persistent grid: one CTA per SM, or fewer when there are fewer work items
+  const int work = p.num_m * p.num_n * p.splits * p.batch;
+  const int ctas = work < sm_count() ? work : sm_count();
+  launch_pdl(gemm_kernel<EPI, A_MN, B_MN, ELEM>, dim3(ctas), dim3(THREADS), SMEM_BYTES, st, ta, ta1, ta2, tb, tc, tc2, p);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : (int)e;
 }
@@ -849,26 +813,21 @@ static int launch(const void* A, const void* B, void* C, void* aux, int M, int N
 ODB_EXPORT int odb_gemm_bf16_tn(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb,
                                 long long ldc, cudaStream_t st) {
   if (K % 8 || lda % 8 || ldb % 8 || ldc % 8) return -1;
-  return gemm::launch<gemm::kStore, false, false>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st);
-}
-
-// as odb_gemm_bf16_tn, computed by clusters of two CTAs that share (multicast) the B tile
-ODB_EXPORT int odb_gemm2_bf16_tn(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb,
-                                 long long ldc, cudaStream_t st) {
-  if (K % 8 || lda % 8 || ldb % 8 || ldc % 8) return -1;
-  return gemm::launch<gemm::kStore, false, false, 2>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st);
+  gemm::Operands o;
+  o.A = A; o.lda = lda; o.B = B; o.ldb = ldb;
+  gemm::Params p{};
+  p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc;
+  return gemm::launch<gemm::kStore, false, false>(o, p, st);
 }
 
 // gu[M,2I] = x[M,K] * Wgu[2I,K]^T and act[M,I] = silu(gu[:, :I]) * gu[:, I:]   (I % 64 == 0)
 ODB_EXPORT int odb_gemm_swiglu(const void* X, const void* Wgu, void* gu, void* act, int M, int I, int K, cudaStream_t st) {
   if (K % 8 || I % 64) return -1;
-  return gemm::launch<gemm::kSwiGLU, false, false>(X, Wgu, gu, act, M, 2 * I, K, K, K, 2 * I, I, I, 0, 0, nullptr, nullptr, st);
-}
-
-// as odb_gemm_swiglu, computed by clusters of two CTAs (one loads the gate half of B, the other the up half)
-ODB_EXPORT int odb_gemm2_swiglu(const void* X, const void* Wgu, void* gu, void* act, int M, int I, int K, cudaStream_t st) {
-  if (K % 8 || I % 64) return -1;
-  return gemm::launch<gemm::kSwiGLU, false, false, 2>(X, Wgu, gu, act, M, 2 * I, K, K, K, 2 * I, I, I, 0, 0, nullptr, nullptr, st);
+  gemm::Operands o;
+  o.A = X; o.lda = K; o.B = Wgu; o.ldb = K;
+  gemm::Params p{};
+  p.M = M; p.N = 2 * I; p.K = K; p.C = gu; p.ldc = 2 * I; p.aux = act; p.ldaux = I; p.I = I;
+  return gemm::launch<gemm::kSwiGLU, false, false>(o, p, st);
 }
 
 // Backward of the SwiGLU MLP's middle: gu[M,2I] (gate|up, bf16) is replaced IN PLACE by d(gate)|d(up), where
@@ -877,59 +836,59 @@ ODB_EXPORT int odb_gemm2_swiglu(const void* X, const void* Wgu, void* gu, void* 
 ODB_EXPORT int odb_gemm_swiglu_bwd(const void* dY, const void* WdT, void* gu, int M, int I, int K, long long lda, long long ldb,
                                    cudaStream_t st) {
   if (K % 8 || I % 64 || lda % 8 || ldb % 8) return -1;
-  return gemm::launch<gemm::kSwiGLUBwd, false, false>(dY, WdT, gu, nullptr, M, I, K, lda, ldb, 2 * I, 0, I, 0, 0, nullptr, nullptr, st);
+  gemm::Operands o;
+  o.A = dY; o.lda = lda; o.B = WdT; o.ldb = ldb;
+  gemm::Params p{};
+  p.M = M; p.N = I; p.K = K; p.C = gu; p.ldc = 2 * I; p.I = I;
+  return gemm::launch<gemm::kSwiGLUBwd, false, false>(o, p, st);
 }
 
 // qkv[M,N] = x[M,K] * Wqkv[N,K]^T with RoPE applied to the first rope_cols columns (head_dim 64, position = row % S)
 ODB_EXPORT int odb_gemm_qkv_rope(const void* X, const void* W, void* qkv, int M, int N, int K, int S, int rope_cols,
                                  const void* cos_t, const void* sin_t, cudaStream_t st) {
   if (K % 8 || N % 64 || rope_cols % 64) return -1;
-  return gemm::launch<gemm::kRoPE, false, false>(X, W, qkv, nullptr, M, N, K, K, K, N, 0, 0, S, rope_cols, (const float*)cos_t,
-                                                 (const float*)sin_t, st);
-}
-
-// as odb_gemm_qkv_rope, computed by clusters of two CTAs that share (multicast) the B tile
-ODB_EXPORT int odb_gemm2_qkv_rope(const void* X, const void* W, void* qkv, int M, int N, int K, int S, int rope_cols,
-                                  const void* cos_t, const void* sin_t, cudaStream_t st) {
-  if (K % 8 || N % 64 || rope_cols % 64) return -1;
-  return gemm::launch<gemm::kRoPE, false, false, 2>(X, W, qkv, nullptr, M, N, K, K, K, N, 0, 0, S, rope_cols, (const float*)cos_t,
-                                                    (const float*)sin_t, st);
-}
-
-// C[M,N] = [A0 | A1 | A2][M, K0+K1+K2] * B[N, K0+K1+K2]^T with the three A pieces read in place (K0, K1, K2 % 64 == 0)
-ODB_EXPORT int odb_gemm_bf16_tn_a3(const void* A0, const void* A1, const void* A2, long long lda0, long long lda1, long long lda2,
-                                   int K0, int K1, int K2, const void* B, void* C, int M, int N, long long ldb, long long ldc,
-                                   cudaStream_t st) {
-  if (K0 % 64 || K1 % 64 || K2 % 64 || K0 <= 0 || K1 <= 0 || K2 <= 0) return -1;
-  gemm::ASplit sp;
-  sp.A1 = A1; sp.A2 = A2; sp.lda1 = lda1; sp.lda2 = lda2; sp.K0 = K0; sp.K1 = K1; sp.K2 = K2;
-  return gemm::launch<gemm::kStore, false, false>(A0, B, C, nullptr, M, N, K0 + K1 + K2, lda0, ldb, ldc, 0, 0, 0, 0, nullptr,
-                                                  nullptr, st, sp);
+  gemm::Operands o;
+  o.A = X; o.lda = K; o.B = W; o.ldb = K;
+  gemm::Params p{};
+  p.M = M; p.N = N; p.K = K; p.C = qkv; p.ldc = N;
+  p.S = S; p.rope_cols = rope_cols; p.cos_t = (const float*)cos_t; p.sin_t = (const float*)sin_t;
+  return gemm::launch<gemm::kRoPE, false, false>(o, p, st);
 }
 
 // C[M,N] = A[M,K] * B[K,N] with B row-major (the dgrad dX = dY W on the forward [out, in] weight layout)
 ODB_EXPORT int odb_gemm_bf16_nn(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb,
                                 long long ldc, cudaStream_t st) {
   if (K % 8 || N % 8 || lda % 8 || ldb % 8 || ldc % 8) return -1;
-  return gemm::launch<gemm::kStore, false, true>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st);
+  gemm::Operands o;
+  o.A = A; o.lda = lda; o.B = B; o.ldb = ldb;
+  gemm::Params p{};
+  p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc;
+  return gemm::launch<gemm::kStore, false, true>(o, p, st);
 }
 
-// as odb_gemm_bf16_tn_a3 with B = W[K0+K1+K2, N] in its forward layout (dgrad of the fused QKV projection)
+// C[M,N] = [A0 | A1 | A2][M, K0+K1+K2] * W[K0+K1+K2, N] with the three A pieces read in place and W in its forward layout
+// (K0, K1, K2 % 64 == 0; dgrad of the fused QKV projection)
 ODB_EXPORT int odb_gemm_bf16_nn_a3(const void* A0, const void* A1, const void* A2, long long lda0, long long lda1, long long lda2,
                                    int K0, int K1, int K2, const void* B, void* C, int M, int N, long long ldb, long long ldc,
                                    cudaStream_t st) {
   if (K0 % 64 || K1 % 64 || K2 % 64 || K0 <= 0 || K1 <= 0 || K2 <= 0 || N % 8 || ldb % 8) return -1;
-  gemm::ASplit sp;
-  sp.A1 = A1; sp.A2 = A2; sp.lda1 = lda1; sp.lda2 = lda2; sp.K0 = K0; sp.K1 = K1; sp.K2 = K2;
-  return gemm::launch<gemm::kStore, false, true>(A0, B, C, nullptr, M, N, K0 + K1 + K2, lda0, ldb, ldc, 0, 0, 0, 0, nullptr,
-                                                 nullptr, st, sp);
+  gemm::Operands o;
+  o.A = A0; o.lda = lda0; o.B = B; o.ldb = ldb;
+  o.A1 = A1; o.lda1 = lda1; o.A2 = A2; o.lda2 = lda2; o.K0 = K0; o.K1 = K1; o.K2 = K2;
+  gemm::Params p{};
+  p.M = M; p.N = N; p.K = K0 + K1 + K2; p.C = C; p.ldc = ldc;
+  return gemm::launch<gemm::kStore, false, true>(o, p, st);
 }
 
 // as odb_gemm_swiglu_bwd with the down-projection weight Wd[K, I] in its forward layout (MN-major B operand)
 ODB_EXPORT int odb_gemm_swiglu_bwd_nn(const void* dY, const void* Wd, void* gu, int M, int I, int K, long long lda, long long ldb,
                                       cudaStream_t st) {
   if (K % 8 || I % 64 || lda % 8 || ldb % 8) return -1;
-  return gemm::launch<gemm::kSwiGLUBwd, false, true>(dY, Wd, gu, nullptr, M, I, K, lda, ldb, 2 * I, 0, I, 0, 0, nullptr, nullptr, st);
+  gemm::Operands o;
+  o.A = dY; o.lda = lda; o.B = Wd; o.ldb = ldb;
+  gemm::Params p{};
+  p.M = M; p.N = I; p.K = K; p.C = gu; p.ldc = 2 * I; p.I = I;
+  return gemm::launch<gemm::kSwiGLUBwd, false, true>(o, p, st);
 }
 
 // ---------------------------------------------------------------------------------------------------- fused linear-cross-entropy
@@ -937,10 +896,12 @@ ODB_EXPORT int odb_gemm_swiglu_bwd_nn(const void* dY, const void* Wd, void* gu, 
 ODB_EXPORT int odb_lce_fwd(const void* X, const void* W, void* E, int M, int V, int K, long long ldx, long long ldw, long long lde,
                            const void* row_shift, void* partials, int want_sumsq, int store, cudaStream_t st) {
   if (K % 8 || ldx % 8 || ldw % 8 || (store && (lde % 8 || !E))) return -1;
-  gemm::LceArgs a;
-  a.row_shift = (const float*)row_shift; a.partials = (float*)partials; a.want_sumsq = want_sumsq; a.store = store;
-  return gemm::launch<gemm::kLCEFwd, false, false>(X, W, E, nullptr, M, V, K, ldx, ldw, lde, 0, 0, 0, 0, nullptr, nullptr, st,
-                                                   gemm::ASplit(), a);
+  gemm::Operands o;
+  o.A = X; o.lda = ldx; o.B = W; o.ldb = ldw;
+  gemm::Params p{};
+  p.M = M; p.N = V; p.K = K; p.C = E; p.ldc = lde;
+  p.row_shift = (const float*)row_shift; p.partials = (float*)partials; p.want_sumsq = want_sumsq; p.store = store;
+  return gemm::launch<gemm::kLCEFwd, false, false>(o, p, st);
 }
 
 ODB_EXPORT int odb_lce_planes(int V) { return (V + gemm::BN - 1) / gemm::BN; }
@@ -949,11 +910,13 @@ ODB_EXPORT int odb_lce_planes(int V) { return (V + gemm::BN - 1) / gemm::BN; }
 ODB_EXPORT int odb_lce_dx(const void* E, const void* W, void* dX, int M, int N, int V, long long lde, long long ldw, long long ldd,
                           const void* rowscale, const void* labels, const void* gscale, cudaStream_t st) {
   if (V % 8 || N % 64 || lde % 8 || ldw % 8 || ldd % 8) return -1;
-  gemm::LceArgs a;
-  a.rowscale = (const float*)rowscale; a.labels = (const long long*)labels; a.gscale = (const float*)gscale;
-  a.wlab = W; a.ldwlab = ldw;
-  return gemm::launch<gemm::kLCEdX, false, true>(E, W, dX, nullptr, M, N, V, lde, ldw, ldd, 0, 0, 0, 0, nullptr, nullptr, st,
-                                                 gemm::ASplit(), a);
+  gemm::Operands o;
+  o.A = E; o.lda = lde; o.B = W; o.ldb = ldw;
+  gemm::Params p{};
+  p.M = M; p.N = N; p.K = V; p.C = dX; p.ldc = ldd;
+  p.rowscale = (const float*)rowscale; p.labels = (const long long*)labels; p.gscale = (const float*)gscale;
+  p.wlab = (const __nv_bfloat16*)W; p.ldwlab = ldw;
+  return gemm::launch<gemm::kLCEdX, false, true>(o, p, st);
 }
 
 // Scoring statistics of logits Z = X W^T without writing Z: per row and 256-column plane pl (planes = odb_lce_planes(V))
@@ -962,11 +925,12 @@ ODB_EXPORT int odb_lce_dx(const void* E, const void* W, void* dX, int M, int N, 
 ODB_EXPORT int odb_lce_score(const void* X, const void* W, int M, int V, int K, long long ldx, long long ldw, const void* labels,
                              void* pmax, void* psum, void* pidx, void* zlab, cudaStream_t st) {
   if (K % 8 || ldx % 8 || ldw % 8) return -1;
-  gemm::LceArgs a;
-  a.labels = (const long long*)labels;
-  a.sc_max = (float*)pmax; a.sc_sum = (float*)psum; a.sc_idx = (int*)pidx; a.sc_zlab = (float*)zlab;
-  return gemm::launch<gemm::kLCEScore, false, false>(X, W, nullptr, nullptr, M, V, K, ldx, ldw, 0, 0, 0, 0, 0, nullptr, nullptr, st,
-                                                     gemm::ASplit(), a);
+  gemm::Operands o;
+  o.A = X; o.lda = ldx; o.B = W; o.ldb = ldw;
+  gemm::Params p{};
+  p.M = M; p.N = V; p.K = K; p.labels = (const long long*)labels;
+  p.sc_max = (float*)pmax; p.sc_sum = (float*)psum; p.sc_idx = (int*)pidx; p.sc_zlab = (float*)zlab;
+  return gemm::launch<gemm::kLCEScore, false, false>(o, p, st);
 }
 
 // ---------------------------------------------------------------------------------------------------- weight gradient
@@ -980,10 +944,12 @@ ODB_EXPORT int odb_wgrad_bf16(const void* dY0, const void* dY1, const void* dY2,
   const int N_out = n0 + n1 + n2;
   if ((n1 || n2) && (n0 % 256 || n1 % 256 || n2 % 256)) return -1;
   if (ld0 % 8 || ldx % 8 || ldw % 4 || T <= 0) return -1;
-  gemm::ASplit sp;
-  if (n1 || n2) { sp.A1 = dY1; sp.A2 = dY2; sp.lda1 = ld1; sp.lda2 = ld2; sp.K0 = n0; sp.K1 = n1; sp.K2 = n2; }
-  return gemm::launch<gemm::kWgradAcc, true, true>(dY0, X, dW, nullptr, N_out, K_out, T, ld0, ldx, ldw, 0, 0, 0, 0, nullptr,
-                                                   nullptr, st, sp);
+  gemm::Operands o;
+  o.A = dY0; o.lda = ld0; o.B = X; o.ldb = ldx;
+  if (n1 || n2) { o.A1 = dY1; o.A2 = dY2; o.lda1 = ld1; o.lda2 = ld2; o.K0 = n0; o.K1 = n1; o.K2 = n2; }
+  gemm::Params p{};
+  p.M = N_out; p.N = K_out; p.K = T; p.C = dW; p.ldc = ldw;
+  return gemm::launch<gemm::kWgradAcc, true, true>(o, p, st);
 }
 
 // ---------------------------------------------------------------------------------------------------- FP8 (e4m3 / e5m2)
@@ -996,37 +962,48 @@ static bool fp8_ok(int K, long long lda, long long ldb) { return K % 16 == 0 && 
 ODB_EXPORT int odb_gemm_fp8_tn(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
                                int a_e5m2, const void* inv_a, const void* inv_b, cudaStream_t st) {
   if (!fp8_ok(K, lda, ldb) || ldc % 8) return -1;
-  if (a_e5m2)
-    return gemm::launch<gemm::kStore, false, false, 1, 2>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st,
-                                                          gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a, (const float*)inv_b);
-  return gemm::launch<gemm::kStore, false, false, 1, 1>(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, nullptr, nullptr, st,
-                                                        gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a, (const float*)inv_b);
+  gemm::Operands o;
+  o.A = A; o.lda = lda; o.B = B; o.ldb = ldb;
+  gemm::Params p{};
+  p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.inv_a = (const float*)inv_a; p.inv_b = (const float*)inv_b;
+  return a_e5m2 ? gemm::launch<gemm::kStore, false, false, 2>(o, p, st) : gemm::launch<gemm::kStore, false, false, 1>(o, p, st);
 }
 
 // as odb_gemm_qkv_rope with e4m3 x[M,K] and Wqkv[N,K]
 ODB_EXPORT int odb_gemm_fp8_qkv_rope(const void* X, const void* W, void* qkv, int M, int N, int K, int S, int rope_cols,
                                      const void* cos_t, const void* sin_t, const void* inv_a, const void* inv_b, cudaStream_t st) {
   if (!fp8_ok(K, K, K) || N % 64 || rope_cols % 64) return -1;
-  return gemm::launch<gemm::kRoPE, false, false, 1, 1>(X, W, qkv, nullptr, M, N, K, K, K, N, 0, 0, S, rope_cols, (const float*)cos_t,
-                                                       (const float*)sin_t, st, gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a,
-                                                       (const float*)inv_b);
+  gemm::Operands o;
+  o.A = X; o.lda = K; o.B = W; o.ldb = K;
+  gemm::Params p{};
+  p.M = M; p.N = N; p.K = K; p.C = qkv; p.ldc = N;
+  p.S = S; p.rope_cols = rope_cols; p.cos_t = (const float*)cos_t; p.sin_t = (const float*)sin_t;
+  p.inv_a = (const float*)inv_a; p.inv_b = (const float*)inv_b;
+  return gemm::launch<gemm::kRoPE, false, false, 1>(o, p, st);
 }
 
 // as odb_gemm_swiglu with e4m3 x[M,K] and Wgu[2I,K]
 ODB_EXPORT int odb_gemm_fp8_swiglu(const void* X, const void* Wgu, void* gu, void* act, int M, int I, int K, const void* inv_a,
                                    const void* inv_b, cudaStream_t st) {
   if (!fp8_ok(K, K, K) || I % 64) return -1;
-  return gemm::launch<gemm::kSwiGLU, false, false, 1, 1>(X, Wgu, gu, act, M, 2 * I, K, K, K, 2 * I, I, I, 0, 0, nullptr, nullptr, st,
-                                                         gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a, (const float*)inv_b);
+  gemm::Operands o;
+  o.A = X; o.lda = K; o.B = Wgu; o.ldb = K;
+  gemm::Params p{};
+  p.M = M; p.N = 2 * I; p.K = K; p.C = gu; p.ldc = 2 * I; p.aux = act; p.ldaux = I; p.I = I;
+  p.inv_a = (const float*)inv_a; p.inv_b = (const float*)inv_b;
+  return gemm::launch<gemm::kSwiGLU, false, false, 1>(o, p, st);
 }
 
 // as odb_gemm_swiglu_bwd with e5m2 dY[M,K] and e4m3 WdT[I,K] (the transposed down-projection weight)
 ODB_EXPORT int odb_gemm_fp8_swiglu_bwd(const void* dY, const void* WdT, void* gu, int M, int I, int K, long long lda, long long ldb,
                                        const void* inv_a, const void* inv_b, cudaStream_t st) {
   if (!fp8_ok(K, lda, ldb) || I % 64) return -1;
-  return gemm::launch<gemm::kSwiGLUBwd, false, false, 1, 2>(dY, WdT, gu, nullptr, M, I, K, lda, ldb, 2 * I, 0, I, 0, 0, nullptr, nullptr,
-                                                            st, gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a,
-                                                            (const float*)inv_b);
+  gemm::Operands o;
+  o.A = dY; o.lda = lda; o.B = WdT; o.ldb = ldb;
+  gemm::Params p{};
+  p.M = M; p.N = I; p.K = K; p.C = gu; p.ldc = 2 * I; p.I = I;
+  p.inv_a = (const float*)inv_a; p.inv_b = (const float*)inv_b;
+  return gemm::launch<gemm::kSwiGLUBwd, false, false, 2>(o, p, st);
 }
 
 // dW[N_out, K_out] (fp32, row stride ldw) += dYt[N_out, T] * Xt[K_out, T]^T with e5m2 dYt and e4m3 Xt: the transposed
@@ -1034,9 +1011,11 @@ ODB_EXPORT int odb_gemm_fp8_swiglu_bwd(const void* dY, const void* WdT, void* gu
 ODB_EXPORT int odb_wgrad_fp8(const void* dYt, const void* Xt, void* dW, int N_out, int K_out, int T, long long ld_dyt, long long ld_xt,
                              long long ldw, const void* inv_a, const void* inv_b, cudaStream_t st) {
   if (!fp8_ok(T, ld_dyt, ld_xt) || ldw % 4 || T <= 0) return -1;
-  return gemm::launch<gemm::kWgradAcc, false, false, 1, 2>(dYt, Xt, dW, nullptr, N_out, K_out, T, ld_dyt, ld_xt, ldw, 0, 0, 0, 0,
-                                                           nullptr, nullptr, st, gemm::ASplit(), gemm::LceArgs(), (const float*)inv_a,
-                                                           (const float*)inv_b);
+  gemm::Operands o;
+  o.A = dYt; o.lda = ld_dyt; o.B = Xt; o.ldb = ld_xt;
+  gemm::Params p{};
+  p.M = N_out; p.N = K_out; p.K = T; p.C = dW; p.ldc = ldw; p.inv_a = (const float*)inv_a; p.inv_b = (const float*)inv_b;
+  return gemm::launch<gemm::kWgradAcc, false, false, 2>(o, p, st);
 }
 
 // Batched C[b] = alpha * A[b] * B[b]^T + beta * D[b] over `batch` problems stacked along rows: A[b] is [M, K] at row b * M
@@ -1045,18 +1024,22 @@ ODB_EXPORT int odb_wgrad_fp8(const void* dYt, const void* Xt, void* dW, int N_ou
 ODB_EXPORT int odb_gemm_batched_axpby_tn(const void* A, const void* B, void* C, const void* D, int batch, int M, int N, int K,
                                          long long ldc, float alpha, float beta, cudaStream_t st) {
   if (batch <= 0 || M % 64 || N % 64 || K % 64 || ldc % 8 || ldc < N) return -1;
-  gemm::BatchArgs ba;
-  ba.batch = batch; ba.a_rows = M; ba.b_rows = N; ba.c_bstride = (long long)M * ldc; ba.alpha = alpha; ba.beta = beta;
-  return gemm::launch<gemm::kAxpby, false, false>(A, B, C, const_cast<void*>(D), M, N, K, K, K, ldc, ldc, 0, 0, 0, nullptr,
-                                                  nullptr, st, gemm::ASplit(), gemm::LceArgs(), nullptr, nullptr, ba);
+  gemm::Operands o;
+  o.A = A; o.lda = K; o.B = B; o.ldb = K;
+  gemm::Params p{};
+  p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.aux = const_cast<void*>(D); p.ldaux = ldc;
+  p.batch = batch; p.a_rows = M; p.b_rows = N; p.c_bstride = (long long)M * ldc; p.alpha = alpha; p.beta = beta;
+  return gemm::launch<gemm::kAxpby, false, false>(o, p, st);
 }
 
 // as odb_gemm_batched_axpby_tn with B[b] = [K, N] row-major at row b * K of B (MN-major operand): C[b] = alpha A[b] B[b] + beta D[b]
 ODB_EXPORT int odb_gemm_batched_axpby_nn(const void* A, const void* B, void* C, const void* D, int batch, int M, int N, int K,
                                          long long ldc, float alpha, float beta, cudaStream_t st) {
   if (batch <= 0 || M % 64 || N % 64 || K % 64 || ldc % 8 || ldc < N) return -1;
-  gemm::BatchArgs ba;
-  ba.batch = batch; ba.a_rows = M; ba.b_rows = K; ba.c_bstride = (long long)M * ldc; ba.alpha = alpha; ba.beta = beta;
-  return gemm::launch<gemm::kAxpby, false, true>(A, B, C, const_cast<void*>(D), M, N, K, K, N, ldc, ldc, 0, 0, 0, nullptr,
-                                                 nullptr, st, gemm::ASplit(), gemm::LceArgs(), nullptr, nullptr, ba);
+  gemm::Operands o;
+  o.A = A; o.lda = K; o.B = B; o.ldb = N;
+  gemm::Params p{};
+  p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.aux = const_cast<void*>(D); p.ldaux = ldc;
+  p.batch = batch; p.a_rows = M; p.b_rows = K; p.c_bstride = (long long)M * ldc; p.alpha = alpha; p.beta = beta;
+  return gemm::launch<gemm::kAxpby, false, true>(o, p, st);
 }

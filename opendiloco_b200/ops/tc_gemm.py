@@ -20,12 +20,6 @@ _lib.register_optional("odb_gemm_bf16_tn", [c_void_p, c_void_p, c_void_p, c_int,
 _lib.register_optional("odb_gemm_swiglu", [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p])
 _lib.register_optional("odb_gemm_qkv_rope", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p])
 
-for _n in ("odb_gemm2_bf16_tn", "odb_gemm2_swiglu", "odb_gemm2_qkv_rope"):
-    _lib.register_optional(_n, _lib._OPTIONAL_SIGS[_n.replace("gemm2", "gemm")])
-
-_lib.register_optional("odb_gemm_bf16_tn_a3", [c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_void_p, c_void_p,
-                                              c_int, c_int, c_ll, c_ll, c_void_p])
-
 _lib.register_optional("odb_wgrad_bf16", [c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_void_p, c_ll, c_void_p,
                                          c_ll, c_int, c_int, c_void_p])
 
@@ -45,31 +39,6 @@ _lib.register_optional("odb_lce_score", [c_void_p, c_void_p, c_int, c_int, c_int
 SCORE_PLANE = 256                   # vocabulary columns per plane of the scoring statistics (the GEMM's tile width)
 
 ENABLED = os.environ.get("ODB_TC_GEMM", "1") != "0"
-FUSE_SWIGLU_BWD = os.environ.get("ODB_TC_SWIGLU_BWD", "1") != "0"
-# 2-CTA cluster kernels (256x256 tiles, B tile multicast): off by default.  Llama-150M bench.py step, H100 SXM at 700 W,
-# three alternating runs each: 1652-1658 ms with the 1-CTA kernels vs 1728-1740 ms with the cluster kernels (-4.7 %
-# tokens/s): with one 193 KB CTA per SM, co-scheduling CTA pairs costs more than the halved B traffic wins.
-TWO_CTA = os.environ.get("ODB_TC_GEMM_2CTA", "0") == "1"
-
-
-_PAIRS: int | None = None
-
-
-def _pairs() -> int:
-    """CTA pairs the device runs at once (SM count // 2): below one full wave of pair tiles the 128x256 single-CTA tiles
-    fill it better."""
-    global _PAIRS
-    if _PAIRS is None:
-        _PAIRS = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count // 2 if torch.cuda.is_available() else 66
-    return _PAIRS
-
-
-def _fn(name: str, M: int = 1 << 30, N: int = 1 << 30):
-    """2-CTA cluster kernel (256x256 tiles) for problems with at least one full wave of pair tiles, else 128x256 tiles."""
-    lib = _lib.cuda_lib()
-    pair_tiles = ((M + 255) // 256) * ((N + 255) // 256)
-    two = TWO_CTA and pair_tiles >= _pairs()
-    return getattr(lib, name.replace("odb_gemm_", "odb_gemm2_") if two else name)
 
 
 def usable(*tensors: torch.Tensor) -> bool:
@@ -77,8 +46,7 @@ def usable(*tensors: torch.Tensor) -> bool:
     and whose base is 16-byte aligned (TMA reads the operands and stores the output); anything else (e.g. an odd
     vocabulary size, a view starting at an odd column) takes the library GEMM."""
     return ENABLED and all(t.is_cuda and t.dtype == torch.bfloat16 and t.stride(-1) == 1 and t.data_ptr() % 16 == 0 and
-                           (t.dim() < 2 or (t.stride(0) % 8 == 0 and t.shape[-1] % 8 == 0)) for t in tensors) and \
-        _lib.has_symbol("odb_gemm_bf16_tn")
+                           (t.dim() < 2 or (t.stride(0) % 8 == 0 and t.shape[-1] % 8 == 0)) for t in tensors)
 
 
 def linear(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
@@ -86,8 +54,8 @@ def linear(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor | None = None) ->
     N = w.shape[0]
     if out is None:
         out = torch.empty(M, N, dtype=x.dtype, device=x.device)
-    _lib.check(_fn("odb_gemm_bf16_tn", M, N)(x.data_ptr(), w.data_ptr(), out.data_ptr(), M, N, K, x.stride(0), w.stride(0),
-                                                out.stride(0), _lib.stream_ptr(x)), "gemm_bf16_tn")
+    _lib.check(_lib.cuda_lib().odb_gemm_bf16_tn(x.data_ptr(), w.data_ptr(), out.data_ptr(), M, N, K, x.stride(0), w.stride(0),
+                                                 out.stride(0), _lib.stream_ptr(x)), "gemm_bf16_tn")
     _lib.count_launch()
     return out
 
@@ -96,17 +64,17 @@ def linear_swiglu(x: torch.Tensor, w_gu: torch.Tensor, gu: torch.Tensor, act: to
     M, K = x.shape
     I = w_gu.shape[0] // 2
     assert x.is_contiguous() and w_gu.is_contiguous() and gu.is_contiguous() and act.is_contiguous()
-    _lib.check(_fn("odb_gemm_swiglu", M, I // 128 * 256)(x.data_ptr(), w_gu.data_ptr(), gu.data_ptr(), act.data_ptr(), M, I, K,
-                                               _lib.stream_ptr(x)), "gemm_swiglu")
+    _lib.check(_lib.cuda_lib().odb_gemm_swiglu(x.data_ptr(), w_gu.data_ptr(), gu.data_ptr(), act.data_ptr(), M, I, K,
+                                                _lib.stream_ptr(x)), "gemm_swiglu")
     _lib.count_launch()
 
 
 def swiglu_bwd_usable(dy: torch.Tensor, w_down: torch.Tensor, gu: torch.Tensor) -> bool:
     """The fused down-proj dgrad + SwiGLU backward (``w_down`` is the weight in its forward [h, I] layout)."""
-    if not (FUSE_SWIGLU_BWD and usable(dy, w_down, gu)):
+    if not usable(dy, w_down, gu):
         return False
     I = w_down.shape[1]
-    return I % 64 == 0 and gu.is_contiguous() and gu.shape[1] == 2 * I and _lib.has_symbol("odb_gemm_swiglu_bwd_nn")
+    return I % 64 == 0 and gu.is_contiguous() and gu.shape[1] == 2 * I
 
 
 def linear_swiglu_bwd(dy: torch.Tensor, w_down: torch.Tensor, gu: torch.Tensor) -> None:
@@ -130,8 +98,7 @@ def linear_swiglu_bwd_t(dy: torch.Tensor, w_down_t: torch.Tensor, gu: torch.Tens
 
 
 def nn_usable(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor | None = None) -> bool:
-    return (usable(a, b) and (out is None or usable(out)) and b.shape[1] % 8 == 0 and a.shape[1] % 8 == 0
-            and _lib.has_symbol("odb_gemm_bf16_nn"))
+    return usable(a, b) and (out is None or usable(out)) and b.shape[1] % 8 == 0 and a.shape[1] % 8 == 0
 
 
 def linear_nn(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
@@ -160,7 +127,7 @@ def linear_nn_a3(a0: torch.Tensor, a1: torch.Tensor, a2: torch.Tensor, w: torch.
 
 # ------------------------------------------------------------------------------------------------ fused linear-cross-entropy
 def lce_usable(x: torch.Tensor, w: torch.Tensor) -> bool:
-    return usable(x, w) and w.shape[1] % 64 == 0 and w.shape[0] % 8 == 0 and _lib.has_symbol("odb_lce_fwd")
+    return usable(x, w) and w.shape[1] % 64 == 0 and w.shape[0] % 8 == 0
 
 
 def lce_planes(V: int) -> int:
@@ -204,7 +171,7 @@ def lce_score(x: torch.Tensor, w: torch.Tensor, labels: torch.Tensor, pmax: torc
     planes = (V + SCORE_PLANE - 1) // SCORE_PLANE
     assert pmax.numel() >= planes * M and psum.numel() >= planes * M and pidx.numel() >= planes * M and zlab.numel() >= M
     assert pidx.dtype == torch.int32 and labels.dtype == torch.int64 and labels.is_contiguous()
-    if lce_usable(x, w) and _lib.has_symbol("odb_lce_score"):
+    if lce_usable(x, w):
         _lib.check(_lib.cuda_lib().odb_lce_score(x.data_ptr(), w.data_ptr(), M, V, x.shape[1], x.stride(0), w.stride(0), labels.data_ptr(),
                                                  pmax.data_ptr(), psum.data_ptr(), pidx.data_ptr(), zlab.data_ptr(), _lib.stream_ptr(x)),
                    "lce_score")
@@ -227,27 +194,13 @@ def linear_qkv_rope(x: torch.Tensor, w: torch.Tensor, qkv: torch.Tensor, cos: to
     M, K = x.shape
     N = w.shape[0]
     assert x.is_contiguous() and w.is_contiguous() and qkv.is_contiguous() and cos.shape[1] == 32
-    _lib.check(_fn("odb_gemm_qkv_rope", M, N)(x.data_ptr(), w.data_ptr(), qkv.data_ptr(), M, N, K, S, rope_cols, cos.data_ptr(),
-                                                 sin.data_ptr(), _lib.stream_ptr(x)), "gemm_qkv_rope")
+    _lib.check(_lib.cuda_lib().odb_gemm_qkv_rope(x.data_ptr(), w.data_ptr(), qkv.data_ptr(), M, N, K, S, rope_cols, cos.data_ptr(),
+                                                  sin.data_ptr(), _lib.stream_ptr(x)), "gemm_qkv_rope")
     _lib.count_launch()
-
-
-def linear_a3(a0: torch.Tensor, a1: torch.Tensor, a2: torch.Tensor, w: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
-    """out = cat([a0, a1, a2], dim=1) @ w^T with the three A pieces read in place (dq|dk|dv -> dgrad of the fused QKV)."""
-    M = a0.shape[0]
-    N = w.shape[0]
-    _lib.check(_lib.cuda_lib().odb_gemm_bf16_tn_a3(a0.data_ptr(), a1.data_ptr(), a2.data_ptr(), a0.stride(0), a1.stride(0),
-                                                    a2.stride(0), a0.shape[1], a1.shape[1], a2.shape[1], w.data_ptr(), out.data_ptr(),
-                                                    M, N, w.stride(0), out.stride(0), _lib.stream_ptr(out)), "gemm_bf16_tn_a3")
-    _lib.count_launch()
-    return out
-
-
-WGRAD = os.environ.get("ODB_TC_WGRAD", "1") != "0"
 
 
 def wgrad_usable(*tensors: torch.Tensor) -> bool:
-    return WGRAD and usable(*tensors) and _lib.has_symbol("odb_wgrad_bf16")
+    return usable(*tensors)
 
 
 def wgrad_acc(dy, x: torch.Tensor, dw: torch.Tensor) -> None:

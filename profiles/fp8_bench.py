@@ -47,7 +47,7 @@ def time_steps(model, ids, steps: int, warmup: int) -> float:
 
 
 def classify(name: str) -> str:
-    if re.search(r"gemm_kernel<\d+, false, false, 1, [12]>", name):      # demangled FP8 instantiations
+    if re.search(r"gemm_kernel<\d+, false, false, [12]>", name):      # demangled FP8 instantiations
         return "fp8 GEMM"
     if "amax_kernel" in name or "cast_kernel" in name:
         return "fp8 amax/cast"

@@ -1,5 +1,4 @@
-"""wgmma GEMM family (1-CTA and 2-CTA cluster kernels, fused SwiGLU / RoPE epilogues, weight gradient, MN-major operands)
-against fp32 PyTorch references."""
+"""wgmma GEMM family (fused SwiGLU / RoPE epilogues, weight gradient, MN-major operands) against fp32 PyTorch references."""
 import pytest
 import torch
 
@@ -14,14 +13,9 @@ def rel(a, b):
     return ((a.float() - b.float()).norm() / (b.float().norm() + 1e-12)).item()
 
 
-@pytest.fixture(params=[False, True], ids=["1cta", "2cta"])
-def two_cta(request, monkeypatch):
-    monkeypatch.setattr(T, "TWO_CTA", request.param)
-    return request.param
-
-
-@pytest.mark.parametrize("M,N,Kd", [(128, 256, 64), (300, 520, 200), (1000, 136, 72), (4096, 1024, 1024), (20000, 768, 2688)])
-def test_linear_matches_fp32(two_cta, M, N, Kd):
+@pytest.mark.parametrize("M,N,Kd", [(128, 256, 64), (300, 520, 200), (1000, 136, 72), (4096, 1024, 1024), (20000, 768, 2688),
+                                    (256, 128, 128), (513, 264, 136), (2048, 2048, 512), (8192, 2304, 768), (16384, 1024, 256)])
+def test_linear_matches_fp32(M, N, Kd):
     torch.manual_seed(0)
     x = torch.randn(M, Kd, device="cuda").to(BF)
     w = (torch.randn(N, Kd, device="cuda") * 0.1).to(BF)
@@ -31,19 +25,21 @@ def test_linear_matches_fp32(two_cta, M, N, Kd):
     assert torch.equal(out, torch.mm(x, w.t()))        # same fp32 accumulation + single bf16 rounding as cuBLAS
 
 
-def test_linear_strided_views(two_cta):
+@pytest.mark.parametrize("M,c0,N", [(600, 256, 320), (1000, 128, 200)])
+def test_linear_strided_views(M, c0, N):
     torch.manual_seed(1)
-    big = torch.randn(600, 1024, device="cuda").to(BF)
-    x = big[:, 256:768]                                  # row stride 1024, 512 columns
-    w = (torch.randn(320, 512, device="cuda") * 0.1).to(BF)
-    outbuf = torch.zeros(600, 640, device="cuda", dtype=BF)
-    T.linear(x, w, outbuf[:, 320:])
-    assert rel(outbuf[:, 320:], x.float() @ w.float().t()) < 4e-3
-    assert torch.count_nonzero(outbuf[:, :320]) == 0     # TMA store clipped to the view
+    big = torch.randn(M, 1024, device="cuda").to(BF)
+    x = big[:, c0:c0 + 512]                              # row stride 1024, 512 columns
+    w = (torch.randn(N, 512, device="cuda") * 0.1).to(BF)
+    outbuf = torch.zeros(M, 2 * N, device="cuda", dtype=BF)
+    T.linear(x, w, outbuf[:, N:])
+    assert rel(outbuf[:, N:], x.float() @ w.float().t()) < 4e-3
+    assert torch.count_nonzero(outbuf[:, :N]) == 0       # TMA store clipped to the view
 
 
-@pytest.mark.parametrize("M,I,Kd", [(256, 128, 64), (777, 384, 192), (20000, 2688, 1024)])
-def test_swiglu_epilogue(two_cta, M, I, Kd):
+@pytest.mark.parametrize("M,I,Kd", [(256, 128, 64), (777, 384, 192), (20000, 2688, 1024), (300, 192, 136), (1024, 640, 256),
+                                    (4096, 1408, 512)])
+def test_swiglu_epilogue(M, I, Kd):
     torch.manual_seed(2)
     x = torch.randn(M, Kd, device="cuda").to(BF)
     w = (torch.randn(2 * I, Kd, device="cuda") * 0.1).to(BF)
@@ -55,8 +51,9 @@ def test_swiglu_epilogue(two_cta, M, I, Kd):
     assert rel(act, torch.nn.functional.silu(g) * u) < 4e-3
 
 
-@pytest.mark.parametrize("B,S,Hq,Hkv,Kd", [(2, 128, 4, 4, 256), (3, 256, 8, 2, 512), (16, 1024, 16, 16, 1024)])
-def test_qkv_rope_epilogue(two_cta, B, S, Hq, Hkv, Kd):
+@pytest.mark.parametrize("B,S,Hq,Hkv,Kd", [(2, 128, 4, 4, 256), (3, 256, 8, 2, 512), (16, 1024, 16, 16, 1024), (1, 64, 2, 1, 128),
+                                             (5, 200, 6, 3, 320), (4, 512, 12, 4, 768)])
+def test_qkv_rope_epilogue(B, S, Hq, Hkv, Kd):
     torch.manual_seed(3)
     M, N = B * S, (Hq + 2 * Hkv) * 64
     x = torch.randn(M, Kd, device="cuda").to(BF)
