@@ -6,12 +6,16 @@
 //   odb_dec_kv_fill       prefill: copy the (already rotated) k|v columns of the packed qkv rows into the cache
 //   odb_dec_attn          split-KV decode attention (flash-decoding) + a combine kernel
 //   odb_dec_sample        greedy / temperature + top-k + top-p sampler, one CTA per row
+//   odb_dec_beam_topk     beam search: per vocabulary split of a row, the (max, sum-exp) partial and the local top-K logits
+//   odb_dec_beam_step     beam search: one CTA per prompt merges the candidates and does HF's selection and bookkeeping
+//   odb_dec_beam_reorder  beam search: chunk-table update and partial-chunk K/V copy for beams that changed parent
 //
 // KV cache layout, per layer: K and V each [B, Hkv, Smax, 64] bf16, so the keys of one (row, kv head) are contiguous and a
 // chunk of them is ONE bulk copy.
 #include <curand_kernel.h>
 
 #include <algorithm>
+#include <climits>
 
 #include "common.cuh"
 #include "sm90_ptx.cuh"
@@ -82,10 +86,10 @@ rope_append_multi_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const fl
 }
 
 // ------------------------------------------------------------------------------------------------ prefill cache fill
-// grid (Sp, B), block 128: row s < len[b] of batch row b: 16-byte copies of the k and v heads.
+// grid (Sp, B), block 128: row s < len[b] of batch row b -> cache row b * row_stride: 16-byte copies of the k and v heads.
 __global__ void __launch_bounds__(128)
 kv_fill_kernel(const __nv_bfloat16* __restrict__ qkv, long long ld, const int* __restrict__ len, __nv_bfloat16* __restrict__ kc,
-               __nv_bfloat16* __restrict__ vc, int Sp, int Hq, int Hkv, int Smax) {
+               __nv_bfloat16* __restrict__ vc, int Sp, int Hq, int Hkv, int Smax, int row_stride) {
   pdl_launch_dependents();
   pdl_wait();
   const int s = blockIdx.x, b = blockIdx.y;
@@ -94,7 +98,7 @@ kv_fill_kernel(const __nv_bfloat16* __restrict__ qkv, long long ld, const int* _
   for (int i = threadIdx.x; i < 2 * Hkv * (D / 8); i += blockDim.x) {
     const int kv = i / (Hkv * (D / 8)), r = i % (Hkv * (D / 8)), hk = r / (D / 8), c = r % (D / 8);
     const uint4 v = ld_nc_v4(row + (kv * Hkv + hk) * D + c * 8);
-    __nv_bfloat16* dst = (kv ? vc : kc) + (((long long)b * Hkv + hk) * Smax + s) * D + c * 8;
+    __nv_bfloat16* dst = (kv ? vc : kc) + (((long long)b * row_stride * Hkv + hk) * Smax + s) * D + c * 8;
     st_v4(dst, v);
   }
 }
@@ -103,7 +107,8 @@ kv_fill_kernel(const __nv_bfloat16* __restrict__ qkv, long long ld, const int* _
 // grid (ceil(Smax / CH), Hkv, B), block 128.  CTA (c, hk, b) serves the G = Hq / Hkv query heads of kv head hk against keys
 // [c*CH, min((c+1)*CH, pos[b]+1)) of row b: K and V of the chunk arrive by two bulk copies, scores are one thread per key,
 // P V is one warp per 32 keys (lanes over dimension pairs) summed across the four warps.  Writes the unnormalised partial
-// output and its (max, sum) in the log2 domain; chunks past the row's length exit at once.
+// output and its (max, sum) in the log2 domain; chunks past the row's length exit at once.  With a chunk table (beam
+// search), the keys of chunk c of row b are read from physical row table[b * nchunks + c]; without one, from row b.
 template <int G>
 struct AttSmem {
   static constexpr int K_OFF = 0;
@@ -120,7 +125,7 @@ template <int G>
 __global__ void __launch_bounds__(ATT_THREADS)
 decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __nv_bfloat16* __restrict__ kc,
                    const __nv_bfloat16* __restrict__ vc, const int* __restrict__ pos, float* __restrict__ part_o,
-                   float* __restrict__ part_ml, int Hkv, int Smax, int nchunks, float scale_log2) {
+                   float* __restrict__ part_ml, const int* __restrict__ table, int Hkv, int Smax, int nchunks, float scale_log2) {
   using L = AttSmem<G>;
   extern __shared__ __align__(128) uint8_t smem[];
   __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(smem + L::K_OFF);
@@ -144,7 +149,8 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __n
   const int j0 = c * CH;
   if (j0 >= len) return;                         // uniform over the CTA
   const int n = min(CH, len - j0);
-  const long long kv_off = (((long long)b * Hkv + hk) * Smax + j0) * D;
+  const int phys = table != nullptr ? table[b * nchunks + c] : b;
+  const long long kv_off = (((long long)phys * Hkv + hk) * Smax + j0) * D;
   if (tid == 0) {
     mbar_arrive_expect_tx(bar, 2u * n * D * 2);
     bulk_load_1d(sK, kc + kv_off, n * D * 2, bar);
@@ -291,11 +297,9 @@ __device__ uint32_t bisect_threshold(const float* e, int V, float target, float*
   return lo;
 }
 
-// Block-wide argmax of a bf16 row (ties to the lowest index); am: 32 shared slots.  Every thread gets the result.
-__device__ ArgMax block_argmax(const __nv_bfloat16* __restrict__ row, int V, ArgMax* am) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  ArgMax best = {-INFINITY, V};
-  for (int i = tid; i < V; i += blockDim.x) best = argmax_merge(best, ArgMax{__bfloat162float(row[i]), i});
+// Block-wide argmax_merge of one (value, index) per thread; am: 32 shared slots.  Every thread gets the result.
+__device__ ArgMax block_reduce_argmax(ArgMax best, ArgMax* am) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     ArgMax other{__shfl_xor_sync(0xffffffffu, best.v, o), __shfl_xor_sync(0xffffffffu, best.i, o)};
@@ -305,7 +309,7 @@ __device__ ArgMax block_argmax(const __nv_bfloat16* __restrict__ row, int V, Arg
   if (lane == 0) am[warp] = best;
   __syncthreads();
   if (warp == 0) {
-    best = am[lane];
+    best = lane < (int)(blockDim.x >> 5) ? am[lane] : ArgMax{-INFINITY, INT_MAX};
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       ArgMax other{__shfl_xor_sync(0xffffffffu, best.v, o), __shfl_xor_sync(0xffffffffu, best.i, o)};
@@ -314,7 +318,14 @@ __device__ ArgMax block_argmax(const __nv_bfloat16* __restrict__ row, int V, Arg
     if (lane == 0) am[0] = best;
   }
   __syncthreads();
-  best = am[0];
+  return am[0];
+}
+
+// Block-wide argmax of a bf16 row (ties to the lowest index); am: 32 shared slots.  Every thread gets the result.
+__device__ ArgMax block_argmax(const __nv_bfloat16* __restrict__ row, int V, ArgMax* am) {
+  ArgMax best = {-INFINITY, V};
+  for (int i = threadIdx.x; i < V; i += blockDim.x) best = argmax_merge(best, ArgMax{__bfloat162float(row[i]), i});
+  best = block_reduce_argmax(best, am);
   if (best.i >= V) best.i = 0;                   // all-NaN row: token 0 rather than an out-of-range id
   return best;
 }
@@ -736,9 +747,286 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
   }
 }
 
+// ------------------------------------------------------------------------------------------------ beam search
+// Deterministic beam search as transformers' GenerationMixin._beam_search (do_sample=False), one step per generated token:
+// beam_topk + beam_step select, beam_reorder shares the history of the selected parents through a per-row chunk table.
+constexpr int MAX_BEAMS = 8;
+constexpr int MAX_KEEP = (1 + MAX_EOS) * MAX_BEAMS;  // beams_to_keep = max(2, 1 + n_eos) * num_beams
+constexpr int MAX_TABLE = 256;                       // chunks of 128 positions per row: Smax <= 32768
+constexpr int TOPK_THREADS = 128;
+constexpr int TOPK_PER = 8;
+constexpr int TOPK_SPLIT = TOPK_THREADS * TOPK_PER;  // vocabulary entries per beam_topk CTA
+constexpr int STEP_THREADS = 512;                    // beam_step: one thread per (beam, split) candidate list
+constexpr float NEG = -1.0e9f;                       // HF's score offset of a continuation that must not be chosen
+
+// grid (splits, rows), block 128.  Split s of row r is logits[r, s*1024 .. s*1024 + 1024); thread t holds entries
+// s*1024 + 128*e + t in registers.  Writes part_ml[r][s] = (max, sum exp(x - max)) in fp32 and cand[r][s][0..K) = the
+// split's K largest logits, by value descending and then index ascending (index -1, value -inf past the split's end).
+// Within one row this is also the order of the log-probabilities.
+__global__ void __launch_bounds__(TOPK_THREADS)
+beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, int K, float* __restrict__ part_ml,
+                 float* __restrict__ cand_v, int* __restrict__ cand_i) {
+  __shared__ float red[33];
+  __shared__ ArgMax am[32];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int s = blockIdx.x, r = blockIdx.y, ns = gridDim.x, tid = threadIdx.x;
+  const int base = s * TOPK_SPLIT;
+  const __nv_bfloat16* row = logits + (long long)r * ld;
+  float x[TOPK_PER];
+  float mx = -INFINITY;
+#pragma unroll
+  for (int e = 0; e < TOPK_PER; ++e) {
+    const int i = base + e * TOPK_THREADS + tid;
+    const float v = i < V ? __bfloat162float(row[i]) : -INFINITY;
+    x[e] = v == v ? v : -INFINITY;               // NaN is never preferred
+    mx = fmaxf(mx, x[e]);
+  }
+  mx = block_max(mx, red);
+  float se = 0.f;
+  if (mx > -INFINITY) {
+#pragma unroll
+    for (int e = 0; e < TOPK_PER; ++e) se += expf(x[e] - mx);
+  }
+  se = block_sum(se, red);
+  const long long rs = (long long)r * ns + s;
+  if (tid == 0) {
+    part_ml[2 * rs] = mx;
+    part_ml[2 * rs + 1] = se;
+  }
+  unsigned taken = 0u;                           // bit e: entry e of this thread is already a candidate
+  for (int k = 0; k < K; ++k) {
+    ArgMax best{-INFINITY, INT_MAX};
+#pragma unroll
+    for (int e = 0; e < TOPK_PER; ++e) {
+      const int i = base + e * TOPK_THREADS + tid;
+      if (i < V && !((taken >> e) & 1u)) best = argmax_merge(best, ArgMax{x[e], i});
+    }
+    best = block_reduce_argmax(best, am);
+    const bool none = best.i == INT_MAX;
+    if (!none && (best.i - base) % TOPK_THREADS == tid) taken |= 1u << ((best.i - base) / TOPK_THREADS);
+    if (tid == 0) {
+      cand_v[rs * K + k] = none ? -INFINITY : best.v;
+      cand_i[rs * K + k] = none ? -1 : best.i;
+    }
+  }
+}
+
+// One CTA per prompt g, whose beams are rows g*nb .. g*nb + nb-1.  One step of HF's beam search (t = tokens generated so
+// far, tstep[g]):
+//   c. score = logit - lse(row) + run_score(row); the K best over all beams (ties: lower beam * V + token), by a K-way
+//      merge of the nb * splits sorted lists of beam_topk
+//   d. a candidate hits the stopping criteria if its token is an EOS id (ictl, as the sampler) or t + 1 == max_new
+//   e. the next running beams: the nb best of score + hit * -1e9
+//   f. the finished hypotheses: the nb best of the old ones and score / (t+1)^length_penalty, plus -1e9 when the prompt's
+//      finished set is full (early_stopping True), when the early-stop heuristic is satisfied, and for every candidate that
+//      is not among the first nb or did not hit the stopping criteria
+//   g. the early-stop heuristic (early_stopping: 0 False, 1 True, 2 "never") and done[g]
+// Histories are int32 [2][rows][max_new], double-buffered by the parity of t: step t reads buffer t & 1 and writes the
+// other one, so beams may swap parents.  Writes ids_next / parent (global row) / run_score of the new running beams, pos
+// += 1, and the finished scores, flags and histories.  A prompt that is done is left untouched (parents = itself).
+__global__ void __launch_bounds__(STEP_THREADS)
+beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ cand_v, const int* __restrict__ cand_i, int ns, int V,
+                 int nb, int K, const long long* __restrict__ ictl, float length_penalty, int early_stopping, int max_new,
+                 float* __restrict__ run_score, float* __restrict__ fin_score, int* __restrict__ fin_flag, int* __restrict__ run_seq,
+                 int* __restrict__ fin_seq, int* __restrict__ unsat, int* __restrict__ done, int* __restrict__ tstep,
+                 int* __restrict__ pos, long long* __restrict__ ids_next, int* __restrict__ parent) {
+  __shared__ ArgMax am[32];
+  __shared__ float lse[MAX_BEAMS];
+  __shared__ float sel_v[MAX_KEEP], fcand[MAX_KEEP];
+  __shared__ int sel_f[MAX_KEEP], hit[MAX_KEEP], taken[MAX_BEAMS + MAX_KEEP];
+  __shared__ int run_src[MAX_BEAMS], fin_src[MAX_BEAMS], new_ff[MAX_BEAMS];
+  __shared__ float new_rs[MAX_BEAMS], new_fs[MAX_BEAMS];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int g = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int row0 = g * nb;
+  if (done[g]) {
+    if (tid < nb) parent[row0 + tid] = row0 + tid;
+    return;
+  }
+  const int t = tstep[g];
+
+  // ---- log-sum-exp of each beam row from the split partials: warp j takes row j
+  if (warp < nb) {
+    const float* ml = part_ml + (long long)(row0 + warp) * ns * 2;
+    float m = -INFINITY;
+    for (int s = lane; s < ns; s += 32) m = fmaxf(m, ml[2 * s]);
+    m = warp_max(m);
+    float z = 0.f;
+    for (int s = lane; s < ns; s += 32)
+      if (ml[2 * s] > -INFINITY) z += ml[2 * s + 1] * expf(ml[2 * s] - m);
+    z = warp_sum(z);
+    if (lane == 0) lse[warp] = m + logf(z);
+  }
+  __syncthreads();
+
+  // ---- c. K-way merge: thread l owns the sorted list of beam l / ns, split l % ns; its head advances when it wins
+  const int nl = nb * ns, jb = tid / ns, sp = tid % ns;
+  int head = 0;
+  for (int k = 0; k < K; ++k) {
+    ArgMax c{-INFINITY, INT_MAX};
+    if (tid < nl && head < K) {
+      const long long at = ((long long)(row0 + jb) * ns + sp) * K + head;
+      const int ci = cand_i[at];
+      if (ci >= 0) c = ArgMax{(cand_v[at] - lse[jb]) + run_score[row0 + jb], jb * V + ci};
+    }
+    const ArgMax w = block_reduce_argmax(c, am);
+    if (tid < nl && c.i != INT_MAX && w.i == c.i) ++head;     // beam * V + token is unique to one list
+    if (tid == 0) {
+      sel_v[k] = w.v;
+      sel_f[k] = w.i;
+    }
+  }
+  __syncthreads();
+
+  // ---- d-g: K <= 72 candidates and nb <= 8 beams, one thread
+  if (tid == 0) {
+    const int n_eos = (int)min(ictl[4], (long long)MAX_EOS);
+    const bool last = t + 1 >= max_new;
+    for (int k = 0; k < K; ++k) {
+      const long long tok = sel_f[k] % V;
+      bool h = last;
+      for (int e = 0; e < n_eos; ++e) h = h || tok == ictl[5 + e];
+      hit[k] = h;
+      taken[k] = 0;
+    }
+    // e. running beams: the nb best of score + hit * -1e9, ties to the lower candidate
+    for (int j = 0; j < nb; ++j) {
+      int bk = -1;
+      float bv = -INFINITY;
+      for (int k = 0; k < K; ++k) {
+        if (taken[k]) continue;
+        const float v = hit[k] ? sel_v[k] + NEG : sel_v[k];
+        if (bk < 0 || v > bv) { bk = k; bv = v; }
+      }
+      taken[bk] = 1;
+      run_src[j] = bk;
+      new_rs[j] = bv;
+    }
+    // f. finished hypotheses: merge the old nb with the K candidates, keep the nb best (ties to the lower merged index)
+    const float denom = (float)pow((double)(t + 1), (double)length_penalty);
+    bool full = early_stopping == 1;
+    for (int j = 0; j < nb; ++j) full = full && fin_flag[row0 + j] != 0;
+    const bool uns = unsat[g] != 0;
+    for (int k = 0; k < K; ++k) {
+      float f = __fdiv_rn(sel_v[k], denom);
+      if (full) f += NEG;
+      if (!uns) f += NEG;
+      if (!(hit[k] && k < nb)) f += NEG;
+      fcand[k] = f;
+    }
+    for (int m = 0; m < nb + K; ++m) taken[m] = 0;
+    for (int j = 0; j < nb; ++j) {
+      int bm = -1;
+      float bv = -INFINITY;
+      for (int m = 0; m < nb + K; ++m) {
+        if (taken[m]) continue;
+        const float v = m < nb ? fin_score[row0 + m] : fcand[m - nb];
+        if (bm < 0 || v > bv) { bm = m; bv = v; }
+      }
+      taken[bm] = 1;
+      fin_src[j] = bm;
+      new_fs[j] = bv;
+      new_ff[j] = bm < nb ? fin_flag[row0 + bm] != 0 : (hit[bm - nb] && bm - nb < nb);
+    }
+    // g. early-stop heuristic on the new running and finished beams, at length t + 1
+    const int best_len = (early_stopping == 2 && length_penalty > 0.f) ? max_new : t + 1;
+    const float best_possible = __fdiv_rn(new_rs[0], (float)pow((double)best_len, (double)length_penalty));
+    float worst = new_fs[0];
+    bool all_fin = true;
+    for (int j = 0; j < nb; ++j) {
+      worst = fminf(worst, new_fs[j]);
+      all_fin = all_fin && new_ff[j];
+    }
+    bool improvable = false;
+    for (int j = 0; j < nb; ++j) improvable = improvable || best_possible > (new_ff[j] ? worst : NEG);
+    const bool u = uns && improvable;
+    unsat[g] = u;
+    done[g] = !u || (early_stopping == 1 && all_fin) || last;
+  }
+  __syncthreads();
+
+  // ---- histories [0, t] of the new running and finished beams, gathered through their sources
+  const long long M = max_new, rows = (long long)gridDim.x * nb;
+  const int* rsrc = run_seq + (t & 1) * rows * M;
+  int* rdst = run_seq + ((t & 1) ^ 1) * rows * M;
+  const int* fsrc = fin_seq + (t & 1) * rows * M;
+  int* fdst = fin_seq + ((t & 1) ^ 1) * rows * M;
+  const int n = t + 1;
+  for (int i = tid; i < nb * n; i += blockDim.x) {
+    const int j = i / n, c = i % n;
+    const int f = sel_f[run_src[j]];
+    rdst[(row0 + j) * M + c] = c < t ? rsrc[(row0 + f / V) * M + c] : f % V;
+    const int m = fin_src[j];
+    int v;
+    if (m < nb) {
+      v = fsrc[(row0 + m) * M + c];
+    } else {
+      const int fk = sel_f[m - nb];
+      v = c < t ? rsrc[(row0 + fk / V) * M + c] : fk % V;
+    }
+    fdst[(row0 + j) * M + c] = v;
+  }
+  if (tid < nb) {
+    const int f = sel_f[run_src[tid]];
+    run_score[row0 + tid] = new_rs[tid];
+    parent[row0 + tid] = row0 + f / V;
+    ids_next[row0 + tid] = f % V;
+    pos[row0 + tid] += 1;
+    fin_score[row0 + tid] = new_fs[tid];
+    fin_flag[row0 + tid] = new_ff[tid];
+  }
+  if (tid == 0) tstep[g] = t + 1;
+}
+
+// grid (L * 2 * Hkv, B), block 256, dynamic shared memory nb * CH * 64 * 2 bytes.  kv [L][2][rows][Hkv][Smax][64]: CTA
+// (x, g) serves slab x / Hkv (a layer's K or V) and kv head x % Hkv of prompt g, whose beams all sit at position p =
+// pos[g*nb].  Chunks c < p / CH are complete and never written again, so a child whose parent is another row takes the
+// parent's table entries for them; only the partial chunk [CH * (p / CH), p) is copied, from the parent's row (which owns
+// its current chunk) to the child's own row, and the child's entry for that chunk becomes itself.  Every source is staged
+// in shared memory before any destination is written (beams may swap parents); the table is updated by the CTAs x = 0.
+// generate() ends with p = P + max_new_tokens - 1 < Smax; a position of Smax (a full cache) copies nothing and writes
+// only entries below Smax / CH.
+__global__ void __launch_bounds__(256)
+beam_reorder_kernel(__nv_bfloat16* __restrict__ kv, int* __restrict__ table, const int* __restrict__ parent,
+                    const int* __restrict__ pos, int nb, int Hkv, int Smax, int nchunks) {
+  extern __shared__ __align__(16) uint4 stage[];  // [nb][CH * D / 8]
+  __shared__ int tstage[MAX_BEAMS * MAX_TABLE];
+  constexpr int RV = D / 8;                      // 16-byte pieces per position
+  pdl_launch_dependents();
+  pdl_wait();
+  const int slab = blockIdx.x / Hkv, hk = blockIdx.x % Hkv, g = blockIdx.y, tid = threadIdx.x;
+  const long long rows = (long long)gridDim.y * nb;
+  const int row0 = g * nb;
+  const int p = pos[row0], c = p / CH, n = p - c * CH;
+  __nv_bfloat16* base = kv + (long long)slab * rows * Hkv * Smax * D;
+  for (int j = 0; j < nb; ++j) {
+    const int par = parent[row0 + j];
+    if (par == row0 + j) continue;
+    const uint4* src = reinterpret_cast<const uint4*>(base + (((long long)par * Hkv + hk) * Smax + c * CH) * D);
+    for (int i = tid; i < n * RV; i += blockDim.x) stage[j * CH * RV + i] = src[i];
+  }
+  if (blockIdx.x == 0)
+    for (int i = tid; i < nb * c; i += blockDim.x) tstage[i] = table[parent[row0 + i / c] * nchunks + i % c];
+  __syncthreads();
+  for (int j = 0; j < nb; ++j) {
+    if (parent[row0 + j] == row0 + j) continue;
+    uint4* dst = reinterpret_cast<uint4*>(base + (((long long)(row0 + j) * Hkv + hk) * Smax + c * CH) * D);
+    for (int i = tid; i < n * RV; i += blockDim.x) dst[i] = stage[j * CH * RV + i];
+  }
+  if (blockIdx.x == 0) {
+    for (int i = tid; i < nb * (c + 1); i += blockDim.x) {
+      const int j = i / (c + 1), cc = i % (c + 1);
+      if (parent[row0 + j] == row0 + j || cc >= nchunks) continue;   // p == Smax: no current chunk to point at
+      table[(row0 + j) * nchunks + cc] = cc < c ? tstage[j * c + cc] : row0 + j;
+    }
+  }
+}
+
 template <int G>
 int launch_attn(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml, void* out,
-                long long ldo, int B, int Hkv, int Smax, float scale, cudaStream_t st) {
+                long long ldo, const void* table, int B, int Hkv, int Smax, float scale, cudaStream_t st) {
   static bool attr_set = false;
   const int smem = AttSmem<G>::BYTES;
   if (!attr_set) {
@@ -748,8 +1036,8 @@ int launch_attn(const void* q, long long ldq, const void* kc, const void* vc, co
   }
   const int nchunks = ceil_div(Smax, CH);
   launch_pdl(decode_attn_kernel<G>, dim3(nchunks, Hkv, B), dim3(ATT_THREADS), smem, st, (const __nv_bfloat16*)q, ldq,
-             (const __nv_bfloat16*)kc, (const __nv_bfloat16*)vc, (const int*)pos, (float*)part_o, (float*)part_ml, Hkv, Smax,
-             nchunks, scale * 1.4426950408889634f);
+             (const __nv_bfloat16*)kc, (const __nv_bfloat16*)vc, (const int*)pos, (float*)part_o, (float*)part_ml, (const int*)table, Hkv,
+             Smax, nchunks, scale * 1.4426950408889634f);
   ODB_CHECK_LAST();
   launch_pdl(decode_combine_kernel, dim3(Hkv * G, B), dim3(D), 0, st, (const float*)part_o, (const float*)part_ml, (const int*)pos,
              (__nv_bfloat16*)out, ldo, nchunks);
@@ -769,12 +1057,12 @@ ODB_EXPORT int odb_dec_rope_append(void* qkv, long long ld, const void* cos_t, c
   return 0;
 }
 
-// qkv [B*Sp, ld] bf16 (rotated prefill projections); len int32 [B]: rows s < len[b] are copied into the cache
+// qkv [B*Sp, ld] bf16 (rotated prefill projections); len int32 [B]: rows s < len[b] are copied into cache row b * row_stride
 ODB_EXPORT int odb_dec_kv_fill(const void* qkv, long long ld, const void* len, void* kc, void* vc, int B, int Sp, int Hq, int Hkv,
-                               int Smax, cudaStream_t st) {
-  if (ld % 8) return -1;
+                               int Smax, int row_stride, cudaStream_t st) {
+  if (ld % 8 || row_stride < 1) return -1;
   launch_pdl(dec::kv_fill_kernel, dim3(Sp, B), dim3(128), 0, st, (const __nv_bfloat16*)qkv, ld, (const int*)len, (__nv_bfloat16*)kc,
-             (__nv_bfloat16*)vc, Sp, Hq, Hkv, Smax);
+             (__nv_bfloat16*)vc, Sp, Hq, Hkv, Smax, row_stride);
   ODB_CHECK_LAST();
   return 0;
 }
@@ -783,15 +1071,17 @@ ODB_EXPORT int odb_dec_kv_fill(const void* qkv, long long ld, const void* len, v
 ODB_EXPORT int odb_dec_attn_chunks(int Smax) { return odb::ceil_div(Smax, dec::CH); }
 
 // q [B, ldq] bf16 (the q heads first); kc/vc [B, Hkv, Smax, 64]; pos int32 [B] (keys 0..pos[b] are attended);
-// part_o fp32 [B, Hq, chunks, 64]; part_ml fp32 [B, Hq, chunks, 2]; out [B, ldo] bf16
+// part_o fp32 [B, Hq, chunks, 64]; part_ml fp32 [B, Hq, chunks, 2]; out [B, ldo] bf16; table: nullptr, or int32 [B, chunks]
+// (chunk c of row b is read from physical cache row table[b][c])
 ODB_EXPORT int odb_dec_attn(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml,
-                            void* out, long long ldo, int B, int Hq, int Hkv, int Smax, float softmax_scale, cudaStream_t st) {
+                            void* out, long long ldo, const void* table, int B, int Hq, int Hkv, int Smax, float softmax_scale,
+                            cudaStream_t st) {
   if (Hq % Hkv || ldq % 8) return -1;
   switch (Hq / Hkv) {
-    case 1: return dec::launch_attn<1>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, B, Hkv, Smax, softmax_scale, st);
-    case 2: return dec::launch_attn<2>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, B, Hkv, Smax, softmax_scale, st);
-    case 4: return dec::launch_attn<4>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, B, Hkv, Smax, softmax_scale, st);
-    case 8: return dec::launch_attn<8>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, B, Hkv, Smax, softmax_scale, st);
+    case 1: return dec::launch_attn<1>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, softmax_scale, st);
+    case 2: return dec::launch_attn<2>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, softmax_scale, st);
+    case 4: return dec::launch_attn<4>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, softmax_scale, st);
+    case 8: return dec::launch_attn<8>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, softmax_scale, st);
     default: return -2;                          // GQA groups of 1, 2, 4 or 8 query heads
   }
 }
@@ -877,6 +1167,57 @@ ODB_EXPORT int odb_dec_accept(const void* plog, long long ldp, const void* qlog,
   launch_pdl(dec::accept_kernel, dim3(B), dim3(dec::SAMPLE_THREADS), smem, st, (const __nv_bfloat16*)plog, ldp,
              (const __nv_bfloat16*)qlog, ldq, V, K, (const long long*)ictl, (const float*)fctl, (long long*)tok, (int*)pos, (int*)gen,
              (int*)finished, (long long*)out, ld_out, max_new, (int*)draft_pos, (long long*)stats);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+// Vocabulary splits of beam_topk for a vocabulary of V (sizes its partials).
+ODB_EXPORT int odb_dec_beam_splits(int V) { return odb::ceil_div(V, dec::TOPK_SPLIT); }
+
+// logits [rows, ld] bf16; part_ml fp32 [rows, splits, 2]; cand_v fp32 / cand_i int32 [rows, splits, K]; K <= 72.
+ODB_EXPORT int odb_dec_beam_topk(const void* logits, long long ld, int V, int K, void* part_ml, void* cand_v, void* cand_i, int rows,
+                                 cudaStream_t st) {
+  if (K < 1 || K > dec::MAX_KEEP || V < K) return -1;
+  launch_pdl(dec::beam_topk_kernel, dim3(odb::ceil_div(V, dec::TOPK_SPLIT), rows), dim3(dec::TOPK_THREADS), 0, st,
+             (const __nv_bfloat16*)logits, ld, V, K, (float*)part_ml, (float*)cand_v, (int*)cand_i);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+// B prompts of nb <= 8 beams (rows = B * nb); the beam_topk partials of V; ictl: the sampler's control block (EOS ids);
+// early_stopping 0 False, 1 True, 2 "never"; run_score / fin_score fp32 [rows]; fin_flag / pos / parent int32 [rows];
+// run_seq / fin_seq int32 [2, rows, max_new]; unsat / done / tstep int32 [B]; ids_next int64 [rows].  See dec::beam_step_kernel.
+ODB_EXPORT int odb_dec_beam_step(const void* part_ml, const void* cand_v, const void* cand_i, int V, int nb, int K, const void* ictl,
+                                 float length_penalty, int early_stopping, int max_new, void* run_score, void* fin_score, void* fin_flag,
+                                 void* run_seq, void* fin_seq, void* unsat, void* done, void* tstep, void* pos, void* ids_next,
+                                 void* parent, int B, cudaStream_t st) {
+  const int ns = odb::ceil_div(V, dec::TOPK_SPLIT);
+  if (nb < 1 || nb > dec::MAX_BEAMS || K < 1 || K > dec::MAX_KEEP || nb * ns > dec::STEP_THREADS || early_stopping < 0 ||
+      early_stopping > 2 || max_new < 1)
+    return -1;
+  launch_pdl(dec::beam_step_kernel, dim3(B), dim3(dec::STEP_THREADS), 0, st, (const float*)part_ml, (const float*)cand_v,
+             (const int*)cand_i, ns, V, nb, K, (const long long*)ictl, length_penalty, early_stopping, max_new, (float*)run_score,
+             (float*)fin_score, (int*)fin_flag, (int*)run_seq, (int*)fin_seq, (int*)unsat, (int*)done, (int*)tstep, (int*)pos,
+             (long long*)ids_next, (int*)parent);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+// kv bf16 [L, 2, B*nb, Hkv, Smax, 64] (every layer's K and V of the beam rows, one allocation); table int32 [B*nb, Smax/128];
+// parent / pos int32 [B*nb] (pos: the next position to be written, equal over a prompt's beams).  See dec::beam_reorder_kernel.
+ODB_EXPORT int odb_dec_beam_reorder(void* kv, void* table, const void* parent, const void* pos, int B, int nb, int L, int Hkv, int Smax,
+                                    cudaStream_t st) {
+  if (nb < 1 || nb > dec::MAX_BEAMS || Smax % dec::CH || Smax / dec::CH > dec::MAX_TABLE) return -1;
+  const int smem = nb * dec::CH * dec::D * 2;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(dec::beam_reorder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         dec::MAX_BEAMS * dec::CH * dec::D * 2);
+    if (e != cudaSuccess) return (int)e;
+    attr_set = true;
+  }
+  launch_pdl(dec::beam_reorder_kernel, dim3(L * 2 * Hkv, B), dim3(256), smem, st, (__nv_bfloat16*)kv, (int*)table, (const int*)parent,
+             (const int*)pos, nb, Hkv, Smax, Smax / dec::CH);
   ODB_CHECK_LAST();
   return 0;
 }

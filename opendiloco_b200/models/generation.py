@@ -18,12 +18,20 @@ multi-token pass (verify attention over its cache), and one acceptance kernel ke
 one target token per row.  The whole round is one CUDA graph.  Rejected cache entries are left in place: attention reads
 only up to each row's position, so moving ``pos`` back is the whole rollback.
 
+Beam search, ``generate(num_beams=...)``: transformers' deterministic beam search step for step, on B * num_beams rows of
+a DecodeState of its own.  The prompts are prefilled once, into the beam-0 rows; every later step is one CUDA graph: the
+decode layers, the LM head, the selection kernels and the cache reorder.  All beams of a prompt sit at the same position,
+so every 128-key chunk behind the current one is immutable history: a beam that continues another row takes that row's
+chunks through a per-row chunk table and copies only the current partial chunk.
+
 Nothing here goes through ``LlamaEngine.workspace`` or its captured training graphs: generating between training steps
 leaves the training buffers and graph untouched.
 """
 from __future__ import annotations
 
 import os
+import warnings
+from dataclasses import dataclass
 
 import torch
 
@@ -70,8 +78,9 @@ class DecodeState:
         i32 = lambda: torch.zeros(B, dtype=torch.int32, device=device)      # noqa: E731
         self.cfg, self.B, self.Smax, self.device, self.dtype = cfg, B, Smax, torch.device(device), dtype
         self.key = (B, Smax, str(device), dtype)
-        self.kc = [torch.zeros(B, Hkv, Smax, D, dtype=dtype, device=device) for _ in range(L)]
-        self.vc = [torch.zeros(B, Hkv, Smax, D, dtype=dtype, device=device) for _ in range(L)]
+        self.kv = torch.zeros(L, 2, B, Hkv, Smax, D, dtype=dtype, device=device)      # one allocation: beam search reorders all
+        self.kc = [self.kv[l, 0] for l in range(L)]
+        self.vc = [self.kv[l, 1] for l in range(L)]
         n_rope = _round_up(max(cfg.max_position_embeddings, Smax), 128)
         self.cos, self.sin = K.rope_tables(n_rope, D, cfg.rope_theta, device)
         # one-token-per-row buffers of the decode step
@@ -179,9 +188,13 @@ def _mlp(cfg, ar, l: int, xn, gu, act) -> None:
         K.swiglu_fwd(gu, out=act)
 
 
-def _head_and_sample(cfg, ar, st: DecodeState, delta) -> None:
+def _head(cfg, ar, st: DecodeState, delta) -> None:
     K.rmsnorm_fwd(st.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=st.xn, rstd=st.rstd, x_out=st.res)
     G.mm_nt(st.xn, ar.w("lm_head.weight"), out=st.logits)
+
+
+def _head_and_sample(cfg, ar, st: DecodeState, delta) -> None:
+    _head(cfg, ar, st, delta)
     DK.sample(st.logits, st.ictl, st.fctl, st.pos, st.gen, st.finished, st.out, st.ids)
 
 
@@ -207,14 +220,15 @@ def _layers(model, buf, ids: torch.Tensor, attend):
     return delta
 
 
-def _one_token_layers(model, st: DecodeState, ids: torch.Tensor):
-    """One token per row at st.pos: the decode layers with single-query RoPE+append and split-KV attention."""
+def _one_token_layers(model, st: DecodeState, ids: torch.Tensor, table: torch.Tensor | None = None):
+    """One token per row at st.pos: the decode layers with single-query RoPE+append and split-KV attention (through the
+    chunk table, if given)."""
     cfg = model.config
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
 
     def attend(l, qkv, att):
         DK.rope_append(qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D)
-        DK.attention(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.part_o, st.part_ml)
+        DK.attention(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.part_o, st.part_ml, table=table)
 
     return _layers(model, st, ids, attend)
 
@@ -410,6 +424,174 @@ def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int
     return tst.out[:, :max_new_tokens].clone()
 
 
+# ------------------------------------------------------------------------------------------------ beam search
+MAX_BEAMS = 8
+
+
+@dataclass
+class GenerateOutput:
+    """``generate(..., return_dict_in_generate=True)``: the sequences [B * num_return_sequences, P + max_new_tokens] and,
+    with beam search, the fp32 score of each (sum of its log-probabilities / generated_len ** length_penalty)."""
+    sequences: torch.Tensor
+    sequences_scores: torch.Tensor | None = None
+
+
+class BeamState:
+    """Beam search over B prompts of nb beams (row b * nb + j is beam j of prompt b): its own DecodeState for the B * nb
+    rows (the model's ``decode_state`` is left alone), the selection state of ``ops.decode.beam_select``, the chunk table
+    and selection partials of the kernel path, and the step graph."""
+
+    def __init__(self, cfg, B: int, nb: int, K: int, max_new: int, Smax: int, device, dtype):
+        rows = B * nb
+        i32 = lambda *shape: torch.zeros(*shape, dtype=torch.int32, device=device)     # noqa: E731
+        f32 = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=device)   # noqa: E731
+        self.B, self.nb, self.K, self.max_new = B, nb, K, max_new
+        self.key = (B, nb, K, max_new, Smax, str(device), dtype)
+        self.dec = DecodeState(cfg, rows, Smax, device, dtype)
+        self.run_score, self.fin_score = f32(rows), f32(rows)
+        self.fin_flag, self.parent = i32(rows), i32(rows)
+        self.run_seq, self.fin_seq = i32(2, rows, max_new), i32(2, rows, max_new)
+        self.unsat, self.done, self.tstep = i32(B), i32(B), i32(B)
+        self.kernels = DK.usable_beam(self.dec.res, cfg.head_dim, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.vocab_size,
+                                      nb, Smax)
+        if self.dec.kernels and not self.kernels:
+            warnings.warn(f"beam search: the selection and reorder kernels take num_beams * ceil(vocab_size / 1024) <= 512 and "
+                          f"at most 32768 positions (here {nb} x {DK.beam_splits(cfg.vocab_size)} and {Smax}); this run uses the "
+                          "PyTorch references, with host syncs, whole-cache reorders and no CUDA graph", stacklevel=3)
+        self.table = self.part_ml = self.cand_v = self.cand_i = None
+        if self.kernels:
+            nsp = DK.beam_splits(cfg.vocab_size)
+            self.table = i32(rows, Smax // 128)
+            self.part_ml = f32(rows, nsp, 2)
+            self.cand_v, self.cand_i = f32(rows, nsp, K), i32(rows, nsp, K)
+        self.graph = None
+        self.graph_key = None
+
+    def reset(self, pad: int) -> None:
+        """HF's initial state: running scores [0, -1e9, ...], no finished hypotheses, every table entry its own row."""
+        self.run_score.view(self.B, self.nb).fill_(DK.NEG)[:, 0] = 0.0
+        self.fin_score.fill_(DK.NEG)
+        self.fin_flag.zero_()
+        self.run_seq.fill_(pad)
+        self.fin_seq.fill_(pad)
+        self.unsat.fill_(1)
+        self.done.zero_()
+        self.tstep.zero_()
+        if self.table is not None:
+            self.table.copy_(torch.arange(self.table.shape[0], dtype=torch.int32, device=self.table.device)[:, None].expand_as(self.table))
+
+    def results(self, R: int) -> tuple[torch.Tensor, torch.Tensor]:
+        """The R best finished hypotheses of every prompt: tokens int64 [B * R, max_new] and scores fp32 [B * R]."""
+        B, nb, M = self.B, self.nb, self.max_new
+        par = self.tstep.long() & 1                  # each prompt's latest history buffer
+        seq = self.fin_seq.view(2, B, nb, M)[par, torch.arange(B, device=par.device)]
+        return seq[:, :R].reshape(B * R, M).long(), self.fin_score.view(B, nb)[:, :R].reshape(B * R).clone()
+
+
+def beam_state(model, B: int, nb: int, K: int, max_new: int, Smax: int) -> BeamState:
+    """The model's beam-search state for these shapes, allocated on first use; at most one is resident."""
+    eng, ar = model.engine, model.arena
+    key = (B, nb, K, max_new, Smax, str(ar.device), ar.compute_dtype)
+    bs = eng.beam_state
+    if bs is None or bs.key != key:
+        eng.beam_state = None                         # free the old buffers before allocating the new ones
+        bs = eng.beam_state = BeamState(model.config, B, nb, K, max_new, Smax, ar.device, ar.compute_dtype)
+    return bs
+
+
+@torch.no_grad()
+def beam_prefill(model, bs: BeamState, ids: torch.Tensor, lens: torch.Tensor) -> None:
+    """ids [B, Sp] compacted prompts, lens [B]: the layers run on the B prompts once and fill the beam-0 row of each
+    prompt; the last position's logits go to every beam row of the prompt (st.pos ends at lens - 1)."""
+    cfg, ar = model.config, model.arena
+    st, nb = bs.dec, bs.nb
+    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    B, Sp = ids.shape
+    pb = st.prefill_buffers(B * Sp)
+    st.pos.copy_(lens.repeat_interleave(nb) - 1)
+    pb.ids.copy_(ids.reshape(-1))
+    delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
+                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, row_stride=nb))
+    last = (torch.arange(B, device=st.device, dtype=torch.int64) * Sp + lens.long() - 1).repeat_interleave(nb)
+    K.embedding_fwd(last, pb.res, out=st.res)
+    K.embedding_fwd(last, delta, out=st.proj)
+    _head(cfg, ar, st, st.proj)
+
+
+def beam_select(bs: BeamState, length_penalty: float, early_stopping: int) -> None:
+    """Select from bs.dec.logits and reorder the caches by parent."""
+    st = bs.dec
+    DK.beam_select(st.logits, st.ictl, bs.nb, bs.K, length_penalty, early_stopping, bs.max_new, bs.run_score, bs.fin_score,
+                   bs.fin_flag, bs.run_seq, bs.fin_seq, bs.unsat, bs.done, bs.tstep, st.pos, st.ids, bs.parent, bs.part_ml,
+                   bs.cand_v, bs.cand_i)
+    DK.beam_reorder(st.kv, bs.table, bs.parent, st.pos, bs.nb)
+
+
+def _beam_step_eager(model, bs: BeamState, length_penalty: float, early_stopping: int) -> None:
+    st = bs.dec
+    delta = _one_token_layers(model, st, st.ids, bs.table)
+    _head(model.config, model.arena, st, delta)
+    beam_select(bs, length_penalty, early_stopping)
+
+
+@torch.no_grad()
+def beam_step(model, bs: BeamState, length_penalty: float, early_stopping: int, graph: bool | None = None) -> None:
+    """One beam-search step: the beams' tokens at their position, the LM head, selection and reorder.  With the kernels
+    and ``graph`` (default: ``ODB_CUDA_GRAPH`` != 0) the first call runs eagerly (warm-up), the second captures the step and
+    every call replays it."""
+    if graph is None:
+        graph = _use_graph()
+    if not (graph and bs.kernels):
+        _beam_step_eager(model, bs, length_penalty, early_stopping)
+        return
+    key = (model.arena.version, model.arena.shadow.data_ptr(), float(length_penalty), int(early_stopping))
+    if bs.graph is None or bs.graph_key != key:
+        if bs.graph_key != ("warm",) + key:
+            bs.graph, bs.graph_key = None, ("warm",) + key
+            _beam_step_eager(model, bs, length_penalty, early_stopping)
+            return
+        torch.cuda.synchronize(bs.dec.device)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, capture_error_mode="thread_local"):
+            _beam_step_eager(model, bs, length_penalty, early_stopping)
+        bs.graph, bs.graph_key = g, key
+    bs.graph.replay()
+
+
+def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R: int, length_penalty: float, early_stopping,
+                   pad: int, eos: list[int]) -> tuple[torch.Tensor, torch.Tensor]:
+    B = comp.shape[0]
+    es = DK.EARLY_STOPPING[early_stopping]
+    bs = beam_state(model, B, nb, DK.beams_to_keep(nb, len(eos)), max_new_tokens, Smax)
+    bs.dec.set_controls(False, 1.0, 0, 1.0, 0, pad, eos)
+    bs.reset(pad)
+    beam_prefill(model, bs, comp, lens)
+    beam_select(bs, length_penalty, es)              # step 0 on the prefill logits: only beam 0 has score 0
+    for t in range(1, max_new_tokens):
+        if t % FINISHED_CHECK_EVERY == 0 and bool(bs.done.all()):
+            break
+        beam_step(model, bs, length_penalty, es)
+    return bs.results(R)
+
+
+def _check_beams(num_beams, num_return_sequences, do_sample: bool, assistant_model, early_stopping, vocab_size: int,
+                 n_eos: int) -> None:
+    if isinstance(num_beams, bool) or not isinstance(num_beams, int) or not 1 <= num_beams <= MAX_BEAMS:
+        raise ValueError(f"num_beams must be an integer in [1, {MAX_BEAMS}], got {num_beams!r}")
+    if isinstance(num_return_sequences, bool) or not isinstance(num_return_sequences, int) \
+            or not 1 <= num_return_sequences <= num_beams:
+        raise ValueError(f"num_return_sequences must be an integer in [1, num_beams={num_beams}], got {num_return_sequences!r}")
+    if not (early_stopping is True or early_stopping is False or early_stopping == "never"):
+        raise ValueError(f"early_stopping must be True, False or \"never\", got {early_stopping!r}")
+    if num_beams > 1 and do_sample:
+        raise ValueError("beam search is deterministic here: do_sample=True cannot be combined with num_beams > 1")
+    if num_beams > 1 and assistant_model is not None:
+        raise ValueError("assistant_model cannot be combined with num_beams > 1")
+    if num_beams > 1 and DK.beams_to_keep(num_beams, n_eos) > vocab_size:
+        raise ValueError(f"num_beams {num_beams} with {n_eos} EOS ids needs a vocabulary of at least "
+                         f"{DK.beams_to_keep(num_beams, n_eos)} tokens, the model has {vocab_size}")
+
+
 # ------------------------------------------------------------------------------------------------ generate
 def _eos_list(eos) -> list[int]:
     if eos is None:
@@ -422,7 +604,9 @@ def _eos_list(eos) -> list[int]:
 @torch.no_grad()
 def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, max_new_tokens: int = 20,
              do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
-             pad_token_id: int | None = None, seed: int = 0, assistant_model=None, num_assistant_tokens: int = 4) -> torch.Tensor:
+             pad_token_id: int | None = None, seed: int = 0, assistant_model=None, num_assistant_tokens: int = 4, num_beams: int = 1,
+             length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1,
+             return_dict_in_generate: bool = False) -> torch.Tensor | GenerateOutput:
     """See :meth:`LlamaForCausalLM.generate`."""
     cfg, ar = model.config, model.arena
     if ar.param_sharded:
@@ -441,6 +625,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
         raise ValueError(f"top_p must be in (0, 1], got {top_p}")
     if assistant_model is not None:
         _check_assistant(model, assistant_model, P, max_new_tokens, num_assistant_tokens)
+    eos = _eos_list(cfg.eos_token_id if eos_token_id is None else eos_token_id)
+    _check_beams(num_beams, num_return_sequences, do_sample, assistant_model, early_stopping, cfg.vocab_size, len(eos))
     dev = ar.device
     ids = input_ids.to(dev)
     if attention_mask is None:
@@ -452,7 +638,6 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
         if not bool((m[:, 1:] >= m[:, :-1]).all()) or not bool(m[:, -1].all()):
             raise ValueError("attention_mask must be left-padded: zeros (padding) before ones in every row")
         lens = m.sum(dim=1).to(torch.int32)
-    eos = _eos_list(cfg.eos_token_id if eos_token_id is None else eos_token_id)
     pad = pad_token_id if pad_token_id is not None else (eos[0] if eos else 0)
 
     # compact each row to start at position 0, right-pad to the prefill length
@@ -466,8 +651,14 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     if assistant_model is not None:
         new = _assisted_generate(model, assistant_model, comp, lens, P, max_new_tokens, num_assistant_tokens,
                                  (do_sample, temperature, top_k, top_p, seed), pad, eos)
-        return torch.cat([ids, new], dim=1)
+        out = torch.cat([ids, new], dim=1)
+        return GenerateOutput(out) if return_dict_in_generate else out
     Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))
+    if num_beams > 1:
+        new, scores = _beam_generate(model, comp, lens, Smax, max_new_tokens, num_beams, num_return_sequences, length_penalty,
+                                     early_stopping, pad, eos)
+        out = torch.cat([ids.repeat_interleave(num_return_sequences, dim=0), new], dim=1)
+        return GenerateOutput(out, scores) if return_dict_in_generate else out
     st = decode_state(model, B, Smax)
 
     st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos)
@@ -477,4 +668,5 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
         if eos and t % FINISHED_CHECK_EVERY == 0 and bool(st.finished.all()):
             break
         step(model, st)
-    return torch.cat([ids, st.out[:, :max_new_tokens].clone()], dim=1)
+    out = torch.cat([ids, st.out[:, :max_new_tokens].clone()], dim=1)
+    return GenerateOutput(out) if return_dict_in_generate else out

@@ -193,6 +193,7 @@ class LlamaEngine:
         self._graphs: dict[tuple, dict] = {}       # (B, S, loss_scale, labels-alias) -> captured micro-step
         self.decode_state = None                   # generation's KV caches + decode graph (models/generation.py)
         self.assisted_state = None                 # assisted generation's verify buffers, draft caches + round graph
+        self.beam_state = None                     # beam search's caches, chunk table, selection state + step graph
         self.score_state = None                    # scoring buffers (models/scoring.py)
 
     def workspace(self, B: int, S: int) -> _Workspace:
@@ -691,6 +692,7 @@ class LlamaForCausalLM(nn.Module):
                 self.engine._graphs.clear()
                 self.engine.decode_state = None
                 self.engine.assisted_state = None
+                self.engine.beam_state = None
                 self.engine.score_state = None
                 self.engine.head_grad_tmp = None
                 self._rebind()
@@ -741,7 +743,8 @@ class LlamaForCausalLM(nn.Module):
     def generate(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, max_new_tokens: int = 20,
                  do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
                  pad_token_id: int | None = None, seed: int = 0, assistant_model: "LlamaForCausalLM | None" = None,
-                 num_assistant_tokens: int = 4) -> torch.Tensor:
+                 num_assistant_tokens: int = 4, num_beams: int = 1, length_penalty: float = 1.0, early_stopping=False,
+                 num_return_sequences: int = 1, return_dict_in_generate: bool = False):
         """KV-cached text generation with HF ``generate`` keyword names.  Returns LongTensor [B, P + max_new_tokens]: the
         prompt as given, then the new tokens.
 
@@ -761,12 +764,30 @@ class LlamaForCausalLM(nn.Module):
         between the one- and multi-token attention).  ``engine.assisted_state`` then reports ``verify_passes()`` and
         ``acceptance_rate()``.  Raises ValueError for a different vocabulary, device or compute dtype, a parameter-sharded
         assistant, ``num_assistant_tokens`` outside [1, 7], or a prompt plus ``max_new_tokens`` plus
-        ``num_assistant_tokens`` beyond either model's ``max_position_embeddings``."""
+        ``num_assistant_tokens`` beyond either model's ``max_position_embeddings``.
+
+        ``num_beams`` > 1 (at most 8) runs deterministic beam search as transformers' ``generate(num_beams=...,
+        do_sample=False)``: fp32 log-softmax of the logits without logits processors, ``length_penalty``,
+        ``early_stopping`` (True, False or ``"never"``) and the finished-hypothesis rules of HF, ties to the lower
+        ``beam * V + token``.  It returns ``[B * num_return_sequences, P + max_new_tokens]``: row ``b * R + r`` is prompt b
+        as given, then its r-th best hypothesis (EOS included), then ``pad_token_id``.  bf16-mixed CUDA models run the
+        selection and cache-reorder kernels with each step replayed from a CUDA graph; beams share the complete 128-position
+        cache chunks of their history through a chunk table.  Those kernels take num_beams * ceil(vocab_size / 1024) <= 512
+        and at most 32768 positions; beyond that the step runs on the PyTorch references without a graph, with a warning.
+        Raises ValueError for ``num_beams`` outside [1, 8],
+        ``num_return_sequences`` outside [1, num_beams], an unknown ``early_stopping``, or ``do_sample=True`` or
+        ``assistant_model`` with ``num_beams`` > 1.
+
+        ``return_dict_in_generate=True`` returns a ``GenerateOutput`` with ``sequences`` and ``sequences_scores`` (fp32
+        [B * num_return_sequences]: each hypothesis's summed log-probabilities / generated_len ** length_penalty; None
+        without beam search)."""
         from .generation import generate
 
         return generate(self, input_ids, attention_mask=attention_mask, max_new_tokens=max_new_tokens, do_sample=do_sample,
                         temperature=temperature, top_k=top_k, top_p=top_p, eos_token_id=eos_token_id, pad_token_id=pad_token_id,
-                        seed=seed, assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens)
+                        seed=seed, assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens, num_beams=num_beams,
+                        length_penalty=length_penalty, early_stopping=early_stopping, num_return_sequences=num_return_sequences,
+                        return_dict_in_generate=return_dict_in_generate)
 
     @torch.no_grad()
     def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None):

@@ -8,6 +8,10 @@ KV cache layout, per layer: K and V each ``[B, Hkv, Smax, D]`` in the compute dt
 position of each row's current token: ``rope_append`` writes at ``pos[b]`` and ``attention`` attends to keys
 ``0 .. pos[b]``; the sampler advances it.
 
+Beam search keeps ``num_beams`` rows per prompt (row ``b * num_beams + j`` is beam j of prompt b) and may share cache
+chunks between them: with a chunk table (int32 ``[rows, Smax / 128]``), keys ``[128 c, 128 c + 128)`` of row r live in
+physical row ``table[r, c]`` (``attention``, ``beam_reorder``).
+
 Assisted generation scores n tokens per row in one pass.  Its buffers are slot-major: row ``j*B + b`` is token j of row
 b, at position ``pos[b] + j`` (``rope_append_multi``, ``verify_attention``, ``accept``).
 """
@@ -23,10 +27,11 @@ from .. import _lib
 c_void_p, c_int, c_ll, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float
 _lib.register_optional("odb_dec_rope_append", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                                c_int, c_void_p])
-_lib.register_optional("odb_dec_kv_fill", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p])
+_lib.register_optional("odb_dec_kv_fill", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                           c_void_p])
 _lib.register_optional("odb_dec_attn_chunks", [c_int])
-_lib.register_optional("odb_dec_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int,
-                                        c_int, c_int, c_float, c_void_p])
+_lib.register_optional("odb_dec_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_int,
+                                        c_int, c_int, c_int, c_float, c_void_p])
 _lib.register_optional("odb_dec_sample", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                           c_void_p, c_int, c_void_p])
 _lib.register_optional("odb_dec_rope_append_multi", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
@@ -35,6 +40,12 @@ _lib.register_optional("odb_dec_verify_attn", [c_void_p, c_ll, c_void_p, c_void_
                                                c_int, c_int, c_int, c_int, c_float, c_void_p])
 _lib.register_optional("odb_dec_accept", [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p])
+_lib.register_optional("odb_dec_beam_splits", [c_int])
+_lib.register_optional("odb_dec_beam_topk", [c_void_p, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p])
+_lib.register_optional("odb_dec_beam_step", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_float, c_int, c_int,
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_int, c_void_p])
+_lib.register_optional("odb_dec_beam_reorder", [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p])
 
 MAX_EOS = 8
 # int64 control block of the sampler: do_sample, top_k, seed, pad_token_id, n_eos, eos ids
@@ -53,6 +64,17 @@ def usable_verify(t: torch.Tensor, head_dim: int, Hq: int = 1, Hkv: int = 1) -> 
     """``usable`` plus the assisted-generation kernels (multi-token RoPE+append, verify attention, acceptance)."""
     return (usable(t, head_dim, Hq, Hkv) and _lib.has_symbol("odb_dec_verify_attn") and _lib.has_symbol("odb_dec_accept")
             and _lib.has_symbol("odb_dec_rope_append_multi"))
+
+
+def usable_beam(t: torch.Tensor, head_dim: int, Hq: int, Hkv: int, V: int, num_beams: int, Smax: int) -> bool:
+    """``usable`` plus the beam-search kernels (selection over a vocabulary of V, chunk-table reorder of Smax positions)."""
+    return (usable(t, head_dim, Hq, Hkv) and _lib.has_symbol("odb_dec_beam_step") and _lib.has_symbol("odb_dec_beam_reorder")
+            and num_beams * beam_splits(V) <= 512 and Smax % 128 == 0 and Smax // 128 <= 256)
+
+
+def beam_splits(V: int) -> int:
+    """Vocabulary splits of ``beam_topk`` (1024 entries each): sizes its partials."""
+    return (V + 1023) // 1024
 
 
 def verify_splits(Smax: int) -> int:
@@ -90,13 +112,13 @@ def rope_append(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, pos: to
 
 
 def kv_fill(qkv: torch.Tensor, lens: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, B: int, Sp: int, Hq: int, Hkv: int,
-            D: int) -> None:
-    """Prefill: rows s < lens[b] of the rotated packed projections qkv [B*Sp, row] -> cache[b, :, s]."""
+            D: int, row_stride: int = 1) -> None:
+    """Prefill: rows s < lens[b] of the rotated packed projections qkv [B*Sp, row] -> cache[b * row_stride, :, s]."""
     Smax = kc.shape[2]
     if usable(qkv, D, Hq, Hkv):
         assert qkv.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous() and lens.dtype == torch.int32
         _lib.check(_lib.cuda_lib().odb_dec_kv_fill(qkv.data_ptr(), qkv.stride(0), lens.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, Sp,
-                                                   Hq, Hkv, Smax, _lib.stream_ptr(qkv)), "dec_kv_fill")
+                                                   Hq, Hkv, Smax, row_stride, _lib.stream_ptr(qkv)), "dec_kv_fill")
         _lib.count_launch()
         return
     n = min(Sp, Smax)
@@ -104,26 +126,33 @@ def kv_fill(qkv: torch.Tensor, lens: torch.Tensor, kc: torch.Tensor, vc: torch.T
     k = rows[..., Hq * D:(Hq + Hkv) * D].unflatten(-1, (Hkv, D)).transpose(1, 2)     # [B, Hkv, n, D]
     v = rows[..., (Hq + Hkv) * D:].unflatten(-1, (Hkv, D)).transpose(1, 2)
     keep = (torch.arange(n, device=qkv.device)[None, :] < lens.long()[:, None].to(qkv.device))[:, None, :, None]
-    kc[:, :, :n] = torch.where(keep, k, kc[:, :, :n])
-    vc[:, :, :n] = torch.where(keep, v, vc[:, :, :n])
+    kd, vd = kc[::row_stride], vc[::row_stride]
+    kd[:, :, :n] = torch.where(keep, k, kd[:, :, :n])
+    vd[:, :, :n] = torch.where(keep, v, vd[:, :, :n])
 
 
 # ------------------------------------------------------------------------------------------------ decode attention
 def attention(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, pos: torch.Tensor, out: torch.Tensor, Hq: int, Hkv: int, D: int,
-              part_o: torch.Tensor | None = None, part_ml: torch.Tensor | None = None) -> torch.Tensor:
+              part_o: torch.Tensor | None = None, part_ml: torch.Tensor | None = None, table: torch.Tensor | None = None) -> torch.Tensor:
     """out[b, h*D:(h+1)*D] = softmax(q_bh . K[b, h//G, :pos[b]+1]^T / sqrt(D)) V[b, h//G, :pos[b]+1]  (one query per row).
 
     q: the first Hq*D columns of [B, row].  part_o fp32 [B, Hq, chunks, D] / part_ml fp32 [B, Hq, chunks, 2]: scratch of
-    the split-KV kernel (``attn_chunks(Smax)`` chunks)."""
+    the split-KV kernel (``attn_chunks(Smax)`` chunks).  table: None, or the int32 chunk table [B, Smax / 128] (keys of
+    chunk c of row b are read from row table[b, c]; the reference gathers them, then attends)."""
     B = q.shape[0]
     Smax = kc.shape[2]
     if usable(q, D, Hq, Hkv):
         assert q.stride(1) == 1 and out.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous() and pos.dtype == torch.int32
+        if table is not None:
+            assert table.dtype == torch.int32 and table.is_contiguous() and table.shape == (B, attn_chunks(Smax)) and Smax % 128 == 0
         _lib.check(_lib.cuda_lib().odb_dec_attn(q.data_ptr(), q.stride(0), kc.data_ptr(), vc.data_ptr(), pos.data_ptr(), part_o.data_ptr(),
-                                                part_ml.data_ptr(), out.data_ptr(), out.stride(0), B, Hq, Hkv, Smax,
+                                                part_ml.data_ptr(), out.data_ptr(), out.stride(0),
+                                                table.data_ptr() if table is not None else None, B, Hq, Hkv, Smax,
                                                 1.0 / math.sqrt(D), _lib.stream_ptr(q)), "dec_attn")
         _lib.count_launch(2)
         return out
+    if table is not None:
+        kc, vc = gather_chunks(kc, table), gather_chunks(vc, table)
     G = Hq // Hkv
     qf = q[:, : Hq * D].float().view(B, Hkv, G, D)
     att = torch.einsum("bkgd,bksd->bkgs", qf, kc.float()) / math.sqrt(D)
@@ -132,6 +161,15 @@ def attention(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, pos: torch.Te
     o = torch.einsum("bkgs,bksd->bkgd", torch.softmax(att, dim=-1), vc.float())
     out.copy_(o.reshape(B, Hq * D).to(out.dtype))
     return out
+
+
+def gather_chunks(cache: torch.Tensor, table: torch.Tensor) -> torch.Tensor:
+    """cache [rows, Hkv, Smax, D] read through the chunk table [rows, Smax / 128]: chunk c of row r from row table[r, c]."""
+    rows, Hkv, Smax, D = cache.shape
+    nch = table.shape[1]
+    c5 = cache.view(rows, Hkv, nch, Smax // nch, D).transpose(1, 2)                   # [rows, nch, Hkv, 128, D]
+    g = c5[table.long().to(cache.device), torch.arange(nch, device=cache.device)[None, :]]
+    return g.transpose(1, 2).reshape(rows, Hkv, Smax, D)
 
 
 # ------------------------------------------------------------------------------------------------ assisted generation
@@ -265,6 +303,152 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor, ictl: torch.Tensor, fctl: tor
         gen[b] = g
         t[0, b] = t_new
         draft_pos[b] = pos[b]
+
+
+# ------------------------------------------------------------------------------------------------ beam search
+EARLY_STOPPING = {False: 0, True: 1, "never": 2}    # codes of HF's early_stopping values
+NEG = -1.0e9                                          # HF's score offset of a continuation that must not be chosen
+
+
+def beams_to_keep(num_beams: int, n_eos: int) -> int:
+    """Candidates taken per prompt and step (HF): enough that num_beams of them are not EOS."""
+    return max(2, 1 + n_eos) * num_beams
+
+
+def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int, length_penalty: float, early_stopping: int,
+                max_new: int, run_score: torch.Tensor, fin_score: torch.Tensor, fin_flag: torch.Tensor, run_seq: torch.Tensor,
+                fin_seq: torch.Tensor, unsat: torch.Tensor, done: torch.Tensor, tstep: torch.Tensor, pos: torch.Tensor,
+                ids_next: torch.Tensor, parent: torch.Tensor, part_ml: torch.Tensor | None = None, cand_v: torch.Tensor | None = None,
+                cand_i: torch.Tensor | None = None) -> None:
+    """One step of deterministic beam search (transformers' ``_beam_search`` with do_sample=False) over logits
+    [B * num_beams, V] (row b * num_beams + j: beam j of prompt b).
+
+    Log-probabilities are fp32 log_softmax of the logits; the K = ``beams_to_keep`` best continuations per prompt of
+    log p + run_score (ties: the lower beam * V + token) hit the stopping criteria on an EOS id of ictl or when t + 1 ==
+    max_new (t = tstep[b], tokens generated so far).  The new running beams are the num_beams best of them after -1e9 on
+    those that hit; the finished hypotheses (fin_score / fin_flag / fin_seq) merge the old ones with the first num_beams
+    candidates that hit, scored log p / (t + 1) ** length_penalty, with HF's -1e9 rules; then the early-stop heuristic
+    (``early_stopping`` code of EARLY_STOPPING) updates unsat and done.
+
+    Writes, for prompts not yet done: ids_next (the new beams' tokens), parent (int32, the global row each new beam
+    continues), run_score, pos += 1, tstep += 1, the finished state, and the histories: int32 [2, rows, max_new]
+    double-buffered by the parity of t (step t reads buffer t & 1 and writes the other).  Done prompts keep everything,
+    with parent = the row itself.  With the beam_topk partials (part_ml fp32 [rows, beam_splits(V), 2], cand_v fp32 /
+    cand_i int32 [rows, beam_splits(V), K]) the kernels run, otherwise ``beam_step_reference``."""
+    if part_ml is None:
+        beam_step_reference(logits, ictl, num_beams, K, length_penalty, early_stopping, max_new, run_score, fin_score, fin_flag, run_seq,
+                            fin_seq, unsat, done, tstep, pos, ids_next, parent)
+        return
+    rows, V = logits.shape
+    assert logits.is_cuda and logits.dtype == torch.bfloat16 and logits.stride(1) == 1 and rows % num_beams == 0
+    assert part_ml.shape == (rows, beam_splits(V), 2) and cand_v.shape == (rows, beam_splits(V), K) and cand_i.shape == cand_v.shape
+    assert run_seq.shape == (2, rows, max_new) and fin_seq.shape == (2, rows, max_new) and run_seq.dtype == torch.int32
+    st = _lib.stream_ptr(logits)
+    _lib.check(_lib.cuda_lib().odb_dec_beam_topk(logits.data_ptr(), logits.stride(0), V, K, part_ml.data_ptr(), cand_v.data_ptr(),
+                                                 cand_i.data_ptr(), rows, st), "dec_beam_topk")
+    _lib.check(_lib.cuda_lib().odb_dec_beam_step(part_ml.data_ptr(), cand_v.data_ptr(), cand_i.data_ptr(), V, num_beams, K,
+                                                 ictl.data_ptr(), float(length_penalty), int(early_stopping), max_new,
+                                                 run_score.data_ptr(), fin_score.data_ptr(), fin_flag.data_ptr(), run_seq.data_ptr(),
+                                                 fin_seq.data_ptr(), unsat.data_ptr(), done.data_ptr(), tstep.data_ptr(), pos.data_ptr(),
+                                                 ids_next.data_ptr(), parent.data_ptr(), rows // num_beams, st), "dec_beam_step")
+    _lib.count_launch(2)
+
+
+def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int, length_penalty: float, early_stopping: int,
+                        max_new: int, run_score: torch.Tensor, fin_score: torch.Tensor, fin_flag: torch.Tensor, run_seq: torch.Tensor,
+                        fin_seq: torch.Tensor, unsat: torch.Tensor, done: torch.Tensor, tstep: torch.Tensor, pos: torch.Tensor,
+                        ids_next: torch.Tensor, parent: torch.Tensor) -> None:
+    """``beam_select`` in PyTorch: transformers' ``_get_top_k_continuations``, ``_get_running_beams_for_next_iteration``,
+    ``_update_finished_beams`` and ``_check_early_stop_heuristic`` over [B, num_beams, ...], with stable sorts for the
+    tie rule."""
+    rows, V = logits.shape
+    nb = num_beams
+    B = rows // nb
+    dev = run_score.device
+    c = ictl.tolist()
+    eos = torch.tensor(c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]], dtype=torch.int64, device=dev)
+    t = tstep.long()
+    ts = [int(x) for x in t.tolist()]
+    live = done == 0
+    top = lambda x, k: torch.sort(x, dim=1, descending=True, stable=True).indices[:, :k]   # noqa: E731
+    # c. top-K continuations
+    logp = torch.log_softmax(logits.float(), dim=-1).to(dev).view(B, nb, V) + run_score.view(B, nb, 1)
+    idx = top(logp.view(B, nb * V), K)
+    vals = logp.view(B, nb * V).gather(1, idx)
+    beam, tok = idx // V, idx % V
+    # d. stopping criteria
+    last = (t + 1 >= max_new)[:, None]
+    hits = last | torch.isin(tok, eos)
+    # e. running beams of the next step
+    trs = vals + hits.float() * NEG
+    rsel = top(trs, nb)
+    new_rs = trs.gather(1, rsel)
+    # f. finished hypotheses
+    just = hits & (torch.arange(K, device=dev) < nb)[None, :]
+    denom = torch.tensor([float((x + 1) ** float(length_penalty)) for x in ts], dtype=torch.float32, device=dev)
+    f = vals / denom[:, None]
+    fs_old, ff_old = fin_score.view(B, nb), fin_flag.view(B, nb) != 0
+    f = f + (ff_old.all(1, keepdim=True) & (early_stopping == 1)).float() * NEG
+    f = f + (unsat.view(B, 1) == 0).float() * NEG
+    f = f + (~just).float() * NEG
+    merged = torch.cat([fs_old, f], dim=1)
+    msel = top(merged, nb)
+    new_fs = merged.gather(1, msel)
+    new_ff = torch.cat([ff_old, just], dim=1).gather(1, msel)
+    # histories: candidate k = the running history of its beam + its token at t
+    M = max_new
+    ar = torch.arange(B, device=dev)
+    par = t & 1
+    run_all, fin_all = run_seq.view(2, B, nb, M), fin_seq.view(2, B, nb, M)
+    cand = run_all[par, ar].gather(1, beam[:, :, None].expand(B, K, M))
+    cand = torch.where(torch.arange(M, device=dev)[None, None, :] == t[:, None, None], tok[:, :, None].to(cand.dtype), cand)
+    new_run = cand.gather(1, rsel[:, :, None].expand(B, nb, M))
+    new_fin = torch.cat([fin_all[par, ar], cand], dim=1).gather(1, msel[:, :, None].expand(B, nb, M))
+    # g. early-stop heuristic
+    best_len = [max_new if (early_stopping == 2 and length_penalty > 0) else x + 1 for x in ts]
+    bden = torch.tensor([float(n ** float(length_penalty)) for n in best_len], dtype=torch.float32, device=dev)
+    best_possible = new_rs[:, :1] / bden[:, None]
+    worst = torch.where(new_ff, new_fs.min(dim=1, keepdim=True).values, torch.full_like(new_fs, NEG))
+    new_unsat = (unsat != 0) & (best_possible > worst).any(dim=1)
+    new_done = ~new_unsat | ((early_stopping == 1) & new_ff.all(dim=1)) | last[:, 0]
+    # write back the prompts that were not done
+    lr = live.repeat_interleave(nb)
+    run_all[1 - par[live], ar[live]] = new_run[live]
+    fin_all[1 - par[live], ar[live]] = new_fin[live]
+    run_score.copy_(torch.where(lr, new_rs.reshape(-1), run_score))
+    fin_score.copy_(torch.where(lr, new_fs.reshape(-1), fin_score))
+    fin_flag.copy_(torch.where(lr, new_ff.reshape(-1).to(fin_flag.dtype), fin_flag))
+    rows_idx = torch.arange(rows, device=dev)
+    parent.copy_(torch.where(lr, (ar[:, None] * nb + beam.gather(1, rsel)).reshape(-1), rows_idx).to(parent.dtype))
+    ids_next.copy_(torch.where(lr, tok.gather(1, rsel).reshape(-1), ids_next))
+    pos.add_(lr.to(pos.dtype))
+    unsat.copy_(torch.where(live, new_unsat.to(unsat.dtype), unsat))
+    done.copy_(torch.where(live, new_done.to(done.dtype), done))
+    tstep.add_(live.to(tstep.dtype))
+
+
+def beam_reorder(kv: torch.Tensor, table: torch.Tensor | None, parent: torch.Tensor, pos: torch.Tensor, num_beams: int) -> None:
+    """After a selection, make every beam row's cache the history of its parent row (int32 [rows], pos: the next position
+    to write, the same for all beams of a prompt).  kv: every layer's K and V of the beam rows, [L, 2, rows, Hkv, Smax, D].
+
+    With a chunk table (the kernel path), complete 128-position chunks are shared: a child whose parent is another row
+    takes the parent's table entries below pos // 128 and gets a copy of positions [128 * (pos // 128), pos) in its own
+    row.  Without one, ``beam_reorder_reference`` moves whole rows."""
+    if table is None:
+        beam_reorder_reference(kv, parent)
+        return
+    L, two, rows, Hkv, Smax, D = kv.shape
+    assert kv.is_cuda and kv.dtype == torch.bfloat16 and kv.is_contiguous() and two == 2 and D == 64 and rows % num_beams == 0
+    assert table.shape == (rows, Smax // 128) and table.dtype == torch.int32 and parent.dtype == torch.int32 and pos.dtype == torch.int32
+    _lib.check(_lib.cuda_lib().odb_dec_beam_reorder(kv.data_ptr(), table.data_ptr(), parent.data_ptr(), pos.data_ptr(), rows // num_beams,
+                                                    num_beams, L, Hkv, Smax, _lib.stream_ptr(kv)), "dec_beam_reorder")
+    _lib.count_launch()
+
+
+def beam_reorder_reference(kv: torch.Tensor, parent: torch.Tensor) -> None:
+    """Physical reorder: row r of every layer's K and V becomes (a copy of) row parent[r].  The chunk table of
+    ``beam_reorder`` must read exactly like this."""
+    kv.copy_(kv.index_select(2, parent.long().to(kv.device)))
 
 
 # ------------------------------------------------------------------------------------------------ sampler

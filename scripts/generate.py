@@ -6,12 +6,15 @@
         --max-new-tokens 64 --do-sample --temperature 0.8 --top-p 0.95
     python scripts/generate.py --model 1b --checkpoint outputs_1b/model_step_1000 --assistant-model 150m \\
         --assistant-checkpoint outputs_150m/model_step_1000 --num-assistant-tokens 4 --prompt-ids "1 450 4996"
+    python scripts/generate.py --model 1b --checkpoint outputs_1b/model_step_1000 --num-beams 4 --num-return-sequences 2 \\
+        --prompt-ids "1 450 4996"
 
 ``--checkpoint`` reads a checkpoint directory written by train_fsdp / utils/ckpt.save_checkpoint (the one holding the
 ``*.distcp`` shards, i.e. ``model_step_N`` or its ``diloco_rank_R`` sub-directory).  ``--weights local`` takes the
 worker's own weights (``model``), ``--weights outer`` the DiLoCo global model (``theta_outer``).  Tokenizers are only
 read from a local directory.  ``--assistant-model`` (with ``--assistant-checkpoint`` / ``--assistant-weights``) loads a
-draft model the same way and turns on assisted (speculative) generation.
+draft model the same way and turns on assisted (speculative) generation.  ``--num-beams`` > 1 runs beam search and prints
+each returned hypothesis with its score (``--num-return-sequences`` per prompt).
 """
 import argparse
 import json
@@ -96,6 +99,11 @@ def main(argv=None) -> None:
     ap.add_argument("--assistant-weights", choices=["local", "outer"], default="local",
                     help="with --assistant-checkpoint: local or DiLoCo outer weights")
     ap.add_argument("--num-assistant-tokens", type=int, default=4, help="draft tokens proposed per round (1..7)")
+    ap.add_argument("--num-beams", type=int, default=1, help="beam search with this many beams (1..8); 1: greedy / sampling")
+    ap.add_argument("--length-penalty", type=float, default=1.0, help="beam search: hypothesis score = sum log p / length ** this")
+    ap.add_argument("--early-stopping", choices=["true", "false", "never"], default="false",
+                    help="beam search: HF's early_stopping (true, false or never)")
+    ap.add_argument("--num-return-sequences", type=int, default=1, help="beam search: hypotheses returned per prompt")
     a = ap.parse_args(argv)
     if a.assistant_model is None and a.assistant_checkpoint is not None:
         ap.error("--assistant-checkpoint needs --assistant-model")
@@ -127,15 +135,22 @@ def main(argv=None) -> None:
     for i, p in enumerate(prompts):
         ids[i, P - len(p):] = torch.tensor(p)
         mask[i, P - len(p):] = 1
-    out = model.generate(ids.to(device), attention_mask=mask.to(device), max_new_tokens=a.max_new_tokens, do_sample=a.do_sample,
+    early_stopping = {"true": True, "false": False, "never": "never"}[a.early_stopping]
+    res = model.generate(ids.to(device), attention_mask=mask.to(device), max_new_tokens=a.max_new_tokens, do_sample=a.do_sample,
                          temperature=a.temperature, top_k=a.top_k, top_p=a.top_p, eos_token_id=a.eos_token_id,
                          pad_token_id=a.pad_token_id, seed=a.seed, assistant_model=assistant,
-                         num_assistant_tokens=a.num_assistant_tokens).cpu()
+                         num_assistant_tokens=a.num_assistant_tokens, num_beams=a.num_beams, length_penalty=a.length_penalty,
+                         early_stopping=early_stopping, num_return_sequences=a.num_return_sequences, return_dict_in_generate=True)
+    out = res.sequences.cpu()
+    R = out.shape[0] // len(prompts)
     for i, p in enumerate(prompts):
-        new = out[i, P:].tolist()
-        print("ids:", " ".join(str(t) for t in p + new))
-        if tok is not None:
-            print("text:", tok.decode(p + new, skip_special_tokens=True))
+        for r in range(R):
+            new = out[i * R + r, P:].tolist()
+            if res.sequences_scores is not None:
+                print(f"score: {float(res.sequences_scores[i * R + r]):.6f}")
+            print("ids:", " ".join(str(t) for t in p + new))
+            if tok is not None:
+                print("text:", tok.decode(p + new, skip_special_tokens=True))
     if assistant is not None:
         st = model.engine.assisted_state
         print(f"assisted: {st.verify_passes()} verify passes, acceptance {st.acceptance_rate():.3f}")
