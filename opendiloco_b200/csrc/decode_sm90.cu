@@ -5,7 +5,8 @@
 //                         captured graph stays valid at every step), write k and v into the layer's cache at (b, pos[b])
 //   odb_dec_kv_fill       prefill: copy the (already rotated) k|v columns of the packed qkv rows into the cache
 //   odb_dec_attn          split-KV decode attention (flash-decoding) + a combine kernel
-//   odb_dec_sample        greedy / temperature + top-k + top-p sampler, one CTA per row
+//   odb_dec_sample        greedy / temperature + top-k + top-p sampler, one CTA per row, with HF's repetition penalty, n-gram
+//                         ban and min-new-tokens over the row's device-side token history when the control blocks ask
 //   odb_dec_beam_topk     beam search: per vocabulary split of a row, the (max, sum-exp) partial and the local top-K logits
 //   odb_dec_beam_step     beam search: one CTA per prompt merges the candidates and does HF's selection and bookkeeping
 //   odb_dec_beam_reorder  beam search: chunk-table update and partial-chunk K/V copy for beams that changed parent
@@ -264,10 +265,82 @@ decode_combine_kernel(const float* __restrict__ part_o, const float* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------ sampler
-// ictl (int64, device): [0] do_sample, [1] top_k, [2] seed, [3] pad_token_id, [4] number of EOS ids (<= 8), [5..12] EOS ids
-// fctl (fp32, device):  [0] temperature, [1] top_p
+// ictl (int64, device): [0] do_sample, [1] top_k, [2] seed, [3] pad_token_id, [4] number of EOS ids (<= 8), [5..12] EOS ids,
+//                       [13] no_repeat_ngram_size, [14] min_new_tokens
+// fctl (fp32, device):  [0] temperature, [1] top_p, [2] repetition_penalty
 constexpr int SAMPLE_THREADS = 1024;
 constexpr int MAX_EOS = 8;
+constexpr int CTL_NGRAM = 13, CTL_MIN_NEW = 14;
+
+// ------------------------------------------------------------------------------------------------ logits processors
+// HF's repetition penalty, n-gram ban and min-new-tokens, applied to the fp32 value of each logit (sampler) or log-prob
+// (beam search).  The settings live in the control blocks, so a captured graph serves every value, "off" included.
+__device__ __forceinline__ bool processors_on(const long long* __restrict__ ictl, const float* __restrict__ fctl) {
+  return fctl[2] != 1.f || ictl[CTL_NGRAM] > 0 || (ictl[CTL_MIN_NEW] > 0 && ictl[4] > 0);
+}
+
+// HF's RepetitionPenaltyLogitsProcessor on one value.
+__device__ __forceinline__ float penalise(float x, float p) { return x < 0.f ? __fmul_rn(x, p) : __fdiv_rn(x, p); }
+
+// A row's token history h[0, L): h[0, n0) from a, then h[n0, L) from b (beam search: the prompt, then the beam's running
+// sequence; plain decode: one buffer).
+struct History {
+  const int* a;
+  const int* b;
+  int n0, L;
+  __device__ __forceinline__ int operator[](int i) const { return i < n0 ? a[i] : b[i - n0]; }
+};
+
+// Marks, for the tokens in [lo, hi), bit (token - lo) of pen (the token occurs in the history; only with penalise) and of
+// ban (the token follows an earlier occurrence of the last n-1 tokens, n = ngram; or it is an EOS id and min_new_active).
+// The n-gram scan looks at the follower h[s + n - 1] of every start s <= L - n first, so only starts whose follower is in
+// range compare their n - 1 tokens.  The bitmaps must be zero on entry; the caller synchronises afterwards.
+__device__ void mark_history(const History& h, int lo, int hi, bool penalise_on, int ngram, bool min_new_active,
+                             const long long* __restrict__ ictl, unsigned* pen, unsigned* ban) {
+  const int tid = threadIdx.x;
+  if (penalise_on) {
+    for (int i = tid; i < h.L; i += blockDim.x) {
+      const int t = h[i];
+      if (t >= lo && t < hi) atomicOr(pen + ((t - lo) >> 5), 1u << ((t - lo) & 31));
+    }
+  }
+  if (ngram > 0 && h.L + 1 >= ngram) {
+    const int q = h.L - ngram + 1;               // the last n - 1 tokens: h[q, L)
+    for (int s = tid; s <= h.L - ngram; s += blockDim.x) {
+      const int f = h[s + ngram - 1];
+      if (f < lo || f >= hi) continue;
+      bool eq = true;
+      for (int k = 0; k < ngram - 1 && eq; ++k) eq = h[s + k] == h[q + k];
+      if (eq) atomicOr(ban + ((f - lo) >> 5), 1u << ((f - lo) & 31));
+    }
+  }
+  if (min_new_active && tid == 0) {
+    const int n_eos = (int)min(ictl[4], (long long)MAX_EOS);
+    for (int k = 0; k < n_eos; ++k) {
+      const long long t = ictl[5 + k];
+      if (t >= lo && t < hi) atomicOr(ban + ((t - lo) >> 5), 1u << ((t - lo) & 31));
+    }
+  }
+}
+
+// The value the sampler works on: the bf16 logit, or its processed fp32 value (bitmaps in global scratch, read past L1).
+struct RawLogit {
+  const __nv_bfloat16* row;
+  __device__ __forceinline__ float operator()(int i) const { return __bfloat162float(row[i]); }
+};
+struct ProcessedLogit {
+  const __nv_bfloat16* row;
+  const unsigned* pen;
+  const unsigned* ban;
+  float p;
+  __device__ __forceinline__ float operator()(int i) const {
+    float x = __bfloat162float(row[i]);
+    const unsigned bit = 1u << (i & 31);
+    if (__ldcg(pen + (i >> 5)) & bit) x = penalise(x, p);
+    if (__ldcg(ban + (i >> 5)) & bit) x = -INFINITY;
+    return x;
+  }
+};
 
 struct ArgMax {
   float v;
@@ -321,14 +394,16 @@ __device__ ArgMax block_reduce_argmax(ArgMax best, ArgMax* am) {
   return am[0];
 }
 
-// Block-wide argmax of a bf16 row (ties to the lowest index); am: 32 shared slots.  Every thread gets the result.
-__device__ ArgMax block_argmax(const __nv_bfloat16* __restrict__ row, int V, ArgMax* am) {
+// Block-wide argmax of a row's values x(i) (ties to the lowest index); am: 32 shared slots.  Every thread gets the result.
+template <class Load>
+__device__ ArgMax block_argmax(Load x, int V, ArgMax* am) {
   ArgMax best = {-INFINITY, V};
-  for (int i = threadIdx.x; i < V; i += blockDim.x) best = argmax_merge(best, ArgMax{__bfloat162float(row[i]), i});
+  for (int i = threadIdx.x; i < V; i += blockDim.x) best = argmax_merge(best, ArgMax{x(i), i});
   best = block_reduce_argmax(best, am);
   if (best.i >= V) best.i = 0;                   // all-NaN row: token 0 rather than an out-of-range id
   return best;
 }
+__device__ ArgMax block_argmax(const __nv_bfloat16* __restrict__ row, int V, ArgMax* am) { return block_argmax(RawLogit{row}, V, am); }
 
 // The unnormalised warped probability of logit x: exp(x / temp - mx).  Every user goes through this one expression, so
 // a weight recomputed from the logits is bit-identical to the one the thresholds were found on.
@@ -338,11 +413,11 @@ __device__ __forceinline__ float warped_weight(float x, float temp, float mx) {
 
 // HF warper order: temperature, then top-k, then top-p.  Fills e[i] with the kept weights (0 elsewhere) and returns the
 // threshold T on the weight's bit pattern: token i is kept iff bits(warped_weight(x_i)) >= T.  mx = max logit / temp.
-__device__ uint32_t warp_weights(const __nv_bfloat16* __restrict__ row, int V, float temp, int top_k, float top_p, float mx, float* e,
-                                 float* red) {
+template <class Load>
+__device__ uint32_t warp_weights(Load x, int V, float temp, int top_k, float top_p, float mx, float* e, float* red) {
   const int tid = threadIdx.x;
   uint32_t T = 0;
-  for (int i = tid; i < V; i += blockDim.x) e[i] = warped_weight(__bfloat162float(row[i]), temp, mx);
+  for (int i = tid; i < V; i += blockDim.x) e[i] = warped_weight(x(i), temp, mx);
   __syncthreads();
   if (top_k > 0 && top_k < V) {
     T = bisect_threshold<false>(e, V, (float)top_k, red);
@@ -361,6 +436,10 @@ __device__ uint32_t warp_weights(const __nv_bfloat16* __restrict__ row, int V, f
     T = max(T, t);
   }
   return T;
+}
+__device__ uint32_t warp_weights(const __nv_bfloat16* __restrict__ row, int V, float temp, int top_k, float top_p, float mx, float* e,
+                                 float* red) {
+  return warp_weights(RawLogit{row}, V, temp, top_k, top_p, mx, e, red);
 }
 
 // Inverse CDF in index order over the weights e[0, V): u in (0, 1] picks the token; `fallback` when rounding leaves r
@@ -410,10 +489,33 @@ __device__ int draw_index(const float* e, int V, float u, int fallback, float* r
   return *tok_sm;
 }
 
+// One row's token from its values x(i): the argmax (greedy, and the reference point of the exponentials), or a draw from
+// the warped weights.  finite_only: a row with no finite value keeps its argmax instead of drawing.
+template <class Load>
+__device__ int pick_token(Load x, int V, const long long* __restrict__ ictl, const float* __restrict__ fctl, int b, int g,
+                          bool finite_only, float* e, float* red, ArgMax* am, int* tok_sm) {
+  const ArgMax best = block_argmax(x, V, am);
+  const bool do_sample = ictl[0] != 0;
+  const int top_k = (int)ictl[1];
+  int tok = best.i;
+  if (do_sample && top_k != 1 && (!finite_only || best.v > -INFINITY)) {
+    const float temp = fctl[0], top_p = fctl[1];
+    warp_weights(x, V, temp, top_k, top_p, best.v / temp, e, red);
+    curandStatePhilox4_32_10_t rng;
+    curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)g, &rng);
+    tok = draw_index(e, V, curand_uniform(&rng), best.i, red, tok_sm);   // u in (0, 1]
+  }
+  return tok;
+}
+
+// With a history (hist int32 [B, ldh]: row b's tokens at positions 0 .. pos[b]), the logits processors run when the control
+// blocks turn them on: the row's bitmaps (scratch [B][2][nw] words, nw = ceil(V / 32): penalised, banned) are cleared and
+// marked, and the token is picked from the processed values.  The emitted token is appended at hist[b, pos[b] + 1].
 __global__ void __launch_bounds__(SAMPLE_THREADS)
 sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const long long* __restrict__ ictl,
               const float* __restrict__ fctl, int* __restrict__ pos, int* __restrict__ gen, int* __restrict__ finished,
-              long long* __restrict__ out, int max_new, long long* __restrict__ ids_next) {
+              long long* __restrict__ out, int max_new, long long* __restrict__ ids_next, int* __restrict__ hist, int ldh,
+              unsigned* __restrict__ scratch) {
   extern __shared__ __align__(16) float e[];     // [V] exp(x - max) of the kept tokens, 0 elsewhere
   __shared__ float red[33];
   __shared__ ArgMax am[32];
@@ -422,18 +524,20 @@ sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, con
   pdl_wait();
   const int b = blockIdx.x, tid = threadIdx.x;
   const __nv_bfloat16* row = logits + (long long)b * ld;
-
-  // ---- argmax (greedy, and the reference point of the exponentials)
-  const ArgMax best = block_argmax(row, V, am);
-  const bool do_sample = ictl[0] != 0;
-  const int top_k = (int)ictl[1];
-  int tok = best.i;
-  if (do_sample && top_k != 1) {
-    const float temp = fctl[0], top_p = fctl[1];
-    warp_weights(row, V, temp, top_k, top_p, best.v / temp, e, red);
-    curandStatePhilox4_32_10_t rng;
-    curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)gen[b], &rng);
-    tok = draw_index(e, V, curand_uniform(&rng), best.i, red, &tok_sm);   // u in (0, 1]
+  int tok;
+  if (hist != nullptr && processors_on(ictl, fctl)) {
+    const int nw = ceil_div(V, 32), L = pos[b] + 1, g = gen[b];
+    unsigned* pen = scratch + (long long)b * 2 * nw;
+    unsigned* ban = pen + nw;
+    for (int i = tid; i < 2 * nw; i += blockDim.x) pen[i] = 0u;
+    __syncthreads();
+    const float p = fctl[2];
+    const int* h = hist + (long long)b * ldh;
+    mark_history(History{h, h, L, L}, 0, V, p != 1.f, (int)ictl[CTL_NGRAM], g < ictl[CTL_MIN_NEW], ictl, pen, ban);
+    __syncthreads();
+    tok = pick_token(ProcessedLogit{row, pen, ban, p}, V, ictl, fctl, b, g, true, e, red, am, &tok_sm);
+  } else {
+    tok = pick_token(RawLogit{row}, V, ictl, fctl, b, gen[b], false, e, red, am, &tok_sm);
   }
   if (tid == 0) {
     const int g = gen[b];
@@ -442,6 +546,7 @@ sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, con
     if (g < max_new) out[(long long)b * max_new + g] = t;
     ids_next[b] = t;
     gen[b] = g + 1;
+    if (hist != nullptr && pos[b] + 1 < ldh) hist[(long long)b * ldh + pos[b] + 1] = (int)t;
     pos[b] = pos[b] + 1;
     if (!fin) {
       const int n_eos = (int)min(ictl[4], (long long)MAX_EOS);
@@ -759,15 +864,43 @@ constexpr int TOPK_SPLIT = TOPK_THREADS * TOPK_PER;  // vocabulary entries per b
 constexpr int STEP_THREADS = 512;                    // beam_step: one thread per (beam, split) candidate list
 constexpr float NEG = -1.0e9f;                       // HF's score offset of a continuation that must not be chosen
 
+// The K best of the entries in `avail` (bit e: key[e] of this thread, entry base + 128*e + tid), by value descending and
+// then index ascending, to cv / ci[0..K) (index -1, value -inf once none is left).
+__device__ __forceinline__ void split_topk(const float* key, unsigned avail, int base, int K, ArgMax* am, float* __restrict__ cv, int* __restrict__ ci) {
+  const int tid = threadIdx.x;
+  for (int k = 0; k < K; ++k) {
+    ArgMax best{-INFINITY, INT_MAX};
+#pragma unroll
+    for (int e = 0; e < TOPK_PER; ++e)
+      if ((avail >> e) & 1u) best = argmax_merge(best, ArgMax{key[e], base + e * TOPK_THREADS + tid});
+    best = block_reduce_argmax(best, am);
+    const bool none = best.i == INT_MAX;
+    if (!none && (best.i - base) % TOPK_THREADS == tid) avail &= ~(1u << ((best.i - base) / TOPK_THREADS));
+    if (tid == 0) {
+      cv[k] = none ? -INFINITY : best.v;
+      ci[k] = none ? -1 : best.i;
+    }
+  }
+}
+
 // grid (splits, rows), block 128.  Split s of row r is logits[r, s*1024 .. s*1024 + 1024); thread t holds entries
 // s*1024 + 128*e + t in registers.  Writes part_ml[r][s] = (max, sum exp(x - max)) in fp32 and cand[r][s][0..K) = the
 // split's K largest logits, by value descending and then index ascending (index -1, value -inf past the split's end).
-// Within one row this is also the order of the log-probabilities.
+// Within one row this is also the order of the log-probabilities.  cand rows hold ck >= K entries.
+//
+// With the logits processors on (fctl not null and the control blocks turn them on), the row's history is its prompt
+// (prompt[g, 0 .. plens[g]), g = r / nb) followed by run_seq[tstep[g] & 1][r, 0 .. tstep[g]), and ck >= 2K.  A penalised
+// token's log-prob (z - lse) * p is monotone in z within the penalised tokens, but not against the others, so the split
+// gives two lists: cand[..][0..K) the best of the unpenalised tokens, with the banned ones (any class) as -inf, and
+// cand[..][K..2K) the best of the penalised tokens that are not banned, by their raw logits.  beam_step maps and merges them.
 __global__ void __launch_bounds__(TOPK_THREADS)
-beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, int K, float* __restrict__ part_ml,
-                 float* __restrict__ cand_v, int* __restrict__ cand_i) {
+beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, int K, int ck, float* __restrict__ part_ml,
+                 float* __restrict__ cand_v, int* __restrict__ cand_i, const long long* __restrict__ ictl, const float* __restrict__ fctl,
+                 const int* __restrict__ prompt, int ldp, const int* __restrict__ plens, const int* __restrict__ run_seq,
+                 const int* __restrict__ tstep, int nb, int max_new) {
   __shared__ float red[33];
   __shared__ ArgMax am[32];
+  __shared__ unsigned pen_sm[TOPK_SPLIT / 32], ban_sm[TOPK_SPLIT / 32];
   pdl_launch_dependents();
   pdl_wait();
   const int s = blockIdx.x, r = blockIdx.y, ns = gridDim.x, tid = threadIdx.x;
@@ -794,22 +927,33 @@ beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, 
     part_ml[2 * rs] = mx;
     part_ml[2 * rs + 1] = se;
   }
-  unsigned taken = 0u;                           // bit e: entry e of this thread is already a candidate
-  for (int k = 0; k < K; ++k) {
-    ArgMax best{-INFINITY, INT_MAX};
+  unsigned valid = 0u;                           // bit e: entry e of this thread is inside the vocabulary
 #pragma unroll
-    for (int e = 0; e < TOPK_PER; ++e) {
-      const int i = base + e * TOPK_THREADS + tid;
-      if (i < V && !((taken >> e) & 1u)) best = argmax_merge(best, ArgMax{x[e], i});
-    }
-    best = block_reduce_argmax(best, am);
-    const bool none = best.i == INT_MAX;
-    if (!none && (best.i - base) % TOPK_THREADS == tid) taken |= 1u << ((best.i - base) / TOPK_THREADS);
-    if (tid == 0) {
-      cand_v[rs * K + k] = none ? -INFINITY : best.v;
-      cand_i[rs * K + k] = none ? -1 : best.i;
-    }
+  for (int e = 0; e < TOPK_PER; ++e)
+    if (base + e * TOPK_THREADS + tid < V) valid |= 1u << e;
+  if (fctl == nullptr || !processors_on(ictl, fctl)) {
+    split_topk(x, valid, base, K, am, cand_v + rs * ck, cand_i + rs * ck);
+    return;
   }
+  // ---- processors: this split's bits of the row's penalised and banned tokens
+  const int g = r / nb, t = tstep[g], rows = gridDim.y;
+  for (int i = tid; i < TOPK_SPLIT / 32; i += TOPK_THREADS) pen_sm[i] = ban_sm[i] = 0u;
+  __syncthreads();
+  const float p = fctl[2];
+  const History h{prompt + (long long)g * ldp, run_seq + ((long long)(t & 1) * rows + r) * max_new, plens[g], plens[g] + t};
+  mark_history(h, base, base + TOPK_SPLIT, p != 1.f, (int)ictl[CTL_NGRAM], t < ictl[CTL_MIN_NEW], ictl, pen_sm, ban_sm);
+  __syncthreads();
+  unsigned in_pen = 0u;
+#pragma unroll
+  for (int e = 0; e < TOPK_PER; ++e) {
+    const int j = e * TOPK_THREADS + tid;
+    const unsigned bit = 1u << (j & 31);
+    if (ban_sm[j >> 5] & bit) x[e] = -INFINITY;
+    else if (pen_sm[j >> 5] & bit) in_pen |= 1u << e;
+  }
+  in_pen &= valid;
+  split_topk(x, valid & ~in_pen, base, K, am, cand_v + rs * ck, cand_i + rs * ck);
+  split_topk(x, in_pen, base, K, am, cand_v + rs * ck + K, cand_i + rs * ck + K);
 }
 
 // One CTA per prompt g, whose beams are rows g*nb .. g*nb + nb-1.  One step of HF's beam search (t = tokens generated so
@@ -825,12 +969,14 @@ beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, 
 // Histories are int32 [2][rows][max_new], double-buffered by the parity of t: step t reads buffer t & 1 and writes the
 // other one, so beams may swap parents.  Writes ids_next / parent (global row) / run_score of the new running beams, pos
 // += 1, and the finished scores, flags and histories.  A prompt that is done is left untouched (parents = itself).
+// Candidate rows hold ck entries.  With the logits processors on (fctl not null; see beam_topk_kernel) each thread also
+// owns the split's penalised list, scored penalise(logit - lse, p) + run_score, and offers the better of its two heads.
 __global__ void __launch_bounds__(STEP_THREADS)
 beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ cand_v, const int* __restrict__ cand_i, int ns, int V,
-                 int nb, int K, const long long* __restrict__ ictl, float length_penalty, int early_stopping, int max_new,
-                 float* __restrict__ run_score, float* __restrict__ fin_score, int* __restrict__ fin_flag, int* __restrict__ run_seq,
-                 int* __restrict__ fin_seq, int* __restrict__ unsat, int* __restrict__ done, int* __restrict__ tstep,
-                 int* __restrict__ pos, long long* __restrict__ ids_next, int* __restrict__ parent) {
+                 int nb, int K, int ck, const long long* __restrict__ ictl, const float* __restrict__ fctl, float length_penalty,
+                 int early_stopping, int max_new, float* __restrict__ run_score, float* __restrict__ fin_score, int* __restrict__ fin_flag,
+                 int* __restrict__ run_seq, int* __restrict__ fin_seq, int* __restrict__ unsat, int* __restrict__ done,
+                 int* __restrict__ tstep, int* __restrict__ pos, long long* __restrict__ ids_next, int* __restrict__ parent) {
   __shared__ ArgMax am[32];
   __shared__ float lse[MAX_BEAMS];
   __shared__ float sel_v[MAX_KEEP], fcand[MAX_KEEP];
@@ -863,16 +1009,34 @@ beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ ca
 
   // ---- c. K-way merge: thread l owns the sorted list of beam l / ns, split l % ns; its head advances when it wins
   const int nl = nb * ns, jb = tid / ns, sp = tid % ns;
-  int head = 0;
+  const bool two = fctl != nullptr && processors_on(ictl, fctl);
+  const float pen = two ? fctl[2] : 1.f;
+  int head = 0, head2 = 0;
   for (int k = 0; k < K; ++k) {
     ArgMax c{-INFINITY, INT_MAX};
-    if (tid < nl && head < K) {
-      const long long at = ((long long)(row0 + jb) * ns + sp) * K + head;
-      const int ci = cand_i[at];
-      if (ci >= 0) c = ArgMax{(cand_v[at] - lse[jb]) + run_score[row0 + jb], jb * V + ci};
+    bool second = false;
+    if (tid < nl) {
+      const long long at = ((long long)(row0 + jb) * ns + sp) * ck;
+      if (head < K) {
+        const int ci = cand_i[at + head];
+        if (ci >= 0) c = ArgMax{(cand_v[at + head] - lse[jb]) + run_score[row0 + jb], jb * V + ci};
+      }
+      if (two && head2 < K) {
+        const int ci = cand_i[at + K + head2];
+        if (ci >= 0) {
+          const ArgMax c2{penalise(cand_v[at + K + head2] - lse[jb], pen) + run_score[row0 + jb], jb * V + ci};
+          if (argmax_merge(c, c2).i == c2.i) {
+            c = c2;
+            second = true;
+          }
+        }
+      }
     }
     const ArgMax w = block_reduce_argmax(c, am);
-    if (tid < nl && c.i != INT_MAX && w.i == c.i) ++head;     // beam * V + token is unique to one list
+    if (tid < nl && c.i != INT_MAX && w.i == c.i) {           // beam * V + token is unique to one list
+      if (second) ++head2;
+      else ++head;
+    }
     if (tid == 0) {
       sel_v[k] = w.v;
       sel_f[k] = w.i;
@@ -1087,9 +1251,11 @@ ODB_EXPORT int odb_dec_attn(const void* q, long long ldq, const void* kc, const 
 }
 
 // logits [B, ld] bf16; ictl / fctl: see dec::sample_kernel; pos / gen / finished int32 [B]; out int64 [B, max_new];
-// ids_next int64 [B].  The vocabulary lives in shared memory as fp32: V <= 56000.
+// ids_next int64 [B]; hist: nullptr (no logits processors), or int32 [B, ldh] with scratch int32 [B, 2 * ceil(V / 32)].
+// The vocabulary lives in shared memory as fp32: V <= 56000.
 ODB_EXPORT int odb_dec_sample(const void* logits, long long ld, int V, const void* ictl, const void* fctl, void* pos, void* gen,
-                              void* finished, void* out, int max_new, void* ids_next, int B, cudaStream_t st) {
+                              void* finished, void* out, int max_new, void* ids_next, void* hist, int ldh, void* scratch, int B,
+                              cudaStream_t st) {
   const int smem = V * 4;
   if (smem > 224000) return -1;
   static int attr = 0;
@@ -1100,7 +1266,7 @@ ODB_EXPORT int odb_dec_sample(const void* logits, long long ld, int V, const voi
   }
   launch_pdl(dec::sample_kernel, dim3(B), dim3(dec::SAMPLE_THREADS), smem, st, (const __nv_bfloat16*)logits, ld, V,
              (const long long*)ictl, (const float*)fctl, (int*)pos, (int*)gen, (int*)finished, (long long*)out, max_new,
-             (long long*)ids_next);
+             (long long*)ids_next, (int*)hist, ldh, (unsigned*)scratch);
   ODB_CHECK_LAST();
   return 0;
 }
@@ -1174,29 +1340,35 @@ ODB_EXPORT int odb_dec_accept(const void* plog, long long ldp, const void* qlog,
 // Vocabulary splits of beam_topk for a vocabulary of V (sizes its partials).
 ODB_EXPORT int odb_dec_beam_splits(int V) { return odb::ceil_div(V, dec::TOPK_SPLIT); }
 
-// logits [rows, ld] bf16; part_ml fp32 [rows, splits, 2]; cand_v fp32 / cand_i int32 [rows, splits, K]; K <= 72.
-ODB_EXPORT int odb_dec_beam_topk(const void* logits, long long ld, int V, int K, void* part_ml, void* cand_v, void* cand_i, int rows,
-                                 cudaStream_t st) {
-  if (K < 1 || K > dec::MAX_KEEP || V < K) return -1;
+// logits [rows, ld] bf16; part_ml fp32 [rows, splits, 2]; cand_v fp32 / cand_i int32 [rows, splits, ck]; K <= 72.
+// fctl: nullptr (no logits processors), or the sampler's fp32 control block with ck >= 2K, prompt int32 [rows / nb, ldp],
+// plens / tstep int32 [rows / nb] and run_seq int32 [2, rows, max_new] (see dec::beam_topk_kernel).
+ODB_EXPORT int odb_dec_beam_topk(const void* logits, long long ld, int V, int K, int ck, void* part_ml, void* cand_v, void* cand_i,
+                                 const void* ictl, const void* fctl, const void* prompt, int ldp, const void* plens, const void* run_seq,
+                                 const void* tstep, int nb, int max_new, int rows, cudaStream_t st) {
+  if (K < 1 || K > dec::MAX_KEEP || V < K || ck < K || (fctl != nullptr && (ck < 2 * K || nb < 1 || rows % nb))) return -1;
   launch_pdl(dec::beam_topk_kernel, dim3(odb::ceil_div(V, dec::TOPK_SPLIT), rows), dim3(dec::TOPK_THREADS), 0, st,
-             (const __nv_bfloat16*)logits, ld, V, K, (float*)part_ml, (float*)cand_v, (int*)cand_i);
+             (const __nv_bfloat16*)logits, ld, V, K, ck, (float*)part_ml, (float*)cand_v, (int*)cand_i, (const long long*)ictl,
+             (const float*)fctl, (const int*)prompt, ldp, (const int*)plens, (const int*)run_seq, (const int*)tstep, nb, max_new);
   ODB_CHECK_LAST();
   return 0;
 }
 
 // B prompts of nb <= 8 beams (rows = B * nb); the beam_topk partials of V; ictl: the sampler's control block (EOS ids);
 // early_stopping 0 False, 1 True, 2 "never"; run_score / fin_score fp32 [rows]; fin_flag / pos / parent int32 [rows];
-// run_seq / fin_seq int32 [2, rows, max_new]; unsat / done / tstep int32 [B]; ids_next int64 [rows].  See dec::beam_step_kernel.
-ODB_EXPORT int odb_dec_beam_step(const void* part_ml, const void* cand_v, const void* cand_i, int V, int nb, int K, const void* ictl,
-                                 float length_penalty, int early_stopping, int max_new, void* run_score, void* fin_score, void* fin_flag,
-                                 void* run_seq, void* fin_seq, void* unsat, void* done, void* tstep, void* pos, void* ids_next,
-                                 void* parent, int B, cudaStream_t st) {
+// run_seq / fin_seq int32 [2, rows, max_new]; unsat / done / tstep int32 [B]; ids_next int64 [rows]; candidate rows of ck
+// entries; fctl: nullptr, or the processors' control block as for beam_topk.  See dec::beam_step_kernel.
+ODB_EXPORT int odb_dec_beam_step(const void* part_ml, const void* cand_v, const void* cand_i, int V, int nb, int K, int ck,
+                                 const void* ictl, const void* fctl, float length_penalty, int early_stopping, int max_new, void* run_score,
+                                 void* fin_score, void* fin_flag, void* run_seq, void* fin_seq, void* unsat, void* done, void* tstep,
+                                 void* pos, void* ids_next, void* parent, int B, cudaStream_t st) {
   const int ns = odb::ceil_div(V, dec::TOPK_SPLIT);
   if (nb < 1 || nb > dec::MAX_BEAMS || K < 1 || K > dec::MAX_KEEP || nb * ns > dec::STEP_THREADS || early_stopping < 0 ||
-      early_stopping > 2 || max_new < 1)
+      early_stopping > 2 || max_new < 1 || ck < K || (fctl != nullptr && ck < 2 * K))
     return -1;
   launch_pdl(dec::beam_step_kernel, dim3(B), dim3(dec::STEP_THREADS), 0, st, (const float*)part_ml, (const float*)cand_v,
-             (const int*)cand_i, ns, V, nb, K, (const long long*)ictl, length_penalty, early_stopping, max_new, (float*)run_score,
+             (const int*)cand_i, ns, V, nb, K, ck, (const long long*)ictl, (const float*)fctl, length_penalty, early_stopping, max_new,
+             (float*)run_score,
              (float*)fin_score, (int*)fin_flag, (int*)run_seq, (int*)fin_seq, (int*)unsat, (int*)done, (int*)tstep, (int*)pos,
              (long long*)ids_next, (int*)parent);
   ODB_CHECK_LAST();

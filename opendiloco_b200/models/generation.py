@@ -29,6 +29,7 @@ leaves the training buffers and graph untouched.
 """
 from __future__ import annotations
 
+import math
 import os
 import warnings
 from dataclasses import dataclass
@@ -92,6 +93,9 @@ class DecodeState:
         self.pos, self.gen, self.finished, self.lens = i32(), i32(), i32(), i32()
         self.out = torch.zeros(B, Smax, dtype=torch.int64, device=device)
         self.ictl, self.fctl = DK.make_controls(False, 1.0, 0, 1.0, 0, 0, [], device)
+        # token histories of the logits processors: the real prompt tokens, then the generated ones (the sampler appends)
+        self.hist = torch.zeros(B, Smax, dtype=torch.int32, device=device)
+        self.proc_scratch = torch.zeros(B, 2 * ((V + 31) // 32), dtype=torch.int32, device=device)
         self.kernels = DK.usable(self.res, D, Hq, Hkv)
         self.part_o = self.part_ml = None
         if self.kernels:
@@ -108,8 +112,10 @@ class DecodeState:
             self._prefill = _PrefillBuffers(self.cfg, T, self.device, self.dtype)
         return self._prefill
 
-    def set_controls(self, do_sample: bool, temperature: float, top_k: int, top_p: float, seed: int, pad: int, eos: list[int]):
-        ictl, fctl = DK.make_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, "cpu")
+    def set_controls(self, do_sample: bool, temperature: float, top_k: int, top_p: float, seed: int, pad: int, eos: list[int],
+                     repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_new_tokens: int = 0):
+        ictl, fctl = DK.make_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, "cpu", repetition_penalty,
+                                      no_repeat_ngram_size, min_new_tokens)
         self.ictl.copy_(ictl)
         self.fctl.copy_(fctl)
 
@@ -141,6 +147,8 @@ def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor) -> No
     st.pos.copy_(lens - 1)
     st.gen.zero_()
     st.finished.zero_()
+    n = min(Sp, st.Smax)
+    st.hist[:, :n].copy_(ids[:, :n])
     pb.ids.copy_(ids.reshape(-1))
     delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
                            on_qkv=lambda l, qkv: DK.kv_fill(qkv, st.lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D))
@@ -195,7 +203,7 @@ def _head(cfg, ar, st: DecodeState, delta) -> None:
 
 def _head_and_sample(cfg, ar, st: DecodeState, delta) -> None:
     _head(cfg, ar, st, delta)
-    DK.sample(st.logits, st.ictl, st.fctl, st.pos, st.gen, st.finished, st.out, st.ids)
+    DK.sample(st.logits, st.ictl, st.fctl, st.pos, st.gen, st.finished, st.out, st.ids, st.hist, st.proc_scratch)
 
 
 # ------------------------------------------------------------------------------------------------ decode step
@@ -458,12 +466,14 @@ class BeamState:
             warnings.warn(f"beam search: the selection and reorder kernels take num_beams * ceil(vocab_size / 1024) <= 512 and "
                           f"at most 32768 positions (here {nb} x {DK.beam_splits(cfg.vocab_size)} and {Smax}); this run uses the "
                           "PyTorch references, with host syncs, whole-cache reorders and no CUDA graph", stacklevel=3)
+        self.prompt, self.plens = i32(B, Smax), i32(B)              # the compacted prompts: the start of every beam's history
         self.table = self.part_ml = self.cand_v = self.cand_i = None
         if self.kernels:
             nsp = DK.beam_splits(cfg.vocab_size)
             self.table = i32(rows, Smax // 128)
             self.part_ml = f32(rows, nsp, 2)
-            self.cand_v, self.cand_i = f32(rows, nsp, K), i32(rows, nsp, K)
+            # two lists of K per split: the unpenalised and the penalised tokens (the second one only with the processors on)
+            self.cand_v, self.cand_i = f32(rows, nsp, 2 * K), i32(rows, nsp, 2 * K)
         self.graph = None
         self.graph_key = None
 
@@ -523,7 +533,7 @@ def beam_select(bs: BeamState, length_penalty: float, early_stopping: int) -> No
     st = bs.dec
     DK.beam_select(st.logits, st.ictl, bs.nb, bs.K, length_penalty, early_stopping, bs.max_new, bs.run_score, bs.fin_score,
                    bs.fin_flag, bs.run_seq, bs.fin_seq, bs.unsat, bs.done, bs.tstep, st.pos, st.ids, bs.parent, bs.part_ml,
-                   bs.cand_v, bs.cand_i)
+                   bs.cand_v, bs.cand_i, fctl=st.fctl, prompt=bs.prompt, plens=bs.plens)
     DK.beam_reorder(st.kv, bs.table, bs.parent, st.pos, bs.nb)
 
 
@@ -559,12 +569,14 @@ def beam_step(model, bs: BeamState, length_penalty: float, early_stopping: int, 
 
 
 def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R: int, length_penalty: float, early_stopping,
-                   pad: int, eos: list[int]) -> tuple[torch.Tensor, torch.Tensor]:
-    B = comp.shape[0]
+                   pad: int, eos: list[int], processors: tuple = (1.0, 0, 0)) -> tuple[torch.Tensor, torch.Tensor]:
+    B, Sp = comp.shape
     es = DK.EARLY_STOPPING[early_stopping]
     bs = beam_state(model, B, nb, DK.beams_to_keep(nb, len(eos)), max_new_tokens, Smax)
-    bs.dec.set_controls(False, 1.0, 0, 1.0, 0, pad, eos)
+    bs.dec.set_controls(False, 1.0, 0, 1.0, 0, pad, eos, *processors)
     bs.reset(pad)
+    bs.prompt[:, :Sp].copy_(comp)
+    bs.plens.copy_(lens)
     beam_prefill(model, bs, comp, lens)
     beam_select(bs, length_penalty, es)              # step 0 on the prefill logits: only beam 0 has score 0
     for t in range(1, max_new_tokens):
@@ -592,6 +604,23 @@ def _check_beams(num_beams, num_return_sequences, do_sample: bool, assistant_mod
                          f"{DK.beams_to_keep(num_beams, n_eos)} tokens, the model has {vocab_size}")
 
 
+def _check_processors(repetition_penalty, no_repeat_ngram_size, min_new_tokens, assistant_model) -> bool:
+    """Validates the logits-processor arguments (HF's terms); True when one of them is on."""
+    if isinstance(repetition_penalty, bool) or not isinstance(repetition_penalty, (int, float)) \
+            or not math.isfinite(repetition_penalty) or not repetition_penalty > 0:
+        raise ValueError(f"repetition_penalty must be a finite float > 0 (1.0: off), got {repetition_penalty!r}")
+    if isinstance(no_repeat_ngram_size, bool) or not isinstance(no_repeat_ngram_size, int) \
+            or not 0 <= no_repeat_ngram_size <= DK.MAX_NGRAM:
+        raise ValueError(f"no_repeat_ngram_size must be an integer in [0, {DK.MAX_NGRAM}] (0: off), got {no_repeat_ngram_size!r}")
+    if isinstance(min_new_tokens, bool) or not isinstance(min_new_tokens, int) or min_new_tokens < 0:
+        raise ValueError(f"min_new_tokens must be an integer >= 0 (0: off), got {min_new_tokens!r}")
+    on = repetition_penalty != 1.0 or no_repeat_ngram_size > 0 or min_new_tokens > 0
+    if on and assistant_model is not None:
+        raise ValueError("repetition_penalty, no_repeat_ngram_size and min_new_tokens are not supported yet together with "
+                         "assistant_model")
+    return on
+
+
 # ------------------------------------------------------------------------------------------------ generate
 def _eos_list(eos) -> list[int]:
     if eos is None:
@@ -606,7 +635,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
              do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
              pad_token_id: int | None = None, seed: int = 0, assistant_model=None, num_assistant_tokens: int = 4, num_beams: int = 1,
              length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1,
-             return_dict_in_generate: bool = False) -> torch.Tensor | GenerateOutput:
+             return_dict_in_generate: bool = False, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
+             min_new_tokens: int = 0) -> torch.Tensor | GenerateOutput:
     """See :meth:`LlamaForCausalLM.generate`."""
     cfg, ar = model.config, model.arena
     if ar.param_sharded:
@@ -627,6 +657,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
         _check_assistant(model, assistant_model, P, max_new_tokens, num_assistant_tokens)
     eos = _eos_list(cfg.eos_token_id if eos_token_id is None else eos_token_id)
     _check_beams(num_beams, num_return_sequences, do_sample, assistant_model, early_stopping, cfg.vocab_size, len(eos))
+    _check_processors(repetition_penalty, no_repeat_ngram_size, min_new_tokens, assistant_model)
+    processors = (float(repetition_penalty), no_repeat_ngram_size, min_new_tokens)
     dev = ar.device
     ids = input_ids.to(dev)
     if attention_mask is None:
@@ -656,12 +688,12 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))
     if num_beams > 1:
         new, scores = _beam_generate(model, comp, lens, Smax, max_new_tokens, num_beams, num_return_sequences, length_penalty,
-                                     early_stopping, pad, eos)
+                                     early_stopping, pad, eos, processors)
         out = torch.cat([ids.repeat_interleave(num_return_sequences, dim=0), new], dim=1)
         return GenerateOutput(out, scores) if return_dict_in_generate else out
     st = decode_state(model, B, Smax)
 
-    st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos)
+    st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, *processors)
     st.out.fill_(pad)
     prefill(model, st, comp, lens)
     for t in range(1, max_new_tokens):

@@ -744,7 +744,8 @@ class LlamaForCausalLM(nn.Module):
                  do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
                  pad_token_id: int | None = None, seed: int = 0, assistant_model: "LlamaForCausalLM | None" = None,
                  num_assistant_tokens: int = 4, num_beams: int = 1, length_penalty: float = 1.0, early_stopping=False,
-                 num_return_sequences: int = 1, return_dict_in_generate: bool = False):
+                 num_return_sequences: int = 1, return_dict_in_generate: bool = False, repetition_penalty: float = 1.0,
+                 no_repeat_ngram_size: int = 0, min_new_tokens: int = 0):
         """KV-cached text generation with HF ``generate`` keyword names.  Returns LongTensor [B, P + max_new_tokens]: the
         prompt as given, then the new tokens.
 
@@ -767,7 +768,7 @@ class LlamaForCausalLM(nn.Module):
         ``num_assistant_tokens`` beyond either model's ``max_position_embeddings``.
 
         ``num_beams`` > 1 (at most 8) runs deterministic beam search as transformers' ``generate(num_beams=...,
-        do_sample=False)``: fp32 log-softmax of the logits without logits processors, ``length_penalty``,
+        do_sample=False)``: fp32 log-softmax of the logits, then the logits processors below, ``length_penalty``,
         ``early_stopping`` (True, False or ``"never"``) and the finished-hypothesis rules of HF, ties to the lower
         ``beam * V + token``.  It returns ``[B * num_return_sequences, P + max_new_tokens]``: row ``b * R + r`` is prompt b
         as given, then its r-th best hypothesis (EOS included), then ``pad_token_id``.  bf16-mixed CUDA models run the
@@ -778,6 +779,19 @@ class LlamaForCausalLM(nn.Module):
         ``num_return_sequences`` outside [1, num_beams], an unknown ``early_stopping``, or ``do_sample=True`` or
         ``assistant_model`` with ``num_beams`` > 1.
 
+        Logits processors, HF's, applied in HF's order to the fp32 value of each logit (greedy and sampling: before the
+        temperature, top-k and top-p warpers) or log-prob (beam search), on greedy, sampling and beam search:
+        ``repetition_penalty`` (a finite float > 0; 1.0 is off) divides the positive and multiplies the negative values of
+        every token in the row's history, once per distinct token; ``no_repeat_ngram_size`` n (0..64; 0 is off) forbids
+        any n-gram from occurring twice in the history; ``min_new_tokens`` (0 is off) forbids every EOS id until that many
+        tokens have been generated (nothing without EOS ids).  A row's history is its real prompt tokens followed by its
+        generated tokens (beam search: the beam's own running sequence).  Unlike HF, the padding of a left-padded batch is
+        not part of the history, so every row generates what it would alone.  A greedy row whose values are all -inf
+        emits token 0; a sampled one its processed argmax.  With beam search, ``sequences_scores`` sum the processed
+        log-probs, as in HF.  The settings live in device memory: changing them replays the same CUDA graphs.  Raises
+        ValueError for values outside those ranges, or for any of them on together with ``assistant_model`` (not supported
+        yet).
+
         ``return_dict_in_generate=True`` returns a ``GenerateOutput`` with ``sequences`` and ``sequences_scores`` (fp32
         [B * num_return_sequences]: each hypothesis's summed log-probabilities / generated_len ** length_penalty; None
         without beam search)."""
@@ -787,7 +801,8 @@ class LlamaForCausalLM(nn.Module):
                         temperature=temperature, top_k=top_k, top_p=top_p, eos_token_id=eos_token_id, pad_token_id=pad_token_id,
                         seed=seed, assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens, num_beams=num_beams,
                         length_penalty=length_penalty, early_stopping=early_stopping, num_return_sequences=num_return_sequences,
-                        return_dict_in_generate=return_dict_in_generate)
+                        return_dict_in_generate=return_dict_in_generate, repetition_penalty=repetition_penalty,
+                        no_repeat_ngram_size=no_repeat_ngram_size, min_new_tokens=min_new_tokens)
 
     @torch.no_grad()
     def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None):

@@ -33,7 +33,7 @@ _lib.register_optional("odb_dec_attn_chunks", [c_int])
 _lib.register_optional("odb_dec_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_int,
                                         c_int, c_int, c_int, c_float, c_void_p])
 _lib.register_optional("odb_dec_sample", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                          c_void_p, c_int, c_void_p])
+                                          c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p])
 _lib.register_optional("odb_dec_rope_append_multi", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                                      c_int, c_int, c_int, c_void_p])
 _lib.register_optional("odb_dec_verify_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int,
@@ -41,16 +41,22 @@ _lib.register_optional("odb_dec_verify_attn", [c_void_p, c_ll, c_void_p, c_void_
 _lib.register_optional("odb_dec_accept", [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p])
 _lib.register_optional("odb_dec_beam_splits", [c_int])
-_lib.register_optional("odb_dec_beam_topk", [c_void_p, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p])
-_lib.register_optional("odb_dec_beam_step", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_float, c_int, c_int,
-                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                             c_void_p, c_void_p, c_int, c_void_p])
+_lib.register_optional("odb_dec_beam_topk", [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p])
+_lib.register_optional("odb_dec_beam_step", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
+                                             c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_void_p, c_int, c_void_p])
 _lib.register_optional("odb_dec_beam_reorder", [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p])
 
 MAX_EOS = 8
-# int64 control block of the sampler: do_sample, top_k, seed, pad_token_id, n_eos, eos ids
+# int64 control block of the sampler: do_sample, top_k, seed, pad_token_id, n_eos, eos ids, then the logits processors'
+# no_repeat_ngram_size and min_new_tokens.  fp32 block: temperature, top_p, repetition_penalty.
 CTL_DO_SAMPLE, CTL_TOP_K, CTL_SEED, CTL_PAD, CTL_N_EOS, CTL_EOS = range(6)
-CTL_SIZE = CTL_EOS + MAX_EOS
+CTL_NGRAM = CTL_EOS + MAX_EOS
+CTL_MIN_NEW = CTL_NGRAM + 1
+CTL_SIZE = CTL_MIN_NEW + 1
+FCTL_TEMPERATURE, FCTL_TOP_P, FCTL_PENALTY = range(3)
+MAX_NGRAM = 64                    # the largest no_repeat_ngram_size generate() takes
 MAX_SAMPLE_VOCAB = 56000          # the sampler keeps one fp32 per vocabulary entry in shared memory
 
 
@@ -253,7 +259,7 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor, ictl: torch.Tensor, fctl: tor
         _lib.count_launch()
         return
     c = ictl.tolist()
-    temperature, top_p = (float(v) for v in fctl.tolist())
+    temperature, top_p = (float(v) for v in fctl.tolist()[:2])
     greedy = not (c[CTL_DO_SAMPLE] and c[CTL_TOP_K] != 1)
     eos = set(c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]])
     p_all = plog.float().view(K + 1, B, V)
@@ -319,7 +325,8 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
                 max_new: int, run_score: torch.Tensor, fin_score: torch.Tensor, fin_flag: torch.Tensor, run_seq: torch.Tensor,
                 fin_seq: torch.Tensor, unsat: torch.Tensor, done: torch.Tensor, tstep: torch.Tensor, pos: torch.Tensor,
                 ids_next: torch.Tensor, parent: torch.Tensor, part_ml: torch.Tensor | None = None, cand_v: torch.Tensor | None = None,
-                cand_i: torch.Tensor | None = None) -> None:
+                cand_i: torch.Tensor | None = None, fctl: torch.Tensor | None = None, prompt: torch.Tensor | None = None,
+                plens: torch.Tensor | None = None) -> None:
     """One step of deterministic beam search (transformers' ``_beam_search`` with do_sample=False) over logits
     [B * num_beams, V] (row b * num_beams + j: beam j of prompt b).
 
@@ -334,20 +341,37 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
     continues), run_score, pos += 1, tstep += 1, the finished state, and the histories: int32 [2, rows, max_new]
     double-buffered by the parity of t (step t reads buffer t & 1 and writes the other).  Done prompts keep everything,
     with parent = the row itself.  With the beam_topk partials (part_ml fp32 [rows, beam_splits(V), 2], cand_v fp32 /
-    cand_i int32 [rows, beam_splits(V), K]) the kernels run, otherwise ``beam_step_reference``."""
+    cand_i int32 [rows, beam_splits(V), ck >= K]) the kernels run, otherwise ``beam_step_reference``.
+
+    Logits processors: with ``fctl`` (the fp32 control block of ``make_controls``), ``prompt`` (int32 [B, S]: the
+    compacted prompts) and ``plens`` (int32 [B]) given and the processors on in the control blocks, they apply to the
+    fp32 log-probs as in HF's ``_beam_search``: log_softmax of the unprocessed row, then ``process_logits_reference``'s
+    rules (not renormalised), then + run_score.  Beam row r of prompt b has the history ``prompt[b, :plens[b]]`` followed
+    by ``run_seq[t & 1, r, :t]`` and has generated t tokens; at step 0 that is the prompt alone.  Scores are then sums of
+    processed log-probs.  The kernel path needs ck >= 2K: beam_topk lists each split's best unpenalised and best penalised
+    tokens apart, and beam_step maps both to processed scores and merges them."""
+    proc = (fctl is not None and prompt is not None and plens is not None)
     if part_ml is None:
         beam_step_reference(logits, ictl, num_beams, K, length_penalty, early_stopping, max_new, run_score, fin_score, fin_flag, run_seq,
-                            fin_seq, unsat, done, tstep, pos, ids_next, parent)
+                            fin_seq, unsat, done, tstep, pos, ids_next, parent, fctl=fctl if proc else None, prompt=prompt, plens=plens)
         return
     rows, V = logits.shape
+    ck = cand_v.shape[2]
     assert logits.is_cuda and logits.dtype == torch.bfloat16 and logits.stride(1) == 1 and rows % num_beams == 0
-    assert part_ml.shape == (rows, beam_splits(V), 2) and cand_v.shape == (rows, beam_splits(V), K) and cand_i.shape == cand_v.shape
+    assert part_ml.shape == (rows, beam_splits(V), 2) and cand_v.shape == (rows, beam_splits(V), ck) and cand_i.shape == cand_v.shape
+    assert ck >= (2 * K if proc else K) and cand_v.is_contiguous() and cand_i.is_contiguous()
     assert run_seq.shape == (2, rows, max_new) and fin_seq.shape == (2, rows, max_new) and run_seq.dtype == torch.int32
+    if proc:
+        assert prompt.dtype == torch.int32 and prompt.is_contiguous() and prompt.shape[0] == rows // num_beams
+        assert plens.dtype == torch.int32 and fctl.dtype == torch.float32
     st = _lib.stream_ptr(logits)
-    _lib.check(_lib.cuda_lib().odb_dec_beam_topk(logits.data_ptr(), logits.stride(0), V, K, part_ml.data_ptr(), cand_v.data_ptr(),
-                                                 cand_i.data_ptr(), rows, st), "dec_beam_topk")
-    _lib.check(_lib.cuda_lib().odb_dec_beam_step(part_ml.data_ptr(), cand_v.data_ptr(), cand_i.data_ptr(), V, num_beams, K,
-                                                 ictl.data_ptr(), float(length_penalty), int(early_stopping), max_new,
+    fp = fctl.data_ptr() if proc else None
+    _lib.check(_lib.cuda_lib().odb_dec_beam_topk(logits.data_ptr(), logits.stride(0), V, K, ck, part_ml.data_ptr(), cand_v.data_ptr(),
+                                                 cand_i.data_ptr(), ictl.data_ptr(), fp, prompt.data_ptr() if proc else None,
+                                                 prompt.shape[1] if proc else 0, plens.data_ptr() if proc else None, run_seq.data_ptr(),
+                                                 tstep.data_ptr(), num_beams, max_new, rows, st), "dec_beam_topk")
+    _lib.check(_lib.cuda_lib().odb_dec_beam_step(part_ml.data_ptr(), cand_v.data_ptr(), cand_i.data_ptr(), V, num_beams, K, ck,
+                                                 ictl.data_ptr(), fp, float(length_penalty), int(early_stopping), max_new,
                                                  run_score.data_ptr(), fin_score.data_ptr(), fin_flag.data_ptr(), run_seq.data_ptr(),
                                                  fin_seq.data_ptr(), unsat.data_ptr(), done.data_ptr(), tstep.data_ptr(), pos.data_ptr(),
                                                  ids_next.data_ptr(), parent.data_ptr(), rows // num_beams, st), "dec_beam_step")
@@ -357,10 +381,12 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
 def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int, length_penalty: float, early_stopping: int,
                         max_new: int, run_score: torch.Tensor, fin_score: torch.Tensor, fin_flag: torch.Tensor, run_seq: torch.Tensor,
                         fin_seq: torch.Tensor, unsat: torch.Tensor, done: torch.Tensor, tstep: torch.Tensor, pos: torch.Tensor,
-                        ids_next: torch.Tensor, parent: torch.Tensor) -> None:
+                        ids_next: torch.Tensor, parent: torch.Tensor, fctl: torch.Tensor | None = None,
+                        prompt: torch.Tensor | None = None, plens: torch.Tensor | None = None) -> None:
     """``beam_select`` in PyTorch: transformers' ``_get_top_k_continuations``, ``_get_running_beams_for_next_iteration``,
     ``_update_finished_beams`` and ``_check_early_stop_heuristic`` over [B, num_beams, ...], with stable sorts for the
-    tie rule."""
+    tie rule (-inf ties included: the lower beam * V + token).  With fctl / prompt / plens, the logits processors as
+    described in ``beam_select``."""
     rows, V = logits.shape
     nb = num_beams
     B = rows // nb
@@ -372,7 +398,13 @@ def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int
     live = done == 0
     top = lambda x, k: torch.sort(x, dim=1, descending=True, stable=True).indices[:, :k]   # noqa: E731
     # c. top-K continuations
-    logp = torch.log_softmax(logits.float(), dim=-1).to(dev).view(B, nb, V) + run_score.view(B, nb, 1)
+    logp = torch.log_softmax(logits.float(), dim=-1).to(dev)
+    fc = fctl.tolist() if fctl is not None else []
+    if prompt is not None and plens is not None and processors_on(c, fc):
+        tr = t.to(dev).repeat_interleave(nb)
+        logp = process_logits_reference(logp, beam_histories(prompt, plens, run_seq, tstep, nb), plens.long().to(dev).repeat_interleave(nb) + tr,
+                                        tr, fc[FCTL_PENALTY], c[CTL_NGRAM], c[CTL_MIN_NEW], c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]])
+    logp = logp.view(B, nb, V) + run_score.view(B, nb, 1)
     idx = top(logp.view(B, nb * V), K)
     vals = logp.view(B, nb * V).gather(1, idx)
     beam, tok = idx // V, idx % V
@@ -427,6 +459,24 @@ def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int
     tstep.add_(live.to(tstep.dtype))
 
 
+def beam_histories(prompt: torch.Tensor, plens: torch.Tensor, run_seq: torch.Tensor, tstep: torch.Tensor, num_beams: int) -> torch.Tensor:
+    """Every beam row's history, compacted: [rows, S + max_new] int64 whose row r (prompt b = r // num_beams) holds
+    prompt[b, :plens[b]], then run_seq[t & 1, r, :t] with t = tstep[b]; the rest is -1."""
+    dev = run_seq.device
+    _, rows, M = run_seq.shape
+    S = prompt.shape[1]
+    lens = plens.long().to(dev).repeat_interleave(num_beams)
+    t = tstep.long().to(dev).repeat_interleave(num_beams)
+    col = torch.arange(S + M, device=dev)[None, :]
+    r = torch.arange(rows, device=dev)
+    run = run_seq[t & 1, r].long()                                                     # [rows, M]
+    pr = prompt.to(dev).long().repeat_interleave(num_beams, dim=0)
+    from_prompt = pr.gather(1, col.clamp(max=S - 1).expand(rows, -1))
+    from_run = run.gather(1, (col - lens[:, None]).clamp(0, M - 1))
+    h = torch.where(col < lens[:, None], from_prompt, from_run)
+    return torch.where(col < (lens + t)[:, None], h, torch.full_like(h, -1))
+
+
 def beam_reorder(kv: torch.Tensor, table: torch.Tensor | None, parent: torch.Tensor, pos: torch.Tensor, num_beams: int) -> None:
     """After a selection, make every beam row's cache the history of its parent row (int32 [rows], pos: the next position
     to write, the same for all beams of a prompt).  kv: every layer's K and V of the beam rows, [L, 2, rows, Hkv, Smax, D].
@@ -452,38 +502,111 @@ def beam_reorder_reference(kv: torch.Tensor, parent: torch.Tensor) -> None:
 
 
 # ------------------------------------------------------------------------------------------------ sampler
-def make_controls(do_sample: bool, temperature: float, top_k: int, top_p: float, seed: int, pad: int, eos: list[int], device):
-    """(ictl int64 [CTL_SIZE], fctl fp32 [2]) for ``sample``."""
+def make_controls(do_sample: bool, temperature: float, top_k: int, top_p: float, seed: int, pad: int, eos: list[int], device,
+                  repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_new_tokens: int = 0):
+    """(ictl int64 [CTL_SIZE], fctl fp32 [3]) for ``sample`` and ``beam_select``.  The logits processors are off at their
+    defaults (penalty 1.0, n-gram size 0, min_new_tokens 0)."""
     if len(eos) > MAX_EOS:
         raise ValueError(f"at most {MAX_EOS} EOS ids are supported, got {len(eos)}")
     ictl = [int(do_sample), int(top_k), int(seed) & ((1 << 63) - 1), int(pad), len(eos)] + list(eos) + [0] * (MAX_EOS - len(eos))
+    ictl += [int(no_repeat_ngram_size), int(min_new_tokens)]
     return (torch.tensor(ictl, dtype=torch.int64, device=device),
-            torch.tensor([float(temperature), float(top_p)], dtype=torch.float32, device=device))
+            torch.tensor([float(temperature), float(top_p), float(repetition_penalty)], dtype=torch.float32, device=device))
+
+
+def processors_on(ictl: list[int], fctl: list[float]) -> bool:
+    """The control blocks (as lists) turn a logits processor on (the kernels' test, on the same fields)."""
+    return (len(fctl) > FCTL_PENALTY and len(ictl) > CTL_MIN_NEW
+            and (fctl[FCTL_PENALTY] != 1.0 or ictl[CTL_NGRAM] > 0 or (ictl[CTL_MIN_NEW] > 0 and ictl[CTL_N_EOS] > 0)))
+
+
+def process_logits_reference(x: torch.Tensor, histories: torch.Tensor, lens: torch.Tensor, n_generated: torch.Tensor, penalty: float,
+                             n: int, min_new: int, eos: list[int]) -> torch.Tensor:
+    """HF's logits processors, in HF's order, on fp32 values x [rows, V]; returns a new tensor.  Row r's history is
+    histories[r, :lens[r]] (int, [rows, S]); n_generated[r] counts the tokens it has generated.
+
+    - Repetition penalty (``penalty`` != 1): every distinct token of the history gets ``x < 0 ? x * p : x / p``, once.
+    - N-gram ban (``n`` > 0): with h the history and L its length, if L + 1 >= n, every start s <= L - n with
+      ``h[s .. s+n-2] == h[L-n+1 .. L-1]`` bans ``h[s+n-1]`` (-inf); matches may overlap, and n = 1 bans the whole history.
+    - Min new tokens: while n_generated < ``min_new``, every id of ``eos`` gets -inf.
+
+    HF passes the padded ``input_ids``, so for left-padded prompts it also counts the padding ids; here a history holds only
+    the real prompt tokens and the generated ones."""
+    rows, V = x.shape
+    dev = x.device
+    h = histories.to(dev).long()
+    S = h.shape[1]
+    L = lens.to(dev).long()
+    col = torch.arange(S, device=dev)[None, :]
+    x = x.clone()
+    if penalty != 1.0:
+        tok = torch.where((col < L[:, None]) & (h >= 0) & (h < V), h, torch.full_like(h, V))
+        seen = torch.zeros(rows, V + 1, dtype=torch.bool, device=dev).scatter_(1, tok, True)[:, :V]
+        x = torch.where(seen, torch.where(x < 0, x * penalty, x / penalty), x)
+    ban = torch.zeros(rows, V + 1, dtype=torch.bool, device=dev)
+    if n > 0 and S >= n:
+        win = h.unfold(1, n, 1)                                                         # [rows, S - n + 1, n]
+        q = (L[:, None] - n + 1 + torch.arange(n - 1, device=dev)[None, :]).clamp(0, S - 1)
+        prefix = h.gather(1, q)                                                         # h[L-n+1 .. L-1]
+        starts = torch.arange(S - n + 1, device=dev)[None, :]
+        match = (win[:, :, :n - 1] == prefix[:, None, :]).all(dim=-1) & (starts <= (L - n)[:, None])
+        follower = win[:, :, n - 1]
+        follower = torch.where(match & (follower >= 0) & (follower < V), follower, torch.full_like(follower, V))
+        ban.scatter_(1, follower, True)
+    if min_new > 0 and eos:
+        early = n_generated.to(dev).long() < min_new
+        ban[:, torch.tensor(eos, dtype=torch.long, device=dev)] |= early[:, None]
+    return x.masked_fill(ban[:, :V], float("-inf"))
 
 
 def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: torch.Tensor, gen: torch.Tensor, finished: torch.Tensor,
-           out: torch.Tensor, ids_next: torch.Tensor) -> None:
+           out: torch.Tensor, ids_next: torch.Tensor, hist: torch.Tensor | None = None, scratch: torch.Tensor | None = None) -> None:
     """Pick one token per row of logits [B, V] and write it to out[b, gen[b]] and ids_next[b]; then gen += 1, pos += 1.
 
     Greedy (ictl do_sample = 0, or top_k = 1): argmax, ties to the lowest index.  Sampling: logits / temperature, keep the
     top_k largest (0 = all; ties with the k-th value are kept), keep the smallest set of largest probabilities whose mass
     reaches top_p (every token tied with the smallest kept one is kept too), draw from the rest.  A row that has produced an EOS id emits ``pad`` from then on (``finished``).
     CUDA draws use Philox keyed by (seed, row, gen[b]); the reference draws from a torch generator seeded by (seed, step),
-    so the two paths give different (equally distributed) samples for the same seed."""
+    so the two paths give different (equally distributed) samples for the same seed.
+
+    hist (int32 [B, S]): the rows' token histories, row b's tokens at positions 0 .. pos[b] (the real prompt tokens, then
+    the generated ones); the emitted token is appended at hist[b, pos[b] + 1] (when that is < S).  With a history and the
+    processors on in the control blocks (``make_controls``), the logits first go through ``process_logits_reference``'s
+    rules in fp32 (history length pos[b] + 1, gen[b] tokens generated), and greedy and sampling work on the processed
+    values, which are never rounded back to bf16.  A row whose processed values are all -inf emits token 0 greedily; a
+    sampled row with no finite value emits its processed argmax.  The kernel keeps two bitmaps per row in scratch (int32
+    [B, 2 * ceil(V / 32)])."""
     B, V = logits.shape
     if logits.is_cuda and logits.dtype == torch.bfloat16 and _lib.has_symbol("odb_dec_sample"):
         assert logits.stride(1) == 1 and V <= MAX_SAMPLE_VOCAB and out.is_contiguous()
+        if hist is not None:
+            assert hist.dtype == torch.int32 and hist.is_contiguous() and hist.shape[0] == B
+            assert scratch is not None and scratch.is_contiguous() and scratch.numel() >= B * 2 * ((V + 31) // 32)
         _lib.check(_lib.cuda_lib().odb_dec_sample(logits.data_ptr(), logits.stride(0), V, ictl.data_ptr(), fctl.data_ptr(), pos.data_ptr(),
                                                   gen.data_ptr(), finished.data_ptr(), out.data_ptr(), out.shape[1],
-                                                  ids_next.data_ptr(), B, _lib.stream_ptr(logits)), "dec_sample")
+                                                  ids_next.data_ptr(), hist.data_ptr() if hist is not None else None,
+                                                  hist.shape[1] if hist is not None else 0,
+                                                  scratch.data_ptr() if hist is not None else None, B, _lib.stream_ptr(logits)),
+                   "dec_sample")
         _lib.count_launch()
         return
     c = ictl.tolist()
-    temperature, top_p = (float(v) for v in fctl.tolist())
+    fc = fctl.tolist()
+    temperature, top_p = fc[FCTL_TEMPERATURE], fc[FCTL_TOP_P]
     x = logits.float()
+    proc = hist is not None and processors_on(c, fc)
+    if proc:
+        x = process_logits_reference(x, hist, pos.long() + 1, gen, fc[FCTL_PENALTY], c[CTL_NGRAM], c[CTL_MIN_NEW],
+                                     c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]])
     tok = x.argmax(dim=-1)
     if c[CTL_DO_SAMPLE] and c[CTL_TOP_K] != 1:
-        tok = _sample_reference(x, temperature, c[CTL_TOP_K], top_p, c[CTL_SEED], int(gen.min()))
+        if proc:
+            ok = torch.isfinite(x.max(dim=-1).values)
+            drawn = _sample_reference(torch.where(ok[:, None], x, torch.zeros_like(x)), temperature, c[CTL_TOP_K], top_p, c[CTL_SEED],
+                                      int(gen.min()))
+            tok = torch.where(ok, drawn, tok)
+        else:
+            tok = _sample_reference(x, temperature, c[CTL_TOP_K], top_p, c[CTL_SEED], int(gen.min()))
     fin = finished.bool()
     tok = torch.where(fin, torch.full_like(tok, c[CTL_PAD]), tok)
     g = gen.long()
@@ -491,6 +614,10 @@ def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: to
     inside = g < out.shape[1]
     out[rows[inside], g[inside]] = tok[inside]
     ids_next.copy_(tok)
+    if hist is not None:
+        at = pos.long().to(hist.device) + 1
+        ok = at < hist.shape[1]
+        hist[torch.arange(B, device=hist.device)[ok], at[ok]] = tok.to(hist.device, hist.dtype)[ok]
     gen.add_(1)
     pos.add_(1)
     eos = torch.tensor(c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]], dtype=torch.int64, device=logits.device)

@@ -8,13 +8,16 @@
         --assistant-checkpoint outputs_150m/model_step_1000 --num-assistant-tokens 4 --prompt-ids "1 450 4996"
     python scripts/generate.py --model 1b --checkpoint outputs_1b/model_step_1000 --num-beams 4 --num-return-sequences 2 \\
         --prompt-ids "1 450 4996"
+    python scripts/generate.py --model 150m --checkpoint outputs/model_step_1000 --weights outer --num-beams 4 \\
+        --no-repeat-ngram-size 3 --repetition-penalty 1.2 --prompt-ids "1 450 4996"
 
 ``--checkpoint`` reads a checkpoint directory written by train_fsdp / utils/ckpt.save_checkpoint (the one holding the
 ``*.distcp`` shards, i.e. ``model_step_N`` or its ``diloco_rank_R`` sub-directory).  ``--weights local`` takes the
 worker's own weights (``model``), ``--weights outer`` the DiLoCo global model (``theta_outer``).  Tokenizers are only
 read from a local directory.  ``--assistant-model`` (with ``--assistant-checkpoint`` / ``--assistant-weights``) loads a
 draft model the same way and turns on assisted (speculative) generation.  ``--num-beams`` > 1 runs beam search and prints
-each returned hypothesis with its score (``--num-return-sequences`` per prompt).
+each returned hypothesis with its score (``--num-return-sequences`` per prompt).  ``--repetition-penalty``,
+``--no-repeat-ngram-size`` and ``--min-new-tokens`` are HF's repetition controls, for greedy, sampling and beam search.
 """
 import argparse
 import json
@@ -104,6 +107,9 @@ def main(argv=None) -> None:
     ap.add_argument("--early-stopping", choices=["true", "false", "never"], default="false",
                     help="beam search: HF's early_stopping (true, false or never)")
     ap.add_argument("--num-return-sequences", type=int, default=1, help="beam search: hypotheses returned per prompt")
+    ap.add_argument("--repetition-penalty", type=float, default=1.0, help="HF's repetition penalty on the row's history (1.0: off)")
+    ap.add_argument("--no-repeat-ngram-size", type=int, default=0, help="no n-gram of this size occurs twice in a row (0: off)")
+    ap.add_argument("--min-new-tokens", type=int, default=0, help="EOS is forbidden until this many new tokens (0: off)")
     a = ap.parse_args(argv)
     if a.assistant_model is None and a.assistant_checkpoint is not None:
         ap.error("--assistant-checkpoint needs --assistant-model")
@@ -140,7 +146,9 @@ def main(argv=None) -> None:
                          temperature=a.temperature, top_k=a.top_k, top_p=a.top_p, eos_token_id=a.eos_token_id,
                          pad_token_id=a.pad_token_id, seed=a.seed, assistant_model=assistant,
                          num_assistant_tokens=a.num_assistant_tokens, num_beams=a.num_beams, length_penalty=a.length_penalty,
-                         early_stopping=early_stopping, num_return_sequences=a.num_return_sequences, return_dict_in_generate=True)
+                         early_stopping=early_stopping, num_return_sequences=a.num_return_sequences, return_dict_in_generate=True,
+                         repetition_penalty=a.repetition_penalty, no_repeat_ngram_size=a.no_repeat_ngram_size,
+                         min_new_tokens=a.min_new_tokens)
     out = res.sequences.cpu()
     R = out.shape[0] // len(prompts)
     for i, p in enumerate(prompts):
