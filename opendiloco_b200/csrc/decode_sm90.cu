@@ -7,6 +7,8 @@
 //   odb_dec_attn          split-KV decode attention (flash-decoding) + a combine kernel
 //   odb_dec_sample        greedy / temperature + top-k + top-p sampler, one CTA per row, with HF's repetition penalty, n-gram
 //                         ban and min-new-tokens over the row's device-side token history when the control blocks ask
+//   odb_dec_accept        assisted generation / prompt lookup: speculative acceptance of one round's proposals
+//   odb_dec_lookup_propose  prompt lookup: each row's proposals from an earlier occurrence of its last n-gram
 //   odb_dec_beam_topk     beam search: per vocabulary split of a row, the (max, sum-exp) partial and the local top-K logits
 //   odb_dec_beam_step     beam search: one CTA per prompt merges the candidates and does HF's selection and bookkeeping
 //   odb_dec_beam_reorder  beam search: chunk-table update and partial-chunk K/V copy for beams that changed parent
@@ -763,11 +765,20 @@ verify_combine_kernel(const float* __restrict__ part_o, const float* __restrict_
 // new last token goes to tok slot 0 and the draft's position is set to the target's.  A row that finishes keeps its pos
 // (every later round rewrites the same in-range cache positions); finished rows are left alone.
 // stats [B, 2] int64: rounds the row took part in, proposals accepted.
-__global__ void __launch_bounds__(SAMPLE_THREADS)
+//
+// Point-mass mode (qlog == nullptr; prompt lookup): row b has cnt[b] <= K candidates in slots 1..cnt[b] (later slots hold
+// a filler that is never accepted), and the draft is a point mass, q(d_i) = 1.  Greedy: as above, stopping at cnt[b].
+// Sampling: accept d_i with probability p_i(d_i); at the first rejection draw from p_i with d_i removed (renormalised);
+// with no candidate left (slot cnt[b], the bonus slot when cnt[b] = K) draw from p_{cnt[b]}.  The same Philox keys.
+// hist (int32 [B, ldh], nullptr in assisted mode): every emitted token is appended at hist[b, pos[b] + 1 ...], so
+// hist[b, :pos[b] + 1] stays the row's history.  draft_pos may be nullptr.
+// One CTA per SM (the fp32 vocabulary fills shared memory): asking for it lets ptxas go past 32 registers without spilling.
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1)
 accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_bfloat16* __restrict__ qlog, long long ldq, int V,
               int K, const long long* __restrict__ ictl, const float* __restrict__ fctl, long long* __restrict__ tok,
               int* __restrict__ pos, int* __restrict__ gen, int* __restrict__ finished, long long* __restrict__ out, int ld_out,
-              int max_new, int* __restrict__ draft_pos, long long* __restrict__ stats) {
+              int max_new, int* __restrict__ draft_pos, long long* __restrict__ stats, const int* __restrict__ cnt,
+              int* __restrict__ hist, int ldh) {
   extern __shared__ __align__(16) float e[];
   __shared__ float red[33];
   __shared__ ArgMax am[32];
@@ -776,18 +787,19 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
   pdl_wait();
   const int b = blockIdx.x, B = gridDim.x, tid = threadIdx.x;
   if (finished[b]) {
-    if (tid == 0) draft_pos[b] = pos[b];
+    if (tid == 0 && draft_pos != nullptr) draft_pos[b] = pos[b];
     return;
   }
   const bool greedy = !(ictl[0] != 0 && ictl[1] != 1);
   const int top_k = (int)ictl[1];
   const float temp = fctl[0], top_p = fctl[1];
   const int g0 = gen[b];
+  const int c = cnt != nullptr ? min(max(cnt[b], 0), K) : K;   // candidates of this row
   int n_acc = 0, t_new = 0;
-  for (int i = 0; i <= K; ++i) {
+  for (int i = 0; i <= c; ++i) {
     const __nv_bfloat16* prow = plog + ((long long)i * B + b) * ldp;
     const ArgMax pm = block_argmax(prow, V, am);
-    const long long d = i < K ? tok[(long long)(i + 1) * B + b] : -1;
+    const long long d = i < c ? tok[(long long)(i + 1) * B + b] : -1;
     if (greedy) {
       if (d == pm.i) {
         ++n_acc;
@@ -801,7 +813,7 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
     curandStatePhilox4_32_10_t rng;
     curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)g0 * 16ull + 2ull * i, &rng);
     const float u_acc = curand_uniform(&rng), u_draw = curand_uniform(&rng);    // (0, 1]
-    if (i == K) {                                // every proposal accepted: the bonus token from p_{K+1}
+    if (i == c) {                                // no proposal left (assisted: all K accepted): draw from p_c
       t_new = draw_index(e, V, u_acc, pm.i, red, &tok_sm);
       break;
     }
@@ -809,6 +821,21 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
     for (int v = tid; v < V; v += blockDim.x) zp += e[v];
     zp = block_sum(zp, red);
     const float pd = e[d] / zp;
+    if (qlog == nullptr) {                       // point mass: accept with probability p(d), else draw from p without d
+      if (pd > 0.f && u_acc <= pd) {
+        ++n_acc;
+        continue;
+      }
+      __syncthreads();                           // every thread has read e[d]
+      if (tid == 0) e[d] = 0.f;
+      __syncthreads();
+      // fallback of draw_index (r outside every segment by rounding): the residual's largest weight, never d itself
+      ArgMax fb = {-INFINITY, V};
+      for (int v = tid; v < V; v += blockDim.x) fb = argmax_merge(fb, ArgMax{e[v], v});
+      fb = block_reduce_argmax(fb, am);
+      t_new = draw_index(e, V, u_draw, fb.i, red, &tok_sm);
+      break;
+    }
     const __nv_bfloat16* qrow = qlog + ((long long)i * B + b) * ldq;
     const ArgMax qm = block_argmax(qrow, V, am);   // starts with a barrier: every thread has read e[d]
     warp_weights(qrow, V, temp, top_k, top_p, qm.v / temp, e, red);
@@ -837,6 +864,7 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
     for (int t = 0; t <= n_acc && !fin && g < max_new; ++t) {
       const long long x = t < n_acc ? tok[(long long)(t + 1) * B + b] : (long long)t_new;
       out[(long long)b * ld_out + g] = x;
+      if (hist != nullptr && pos[b] + 1 + t < ldh) hist[(long long)b * ldh + pos[b] + 1 + t] = (int)x;
       ++g;
       for (int k = 0; k < n_eos; ++k)
         if (x == ictl[5 + k]) fin = true;
@@ -848,7 +876,68 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
     else pos[b] += n_acc + 1;
     gen[b] = g;
     tok[b] = t_new;
-    draft_pos[b] = pos[b];
+    if (draft_pos != nullptr) draft_pos[b] = pos[b];
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ prompt lookup
+// One CTA per row: the proposals of one prompt-lookup round (transformers' PromptLookupCandidateGenerator).  Row b's history
+// is h = hist[b, :L], L = pos[b] + 1.  For n from min(ngram, L - 1) down to 1, the earliest start s with h[s, s+n) equal to
+// the last n tokens h[L-n, L) and s + n < L (a block-wide minimum over the starts, one pass per n); the first n with such an
+// s wins.  Its candidates are h[s+n, min(s+n+K, L)), cut before the first EOS id of ictl.  They go to tok slots 1..c
+// (slot j of row b: tok[j*B + b]); slots c+1..K get the filler id 0.  cnt[b] = c, proposed[b] += c.  Finished rows are left
+// alone.  Every setting is a kernel argument or lives in device memory, so a captured round graph serves every round.
+constexpr int LOOKUP_THREADS = 256;
+
+__global__ void __launch_bounds__(LOOKUP_THREADS)
+lookup_propose_kernel(const int* __restrict__ hist, int ldh, const int* __restrict__ pos, const int* __restrict__ finished,
+                      const long long* __restrict__ ictl, long long* __restrict__ tok, int* __restrict__ cnt,
+                      long long* __restrict__ proposed, int K, int ngram) {
+  __shared__ int suffix[64];                     // the last n tokens (n <= MAX_NGRAM = 64)
+  __shared__ int best;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x, B = gridDim.x, tid = threadIdx.x;
+  if (finished[b]) return;
+  const int* h = hist + (long long)b * ldh;
+  const int L = min(pos[b] + 1, ldh);
+  int s_win = -1, n_win = 0;
+  for (int n = min(min(ngram, L - 1), 64); n >= 1; --n) {
+    if (tid < n) suffix[tid] = h[L - n + tid];
+    if (tid == 0) best = INT_MAX;
+    __syncthreads();
+    for (int s = tid; s + n < L; s += blockDim.x) {            // the first match of each thread is its smallest
+      bool eq = true;
+      for (int k = 0; k < n && eq; ++k) eq = h[s + k] == suffix[k];
+      if (eq) {
+        atomicMin(&best, s);
+        break;
+      }
+    }
+    __syncthreads();
+    const int s = best;
+    __syncthreads();                             // every thread has read best and suffix before the next pass
+    if (s != INT_MAX) {
+      s_win = s;
+      n_win = n;
+      break;
+    }
+  }
+  if (tid == 0) {
+    int c = 0;
+    if (s_win >= 0) {
+      const int start = s_win + n_win, n_eos = (int)min(ictl[4], (long long)MAX_EOS);
+      const int end = min(start + K, L);
+      for (int i = start; i < end; ++i) {
+        bool is_eos = false;
+        for (int k = 0; k < n_eos; ++k) is_eos |= (long long)h[i] == ictl[5 + k];
+        if (is_eos) break;
+        ++c;
+      }
+    }
+    for (int j = 0; j < K; ++j) tok[(long long)(j + 1) * B + b] = j < c ? (long long)h[s_win + n_win + j] : 0ll;
+    cnt[b] = c;
+    proposed[b] += c;
   }
 }
 
@@ -1319,11 +1408,13 @@ ODB_EXPORT int odb_dec_verify_attn(const void* q, long long ldq, const void* kc,
 
 // plog [(K+1)*B, ldp] / qlog [K*B, ldq] bf16 slot-major; tok int64 [(K+1)*B]; ictl / fctl: see dec::sample_kernel; pos / gen /
 // finished / draft_pos int32 [B]; out int64 [B, ld_out]; stats int64 [B, 2].  V <= 56000 (fp32 vocabulary in shared memory).
+// Point-mass mode (prompt lookup): qlog nullptr, cnt int32 [B] candidate counts, hist int32 [B, ldh] (or nullptr), draft_pos
+// may be nullptr.  See dec::accept_kernel.
 ODB_EXPORT int odb_dec_accept(const void* plog, long long ldp, const void* qlog, long long ldq, int V, int K, const void* ictl,
                               const void* fctl, void* tok, void* pos, void* gen, void* finished, void* out, int ld_out, int max_new,
-                              void* draft_pos, void* stats, int B, cudaStream_t st) {
+                              void* draft_pos, void* stats, const void* cnt, void* hist, int ldh, int B, cudaStream_t st) {
   const int smem = V * 4;
-  if (smem > 224000 || K < 1 || K > 7) return -1;
+  if (smem > 224000 || K < 1 || K > 7 || (qlog == nullptr && cnt == nullptr)) return -1;
   static int attr = 0;
   if (smem > 48 * 1024 && smem > attr) {
     cudaError_t e = cudaFuncSetAttribute(dec::accept_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -1332,7 +1423,18 @@ ODB_EXPORT int odb_dec_accept(const void* plog, long long ldp, const void* qlog,
   }
   launch_pdl(dec::accept_kernel, dim3(B), dim3(dec::SAMPLE_THREADS), smem, st, (const __nv_bfloat16*)plog, ldp,
              (const __nv_bfloat16*)qlog, ldq, V, K, (const long long*)ictl, (const float*)fctl, (long long*)tok, (int*)pos, (int*)gen,
-             (int*)finished, (long long*)out, ld_out, max_new, (int*)draft_pos, (long long*)stats);
+             (int*)finished, (long long*)out, ld_out, max_new, (int*)draft_pos, (long long*)stats, (const int*)cnt, (int*)hist, ldh);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+// hist int32 [B, ldh]; pos / finished / cnt int32 [B]; ictl: see dec::sample_kernel (EOS ids); tok int64 [(K+1)*B] slot-major
+// (slots 1..K written); proposed int64 [B].  1 <= K <= 7, 1 <= ngram <= 64.  See dec::lookup_propose_kernel.
+ODB_EXPORT int odb_dec_lookup_propose(const void* hist, int ldh, const void* pos, const void* finished, const void* ictl, void* tok,
+                                      void* cnt, void* proposed, int K, int ngram, int B, cudaStream_t st) {
+  if (K < 1 || K > 7 || ngram < 1 || ngram > 64 || ldh < 1) return -1;
+  launch_pdl(dec::lookup_propose_kernel, dim3(B), dim3(dec::LOOKUP_THREADS), 0, st, (const int*)hist, ldh, (const int*)pos,
+             (const int*)finished, (const long long*)ictl, (long long*)tok, (int*)cnt, (long long*)proposed, K, ngram);
   ODB_CHECK_LAST();
   return 0;
 }

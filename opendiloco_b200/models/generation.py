@@ -18,6 +18,10 @@ multi-token pass (verify attention over its cache), and one acceptance kernel ke
 one target token per row.  The whole round is one CUDA graph.  Rejected cache entries are left in place: attention reads
 only up to each row's position, so moving ``pos`` back is the whole rollback.
 
+Prompt lookup, ``generate(prompt_lookup_num_tokens=K)``: the same round without a draft model.  One kernel proposes up to K
+tokens per row, the tokens that followed an earlier occurrence of the row's last n-gram in its own history (the device-side
+history of the logits processors, which the acceptance kernel extends); the verify pass and a point-mass acceptance follow.
+
 Beam search, ``generate(num_beams=...)``: transformers' deterministic beam search step for step, on B * num_beams rows of
 a DecodeState of its own.  The prompts are prefilled once, into the beam-0 rows; every later step is one CUDA graph: the
 decode layers, the LM head, the selection kernels and the cache reorder.  All beams of a prompt sit at the same position,
@@ -275,23 +279,29 @@ class AssistedState:
     """The target's buffers of assisted generation over B rows with K proposals: the multi-token verify pass over
     (K+1)*B slot-major rows (row j*B + b is slot j of row b), the draft's proposal logits, the draft's own DecodeState
     (so a model can draft for itself, and the assistant's ``decode_state`` is left alone) and the round graph.  The
-    target's caches, positions and outputs stay in its DecodeState."""
+    target's caches, positions and outputs stay in its DecodeState.
+
+    With ``dcfg`` None (prompt lookup) there is no draft: no draft DecodeState and no proposal logits; the proposals
+    come from the target's token history, and ``cnt`` / ``proposed`` count each row's candidates."""
 
     def __init__(self, cfg, dcfg, B: int, K: int, Smax: int, device, dtype):
         h, i, V, D = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size, cfg.head_dim
         T = (K + 1) * B
         e = lambda *shape: torch.empty(*shape, dtype=dtype, device=device)  # noqa: E731
-        self.B, self.K, self.key = B, K, (B, K, Smax, str(device), dtype, _shape(dcfg))
-        self.draft = DecodeState(dcfg, B, Smax, device, dtype)
+        self.B, self.K, self.key = B, K, (B, K, Smax, str(device), dtype, _shape(dcfg) if dcfg is not None else None)
+        self.draft = DecodeState(dcfg, B, Smax, device, dtype) if dcfg is not None else None
         self.tok = torch.zeros(T, dtype=torch.int64, device=device)          # slot 0: last token; 1..K: proposals
         self.res, self.xn, self.proj = e(T, h), e(T, h), e(T, h)
         self.rstd = torch.empty(T, dtype=torch.float32, device=device)
         self.qkv, self.att, self.gu, self.act = e(T, cfg.qkv_dim), e(T, cfg.q_dim), e(T, 2 * i), e(T, i)
-        self.plog, self.qlog = e(T, V), e(K * B, V)
+        self.plog = e(T, V)
+        self.qlog = e(K * B, V) if dcfg is not None else None
         self.stats = torch.zeros(B, 2, dtype=torch.int64, device=device)     # per row: rounds taken part in, accepted
+        self.cnt = torch.zeros(B, dtype=torch.int32, device=device)          # prompt lookup: this round's candidates per row
+        self.proposed = torch.zeros(B, dtype=torch.int64, device=device)     # prompt lookup: candidates proposed per row
         # the verify kernels follow the target's shapes alone; the round graph needs the draft's decode kernels too
         self.kernels = DK.usable_verify(self.res, D, cfg.num_attention_heads, cfg.num_key_value_heads)
-        self.graphable = self.kernels and self.draft.kernels
+        self.graphable = self.kernels and (self.draft is None or self.draft.kernels)
         self.part_o = self.part_ml = None
         if self.kernels:
             nsp = DK.verify_splits(Smax)
@@ -309,9 +319,10 @@ class AssistedState:
         return int(self.stats[:, 0].max())
 
     def acceptance_rate(self) -> float:
-        """Accepted proposals over proposals made, over the rows and rounds of the last generate call."""
-        rounds = int(self.stats[:, 0].sum())
-        return int(self.stats[:, 1].sum()) / (self.K * rounds) if rounds else float("nan")
+        """Accepted proposals over proposals made, over the rows and rounds of the last generate call (prompt lookup:
+        over the candidates actually proposed; a row without a match proposes none)."""
+        made = int(self.proposed.sum()) if self.draft is None else self.K * int(self.stats[:, 0].sum())
+        return int(self.stats[:, 1].sum()) / made if made else float("nan")
 
 
 def _shape(cfg) -> tuple:
@@ -321,13 +332,14 @@ def _shape(cfg) -> tuple:
 
 def assisted_state(model, assistant, B: int, K: int, Smax: int) -> AssistedState:
     """The model's assisted-generation state for (assistant shapes, B, K, Smax), allocated on first use; at most one is
-    resident, on the target's engine."""
+    resident, on the target's engine.  ``assistant`` None: the draft-less state of prompt lookup."""
     eng, ar = model.engine, model.arena
-    key = (B, K, Smax, str(ar.device), ar.compute_dtype, _shape(assistant.config))
+    dcfg = assistant.config if assistant is not None else None
+    key = (B, K, Smax, str(ar.device), ar.compute_dtype, _shape(dcfg) if dcfg is not None else None)
     st = eng.assisted_state
     if st is None or st.key != key:
         eng.assisted_state = None                     # free the old buffers before allocating the new ones
-        st = eng.assisted_state = AssistedState(model.config, assistant.config, B, K, Smax, ar.device, ar.compute_dtype)
+        st = eng.assisted_state = AssistedState(model.config, dcfg, B, K, Smax, ar.device, ar.compute_dtype)
     return st
 
 
@@ -346,7 +358,13 @@ def _verify(model, tst: DecodeState, ast: AssistedState) -> None:
     G.mm_nt(ast.xn, ar.w("lm_head.weight"), out=ast.plog)
 
 
-def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: int) -> None:
+def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: int, ngram: int) -> None:
+    if draft is None:                                 # prompt lookup: proposals from the history, point-mass acceptance
+        DK.lookup_propose(tst.hist, tst.pos, tst.finished, tst.ictl, ast.tok, ast.cnt, ast.proposed, ngram)
+        _verify(target, tst, ast)
+        DK.accept(ast.plog, None, tst.ictl, tst.fctl, ast.tok, tst.pos, tst.gen, tst.finished, tst.out, max_new, None, ast.stats,
+                  cnt=ast.cnt, hist=tst.hist)
+        return
     B, Kp, dst = ast.B, ast.K, ast.draft
     dcfg, dar = draft.config, draft.arena
     for i in range(Kp + 1):
@@ -363,26 +381,28 @@ def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: i
 
 
 @torch.no_grad()
-def assisted_round(target, draft, tst: DecodeState, ast: AssistedState, max_new: int, graph: bool | None = None) -> None:
-    """One assisted round: K draft proposals, one verify pass of the target, acceptance.  With the kernels and ``graph``
-    (default: ``ODB_CUDA_GRAPH`` != 0) the first call runs eagerly (warm-up), the second captures the round and every
-    call replays it."""
+def assisted_round(target, draft, tst: DecodeState, ast: AssistedState, max_new: int, graph: bool | None = None,
+                   ngram: int = 2) -> None:
+    """One assisted round: K draft proposals, one verify pass of the target, acceptance.  ``draft`` None is a prompt-lookup
+    round: up to K proposals per row from an earlier occurrence of the row's last n-gram (n <= ``ngram``) in its history,
+    one verify pass, point-mass acceptance.  With the kernels and ``graph`` (default: ``ODB_CUDA_GRAPH`` != 0) the first
+    call runs eagerly (warm-up), the second captures the round and every call replays it."""
     if graph is None:
         graph = _use_graph()
     if not (graph and ast.graphable and tst.kernels):
-        _round_eager(target, draft, tst, ast, max_new)
+        _round_eager(target, draft, tst, ast, max_new, ngram)
         return
-    key = (target.arena.version, target.arena.shadow.data_ptr(), draft.arena.version, draft.arena.shadow.data_ptr(), id(tst),
-           max_new)
+    proposer = (draft.arena.version, draft.arena.shadow.data_ptr()) if draft is not None else ("lookup", ngram)
+    key = (target.arena.version, target.arena.shadow.data_ptr(), *proposer, id(tst), max_new)
     if ast.graph is None or ast.graph_key != key:
         if ast.graph_key != ("warm",) + key:
             ast.graph, ast.graph_key, ast.graph_target = None, ("warm",) + key, tst
-            _round_eager(target, draft, tst, ast, max_new)
+            _round_eager(target, draft, tst, ast, max_new, ngram)
             return
         torch.cuda.synchronize(tst.device)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
-            _round_eager(target, draft, tst, ast, max_new)
+            _round_eager(target, draft, tst, ast, max_new, ngram)
         ast.graph, ast.graph_key = g, key
     ast.graph.replay()
 
@@ -408,8 +428,34 @@ def _check_assistant(model, assistant, P: int, max_new_tokens: int, num_assistan
                              f"exceeds max_position_embeddings {c.max_position_embeddings} of {who}")
 
 
+def _check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size, assistant_model, num_beams, processors_on: bool, P: int,
+                  max_new_tokens: int, max_position_embeddings: int) -> int:
+    """Validates the prompt-lookup arguments (transformers' names); returns max_matching_ngram_size (default 2)."""
+    if max_matching_ngram_size is not None and (isinstance(max_matching_ngram_size, bool) or not isinstance(max_matching_ngram_size, int)
+                                                or not 1 <= max_matching_ngram_size <= DK.MAX_NGRAM):
+        raise ValueError(f"max_matching_ngram_size must be an integer in [1, {DK.MAX_NGRAM}], got {max_matching_ngram_size!r}")
+    ngram = 2 if max_matching_ngram_size is None else max_matching_ngram_size
+    if prompt_lookup_num_tokens is None:
+        return ngram
+    K = prompt_lookup_num_tokens
+    if isinstance(K, bool) or not isinstance(K, int) or not 1 <= K <= MAX_ASSISTANT_TOKENS:
+        raise ValueError(f"prompt_lookup_num_tokens must be an integer in [1, {MAX_ASSISTANT_TOKENS}], got {K!r}")
+    if assistant_model is not None:
+        raise ValueError("prompt_lookup_num_tokens cannot be combined with assistant_model")
+    if num_beams > 1:
+        raise ValueError("prompt_lookup_num_tokens cannot be combined with num_beams > 1")
+    if processors_on:
+        raise ValueError("repetition_penalty, no_repeat_ngram_size and min_new_tokens are not supported yet together with "
+                         "prompt_lookup_num_tokens")
+    if P + max_new_tokens + K > max_position_embeddings:
+        raise ValueError(f"prompt length {P} + max_new_tokens {max_new_tokens} + prompt_lookup_num_tokens {K} exceeds "
+                         f"max_position_embeddings {max_position_embeddings}")
+    return ngram
+
+
 def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int, Kp: int, controls: tuple, pad: int,
-                       eos: list[int]) -> torch.Tensor:
+                       eos: list[int], ngram: int = 2) -> torch.Tensor:
+    """Assisted generation with ``assistant``, or prompt lookup (n-grams up to ``ngram``) with ``assistant`` None."""
     B = comp.shape[0]
     Smax = _round_up(P + max_new_tokens + Kp, 128)
     tst = decode_state(model, B, Smax)
@@ -417,18 +463,21 @@ def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int
     dst = ast.draft
     do_sample, temperature, top_k, top_p, seed = controls
     tst.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos)
-    dst.set_controls(do_sample, temperature, top_k, top_p, seed ^ DRAFT_SEED_XOR, 0, [])
+    if dst is not None:
+        dst.set_controls(do_sample, temperature, top_k, top_p, seed ^ DRAFT_SEED_XOR, 0, [])
     tst.out.fill_(pad)
-    prefill(model, tst, comp, lens)
-    prefill(assistant, dst, comp, lens)
-    dst.finished.zero_()                              # the draft never stops by itself; its position follows the target's
-    dst.pos.copy_(tst.pos)
+    prefill(model, tst, comp, lens)                   # also leaves each row's history in tst.hist
+    if dst is not None:
+        prefill(assistant, dst, comp, lens)
+        dst.finished.zero_()                          # the draft never stops by itself; its position follows the target's
+        dst.pos.copy_(tst.pos)
     ast.tok[:B].copy_(tst.ids)
     ast.stats.zero_()
+    ast.proposed.zero_()
     for r in range(max_new_tokens - 1):               # every round emits >= 1 token per unfinished row
         if r % ASSISTED_CHECK_EVERY == 0 and bool(tst.finished.all()):
             break
-        assisted_round(model, assistant, tst, ast, max_new_tokens)
+        assisted_round(model, assistant, tst, ast, max_new_tokens, ngram=ngram)
     return tst.out[:, :max_new_tokens].clone()
 
 
@@ -636,7 +685,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
              pad_token_id: int | None = None, seed: int = 0, assistant_model=None, num_assistant_tokens: int = 4, num_beams: int = 1,
              length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1,
              return_dict_in_generate: bool = False, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
-             min_new_tokens: int = 0) -> torch.Tensor | GenerateOutput:
+             min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
+             max_matching_ngram_size: int | None = None) -> torch.Tensor | GenerateOutput:
     """See :meth:`LlamaForCausalLM.generate`."""
     cfg, ar = model.config, model.arena
     if ar.param_sharded:
@@ -657,7 +707,9 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
         _check_assistant(model, assistant_model, P, max_new_tokens, num_assistant_tokens)
     eos = _eos_list(cfg.eos_token_id if eos_token_id is None else eos_token_id)
     _check_beams(num_beams, num_return_sequences, do_sample, assistant_model, early_stopping, cfg.vocab_size, len(eos))
-    _check_processors(repetition_penalty, no_repeat_ngram_size, min_new_tokens, assistant_model)
+    proc_on = _check_processors(repetition_penalty, no_repeat_ngram_size, min_new_tokens, assistant_model)
+    ngram = _check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size, assistant_model, num_beams, proc_on, P, max_new_tokens,
+                          cfg.max_position_embeddings)
     processors = (float(repetition_penalty), no_repeat_ngram_size, min_new_tokens)
     dev = ar.device
     ids = input_ids.to(dev)
@@ -680,9 +732,10 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     col = (P - lens.long())[:, None] + torch.arange(Sp, device=dev)[None, :]
     comp = ids.gather(1, col.clamp(max=P - 1))
     comp = comp.masked_fill(torch.arange(Sp, device=dev)[None, :] >= lens.long()[:, None], 0)
-    if assistant_model is not None:
-        new = _assisted_generate(model, assistant_model, comp, lens, P, max_new_tokens, num_assistant_tokens,
-                                 (do_sample, temperature, top_k, top_p, seed), pad, eos)
+    if assistant_model is not None or prompt_lookup_num_tokens is not None:
+        K = num_assistant_tokens if assistant_model is not None else prompt_lookup_num_tokens
+        new = _assisted_generate(model, assistant_model, comp, lens, P, max_new_tokens, K, (do_sample, temperature, top_k, top_p, seed),
+                                 pad, eos, ngram)
         out = torch.cat([ids, new], dim=1)
         return GenerateOutput(out) if return_dict_in_generate else out
     Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))

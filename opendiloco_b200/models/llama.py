@@ -745,7 +745,8 @@ class LlamaForCausalLM(nn.Module):
                  pad_token_id: int | None = None, seed: int = 0, assistant_model: "LlamaForCausalLM | None" = None,
                  num_assistant_tokens: int = 4, num_beams: int = 1, length_penalty: float = 1.0, early_stopping=False,
                  num_return_sequences: int = 1, return_dict_in_generate: bool = False, repetition_penalty: float = 1.0,
-                 no_repeat_ngram_size: int = 0, min_new_tokens: int = 0):
+                 no_repeat_ngram_size: int = 0, min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
+                 max_matching_ngram_size: int | None = None):
         """KV-cached text generation with HF ``generate`` keyword names.  Returns LongTensor [B, P + max_new_tokens]: the
         prompt as given, then the new tokens.
 
@@ -766,6 +767,18 @@ class LlamaForCausalLM(nn.Module):
         ``acceptance_rate()``.  Raises ValueError for a different vocabulary, device or compute dtype, a parameter-sharded
         assistant, ``num_assistant_tokens`` outside [1, 7], or a prompt plus ``max_new_tokens`` plus
         ``num_assistant_tokens`` beyond either model's ``max_position_embeddings``.
+
+        ``prompt_lookup_num_tokens`` K (1..7; None is off) turns on prompt lookup decoding, transformers' draft-free
+        speculative generation: each round, every row proposes up to K tokens from its own history (its real prompt tokens,
+        then its generated ones; padding is not history), this model scores them in one pass and the same acceptance as
+        assisted generation keeps an exact sample of its distribution (greedy: its argmax continuation, up to the same
+        bf16 near-ties).  A row's proposals are the tokens that followed the earliest earlier occurrence of its last n
+        tokens, for the largest n <= ``max_matching_ngram_size`` (1..64, default 2) that has one, at most K and cut before
+        the first EOS id; a row with no match proposes nothing and gains one token that round.  ``engine.assisted_state``
+        then reports ``verify_passes()`` and ``acceptance_rate()`` (accepted over proposed tokens).  Works with greedy
+        decoding and sampling, left-padded batches and EOS.  Raises ValueError for K or ``max_matching_ngram_size`` outside
+        those ranges or not an integer, together with ``assistant_model``, ``num_beams`` > 1 or any logits processor below
+        (not supported yet), or for a prompt plus ``max_new_tokens`` plus K beyond ``max_position_embeddings``.
 
         ``num_beams`` > 1 (at most 8) runs deterministic beam search as transformers' ``generate(num_beams=...,
         do_sample=False)``: fp32 log-softmax of the logits, then the logits processors below, ``length_penalty``,
@@ -802,7 +815,8 @@ class LlamaForCausalLM(nn.Module):
                         seed=seed, assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens, num_beams=num_beams,
                         length_penalty=length_penalty, early_stopping=early_stopping, num_return_sequences=num_return_sequences,
                         return_dict_in_generate=return_dict_in_generate, repetition_penalty=repetition_penalty,
-                        no_repeat_ngram_size=no_repeat_ngram_size, min_new_tokens=min_new_tokens)
+                        no_repeat_ngram_size=no_repeat_ngram_size, min_new_tokens=min_new_tokens,
+                        prompt_lookup_num_tokens=prompt_lookup_num_tokens, max_matching_ngram_size=max_matching_ngram_size)
 
     @torch.no_grad()
     def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None):

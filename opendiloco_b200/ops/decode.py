@@ -39,7 +39,10 @@ _lib.register_optional("odb_dec_rope_append_multi", [c_void_p, c_ll, c_void_p, c
 _lib.register_optional("odb_dec_verify_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int,
                                                c_int, c_int, c_int, c_int, c_float, c_void_p])
 _lib.register_optional("odb_dec_accept", [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                          c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p])
+                                          c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                          c_int, c_void_p])
+_lib.register_optional("odb_dec_lookup_propose", [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                                  c_int, c_int, c_void_p])
 _lib.register_optional("odb_dec_beam_splits", [c_int])
 _lib.register_optional("odb_dec_beam_topk", [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p])
@@ -229,9 +232,9 @@ def verify_attention(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, pos: t
     return out
 
 
-def accept(plog: torch.Tensor, qlog: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, tok: torch.Tensor, pos: torch.Tensor,
-           gen: torch.Tensor, finished: torch.Tensor, out: torch.Tensor, max_new: int, draft_pos: torch.Tensor,
-           stats: torch.Tensor) -> None:
+def accept(plog: torch.Tensor, qlog: torch.Tensor | None, ictl: torch.Tensor, fctl: torch.Tensor, tok: torch.Tensor, pos: torch.Tensor,
+           gen: torch.Tensor, finished: torch.Tensor, out: torch.Tensor, max_new: int, draft_pos: torch.Tensor | None,
+           stats: torch.Tensor, cnt: torch.Tensor | None = None, hist: torch.Tensor | None = None) -> None:
     """The acceptance step of one assisted round (speculative sampling; Leviathan et al. 2023, Chen et al. 2023).
 
     plog [(K+1)*B, V]: the target's logits, slot-major, slot i predicting the token at pos[b] + i + 1; qlog [K*B, V]: the
@@ -246,16 +249,31 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor, ictl: torch.Tensor, fctl: tor
     written), gen / pos / finished advance (a row that finishes keeps its pos), tok slot 0 becomes the next round's last
     token and draft_pos = pos.  Finished rows are left alone.  stats int64 [B, 2] += (1, accepted proposals) per row that
     took part.  CUDA draws use Philox keyed by (seed, row, gen[b], slot); the reference draws from a torch generator
-    seeded by (seed, row, gen[b]), so the paths give different (equally distributed) samples for the same seed."""
+    seeded by (seed, row, gen[b]), so the paths give different (equally distributed) samples for the same seed.
+
+    Point-mass mode (prompt lookup): qlog None and cnt (int32 [B]) given.  Row b has cnt[b] <= K candidates in slots
+    1..cnt[b] (later slots hold a filler that is never accepted) and q is a point mass on each.  Greedy: as above,
+    stopping at cnt[b].  Sampling: d_i is accepted with probability p_i(d_i); the first rejection draws from p_i with d_i
+    removed and renormalised; with no candidate left (slot cnt[b]) the token is drawn from p_{cnt[b]}.  This is the law of
+    drawing from p and keeping the candidate while the draw equals it.  hist (int32 [B, S], or None): every emitted token
+    is appended at hist[b, pos[b] + 1 ...] (positions < S), so hist[b, :pos[b] + 1] stays the row's history.  draft_pos
+    may be None."""
     B = pos.shape[0]
-    K = qlog.shape[0] // B
+    K = plog.shape[0] // B - 1
     V = plog.shape[1]
+    assert qlog is not None or cnt is not None
     if plog.is_cuda and plog.dtype == torch.bfloat16 and _lib.has_symbol("odb_dec_accept"):
-        assert plog.stride(1) == 1 and qlog.stride(1) == 1 and V <= MAX_SAMPLE_VOCAB and out.is_contiguous() and 1 <= K <= 7
-        _lib.check(_lib.cuda_lib().odb_dec_accept(plog.data_ptr(), plog.stride(0), qlog.data_ptr(), qlog.stride(0), V, K, ictl.data_ptr(),
-                                                  fctl.data_ptr(), tok.data_ptr(), pos.data_ptr(), gen.data_ptr(), finished.data_ptr(),
-                                                  out.data_ptr(), out.shape[1], max_new, draft_pos.data_ptr(), stats.data_ptr(), B,
-                                                  _lib.stream_ptr(plog)), "dec_accept")
+        assert plog.stride(1) == 1 and V <= MAX_SAMPLE_VOCAB and out.is_contiguous() and 1 <= K <= 7
+        assert qlog is None or (qlog.stride(1) == 1 and qlog.shape[0] == K * B)
+        assert cnt is None or (cnt.dtype == torch.int32 and cnt.is_contiguous())
+        assert hist is None or (hist.dtype == torch.int32 and hist.is_contiguous() and hist.shape[0] == B)
+        _lib.check(_lib.cuda_lib().odb_dec_accept(plog.data_ptr(), plog.stride(0), qlog.data_ptr() if qlog is not None else None,
+                                                  qlog.stride(0) if qlog is not None else 0, V, K, ictl.data_ptr(), fctl.data_ptr(),
+                                                  tok.data_ptr(), pos.data_ptr(), gen.data_ptr(), finished.data_ptr(), out.data_ptr(),
+                                                  out.shape[1], max_new, draft_pos.data_ptr() if draft_pos is not None else None,
+                                                  stats.data_ptr(), cnt.data_ptr() if cnt is not None else None,
+                                                  hist.data_ptr() if hist is not None else None, hist.shape[1] if hist is not None else 0,
+                                                  B, _lib.stream_ptr(plog)), "dec_accept")
         _lib.count_launch()
         return
     c = ictl.tolist()
@@ -263,40 +281,49 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor, ictl: torch.Tensor, fctl: tor
     greedy = not (c[CTL_DO_SAMPLE] and c[CTL_TOP_K] != 1)
     eos = set(c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]])
     p_all = plog.float().view(K + 1, B, V)
-    q_all = qlog.float().view(K, B, V)
+    q_all = qlog.float().view(K, B, V) if qlog is not None else None
     t = tok.view(K + 1, B)
     for b in range(B):
         if finished[b]:
-            draft_pos[b] = pos[b]
+            if draft_pos is not None:
+                draft_pos[b] = pos[b]
             continue
         g0 = int(gen[b])
-        drafts = [int(t[i + 1, b]) for i in range(K)]
+        n_cand = K if cnt is None else min(max(int(cnt[b]), 0), K)
+        drafts = [int(t[i + 1, b]) for i in range(n_cand)]
         n_acc, t_new = 0, 0
         if greedy:
             am = p_all[:, b].argmax(dim=-1).tolist()
-            while n_acc < K and drafts[n_acc] == am[n_acc]:
+            while n_acc < n_cand and drafts[n_acc] == am[n_acc]:
                 n_acc += 1
             t_new = am[n_acc]
         else:
             rng = torch.Generator(device="cpu").manual_seed((int(c[CTL_SEED]) * 1000003 + b * 7919 + g0) & ((1 << 63) - 1))
             p = torch.softmax(warp_logits(p_all[:, b].cpu(), temperature, c[CTL_TOP_K], top_p), dim=-1)          # [K+1, V]
-            q = torch.softmax(warp_logits(q_all[:, b].cpu(), temperature, c[CTL_TOP_K], top_p), dim=-1)          # [K, V]
-            while n_acc < K:
+            q = torch.softmax(warp_logits(q_all[:, b].cpu(), temperature, c[CTL_TOP_K], top_p), dim=-1) if q_all is not None else None
+            while n_acc < n_cand:
                 d = drafts[n_acc]
                 u = float(torch.rand((), generator=rng))
-                if p[n_acc, d] > 0 and u * q[n_acc, d] <= p[n_acc, d]:
+                qd = q[n_acc, d] if q is not None else 1.0
+                if p[n_acc, d] > 0 and u * qd <= p[n_acc, d]:
                     n_acc += 1
                     continue
-                res = (p[n_acc] - q[n_acc]).clamp(min=0)
+                if q is not None:
+                    res = (p[n_acc] - q[n_acc]).clamp(min=0)
+                else:
+                    res = p[n_acc].clone()
+                    res[d] = 0
                 t_new = int(torch.multinomial(res if float(res.sum()) > 0 else p[n_acc], 1, generator=rng))
                 break
             else:
-                t_new = int(torch.multinomial(p[K], 1, generator=rng))
+                t_new = int(torch.multinomial(p[n_cand], 1, generator=rng))
         g, fin = g0, False
         for x in drafts[:n_acc] + [t_new]:
             if fin or g >= max_new:
                 break
             out[b, g] = x
+            if hist is not None and int(pos[b]) + 1 + g - g0 < hist.shape[1]:
+                hist[b, int(pos[b]) + 1 + g - g0] = x
             g += 1
             fin = x in eos
         fin = fin or g >= max_new
@@ -308,7 +335,62 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor, ictl: torch.Tensor, fctl: tor
             pos[b] += n_acc + 1
         gen[b] = g
         t[0, b] = t_new
-        draft_pos[b] = pos[b]
+        if draft_pos is not None:
+            draft_pos[b] = pos[b]
+
+
+def lookup_propose(hist: torch.Tensor, pos: torch.Tensor, finished: torch.Tensor, ictl: torch.Tensor, tok: torch.Tensor,
+                   cnt: torch.Tensor, proposed: torch.Tensor, ngram: int) -> None:
+    """The proposals of one prompt-lookup round (transformers' ``PromptLookupCandidateGenerator``, every row at once).
+
+    Row b's history is h = hist[b, :L] with L = pos[b] + 1 (int32 [B, S]: the real prompt tokens, then the generated
+    ones).  For n from min(ngram, L - 1) down to 1: the earliest start s with h[s:s+n] == h[L-n:L] and s + n < L; the
+    first n that has one wins, and its candidates are h[s+n : min(s+n+K, L)], cut before the first EOS id of ictl.  No
+    such n: no candidates.  tok [(K+1)*B] slot-major: slots 1..c of row b get the c candidates, slots c+1..K the filler
+    id 0; cnt[b] = c (int32) and proposed[b] += c (int64).  Finished rows are left alone.  CUDA tensors run
+    ``lookup_propose_kernel``, others ``lookup_propose_reference``; both give the same result."""
+    B = pos.shape[0]
+    K = tok.shape[0] // B - 1
+    if hist.is_cuda and _lib.has_symbol("odb_dec_lookup_propose"):
+        assert hist.dtype == torch.int32 and hist.is_contiguous() and hist.shape[0] == B and pos.dtype == torch.int32
+        assert cnt.dtype == torch.int32 and proposed.dtype == torch.int64 and tok.dtype == torch.int64 and 1 <= ngram <= MAX_NGRAM
+        _lib.check(_lib.cuda_lib().odb_dec_lookup_propose(hist.data_ptr(), hist.shape[1], pos.data_ptr(), finished.data_ptr(),
+                                                          ictl.data_ptr(), tok.data_ptr(), cnt.data_ptr(), proposed.data_ptr(), K,
+                                                          ngram, B, _lib.stream_ptr(hist)), "dec_lookup_propose")
+        _lib.count_launch()
+        return
+    lookup_propose_reference(hist, pos, finished, ictl, tok, cnt, proposed, ngram)
+
+
+def lookup_candidates(h: list[int], K: int, ngram: int, eos) -> list[int]:
+    """The rule of ``lookup_propose`` on one history h (a list of ids): up to K candidate ids."""
+    L = len(h)
+    for n in range(min(ngram, L - 1), 0, -1):
+        tail = h[L - n:]
+        for s in range(L - n):                                     # s + n < L
+            if h[s:s + n] == tail:
+                cand = h[s + n:min(s + n + K, L)]
+                cut = next((i for i, x in enumerate(cand) if x in eos), len(cand))
+                return cand[:cut]
+    return []
+
+
+def lookup_propose_reference(hist: torch.Tensor, pos: torch.Tensor, finished: torch.Tensor, ictl: torch.Tensor, tok: torch.Tensor,
+                             cnt: torch.Tensor, proposed: torch.Tensor, ngram: int) -> None:
+    """``lookup_propose`` in PyTorch, row by row (``lookup_candidates``)."""
+    B = pos.shape[0]
+    K = tok.shape[0] // B - 1
+    c = ictl.tolist()
+    eos = set(c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]])
+    t = tok.view(K + 1, B)
+    for b in range(B):
+        if finished[b]:
+            continue
+        L = min(int(pos[b]) + 1, hist.shape[1])
+        cand = lookup_candidates(hist[b, :L].tolist(), K, ngram, eos)
+        t[1:, b] = torch.tensor(cand + [0] * (K - len(cand)), dtype=t.dtype)
+        cnt[b] = len(cand)
+        proposed[b] += len(cand)
 
 
 # ------------------------------------------------------------------------------------------------ beam search

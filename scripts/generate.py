@@ -18,6 +18,8 @@ read from a local directory.  ``--assistant-model`` (with ``--assistant-checkpoi
 draft model the same way and turns on assisted (speculative) generation.  ``--num-beams`` > 1 runs beam search and prints
 each returned hypothesis with its score (``--num-return-sequences`` per prompt).  ``--repetition-penalty``,
 ``--no-repeat-ngram-size`` and ``--min-new-tokens`` are HF's repetition controls, for greedy, sampling and beam search.
+``--prompt-lookup-num-tokens`` (with ``--max-matching-ngram-size``) turns on prompt lookup decoding: speculative
+generation whose proposals are copied from the row's own prompt and output, with no draft model.
 """
 import argparse
 import json
@@ -110,6 +112,9 @@ def main(argv=None) -> None:
     ap.add_argument("--repetition-penalty", type=float, default=1.0, help="HF's repetition penalty on the row's history (1.0: off)")
     ap.add_argument("--no-repeat-ngram-size", type=int, default=0, help="no n-gram of this size occurs twice in a row (0: off)")
     ap.add_argument("--min-new-tokens", type=int, default=0, help="EOS is forbidden until this many new tokens (0: off)")
+    ap.add_argument("--prompt-lookup-num-tokens", type=int, default=None,
+                    help="prompt lookup decoding: tokens proposed per round from the row's own history (1..7)")
+    ap.add_argument("--max-matching-ngram-size", type=int, default=None, help="prompt lookup: longest n-gram matched (default 2)")
     a = ap.parse_args(argv)
     if a.assistant_model is None and a.assistant_checkpoint is not None:
         ap.error("--assistant-checkpoint needs --assistant-model")
@@ -148,7 +153,8 @@ def main(argv=None) -> None:
                          num_assistant_tokens=a.num_assistant_tokens, num_beams=a.num_beams, length_penalty=a.length_penalty,
                          early_stopping=early_stopping, num_return_sequences=a.num_return_sequences, return_dict_in_generate=True,
                          repetition_penalty=a.repetition_penalty, no_repeat_ngram_size=a.no_repeat_ngram_size,
-                         min_new_tokens=a.min_new_tokens)
+                         min_new_tokens=a.min_new_tokens, prompt_lookup_num_tokens=a.prompt_lookup_num_tokens,
+                         max_matching_ngram_size=a.max_matching_ngram_size)
     out = res.sequences.cpu()
     R = out.shape[0] // len(prompts)
     for i, p in enumerate(prompts):
@@ -162,6 +168,9 @@ def main(argv=None) -> None:
     if assistant is not None:
         st = model.engine.assisted_state
         print(f"assisted: {st.verify_passes()} verify passes, acceptance {st.acceptance_rate():.3f}")
+    if a.prompt_lookup_num_tokens is not None:
+        st = model.engine.assisted_state
+        print(f"prompt lookup: {st.verify_passes()} verify passes, acceptance {st.acceptance_rate():.3f}")
 
 
 if __name__ == "__main__":
