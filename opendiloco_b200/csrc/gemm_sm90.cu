@@ -779,15 +779,17 @@ static int launch(const Operands& o, Params p, cudaStream_t st) {
   p.splits = 1;
   p.kb_per_split = kb_total;
   if (EPI == kWgradAcc) {
-    // split-K over the tokens so that tiles * splits is close to a whole multiple of the grid (one CTA per SM), so every
-    // persistent CTA gets the same number of work items; >= 16 k-blocks per work item
+    // split-K over the tokens (>= 16 k-blocks per work item), chosen by the time of the busiest persistent CTA: its work
+    // items x (k-blocks per item + the item's fixed cost).  The fixed cost is mostly the epilogue, the fp32 reduce-add of
+    // a whole tile into dW, and measures as about WGRAD_ITEM_KB k-blocks (split-count sweeps on an H100 SXM at 700 W,
+    // Llama-150M and 1B weight-gradient shapes): more, shorter items only pay off when they fill the grid much better.
+    constexpr int WGRAD_ITEM_KB = 32;
     int best = 1;
-    double best_eff = 0.0;
+    long long best_cost = LLONG_MAX;
     for (int s = 1; s <= 64 && kb_total / s >= 16; ++s) {
-      const int work = tiles * s;
-      const int waves = ceil_div(work, sm_count());
-      const double eff = (double)work / (double)(waves * sm_count());
-      if (eff > best_eff + 0.02) { best_eff = eff; best = s; }
+      const int kps = ceil_div(kb_total, s);
+      const long long cost = (long long)ceil_div(tiles * ceil_div(kb_total, kps), sm_count()) * (kps + WGRAD_ITEM_KB);
+      if (cost < best_cost) { best_cost = cost; best = s; }
     }
     p.kb_per_split = ceil_div(kb_total, best);
     p.splits = ceil_div(kb_total, p.kb_per_split);   // no empty slices

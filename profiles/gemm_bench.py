@@ -3,7 +3,8 @@
     python profiles/gemm_bench.py [--root DIR] [--step-only]
 
 --root DIR imports opendiloco_b200 from another built tree (e.g. an older commit, to compare two versions in one run);
---step-only times just the GEMMs of a Llama-150M micro-step (T = 32768) and prints one line per shape."""
+--step-only times every GEMM of a Llama-150M micro-step (T = 32768: forwards, dgrads, the four layer weight gradients, the
+LM-head forward, dX and dW) and prints one line per shape."""
 import argparse, os, sys, torch
 _ap = argparse.ArgumentParser()
 _ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -61,6 +62,8 @@ def step_shapes(Tn=32768, h=1024, I=2688, V=32000, S=1024):
     run("lce_fwd store=1 K1024", lambda: T.lce_fwd(x, w_lm, shift, partials, e), 2 * Tn * V * h)
     rs = torch.full((Tn,), 1e-3, device=dev); lab = torch.randint(0, V, (Tn,), device=dev); gs = torch.ones((), device=dev)
     run("lce_dx K32000", lambda: T.lce_dx(e, w_lm, rs, lab, gs, o), 2 * Tn * V * h)
+    dw_lm = torch.zeros(V, h, device=dev)
+    run(f"lce dW wgrad N{V} K{h}", lambda: T.wgrad_acc(e, x, dw_lm), 2 * Tn * V * h)
     for name, us, tf, spread in rows:
         print(f"STEP {name:32s} {us:9.1f} us {tf:6.1f} TF/s  (spread {spread:.1f} us)")
 
