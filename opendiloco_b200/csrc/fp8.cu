@@ -9,6 +9,10 @@
 //          everywhere (and inv = NaN): a diverging tensor stays visible instead of saturating to finite values.
 // Power-of-two scales make x * scale and the dequantisation exact, so an FP8 GEMM equals the bf16 GEMM of the
 // quantised-dequantised operands up to accumulation order.
+//
+//   quantize_rows : the same rule per ROW of a weight matrix (FP8 weight-only generation, ops/fp8w.py): one warp per row
+//          takes the row's amax, then writes q (e4m3), inv = 1 / scale and the dequantised bf16 row q * inv.  One launch
+//          covers a table of matrices (every projection of every layer).
 #include <cuda_fp8.h>
 #include <float.h>
 
@@ -110,7 +114,63 @@ __global__ void __launch_bounds__(256) cast_kernel(const __nv_bfloat16* __restri
   }
 }
 
+// One warp per row; blockIdx.y selects the matrix of the segment table: {src bf16*, q e4m3*, inv fp32*, deq bf16*, rows, cols}.
+__global__ void __launch_bounds__(256) quantize_rows_kernel(const long long* __restrict__ segs) {
+  const long long* sg = segs + 6 * blockIdx.y;
+  const int rows = (int)sg[4], cols = (int)sg[5];
+  const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= rows) return;
+  const __nv_bfloat16* x = reinterpret_cast<const __nv_bfloat16*>(sg[0]) + (size_t)r * cols;
+  uint8_t* q = reinterpret_cast<uint8_t*>(sg[1]) + (size_t)r * cols;
+  float* inv = reinterpret_cast<float*>(sg[2]);
+  __nv_bfloat16* deq = reinterpret_cast<__nv_bfloat16*>(sg[3]) + (size_t)r * cols;
+  uint32_t m = 0;
+  for (int c = lane * 8; c < cols; c += 256) {
+    const uint4 v = ld_v4(x + c);
+    m = bf16_abs_bits_max(m, v.x);
+    m = bf16_abs_bits_max(m, v.y);
+    m = bf16_abs_bits_max(m, v.z);
+    m = bf16_abs_bits_max(m, v.w);
+  }
+  m = __reduce_max_sync(0xffffffffu, m);
+  float scale;
+  const bool ok = fp8_scale(__uint_as_float(m), kE4M3Max, scale);
+  const float iv = ok ? 1.f / scale : __int_as_float(0x7fffffff);
+  if (lane == 0) inv[r] = iv;
+  for (int c = lane * 8; c < cols; c += 256) {
+    float f[8];
+    unpack8(ld_nc_v4(x + c), f);
+    uint32_t w[2];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const uint32_t lo = cvt2<false>(f[4 * k] * scale, f[4 * k + 1] * scale);
+      const uint32_t hi = cvt2<false>(f[4 * k + 2] * scale, f[4 * k + 3] * scale);
+      w[k] = ok ? (lo | hi << 16) : 0x7f7f7f7fu;
+    }
+    *reinterpret_cast<uint2*>(q + c) = make_uint2(w[0], w[1]);
+    float d[8];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[k >> 1] >> (16 * (k & 1))), __NV_E4M3);
+      const float2 v = __half22float2(*reinterpret_cast<const __half2*>(&h));
+      d[2 * k] = v.x * iv;
+      d[2 * k + 1] = v.y * iv;
+    }
+    st_v4(deq + c, pack8(d));
+  }
+}
+
 }  // namespace
+
+// Per-row e4m3 quantisation of n_seg bf16 matrices described by segs (device memory, 6 int64 per matrix: src, q, inv, deq
+// pointers, rows, cols; cols % 8 == 0 and every row 16-byte aligned): inv[r] = 1 / scale of row r's amax, q = e4m3 copy,
+// deq = bf16 q * inv.  max_rows: the largest rows of the table.
+ODB_EXPORT int odb_fp8_quantize_rows(const void* segs, int n_seg, int max_rows, cudaStream_t st) {
+  if (n_seg <= 0 || max_rows <= 0) return -1;
+  quantize_rows_kernel<<<dim3((unsigned)ceil_div(max_rows, 8), (unsigned)n_seg), 256, 0, st>>>((const long long*)segs);
+  ODB_CHECK_LAST();
+  return 0;
+}
 
 // slot (fp32 device scalar) = max |x| over x[n] (bf16, n % 8 == 0, 16-byte aligned); inf / NaN propagate.
 ODB_EXPORT int odb_fp8_amax(const void* x, long long n, void* slot, cudaStream_t st) {

@@ -28,6 +28,11 @@ decode layers, the LM head, the selection kernels and the cache reorder.  All be
 so every 128-key chunk behind the current one is immutable history: a beam that continues another row takes that row's
 chunks through a per-row chunk table and copies only the current partial chunk.
 
+FP8 weight-only mode, ``generate(fp8_weights=True)``: the layer programs take every projection weight from one helper
+(``_proj``, ``_weight``, ``_mlp``).  Without FP8 weights it returns the arena weight and launches what it always did; with
+them (:mod:`~opendiloco_b200.models.fp8_weights`) rows of M <= 64 run the skinny e4m3 GEMM and wider ones the bf16 GEMM on
+the dequantised weights Ŵ.  Every graph key carries the mode, so switching it recaptures.
+
 Nothing here goes through ``LlamaEngine.workspace`` or its captured training graphs: generating between training steps
 leaves the training buffers and graph untouched.
 """
@@ -45,6 +50,7 @@ from ..ops import decode as DK
 from ..ops import gemm as G
 from ..ops import kernels as K
 from ..ops import tc_gemm as TC
+from . import fp8_weights as W8
 
 FINISHED_CHECK_EVERY = 16           # decode steps between host checks of "every row has finished"
 ASSISTED_CHECK_EVERY = 4            # assisted rounds between host checks (a round emits 1 .. K+1 tokens per row)
@@ -139,9 +145,10 @@ def decode_state(model, B: int, Smax: int) -> DecodeState:
 
 # ------------------------------------------------------------------------------------------------ prefill
 @torch.no_grad()
-def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor) -> None:
+def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, fp8=None) -> None:
     """ids [B, Sp]: prompts compacted to start at position 0 and right-padded; lens [B] real lengths.  Fills the caches,
-    computes the logits at position lens[b]-1 and samples the first new token (st.pos ends at lens)."""
+    computes the logits at position lens[b]-1 and samples the first new token (st.pos ends at lens).  ``fp8``: the
+    model's FP8 weights (None: the arena weights)."""
     cfg, ar = model.config, model.arena
     B, Sp = ids.shape
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
@@ -155,7 +162,7 @@ def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor) -> No
     st.hist[:, :n].copy_(ids[:, :n])
     pb.ids.copy_(ids.reshape(-1))
     delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
-                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, st.lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D))
+                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, st.lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D), fp8=fp8)
     # only the last real position of every row feeds the LM head: gather its residual and delta rows
     last = torch.arange(B, device=st.device, dtype=torch.int64) * Sp + st.lens.long() - 1
     K.embedding_fwd(last, pb.res, out=st.res)
@@ -163,7 +170,7 @@ def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor) -> No
     _head_and_sample(cfg, ar, st, st.proj)
 
 
-def forward_layers(model, pb: _PrefillBuffers, B: int, Sp: int, cos, sin, fused_rope: bool, on_qkv=None):
+def forward_layers(model, pb: _PrefillBuffers, B: int, Sp: int, cos, sin, fused_rope: bool, on_qkv=None, fp8=None):
     """The forward-only layer program over pb.ids [B*Sp] (rows start at position 0; causal attention keeps right padding
     from reaching real positions): embedding, then per layer rmsnorm -> QKV(+RoPE) GEMM -> attention -> o-proj ->
     rmsnorm(+residual) -> SwiGLU GEMM -> down.  ``on_qkv(l, qkv)`` sees the rotated projections of layer l.  Returns the
@@ -176,27 +183,45 @@ def forward_layers(model, pb: _PrefillBuffers, B: int, Sp: int, cos, sin, fused_
     for l in range(L):
         p = f"model.layers.{l}."
         K.rmsnorm_fwd(pb.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
-        if fused_rope and TC.usable(pb.xn, ar.qkv_w(l)):
-            TC.linear_qkv_rope(pb.xn, ar.qkv_w(l), pb.qkv, cos, sin, Sp, (Hq + Hkv) * D)
+        w_qkv = _weight(ar, fp8, "qkv", l)
+        if fused_rope and TC.usable(pb.xn, w_qkv):
+            TC.linear_qkv_rope(pb.xn, w_qkv, pb.qkv, cos, sin, Sp, (Hq + Hkv) * D)
         else:
-            G.mm_nt(pb.xn, ar.qkv_w(l), out=pb.qkv)
+            _proj(ar, fp8, "qkv", l, pb.xn, pb.qkv)
             K.rope_(pb.qkv, cos, sin, Sp, Hq + Hkv, D)
         if on_qkv is not None:
             on_qkv(l, pb.qkv)
         att, _ = A.attention_fwd(pb.qkv, B, Sp, Hq, Hkv, D)
-        G.mm_nt(att, ar.w(p + "self_attn.o_proj.weight"), out=pb.proj)
+        _proj(ar, fp8, "o", l, att, pb.proj)
         K.rmsnorm_fwd(pb.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=pb.proj, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
-        _mlp(cfg, ar, l, pb.xn, pb.gu, pb.act)
-        G.mm_nt(pb.act, ar.w(p + "mlp.down_proj.weight"), out=pb.proj)
+        _mlp(cfg, ar, l, pb.xn, pb.gu, pb.act, fp8)
+        _proj(ar, fp8, "down", l, pb.act, pb.proj)
         delta = pb.proj
     return delta
 
 
-def _mlp(cfg, ar, l: int, xn, gu, act) -> None:
-    if cfg.intermediate_size % 64 == 0 and TC.usable(xn, ar.gu_w(l)):
-        TC.linear_swiglu(xn, ar.gu_w(l), gu, act)
+def _weight(ar, fp8, kind: str, l: int) -> torch.Tensor:
+    """The bf16 weight of projection ``kind`` (``fp8_weights.KINDS``) of layer l: the arena's, or Ŵ in FP8 mode."""
+    return W8.arena_weight(ar, kind, l) if fp8 is None else fp8.weight(kind, l)
+
+
+def _proj(ar, fp8, kind: str, l: int, x, out) -> None:
+    """out = x @ W^T for projection ``kind`` of layer l: the skinny FP8 GEMM where it applies, else the bf16 GEMM."""
+    if fp8 is not None and fp8.skinny(kind, x):
+        fp8.linear(kind, l, x, out)
     else:
-        G.mm_nt(xn, ar.gu_w(l), out=gu)
+        G.mm_nt(x, _weight(ar, fp8, kind, l), out=out)
+
+
+def _mlp(cfg, ar, l: int, xn, gu, act, fp8=None) -> None:
+    if fp8 is not None and fp8.skinny("gu", xn):
+        fp8.linear("gu", l, xn, gu, act=act)
+        return
+    w = _weight(ar, fp8, "gu", l)
+    if cfg.intermediate_size % 64 == 0 and TC.usable(xn, w):
+        TC.linear_swiglu(xn, w, gu, act)
+    else:
+        G.mm_nt(xn, w, out=gu)
         K.swiglu_fwd(gu, out=act)
 
 
@@ -211,7 +236,7 @@ def _head_and_sample(cfg, ar, st: DecodeState, delta) -> None:
 
 
 # ------------------------------------------------------------------------------------------------ decode step
-def _layers(model, buf, ids: torch.Tensor, attend):
+def _layers(model, buf, ids: torch.Tensor, attend, fp8=None):
     """The decode layer program over the rows of ``buf`` (a DecodeState or AssistedState): embedding of ids, then per layer
     rmsnorm -> QKV GEMM -> ``attend(l, qkv, att)`` (RoPE, cache append, attention) -> o-proj -> rmsnorm(+residual) ->
     SwiGLU GEMM -> down.  Returns the last layer's output delta; the residual before it is in buf.res."""
@@ -222,17 +247,17 @@ def _layers(model, buf, ids: torch.Tensor, attend):
     for l in range(cfg.num_hidden_layers):
         p = f"model.layers.{l}."
         K.rmsnorm_fwd(buf.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=buf.xn, rstd=buf.rstd, x_out=buf.res)
-        G.mm_nt(buf.xn, ar.qkv_w(l), out=buf.qkv)
+        _proj(ar, fp8, "qkv", l, buf.xn, buf.qkv)
         attend(l, buf.qkv, buf.att)
-        G.mm_nt(buf.att, ar.w(p + "self_attn.o_proj.weight"), out=buf.proj)
+        _proj(ar, fp8, "o", l, buf.att, buf.proj)
         K.rmsnorm_fwd(buf.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=buf.proj, out=buf.xn, rstd=buf.rstd, x_out=buf.res)
-        _mlp(cfg, ar, l, buf.xn, buf.gu, buf.act)
-        G.mm_nt(buf.act, ar.w(p + "mlp.down_proj.weight"), out=buf.proj)
+        _mlp(cfg, ar, l, buf.xn, buf.gu, buf.act, fp8)
+        _proj(ar, fp8, "down", l, buf.act, buf.proj)
         delta = buf.proj
     return delta
 
 
-def _one_token_layers(model, st: DecodeState, ids: torch.Tensor, table: torch.Tensor | None = None):
+def _one_token_layers(model, st: DecodeState, ids: torch.Tensor, table: torch.Tensor | None = None, fp8=None):
     """One token per row at st.pos: the decode layers with single-query RoPE+append and split-KV attention (through the
     chunk table, if given)."""
     cfg = model.config
@@ -242,34 +267,38 @@ def _one_token_layers(model, st: DecodeState, ids: torch.Tensor, table: torch.Te
         DK.rope_append(qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D)
         DK.attention(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.part_o, st.part_ml, table=table)
 
-    return _layers(model, st, ids, attend)
+    return _layers(model, st, ids, attend, fp8)
 
 
-def _step_eager(model, st: DecodeState) -> None:
-    delta = _one_token_layers(model, st, st.ids)
+def _fp8_key(fp8):
+    return None if fp8 is None else fp8.token
+
+
+def _step_eager(model, st: DecodeState, fp8=None) -> None:
+    delta = _one_token_layers(model, st, st.ids, fp8=fp8)
     _head_and_sample(model.config, model.arena, st, delta)
 
 
 @torch.no_grad()
-def step(model, st: DecodeState, graph: bool | None = None) -> None:
+def step(model, st: DecodeState, graph: bool | None = None, fp8=None) -> None:
     """One decode step: consume st.ids at st.pos, sample the next token into st.ids / st.out.  With the kernels and
     ``graph`` (default: ``ODB_CUDA_GRAPH`` != 0) the first call runs eagerly (warm-up), the second captures the step and
-    every call replays it."""
+    every call replays it.  ``fp8``: the model's FP8 weights (None: the arena weights)."""
     if graph is None:
         graph = _use_graph()
     if not (graph and st.kernels):
-        _step_eager(model, st)
+        _step_eager(model, st, fp8)
         return
-    key = (model.arena.version, model.arena.shadow.data_ptr())
+    key = (model.arena.version, model.arena.shadow.data_ptr(), _fp8_key(fp8))
     if st.graph is None or st.graph_key != key:
         if st.graph_key != ("warm",) + key:
             st.graph, st.graph_key = None, ("warm",) + key
-            _step_eager(model, st)
+            _step_eager(model, st, fp8)
             return
         torch.cuda.synchronize(st.device)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
-            _step_eager(model, st)
+            _step_eager(model, st, fp8)
         st.graph, st.graph_key = g, key
     st.graph.replay()
 
@@ -343,7 +372,7 @@ def assisted_state(model, assistant, B: int, K: int, Smax: int) -> AssistedState
     return st
 
 
-def _verify(model, tst: DecodeState, ast: AssistedState) -> None:
+def _verify(model, tst: DecodeState, ast: AssistedState, fp8=None) -> None:
     """The target scores ast.tok (slot j at tst.pos + j) in one pass: logits of every slot -> ast.plog."""
     cfg, ar = model.config, model.arena
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
@@ -353,15 +382,15 @@ def _verify(model, tst: DecodeState, ast: AssistedState) -> None:
         DK.rope_append_multi(qkv, tst.cos, tst.sin, tst.pos, tst.kc[l], tst.vc[l], Hq, Hkv, D, n)
         DK.verify_attention(qkv, tst.kc[l], tst.vc[l], tst.pos, att, Hq, Hkv, D, n, ast.part_o, ast.part_ml)
 
-    delta = _layers(model, ast, ast.tok, attend)
+    delta = _layers(model, ast, ast.tok, attend, fp8)
     K.rmsnorm_fwd(ast.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=ast.xn, rstd=ast.rstd, x_out=ast.res)
     G.mm_nt(ast.xn, ar.w("lm_head.weight"), out=ast.plog)
 
 
-def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: int, ngram: int) -> None:
+def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: int, ngram: int, fp8=None) -> None:
     if draft is None:                                 # prompt lookup: proposals from the history, point-mass acceptance
         DK.lookup_propose(tst.hist, tst.pos, tst.finished, tst.ictl, ast.tok, ast.cnt, ast.proposed, ngram)
-        _verify(target, tst, ast)
+        _verify(target, tst, ast, fp8)
         DK.accept(ast.plog, None, tst.ictl, tst.fctl, ast.tok, tst.pos, tst.gen, tst.finished, tst.out, max_new, None, ast.stats,
                   cnt=ast.cnt, hist=tst.hist)
         return
@@ -376,33 +405,34 @@ def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: i
         K.rmsnorm_fwd(dst.res, dar.w("model.norm.weight"), dcfg.rms_norm_eps, delta=delta, out=dst.xn, rstd=dst.rstd, x_out=dst.res)
         G.mm_nt(dst.xn, dar.w("lm_head.weight"), out=q)
         DK.sample(q, dst.ictl, dst.fctl, dst.pos, dst.gen, dst.finished, dst.out, ast.tok[(i + 1) * B:(i + 2) * B])
-    _verify(target, tst, ast)
+    _verify(target, tst, ast, fp8)                    # the draft above runs on its own weights
     DK.accept(ast.plog, ast.qlog, tst.ictl, tst.fctl, ast.tok, tst.pos, tst.gen, tst.finished, tst.out, max_new, dst.pos, ast.stats)
 
 
 @torch.no_grad()
 def assisted_round(target, draft, tst: DecodeState, ast: AssistedState, max_new: int, graph: bool | None = None,
-                   ngram: int = 2) -> None:
+                   ngram: int = 2, fp8=None) -> None:
     """One assisted round: K draft proposals, one verify pass of the target, acceptance.  ``draft`` None is a prompt-lookup
     round: up to K proposals per row from an earlier occurrence of the row's last n-gram (n <= ``ngram``) in its history,
     one verify pass, point-mass acceptance.  With the kernels and ``graph`` (default: ``ODB_CUDA_GRAPH`` != 0) the first
-    call runs eagerly (warm-up), the second captures the round and every call replays it."""
+    call runs eagerly (warm-up), the second captures the round and every call replays it.  ``fp8``: the target's FP8
+    weights (None: its arena weights); the draft always runs on its own arena weights."""
     if graph is None:
         graph = _use_graph()
     if not (graph and ast.graphable and tst.kernels):
-        _round_eager(target, draft, tst, ast, max_new, ngram)
+        _round_eager(target, draft, tst, ast, max_new, ngram, fp8)
         return
     proposer = (draft.arena.version, draft.arena.shadow.data_ptr()) if draft is not None else ("lookup", ngram)
-    key = (target.arena.version, target.arena.shadow.data_ptr(), *proposer, id(tst), max_new)
+    key = (target.arena.version, target.arena.shadow.data_ptr(), *proposer, id(tst), max_new, _fp8_key(fp8))
     if ast.graph is None or ast.graph_key != key:
         if ast.graph_key != ("warm",) + key:
             ast.graph, ast.graph_key, ast.graph_target = None, ("warm",) + key, tst
-            _round_eager(target, draft, tst, ast, max_new, ngram)
+            _round_eager(target, draft, tst, ast, max_new, ngram, fp8)
             return
         torch.cuda.synchronize(tst.device)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
-            _round_eager(target, draft, tst, ast, max_new, ngram)
+            _round_eager(target, draft, tst, ast, max_new, ngram, fp8)
         ast.graph, ast.graph_key = g, key
     ast.graph.replay()
 
@@ -454,7 +484,7 @@ def _check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size, assistant_m
 
 
 def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int, Kp: int, controls: tuple, pad: int,
-                       eos: list[int], ngram: int = 2) -> torch.Tensor:
+                       eos: list[int], ngram: int = 2, fp8=None) -> torch.Tensor:
     """Assisted generation with ``assistant``, or prompt lookup (n-grams up to ``ngram``) with ``assistant`` None."""
     B = comp.shape[0]
     Smax = _round_up(P + max_new_tokens + Kp, 128)
@@ -466,7 +496,7 @@ def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int
     if dst is not None:
         dst.set_controls(do_sample, temperature, top_k, top_p, seed ^ DRAFT_SEED_XOR, 0, [])
     tst.out.fill_(pad)
-    prefill(model, tst, comp, lens)                   # also leaves each row's history in tst.hist
+    prefill(model, tst, comp, lens, fp8)              # also leaves each row's history in tst.hist
     if dst is not None:
         prefill(assistant, dst, comp, lens)
         dst.finished.zero_()                          # the draft never stops by itself; its position follows the target's
@@ -477,7 +507,7 @@ def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int
     for r in range(max_new_tokens - 1):               # every round emits >= 1 token per unfinished row
         if r % ASSISTED_CHECK_EVERY == 0 and bool(tst.finished.all()):
             break
-        assisted_round(model, assistant, tst, ast, max_new_tokens, ngram=ngram)
+        assisted_round(model, assistant, tst, ast, max_new_tokens, ngram=ngram, fp8=fp8)
     return tst.out[:, :max_new_tokens].clone()
 
 
@@ -559,7 +589,7 @@ def beam_state(model, B: int, nb: int, K: int, max_new: int, Smax: int) -> BeamS
 
 
 @torch.no_grad()
-def beam_prefill(model, bs: BeamState, ids: torch.Tensor, lens: torch.Tensor) -> None:
+def beam_prefill(model, bs: BeamState, ids: torch.Tensor, lens: torch.Tensor, fp8=None) -> None:
     """ids [B, Sp] compacted prompts, lens [B]: the layers run on the B prompts once and fill the beam-0 row of each
     prompt; the last position's logits go to every beam row of the prompt (st.pos ends at lens - 1)."""
     cfg, ar = model.config, model.arena
@@ -570,7 +600,8 @@ def beam_prefill(model, bs: BeamState, ids: torch.Tensor, lens: torch.Tensor) ->
     st.pos.copy_(lens.repeat_interleave(nb) - 1)
     pb.ids.copy_(ids.reshape(-1))
     delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
-                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, row_stride=nb))
+                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, row_stride=nb),
+                           fp8=fp8)
     last = (torch.arange(B, device=st.device, dtype=torch.int64) * Sp + lens.long() - 1).repeat_interleave(nb)
     K.embedding_fwd(last, pb.res, out=st.res)
     K.embedding_fwd(last, delta, out=st.proj)
@@ -586,39 +617,39 @@ def beam_select(bs: BeamState, length_penalty: float, early_stopping: int) -> No
     DK.beam_reorder(st.kv, bs.table, bs.parent, st.pos, bs.nb)
 
 
-def _beam_step_eager(model, bs: BeamState, length_penalty: float, early_stopping: int) -> None:
+def _beam_step_eager(model, bs: BeamState, length_penalty: float, early_stopping: int, fp8=None) -> None:
     st = bs.dec
-    delta = _one_token_layers(model, st, st.ids, bs.table)
+    delta = _one_token_layers(model, st, st.ids, bs.table, fp8)
     _head(model.config, model.arena, st, delta)
     beam_select(bs, length_penalty, early_stopping)
 
 
 @torch.no_grad()
-def beam_step(model, bs: BeamState, length_penalty: float, early_stopping: int, graph: bool | None = None) -> None:
+def beam_step(model, bs: BeamState, length_penalty: float, early_stopping: int, graph: bool | None = None, fp8=None) -> None:
     """One beam-search step: the beams' tokens at their position, the LM head, selection and reorder.  With the kernels
     and ``graph`` (default: ``ODB_CUDA_GRAPH`` != 0) the first call runs eagerly (warm-up), the second captures the step and
     every call replays it."""
     if graph is None:
         graph = _use_graph()
     if not (graph and bs.kernels):
-        _beam_step_eager(model, bs, length_penalty, early_stopping)
+        _beam_step_eager(model, bs, length_penalty, early_stopping, fp8)
         return
-    key = (model.arena.version, model.arena.shadow.data_ptr(), float(length_penalty), int(early_stopping))
+    key = (model.arena.version, model.arena.shadow.data_ptr(), float(length_penalty), int(early_stopping), _fp8_key(fp8))
     if bs.graph is None or bs.graph_key != key:
         if bs.graph_key != ("warm",) + key:
             bs.graph, bs.graph_key = None, ("warm",) + key
-            _beam_step_eager(model, bs, length_penalty, early_stopping)
+            _beam_step_eager(model, bs, length_penalty, early_stopping, fp8)
             return
         torch.cuda.synchronize(bs.dec.device)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
-            _beam_step_eager(model, bs, length_penalty, early_stopping)
+            _beam_step_eager(model, bs, length_penalty, early_stopping, fp8)
         bs.graph, bs.graph_key = g, key
     bs.graph.replay()
 
 
 def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R: int, length_penalty: float, early_stopping,
-                   pad: int, eos: list[int], processors: tuple = (1.0, 0, 0)) -> tuple[torch.Tensor, torch.Tensor]:
+                   pad: int, eos: list[int], processors: tuple = (1.0, 0, 0), fp8=None) -> tuple[torch.Tensor, torch.Tensor]:
     B, Sp = comp.shape
     es = DK.EARLY_STOPPING[early_stopping]
     bs = beam_state(model, B, nb, DK.beams_to_keep(nb, len(eos)), max_new_tokens, Smax)
@@ -626,12 +657,12 @@ def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R
     bs.reset(pad)
     bs.prompt[:, :Sp].copy_(comp)
     bs.plens.copy_(lens)
-    beam_prefill(model, bs, comp, lens)
+    beam_prefill(model, bs, comp, lens, fp8)
     beam_select(bs, length_penalty, es)              # step 0 on the prefill logits: only beam 0 has score 0
     for t in range(1, max_new_tokens):
         if t % FINISHED_CHECK_EVERY == 0 and bool(bs.done.all()):
             break
-        beam_step(model, bs, length_penalty, es)
+        beam_step(model, bs, length_penalty, es, fp8=fp8)
     return bs.results(R)
 
 
@@ -686,7 +717,7 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
              length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1,
              return_dict_in_generate: bool = False, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
              min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
-             max_matching_ngram_size: int | None = None) -> torch.Tensor | GenerateOutput:
+             max_matching_ngram_size: int | None = None, fp8_weights: bool = False) -> torch.Tensor | GenerateOutput:
     """See :meth:`LlamaForCausalLM.generate`."""
     cfg, ar = model.config, model.arena
     if ar.param_sharded:
@@ -711,6 +742,7 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     ngram = _check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size, assistant_model, num_beams, proc_on, P, max_new_tokens,
                           cfg.max_position_embeddings)
     processors = (float(repetition_penalty), no_repeat_ngram_size, min_new_tokens)
+    W8.check_flag(fp8_weights)
     dev = ar.device
     ids = input_ids.to(dev)
     if attention_mask is None:
@@ -732,26 +764,27 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     col = (P - lens.long())[:, None] + torch.arange(Sp, device=dev)[None, :]
     comp = ids.gather(1, col.clamp(max=P - 1))
     comp = comp.masked_fill(torch.arange(Sp, device=dev)[None, :] >= lens.long()[:, None], 0)
+    fp8 = W8.fp8_weights(model) if fp8_weights else None
     if assistant_model is not None or prompt_lookup_num_tokens is not None:
         K = num_assistant_tokens if assistant_model is not None else prompt_lookup_num_tokens
         new = _assisted_generate(model, assistant_model, comp, lens, P, max_new_tokens, K, (do_sample, temperature, top_k, top_p, seed),
-                                 pad, eos, ngram)
+                                 pad, eos, ngram, fp8)
         out = torch.cat([ids, new], dim=1)
         return GenerateOutput(out) if return_dict_in_generate else out
     Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))
     if num_beams > 1:
         new, scores = _beam_generate(model, comp, lens, Smax, max_new_tokens, num_beams, num_return_sequences, length_penalty,
-                                     early_stopping, pad, eos, processors)
+                                     early_stopping, pad, eos, processors, fp8)
         out = torch.cat([ids.repeat_interleave(num_return_sequences, dim=0), new], dim=1)
         return GenerateOutput(out, scores) if return_dict_in_generate else out
     st = decode_state(model, B, Smax)
 
     st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, *processors)
     st.out.fill_(pad)
-    prefill(model, st, comp, lens)
+    prefill(model, st, comp, lens, fp8)
     for t in range(1, max_new_tokens):
         if eos and t % FINISHED_CHECK_EVERY == 0 and bool(st.finished.all()):
             break
-        step(model, st)
+        step(model, st, fp8=fp8)
     out = torch.cat([ids, st.out[:, :max_new_tokens].clone()], dim=1)
     return GenerateOutput(out) if return_dict_in_generate else out

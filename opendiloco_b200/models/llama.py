@@ -195,6 +195,7 @@ class LlamaEngine:
         self.assisted_state = None                 # assisted generation's verify buffers, draft caches + round graph
         self.beam_state = None                     # beam search's caches, chunk table, selection state + step graph
         self.score_state = None                    # scoring buffers (models/scoring.py)
+        self.fp8_weights = None                    # e4m3 + dequantised projection weights of fp8_weights=True (models/fp8_weights.py)
 
     def workspace(self, B: int, S: int) -> _Workspace:
         key = (B, S, str(self.arena.device), self.arena.compute_dtype)
@@ -694,6 +695,7 @@ class LlamaForCausalLM(nn.Module):
                 self.engine.assisted_state = None
                 self.engine.beam_state = None
                 self.engine.score_state = None
+                self.engine.fp8_weights = None
                 self.engine.head_grad_tmp = None
                 self._rebind()
         return self
@@ -746,7 +748,7 @@ class LlamaForCausalLM(nn.Module):
                  num_assistant_tokens: int = 4, num_beams: int = 1, length_penalty: float = 1.0, early_stopping=False,
                  num_return_sequences: int = 1, return_dict_in_generate: bool = False, repetition_penalty: float = 1.0,
                  no_repeat_ngram_size: int = 0, min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
-                 max_matching_ngram_size: int | None = None):
+                 max_matching_ngram_size: int | None = None, fp8_weights: bool = False):
         """KV-cached text generation with HF ``generate`` keyword names.  Returns LongTensor [B, P + max_new_tokens]: the
         prompt as given, then the new tokens.
 
@@ -807,7 +809,17 @@ class LlamaForCausalLM(nn.Module):
 
         ``return_dict_in_generate=True`` returns a ``GenerateOutput`` with ``sequences`` and ``sequences_scores`` (fp32
         [B * num_return_sequences]: each hypothesis's summed log-probabilities / generated_len ** length_penalty; None
-        without beam search)."""
+        without beam search).
+
+        ``fp8_weights=True`` generates with FP8 weight-only quantisation: at the start of the call the q|k|v, o, gate|up
+        and down projections of every decoder layer are quantised to e4m3 with one power-of-two scale per output row
+        (ops/fp8w.py); the embedding, the norms and the LM head stay in the compute dtype.  The result is the model with
+        every projection weight replaced by its dequantised copy Ŵ: bf16-mixed CUDA models decode on an sm_90a GEMM that
+        streams the e4m3 weights (half the bytes of bf16) wherever a pass has at most 64 rows and run the bf16 GEMMs on Ŵ
+        elsewhere (prefill, wider verify passes and beam steps); other precisions and devices run the reference path on
+        Ŵ.  Works with every mode above; with ``assistant_model`` only this model is quantised.  While in use the e4m3 and
+        dequantised copies take 1.5x the bf16 bytes of the projections (about 2.9 GB at the 1b preset), kept on the engine
+        for the next call; training state is not touched.  Raises ValueError when ``fp8_weights`` is not a bool."""
         from .generation import generate
 
         return generate(self, input_ids, attention_mask=attention_mask, max_new_tokens=max_new_tokens, do_sample=do_sample,
@@ -816,10 +828,12 @@ class LlamaForCausalLM(nn.Module):
                         length_penalty=length_penalty, early_stopping=early_stopping, num_return_sequences=num_return_sequences,
                         return_dict_in_generate=return_dict_in_generate, repetition_penalty=repetition_penalty,
                         no_repeat_ngram_size=no_repeat_ngram_size, min_new_tokens=min_new_tokens,
-                        prompt_lookup_num_tokens=prompt_lookup_num_tokens, max_matching_ngram_size=max_matching_ngram_size)
+                        prompt_lookup_num_tokens=prompt_lookup_num_tokens, max_matching_ngram_size=max_matching_ngram_size,
+                        fp8_weights=fp8_weights)
 
     @torch.no_grad()
-    def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None):
+    def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None,
+              fp8_weights: bool = False):
         """Per-token log-likelihoods.  Returns ``ScoreOutput`` with ``logprobs`` (fp32 [B, S], log p(target_t | tokens < t))
         and ``greedy`` (bool [B, S], the argmax of the prediction at t-1, lowest index on ties, equals target_t), on the
         model's device.
@@ -832,10 +846,14 @@ class LlamaForCausalLM(nn.Module):
         the bf16 path from their bf16 compute weights (no FP8 GEMMs), so their log-likelihoods differ slightly from the
         FP8 eval loss of ``forward``.  Raises ValueError for a
         parameter-sharded (FULL_SHARD) model, a sequence longer than ``max_position_embeddings``, mismatched shapes, a mask
-        that is not one run per row, or token / label ids outside the vocabulary."""
+        that is not one run per row, or token / label ids outside the vocabulary.
+
+        ``fp8_weights=True`` scores the FP8 weight-only quantised model of ``generate(fp8_weights=True)`` (the projections
+        replaced by their per-row e4m3 dequantised copies), which is how the quality cost of that quantisation is measured;
+        a non-bool raises ValueError."""
         from .scoring import score
 
-        return score(self, input_ids, attention_mask=attention_mask, labels=labels)
+        return score(self, input_ids, attention_mask=attention_mask, labels=labels, fp8_weights=fp8_weights)
 
     # ------------------------------------------------------------------ state dict / checkpoints
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):

@@ -23,6 +23,7 @@ import torch
 
 from ..ops import kernels as K
 from ..ops import tc_gemm as TC
+from . import fp8_weights as W8
 from .generation import _PrefillBuffers, _round_up, forward_layers
 
 SCORE_CHUNK = 32768                 # LM-head rows per scoring GEMM on the kernels
@@ -114,21 +115,23 @@ def _plan(cfg, input_ids, attention_mask, labels, kernels: bool):
 
 @torch.no_grad()
 def score(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None,
-          labels: torch.Tensor | None = None) -> ScoreOutput:
+          labels: torch.Tensor | None = None, fp8_weights: bool = False) -> ScoreOutput:
     """See :meth:`LlamaForCausalLM.score`."""
     cfg, ar = model.config, model.arena
     if ar.param_sharded:
         raise ValueError("score() needs the full compute weights on this rank; the arena is parameter-sharded (FULL_SHARD)")
     w_lm = ar.w("lm_head.weight")
     kernels = cfg.head_dim == 64 and TC.usable(w_lm)
+    W8.check_flag(fp8_weights)
     comp, Sp, gidx, lab = _plan(cfg, input_ids, attention_mask, labels, kernels)
+    fp8 = W8.fp8_weights(model) if fp8_weights else None
     B, S = input_ids.shape
     st = score_state(model, B, Sp, S, kernels)
     pb = st.pb
     pb.ids.copy_(comp.reshape(-1))
     st.gidx.copy_(gidx)
     st.labels.copy_(lab)
-    delta = forward_layers(model, pb, B, Sp, st.cos, st.sin, kernels)
+    delta = forward_layers(model, pb, B, Sp, st.cos, st.sin, kernels, fp8=fp8)
     K.rmsnorm_fwd(pb.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
     K.embedding_fwd(st.gidx, pb.xn, out=st.xg)        # the row that predicts each output slot, in output order
     n = B * S

@@ -17,6 +17,10 @@ Multiple choice scores each choice by the sum of its continuation log-probabilit
 (fraction of gold continuations that are the greedy continuation at every token) and ``n`` (requests).  Requests are
 sorted by length and scored in right-padded batches of --batch-size sequences.  ``context`` and ``choices`` may also be
 text when a local ``--tokenizer`` directory is given.
+
+``--fp8-weights`` scores the model with its decoder-layer projections quantised to e4m3, one scale per output row (what
+``generate.py --fp8-weights`` decodes with), and adds ``"fp8_weights": true`` to the result: compare it with a run
+without the flag to see what the quantisation costs.
 """
 import argparse
 import json
@@ -37,7 +41,7 @@ def _sync(device: torch.device) -> None:
         torch.cuda.synchronize(device)
 
 
-def perplexity(model, pattern: str, seq_len: int, batch_size: int, batches: int, seed: int) -> dict:
+def perplexity(model, pattern: str, seq_len: int, batch_size: int, batches: int, seed: int, fp8_weights: bool = False) -> dict:
     from opendiloco_b200.utils.data import TokenFileLoader
 
     dev = model.device
@@ -48,7 +52,7 @@ def perplexity(model, pattern: str, seq_len: int, batch_size: int, batches: int,
             ids = next(loader)["input_ids"].to(dev)
             _sync(dev)
             t0 = time.perf_counter()
-            lp = model.score(ids).logprobs
+            lp = model.score(ids, fp8_weights=fp8_weights).logprobs
             _sync(dev)
             seconds += time.perf_counter() - t0
             nll -= float(lp[:, 1:].double().sum())
@@ -68,7 +72,7 @@ def _ids(x, tok, what: str, special: bool) -> list[int]:
     return [int(t) for t in x]
 
 
-def multiple_choice(model, path: str, batch_size: int, tok) -> dict:
+def multiple_choice(model, path: str, batch_size: int, tok, fp8_weights: bool = False) -> dict:
     requests = []
     with open(path) as f:
         for n, line in enumerate(f, 1):
@@ -99,7 +103,7 @@ def multiple_choice(model, path: str, batch_size: int, tok) -> dict:
             ctx, choices, _ = requests[q]
             ids[i, :n] = torch.tensor(ctx + choices[k])
             mask[i, :n] = 1
-        out = model.score(ids.to(dev), attention_mask=mask.to(dev))
+        out = model.score(ids.to(dev), attention_mask=mask.to(dev), fp8_weights=fp8_weights)
         lp, gr = out.logprobs.cpu(), out.greedy.cpu()
         for i, (n, q, k) in enumerate(batch):
             c0 = len(requests[q][0])
@@ -125,6 +129,9 @@ def main(argv=None) -> None:
     ap.add_argument("--seed", type=int, default=0, help="perplexity: seed of the window order")
     ap.add_argument("--choices", default=None, help="JSONL file of multiple-choice requests")
     ap.add_argument("--tokenizer", default=None, help="local tokenizer directory for text requests (never downloaded)")
+    ap.add_argument("--fp8-weights", action="store_true",
+                    help="score the model with its decoder-layer projections quantised to e4m3 (generate --fp8-weights): "
+                         "compare with a run without it to see what the quantisation costs")
     a = ap.parse_args(argv)
     if a.tokens is None and a.choices is None:
         ap.error("give --tokens (perplexity) and/or --choices (multiple choice)")
@@ -138,9 +145,11 @@ def main(argv=None) -> None:
     model = load_model(a)
     result = {}
     if a.tokens is not None:
-        result.update(perplexity(model, a.tokens, a.seq_len, a.batch_size, a.batches, a.seed))
+        result.update(perplexity(model, a.tokens, a.seq_len, a.batch_size, a.batches, a.seed, a.fp8_weights))
     if a.choices is not None:
-        result.update(multiple_choice(model, a.choices, a.batch_size, tok))
+        result.update(multiple_choice(model, a.choices, a.batch_size, tok, a.fp8_weights))
+    if a.fp8_weights:
+        result["fp8_weights"] = True
     print(json.dumps(result))
 
 

@@ -115,6 +115,8 @@ def main(argv=None) -> None:
     ap.add_argument("--prompt-lookup-num-tokens", type=int, default=None,
                     help="prompt lookup decoding: tokens proposed per round from the row's own history (1..7)")
     ap.add_argument("--max-matching-ngram-size", type=int, default=None, help="prompt lookup: longest n-gram matched (default 2)")
+    ap.add_argument("--fp8-weights", action="store_true",
+                    help="quantise the decoder-layer projections to e4m3 (one scale per output row) and decode on them")
     a = ap.parse_args(argv)
     if a.assistant_model is None and a.assistant_checkpoint is not None:
         ap.error("--assistant-checkpoint needs --assistant-model")
@@ -154,7 +156,7 @@ def main(argv=None) -> None:
                          early_stopping=early_stopping, num_return_sequences=a.num_return_sequences, return_dict_in_generate=True,
                          repetition_penalty=a.repetition_penalty, no_repeat_ngram_size=a.no_repeat_ngram_size,
                          min_new_tokens=a.min_new_tokens, prompt_lookup_num_tokens=a.prompt_lookup_num_tokens,
-                         max_matching_ngram_size=a.max_matching_ngram_size)
+                         max_matching_ngram_size=a.max_matching_ngram_size, fp8_weights=a.fp8_weights)
     out = res.sequences.cpu()
     R = out.shape[0] // len(prompts)
     for i, p in enumerate(prompts):
