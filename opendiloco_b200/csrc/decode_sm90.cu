@@ -15,12 +15,19 @@
 //
 // KV cache layout, per layer: K and V each [B, Hkv, Smax, 64] bf16, so the keys of one (row, kv head) are contiguous and a
 // chunk of them is ONE bulk copy.
+//
+// FP8 KV cache (generate(fp8_kv_cache=True)): K and V each [B, Hkv, Smax, 64] e4m3 plus fp32 inv [B, Hkv, Smax], one
+// power-of-two scale per (position, kv head) row by the rule of fp8_rows.cuh.  The writers quantise the bf16 row the bf16
+// writer would store; the attention kernels dequantise each element as q * inv, which is exactly the bf16 value of the
+// dequantised cache C^ = q * inv, so they compute bit for bit what the bf16 kernels compute on C^.  The kernels are
+// templates on the cache element type T (bf16, or uint8_t for e4m3 bytes); the inv pointers are null for bf16.
 #include <curand_kernel.h>
 
 #include <algorithm>
 #include <climits>
 
 #include "common.cuh"
+#include "fp8_rows.cuh"
 #include "sm90_ptx.cuh"
 
 using namespace odb;
@@ -32,13 +39,37 @@ constexpr int D = 64;
 constexpr int CH = 128;             // keys per attention CTA
 constexpr int ATT_THREADS = 128;    // one thread per key in the score phase, four warps in P V
 
+// ------------------------------------------------------------------------------------------------ FP8 cache rows
+// One warp quantises one 64-value cache row, two values per lane: returns the lane's two e4m3 bytes (x0 low, x1 high); lane
+// 0 writes the row's inv.  The amax is an integer max of the |x| bit patterns, so a NaN or inf reaches it (NaN bytes, inv NaN).
+__device__ __forceinline__ uint32_t quantize_pair(float x0, float x1, float* __restrict__ inv) {
+  const uint32_t m = __reduce_max_sync(0xffffffffu, max(__float_as_uint(fabsf(x0)), __float_as_uint(fabsf(x1))));
+  float scale;
+  const bool ok = fp8_scale(__uint_as_float(m), kE4M3Max, scale);
+  if ((threadIdx.x & 31) == 0) *inv = ok ? 1.f / scale : __int_as_float(0x7fffffff);
+  return ok ? (uint32_t)cvt2<false>(x0 * scale, x1 * scale) : 0x7f7fu;
+}
+
+// 8 e4m3 bytes -> q * inv in fp32 (exactly the bf16 value of C^ for rows above the bf16-normal limit)
+__device__ __forceinline__ void dequant8(const uint2& w, float inv, float (&f)[8]) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float2 v = e4m3x2_to_f2((k < 2 ? w.x : w.y) >> (16 * (k & 1)));
+    f[2 * k] = v.x * inv;
+    f[2 * k + 1] = v.y * inv;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ RoPE + append
 // One block per token.  row: the token's qkv row (q heads, k heads, v heads; unrotated GEMM output); p its position; b its
 // sequence.  q is rotated in place; rotated k and v go to the cache at (b, p).  Rounding: fp32 rotation of the bf16 inputs,
-// one rounding to bf16 (as ops.kernels.rope_).
+// one rounding to bf16 (as ops.kernels.rope_).  FP8 cache: with blockDim a multiple of 32, one warp covers exactly one
+// head per iteration (lane e holds elements e and e + 32 of a rotated head, 2e and 2e + 1 of a v head), so the row amax of
+// the bf16-rounded values is one warp reduction.
+template <typename T>
 __device__ __forceinline__ void rope_append_token(__nv_bfloat16* __restrict__ row, int p, int b, const float* __restrict__ cos_t,
-                                                  const float* __restrict__ sin_t, __nv_bfloat16* __restrict__ kc,
-                                                  __nv_bfloat16* __restrict__ vc, int Hq, int Hkv, int Smax) {
+                                                  const float* __restrict__ sin_t, T* __restrict__ kc, T* __restrict__ vc, int Hq,
+                                                  int Hkv, int Smax, float* __restrict__ kinv, float* __restrict__ vinv) {
   const float* cr = cos_t + (long long)p * (D / 2);
   const float* sr = sin_t + (long long)p * (D / 2);
   const int n_rot = (Hq + Hkv) * (D / 2);
@@ -52,6 +83,11 @@ __device__ __forceinline__ void rope_append_token(__nv_bfloat16* __restrict__ ro
       if (h < Hq) {
         x[e] = lo;
         x[e + D / 2] = hi;
+      } else if constexpr (sizeof(T) == 1) {
+        const long long r = ((long long)b * Hkv + (h - Hq)) * Smax + p;
+        const uint32_t qb = quantize_pair(__bfloat162float(lo), __bfloat162float(hi), kinv + r);
+        kc[r * D + e] = (uint8_t)qb;
+        kc[r * D + e + D / 2] = (uint8_t)(qb >> 8);
       } else {
         __nv_bfloat16* dst = kc + (((long long)b * Hkv + (h - Hq)) * Smax + p) * D;
         dst[e] = lo;
@@ -60,49 +96,70 @@ __device__ __forceinline__ void rope_append_token(__nv_bfloat16* __restrict__ ro
     } else {
       const int j = i - n_rot, hk = j / (D / 2), e = j % (D / 2);
       const uint32_t v = reinterpret_cast<const uint32_t*>(row + (Hq + Hkv + hk) * D)[e];
-      reinterpret_cast<uint32_t*>(vc + (((long long)b * Hkv + hk) * Smax + p) * D)[e] = v;
+      if constexpr (sizeof(T) == 1) {
+        const long long r = ((long long)b * Hkv + hk) * Smax + p;
+        const float2 f = bf2_to_f2(v);
+        reinterpret_cast<uint16_t*>(vc + r * D)[e] = (uint16_t)quantize_pair(f.x, f.y, vinv + r);
+      } else {
+        reinterpret_cast<uint32_t*>(vc + (((long long)b * Hkv + hk) * Smax + p) * D)[e] = v;
+      }
     }
   }
 }
 
 // grid B, block 256: one new token per row at the row's own position pos[b] (read from device memory, so a captured graph
 // stays valid at every step).
+template <typename T>
 __global__ void __launch_bounds__(256)
 rope_append_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const float* __restrict__ cos_t, const float* __restrict__ sin_t,
-                   const int* __restrict__ pos, __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc, int Hq, int Hkv,
-                   int Smax) {
+                   const int* __restrict__ pos, T* __restrict__ kc, T* __restrict__ vc, int Hq, int Hkv, int Smax,
+                   float* __restrict__ kinv, float* __restrict__ vinv) {
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x;
-  rope_append_token(qkv + (long long)b * ld, pos[b], b, cos_t, sin_t, kc, vc, Hq, Hkv, Smax);
+  rope_append_token(qkv + (long long)b * ld, pos[b], b, cos_t, sin_t, kc, vc, Hq, Hkv, Smax, kinv, vinv);
 }
 
 // grid (B, n), block 256: n tokens per row, slot-major rows (row j*B + b is token j of sequence b, at position pos[b] + j).
+template <typename T>
 __global__ void __launch_bounds__(256)
 rope_append_multi_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const float* __restrict__ cos_t,
-                         const float* __restrict__ sin_t, const int* __restrict__ pos, __nv_bfloat16* __restrict__ kc,
-                         __nv_bfloat16* __restrict__ vc, int Hq, int Hkv, int Smax) {
+                         const float* __restrict__ sin_t, const int* __restrict__ pos, T* __restrict__ kc, T* __restrict__ vc, int Hq,
+                         int Hkv, int Smax, float* __restrict__ kinv, float* __restrict__ vinv) {
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x, j = blockIdx.y, B = gridDim.x;
-  rope_append_token(qkv + ((long long)j * B + b) * ld, pos[b] + j, b, cos_t, sin_t, kc, vc, Hq, Hkv, Smax);
+  rope_append_token(qkv + ((long long)j * B + b) * ld, pos[b] + j, b, cos_t, sin_t, kc, vc, Hq, Hkv, Smax, kinv, vinv);
 }
 
 // ------------------------------------------------------------------------------------------------ prefill cache fill
-// grid (Sp, B), block 128: row s < len[b] of batch row b -> cache row b * row_stride: 16-byte copies of the k and v heads.
+// grid (Sp, B), block 128: row s < len[b] of batch row b -> cache row b * row_stride: 16-byte copies of the k and v heads
+// (FP8 cache: one warp quantises one head, two values per lane).
+template <typename T>
 __global__ void __launch_bounds__(128)
-kv_fill_kernel(const __nv_bfloat16* __restrict__ qkv, long long ld, const int* __restrict__ len, __nv_bfloat16* __restrict__ kc,
-               __nv_bfloat16* __restrict__ vc, int Sp, int Hq, int Hkv, int Smax, int row_stride) {
+kv_fill_kernel(const __nv_bfloat16* __restrict__ qkv, long long ld, const int* __restrict__ len, T* __restrict__ kc,
+               T* __restrict__ vc, int Sp, int Hq, int Hkv, int Smax, int row_stride, float* __restrict__ kinv,
+               float* __restrict__ vinv) {
   pdl_launch_dependents();
   pdl_wait();
   const int s = blockIdx.x, b = blockIdx.y;
   if (s >= len[b] || s >= Smax) return;
   const __nv_bfloat16* row = qkv + ((long long)b * Sp + s) * ld + Hq * D;
-  for (int i = threadIdx.x; i < 2 * Hkv * (D / 8); i += blockDim.x) {
-    const int kv = i / (Hkv * (D / 8)), r = i % (Hkv * (D / 8)), hk = r / (D / 8), c = r % (D / 8);
-    const uint4 v = ld_nc_v4(row + (kv * Hkv + hk) * D + c * 8);
-    __nv_bfloat16* dst = (kv ? vc : kc) + (((long long)b * row_stride * Hkv + hk) * Smax + s) * D + c * 8;
-    st_v4(dst, v);
+  if constexpr (sizeof(T) == 1) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int hh = warp; hh < 2 * Hkv; hh += blockDim.x >> 5) {
+      const int kv = hh / Hkv, hk = hh % Hkv;
+      const float2 f = bf2_to_f2(reinterpret_cast<const uint32_t*>(row + hh * D)[lane]);
+      const long long r = ((long long)b * row_stride * Hkv + hk) * Smax + s;
+      reinterpret_cast<uint16_t*>((kv ? vc : kc) + r * D)[lane] = (uint16_t)quantize_pair(f.x, f.y, (kv ? vinv : kinv) + r);
+    }
+  } else {
+    for (int i = threadIdx.x; i < 2 * Hkv * (D / 8); i += blockDim.x) {
+      const int kv = i / (Hkv * (D / 8)), r = i % (Hkv * (D / 8)), hk = r / (D / 8), c = r % (D / 8);
+      const uint4 v = ld_nc_v4(row + (kv * Hkv + hk) * D + c * 8);
+      __nv_bfloat16* dst = (kv ? vc : kc) + (((long long)b * row_stride * Hkv + hk) * Smax + s) * D + c * 8;
+      st_v4(dst, v);
+    }
   }
 }
 
@@ -112,11 +169,16 @@ kv_fill_kernel(const __nv_bfloat16* __restrict__ qkv, long long ld, const int* _
 // P V is one warp per 32 keys (lanes over dimension pairs) summed across the four warps.  Writes the unnormalised partial
 // output and its (max, sum) in the log2 domain; chunks past the row's length exit at once.  With a chunk table (beam
 // search), the keys of chunk c of row b are read from physical row table[b * nchunks + c]; without one, from row b.
-template <int G>
+// FP8 cache (T = uint8_t): the chunk's e4m3 K and V and its two inv runs (rounded up to 16 bytes, in bounds since Smax is a
+// multiple of CH) arrive by four bulk copies, and every element is read as q * inv; the arithmetic is the bf16 kernel's.
+template <int G, typename T = __nv_bfloat16>
 struct AttSmem {
+  static constexpr int E = (int)sizeof(T);
   static constexpr int K_OFF = 0;
-  static constexpr int V_OFF = CH * D * 2;
-  static constexpr int Q_OFF = 2 * CH * D * 2;                   // fp32 [G][64], pre-scaled by softmax_scale * log2(e)
+  static constexpr int V_OFF = CH * D * E;
+  static constexpr int KI_OFF = 2 * CH * D * E;                  // FP8 cache: fp32 [CH] inv of the keys, then of the values
+  static constexpr int VI_OFF = KI_OFF + (E == 1 ? CH * 4 : 0);
+  static constexpr int Q_OFF = VI_OFF + (E == 1 ? CH * 4 : 0);   // fp32 [G][64], pre-scaled by softmax_scale * log2(e)
   static constexpr int S_OFF = Q_OFF + G * D * 4;                 // fp32 [G][CH] scores, then probabilities
   static constexpr int R_OFF = S_OFF + G * CH * 4;                // fp32 [4][G][64] per-warp P V
   static constexpr int M_OFF = R_OFF + 4 * G * D * 4;             // fp32 [G][2] (max, sum)
@@ -124,15 +186,18 @@ struct AttSmem {
   static constexpr int BYTES = BAR_OFF + 16;
 };
 
-template <int G>
+template <int G, typename T>
 __global__ void __launch_bounds__(ATT_THREADS)
-decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __nv_bfloat16* __restrict__ kc,
-                   const __nv_bfloat16* __restrict__ vc, const int* __restrict__ pos, float* __restrict__ part_o,
-                   float* __restrict__ part_ml, const int* __restrict__ table, int Hkv, int Smax, int nchunks, float scale_log2) {
-  using L = AttSmem<G>;
+decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const T* __restrict__ kc, const T* __restrict__ vc,
+                   const int* __restrict__ pos, float* __restrict__ part_o, float* __restrict__ part_ml, const int* __restrict__ table,
+                   int Hkv, int Smax, int nchunks, float scale_log2, const float* __restrict__ kinv, const float* __restrict__ vinv) {
+  using L = AttSmem<G, T>;
+  constexpr bool KV8 = sizeof(T) == 1;
   extern __shared__ __align__(128) uint8_t smem[];
-  __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(smem + L::K_OFF);
-  __nv_bfloat16* sV = reinterpret_cast<__nv_bfloat16*>(smem + L::V_OFF);
+  T* sK = reinterpret_cast<T*>(smem + L::K_OFF);
+  T* sV = reinterpret_cast<T*>(smem + L::V_OFF);
+  const float* sKI = reinterpret_cast<const float*>(smem + L::KI_OFF);
+  const float* sVI = reinterpret_cast<const float*>(smem + L::VI_OFF);
   float* sQ = reinterpret_cast<float*>(smem + L::Q_OFF);
   float* sS = reinterpret_cast<float*>(smem + L::S_OFF);
   float* sR = reinterpret_cast<float*>(smem + L::R_OFF);
@@ -155,9 +220,19 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __n
   const int phys = table != nullptr ? table[b * nchunks + c] : b;
   const long long kv_off = (((long long)phys * Hkv + hk) * Smax + j0) * D;
   if (tid == 0) {
-    mbar_arrive_expect_tx(bar, 2u * n * D * 2);
-    bulk_load_1d(sK, kc + kv_off, n * D * 2, bar);
-    bulk_load_1d(sV, vc + kv_off, n * D * 2, bar);
+    if constexpr (KV8) {
+      const long long i_off = ((long long)phys * Hkv + hk) * Smax + j0;
+      const uint32_t ib = (n * 4 + 15) & ~15;
+      mbar_arrive_expect_tx(bar, 2u * n * D + 2u * ib);
+      bulk_load_1d(sK, kc + kv_off, n * D, bar);
+      bulk_load_1d(sV, vc + kv_off, n * D, bar);
+      bulk_load_1d(smem + L::KI_OFF, kinv + i_off, ib, bar);
+      bulk_load_1d(smem + L::VI_OFF, vinv + i_off, ib, bar);
+    } else {
+      mbar_arrive_expect_tx(bar, 2u * n * D * 2);
+      bulk_load_1d(sK, kc + kv_off, n * D * 2, bar);
+      bulk_load_1d(sV, vc + kv_off, n * D * 2, bar);
+    }
   }
   const __nv_bfloat16* qrow = q + (long long)b * ldq + (long long)hk * G * D;
   for (int i = tid; i < G * D; i += ATT_THREADS) sQ[i] = __bfloat162float(qrow[i]) * scale_log2;
@@ -170,12 +245,12 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __n
 #pragma unroll
     for (int g = 0; g < G; ++g) acc[g] = 0.f;
     if (tid < n) {
-      const uint4* krow = reinterpret_cast<const uint4*>(sK + tid * D);
 #pragma unroll
       for (int cc = 0; cc < D / 8; ++cc) {
         const int ch = (cc + tid) & (D / 8 - 1);
         float kf[8];
-        unpack8(krow[ch], kf);
+        if constexpr (KV8) dequant8(reinterpret_cast<const uint2*>(sK + tid * D)[ch], sKI[tid], kf);
+        else unpack8(reinterpret_cast<const uint4*>(sK + tid * D)[ch], kf);
 #pragma unroll
         for (int g = 0; g < G; ++g) {
           const float* qg = sQ + g * D + ch * 8;
@@ -220,7 +295,13 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __n
     for (int g = 0; g < G; ++g) o[g][0] = o[g][1] = 0.f;
     const int jb = warp * 32, je = min(n, jb + 32);
     for (int j = jb; j < je; ++j) {
-      const float2 vv = bf2_to_f2(reinterpret_cast<const uint32_t*>(sV + j * D)[lane]);
+      float2 vv;
+      if constexpr (KV8) {
+        const float2 f = e4m3x2_to_f2(reinterpret_cast<const uint16_t*>(sV + j * D)[lane]);
+        vv = make_float2(f.x * sVI[j], f.y * sVI[j]);
+      } else {
+        vv = bf2_to_f2(reinterpret_cast<const uint32_t*>(sV + j * D)[lane]);
+      }
 #pragma unroll
       for (int g = 0; g < G; ++g) {
         const float p = sS[g * CH + j];
@@ -570,21 +651,32 @@ sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, con
 //   warps 0-3   one warpgroup: Q gathered into shared memory in the same swizzled layout, S = Q K^T on wgmma m64n64k16,
 //               causal mask + online softmax (exp2 domain) on the accumulators, O += P V with P as the register operand
 // Writes the unnormalised partial output and its (max, sum) per query row; verify_combine_kernel merges the splits.
+//
+// FP8 cache (KV8): warp 4 bulk-copies each tile's e4m3 K and V [64 keys x 64 bytes] and their two inv runs into an FP8
+// stage of the ring; the warpgroup converts them (q * inv, exact in bf16) into ONE pair of bf16 K | V tiles in the same
+// 128-byte swizzled layout the bf16 kernel's TMA writes, fences them for the async proxy and runs the same wgmmas, whose
+// inputs are then exactly the bf16 kernel's on the dequantised cache.
 constexpr int VB = 64;                           // keys per tile
 constexpr int VSTAGES = 2;
 constexpr int VTHREADS = 160;
 constexpr int VTILE = 64 * 128;                  // a [64 x 64] bf16 tile, 128-byte swizzled rows
 constexpr int VSMEM = VTILE + VSTAGES * 2 * VTILE + 1024 /*align*/ + 128 /*barriers*/;
+constexpr int VFSTAGE = 2 * VB * D + 2 * VB * 4; // FP8 stage: e4m3 K, e4m3 V, inv of K, inv of V
+constexpr int VSMEM8 = VTILE + 2 * VTILE + VSTAGES * VFSTAGE + 1024 /*align*/ + 128 /*barriers*/;
 
+template <bool KV8>
 __global__ void __launch_bounds__(VTHREADS)
 verify_attn_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                    const __nv_bfloat16* __restrict__ q, long long ldq, const int* __restrict__ pos, float* __restrict__ part_o,
-                   float* __restrict__ part_ml, int Hkv, int Smax, int cap, int tps, float scale_log2, int lg, int n) {
+                   float* __restrict__ part_ml, int Hkv, int Smax, int cap, int tps, float scale_log2, int lg, int n,
+                   const uint8_t* __restrict__ kc8, const uint8_t* __restrict__ vc8, const float* __restrict__ kinv,
+                   const float* __restrict__ vinv) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
-  uint8_t* sKV = smem + VTILE;                   // [stage][K | V]
-  uint64_t* full = reinterpret_cast<uint64_t*>(sKV + VSTAGES * 2 * VTILE);
+  uint8_t* sKV = smem + VTILE;                   // [stage][K | V]; FP8: the converted K | V, then the FP8 stages
+  uint8_t* s8 = sKV + 2 * VTILE;
+  uint64_t* full = reinterpret_cast<uint64_t*>(KV8 ? s8 + VSTAGES * VFSTAGE : sKV + VSTAGES * 2 * VTILE);
   uint64_t* empty = full + VSTAGES;
 
   pdl_launch_dependents();
@@ -592,8 +684,10 @@ verify_attn_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_cons
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int G = 1 << lg, nq = G * n, Hq = Hkv * G;
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
+    if constexpr (!KV8) {
+      tma_prefetch_desc(&tmap_k);
+      tma_prefetch_desc(&tmap_v);
+    }
     for (int i = 0; i < VSTAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
     fence_barrier_init();
   }
@@ -610,9 +704,19 @@ verify_attn_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_cons
       for (int t = t_begin; t < t_end; ++t) {
         const int i = t - t_begin, st = i % VSTAGES;
         mbar_wait(&empty[st], ((i / VSTAGES) & 1) ^ 1);
-        mbar_arrive_expect_tx(&full[st], 2 * VTILE);
-        tma_load_2d(sKV + st * 2 * VTILE, &tmap_k, &full[st], 0, row0 + t * VB);
-        tma_load_2d(sKV + st * 2 * VTILE + VTILE, &tmap_v, &full[st], 0, row0 + t * VB);
+        if constexpr (KV8) {
+          uint8_t* f8 = s8 + st * VFSTAGE;
+          const long long r = (long long)row0 + t * VB;
+          mbar_arrive_expect_tx(&full[st], VFSTAGE);
+          bulk_load_1d(f8, kc8 + r * D, VB * D, &full[st]);
+          bulk_load_1d(f8 + VB * D, vc8 + r * D, VB * D, &full[st]);
+          bulk_load_1d(f8 + 2 * VB * D, kinv + r, VB * 4, &full[st]);
+          bulk_load_1d(f8 + 2 * VB * D + VB * 4, vinv + r, VB * 4, &full[st]);
+        } else {
+          mbar_arrive_expect_tx(&full[st], 2 * VTILE);
+          tma_load_2d(sKV + st * 2 * VTILE, &tmap_k, &full[st], 0, row0 + t * VB);
+          tma_load_2d(sKV + st * 2 * VTILE + VTILE, &tmap_v, &full[st], 0, row0 + t * VB);
+        }
       }
     }
     return;
@@ -645,7 +749,21 @@ verify_attn_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_cons
   for (int t = t_begin; t < t_end; ++t) {
     const int i = t - t_begin, st = i % VSTAGES;
     mbar_wait(&full[st], (i / VSTAGES) & 1);
-    const uint32_t k_addr = smem_u32(sKV + st * 2 * VTILE);
+    if constexpr (KV8) {
+      named_bar_sync(1, 128);                    // every warp's MMAs on the previous tile have retired: the bf16 tiles are free
+      const uint8_t* f8 = s8 + st * VFSTAGE;
+      const float* fi = reinterpret_cast<const float*>(f8 + 2 * VB * D);
+      for (int x = threadIdx.x; x < 2 * VB * 8; x += 128) {     // (K | V, key r, 16-byte bf16 chunk c)
+        const int kv = x >> 9, r = (x >> 3) & (VB - 1), c = x & 7;
+        float f[8];
+        dequant8(*reinterpret_cast<const uint2*>(f8 + kv * VB * D + r * D + c * 8), fi[kv * VB + r], f);
+        *reinterpret_cast<uint4*>(sKV + kv * VTILE + r * 128 + ((c ^ (r & 7)) << 4)) = pack8(f);
+      }
+      fence_proxy_async_smem();                  // generic-proxy writes -> visible to wgmma
+      named_bar_sync(1, 128);
+      if (threadIdx.x == 0) mbar_arrive(&empty[st]);   // the FP8 stage has been read
+    }
+    const uint32_t k_addr = smem_u32(KV8 ? sKV : sKV + st * 2 * VTILE);
     const uint64_t kdesc = make_smem_desc_sw128(k_addr, 16, 1024);
     const uint64_t vdesc = make_smem_desc_sw128(k_addr + VTILE, VTILE, 1024);   // V: [keys x 64] read MN-major
 
@@ -707,7 +825,7 @@ verify_attn_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_cons
     for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs<1>(o, pf[kk], vdesc + 128 * kk, 1u);
     wgmma_commit();
     wgmma_wait<0>();
-    if (threadIdx.x == 0) mbar_arrive(&empty[st]);   // this warpgroup's MMAs on the stage have retired
+    if (!KV8 && threadIdx.x == 0) mbar_arrive(&empty[st]);   // this warpgroup's MMAs on the stage have retired
   }
 
 #pragma unroll
@@ -1240,25 +1358,33 @@ beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ ca
 // its current chunk) to the child's own row, and the child's entry for that chunk becomes itself.  Every source is staged
 // in shared memory before any destination is written (beams may swap parents); the table is updated by the CTAs x = 0.
 // generate() ends with p = P + max_new_tokens - 1 < Smax; a position of Smax (a full cache) copies nothing and writes
-// only entries below Smax / CH.
+// only entries below Smax / CH.  T is the cache element type, so a position is D * sizeof(T) bytes (128 bf16, 64 e4m3);
+// an FP8 cache also moves the positions' inv [L][2][rows][Hkv][Smax] (staged after the bytes), read through the same table.
+template <typename T>
 __global__ void __launch_bounds__(256)
-beam_reorder_kernel(__nv_bfloat16* __restrict__ kv, int* __restrict__ table, const int* __restrict__ parent,
-                    const int* __restrict__ pos, int nb, int Hkv, int Smax, int nchunks) {
-  extern __shared__ __align__(16) uint4 stage[];  // [nb][CH * D / 8]
+beam_reorder_kernel(T* __restrict__ kv, int* __restrict__ table, const int* __restrict__ parent,
+                    const int* __restrict__ pos, int nb, int Hkv, int Smax, int nchunks, float* __restrict__ inv) {
+  extern __shared__ __align__(16) uint4 stage[];  // [nb][CH * RV] (FP8: then fp32 [nb][CH] inv)
   __shared__ int tstage[MAX_BEAMS * MAX_TABLE];
-  constexpr int RV = D / 8;                      // 16-byte pieces per position
+  constexpr int RV = D * (int)sizeof(T) / 16;    // 16-byte pieces per position
+  constexpr bool KV8 = sizeof(T) == 1;
   pdl_launch_dependents();
   pdl_wait();
   const int slab = blockIdx.x / Hkv, hk = blockIdx.x % Hkv, g = blockIdx.y, tid = threadIdx.x;
   const long long rows = (long long)gridDim.y * nb;
   const int row0 = g * nb;
   const int p = pos[row0], c = p / CH, n = p - c * CH;
-  __nv_bfloat16* base = kv + (long long)slab * rows * Hkv * Smax * D;
+  T* base = kv + (long long)slab * rows * Hkv * Smax * D;
   for (int j = 0; j < nb; ++j) {
     const int par = parent[row0 + j];
     if (par == row0 + j) continue;
     const uint4* src = reinterpret_cast<const uint4*>(base + (((long long)par * Hkv + hk) * Smax + c * CH) * D);
     for (int i = tid; i < n * RV; i += blockDim.x) stage[j * CH * RV + i] = src[i];
+    if constexpr (KV8) {
+      const float* isrc = inv + ((long long)slab * rows * Hkv + (long long)par * Hkv + hk) * Smax + c * CH;
+      float* istage = reinterpret_cast<float*>(stage + nb * CH * RV) + j * CH;
+      for (int i = tid; i < n; i += blockDim.x) istage[i] = isrc[i];
+    }
   }
   if (blockIdx.x == 0)
     for (int i = tid; i < nb * c; i += blockDim.x) tstage[i] = table[parent[row0 + i / c] * nchunks + i % c];
@@ -1267,6 +1393,11 @@ beam_reorder_kernel(__nv_bfloat16* __restrict__ kv, int* __restrict__ table, con
     if (parent[row0 + j] == row0 + j) continue;
     uint4* dst = reinterpret_cast<uint4*>(base + (((long long)(row0 + j) * Hkv + hk) * Smax + c * CH) * D);
     for (int i = tid; i < n * RV; i += blockDim.x) dst[i] = stage[j * CH * RV + i];
+    if constexpr (KV8) {
+      float* idst = inv + ((long long)slab * rows * Hkv + (long long)(row0 + j) * Hkv + hk) * Smax + c * CH;
+      const float* istage = reinterpret_cast<const float*>(stage + nb * CH * RV) + j * CH;
+      for (int i = tid; i < n; i += blockDim.x) idst[i] = istage[i];
+    }
   }
   if (blockIdx.x == 0) {
     for (int i = tid; i < nb * (c + 1); i += blockDim.x) {
@@ -1277,20 +1408,21 @@ beam_reorder_kernel(__nv_bfloat16* __restrict__ kv, int* __restrict__ table, con
   }
 }
 
-template <int G>
+template <int G, typename T>
 int launch_attn(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml, void* out,
-                long long ldo, const void* table, int B, int Hkv, int Smax, float scale, cudaStream_t st) {
+                long long ldo, const void* table, int B, int Hkv, int Smax, float scale, const void* kinv, const void* vinv,
+                cudaStream_t st) {
   static bool attr_set = false;
-  const int smem = AttSmem<G>::BYTES;
+  const int smem = AttSmem<G, T>::BYTES;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(decode_attn_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(decode_attn_kernel<G, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
   const int nchunks = ceil_div(Smax, CH);
-  launch_pdl(decode_attn_kernel<G>, dim3(nchunks, Hkv, B), dim3(ATT_THREADS), smem, st, (const __nv_bfloat16*)q, ldq,
-             (const __nv_bfloat16*)kc, (const __nv_bfloat16*)vc, (const int*)pos, (float*)part_o, (float*)part_ml, (const int*)table, Hkv,
-             Smax, nchunks, scale * 1.4426950408889634f);
+  launch_pdl(decode_attn_kernel<G, T>, dim3(nchunks, Hkv, B), dim3(ATT_THREADS), smem, st, (const __nv_bfloat16*)q, ldq,
+             (const T*)kc, (const T*)vc, (const int*)pos, (float*)part_o, (float*)part_ml, (const int*)table, Hkv, Smax, nchunks,
+             scale * 1.4426950408889634f, (const float*)kinv, (const float*)vinv);
   ODB_CHECK_LAST();
   launch_pdl(decode_combine_kernel, dim3(Hkv * G, B), dim3(D), 0, st, (const float*)part_o, (const float*)part_ml, (const int*)pos,
              (__nv_bfloat16*)out, ldo, nchunks);
@@ -1298,24 +1430,64 @@ int launch_attn(const void* q, long long ldq, const void* kc, const void* vc, co
   return 0;
 }
 
+template <int G>
+int launch_attn_t(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml, void* out,
+                  long long ldo, const void* table, int B, int Hkv, int Smax, float scale, const void* kinv, const void* vinv,
+                  cudaStream_t st) {
+  if (kinv != nullptr)
+    return launch_attn<G, uint8_t>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, scale, kinv, vinv, st);
+  return launch_attn<G, __nv_bfloat16>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, scale, nullptr, nullptr,
+                                       st);
+}
+
+template <typename T>
+int launch_beam_reorder(void* kv, void* inv, void* table, const void* parent, const void* pos, int B, int nb, int L, int Hkv, int Smax,
+                        cudaStream_t st) {
+  constexpr int extra = sizeof(T) == 1 ? CH * 4 : 0;                  // FP8: the staged inv of a position chunk
+  const int smem = nb * (CH * D * (int)sizeof(T) + extra);
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(beam_reorder_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         MAX_BEAMS * (CH * D * (int)sizeof(T) + extra));
+    if (e != cudaSuccess) return (int)e;
+    attr_set = true;
+  }
+  launch_pdl(beam_reorder_kernel<T>, dim3(L * 2 * Hkv, B), dim3(256), smem, st, (T*)kv, (int*)table, (const int*)parent,
+             (const int*)pos, nb, Hkv, Smax, Smax / CH, (float*)inv);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
 }  // namespace dec
 
-// qkv [B, ld] bf16 (one token per row); cos/sin fp32 [max_pos, 32]; pos int32 [B]; kc/vc [B, Hkv, Smax, 64] bf16
+// Every cache argument below is either bf16 (kinv = vinv = nullptr) or an FP8 cache: e4m3 bytes of the same shape plus fp32
+// kinv / vinv [B, Hkv, Smax] (16-byte aligned, Smax a multiple of 128), written and read as described at the top of the file.
+
+// qkv [B, ld] bf16 (one token per row); cos/sin fp32 [max_pos, 32]; pos int32 [B]; kc/vc [B, Hkv, Smax, 64]
 ODB_EXPORT int odb_dec_rope_append(void* qkv, long long ld, const void* cos_t, const void* sin_t, const void* pos, void* kc, void* vc,
-                                   int B, int Hq, int Hkv, int Smax, cudaStream_t st) {
+                                   int B, int Hq, int Hkv, int Smax, void* kinv, void* vinv, cudaStream_t st) {
   if (ld % 2) return -1;
-  launch_pdl(dec::rope_append_kernel, dim3(B), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t, (const float*)sin_t,
-             (const int*)pos, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, Hq, Hkv, Smax);
+  if (kinv != nullptr)
+    launch_pdl(dec::rope_append_kernel<uint8_t>, dim3(B), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t,
+               (const float*)sin_t, (const int*)pos, (uint8_t*)kc, (uint8_t*)vc, Hq, Hkv, Smax, (float*)kinv, (float*)vinv);
+  else
+    launch_pdl(dec::rope_append_kernel<__nv_bfloat16>, dim3(B), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t,
+               (const float*)sin_t, (const int*)pos, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, Hq, Hkv, Smax, (float*)nullptr,
+               (float*)nullptr);
   ODB_CHECK_LAST();
   return 0;
 }
 
 // qkv [B*Sp, ld] bf16 (rotated prefill projections); len int32 [B]: rows s < len[b] are copied into cache row b * row_stride
 ODB_EXPORT int odb_dec_kv_fill(const void* qkv, long long ld, const void* len, void* kc, void* vc, int B, int Sp, int Hq, int Hkv,
-                               int Smax, int row_stride, cudaStream_t st) {
+                               int Smax, int row_stride, void* kinv, void* vinv, cudaStream_t st) {
   if (ld % 8 || row_stride < 1) return -1;
-  launch_pdl(dec::kv_fill_kernel, dim3(Sp, B), dim3(128), 0, st, (const __nv_bfloat16*)qkv, ld, (const int*)len, (__nv_bfloat16*)kc,
-             (__nv_bfloat16*)vc, Sp, Hq, Hkv, Smax, row_stride);
+  if (kinv != nullptr)
+    launch_pdl(dec::kv_fill_kernel<uint8_t>, dim3(Sp, B), dim3(128), 0, st, (const __nv_bfloat16*)qkv, ld, (const int*)len,
+               (uint8_t*)kc, (uint8_t*)vc, Sp, Hq, Hkv, Smax, row_stride, (float*)kinv, (float*)vinv);
+  else
+    launch_pdl(dec::kv_fill_kernel<__nv_bfloat16>, dim3(Sp, B), dim3(128), 0, st, (const __nv_bfloat16*)qkv, ld, (const int*)len,
+               (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, Sp, Hq, Hkv, Smax, row_stride, (float*)nullptr, (float*)nullptr);
   ODB_CHECK_LAST();
   return 0;
 }
@@ -1328,13 +1500,14 @@ ODB_EXPORT int odb_dec_attn_chunks(int Smax) { return odb::ceil_div(Smax, dec::C
 // (chunk c of row b is read from physical cache row table[b][c])
 ODB_EXPORT int odb_dec_attn(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml,
                             void* out, long long ldo, const void* table, int B, int Hq, int Hkv, int Smax, float softmax_scale,
-                            cudaStream_t st) {
-  if (Hq % Hkv || ldq % 8) return -1;
+                            const void* kinv, const void* vinv, cudaStream_t st) {
+  if (Hq % Hkv || ldq % 8 || (kinv != nullptr && Smax % dec::CH)) return -1;
+  const float sc = softmax_scale;
   switch (Hq / Hkv) {
-    case 1: return dec::launch_attn<1>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, softmax_scale, st);
-    case 2: return dec::launch_attn<2>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, softmax_scale, st);
-    case 4: return dec::launch_attn<4>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, softmax_scale, st);
-    case 8: return dec::launch_attn<8>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, softmax_scale, st);
+    case 1: return dec::launch_attn_t<1>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, sc, kinv, vinv, st);
+    case 2: return dec::launch_attn_t<2>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, sc, kinv, vinv, st);
+    case 4: return dec::launch_attn_t<4>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, sc, kinv, vinv, st);
+    case 8: return dec::launch_attn_t<8>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, sc, kinv, vinv, st);
     default: return -2;                          // GQA groups of 1, 2, 4 or 8 query heads
   }
 }
@@ -1363,10 +1536,15 @@ ODB_EXPORT int odb_dec_sample(const void* logits, long long ld, int V, const voi
 // qkv [n*B, ld] bf16, slot-major (row j*B + b: token j of sequence b, at position pos[b] + j); cos/sin fp32 [max_pos, 32];
 // pos int32 [B]; kc/vc [B, Hkv, Smax, 64] bf16
 ODB_EXPORT int odb_dec_rope_append_multi(void* qkv, long long ld, const void* cos_t, const void* sin_t, const void* pos, void* kc,
-                                         void* vc, int B, int n, int Hq, int Hkv, int Smax, cudaStream_t st) {
+                                         void* vc, int B, int n, int Hq, int Hkv, int Smax, void* kinv, void* vinv, cudaStream_t st) {
   if (ld % 2 || n < 1) return -1;
-  launch_pdl(dec::rope_append_multi_kernel, dim3(B, n), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t,
-             (const float*)sin_t, (const int*)pos, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, Hq, Hkv, Smax);
+  if (kinv != nullptr)
+    launch_pdl(dec::rope_append_multi_kernel<uint8_t>, dim3(B, n), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t,
+               (const float*)sin_t, (const int*)pos, (uint8_t*)kc, (uint8_t*)vc, Hq, Hkv, Smax, (float*)kinv, (float*)vinv);
+  else
+    launch_pdl(dec::rope_append_multi_kernel<__nv_bfloat16>, dim3(B, n), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld,
+               (const float*)cos_t, (const float*)sin_t, (const int*)pos, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, Hq, Hkv, Smax,
+               (float*)nullptr, (float*)nullptr);
   ODB_CHECK_LAST();
   return 0;
 }
@@ -1377,28 +1555,44 @@ ODB_EXPORT int odb_dec_rope_append_multi(void* qkv, long long ld, const void* co
 // The keys are split so that about two CTAs per SM run: splits = min(tiles, ceil(264 / (Hkv*B))).
 ODB_EXPORT int odb_dec_verify_attn(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o,
                                    void* part_ml, void* out, long long ldo, int B, int n, int Hq, int Hkv, int Smax, float softmax_scale,
-                                   cudaStream_t st) {
+                                   const void* kinv, const void* vinv, cudaStream_t st) {
   if (Hq % Hkv || ldq % 8 || n < 1 || n > 8 || Smax % dec::VB) return -1;
   const int G = Hq / Hkv;
   const int lg = G == 1 ? 0 : G == 2 ? 1 : G == 4 ? 2 : G == 8 ? 3 : -1;
   if (lg < 0) return -2;                         // GQA groups of 1, 2, 4 or 8 query heads
-  CUtensorMap tk, tv;
-  int rc;
-  const long long rows = (long long)B * Hkv * Smax;
-  if ((rc = make_tmap_2d(&tk, kc, rows, dec::D, dec::D * 2, dec::VB, dec::D, 2))) return rc;
-  if ((rc = make_tmap_2d(&tv, vc, rows, dec::D, dec::D * 2, dec::VB, dec::D, 2))) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(dec::verify_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dec::VSMEM);
-    if (e != cudaSuccess) return (int)e;
-    attr_set = true;
-  }
   const int cap = Smax / dec::VB;
   int splits = std::min(cap, std::max(1, odb::ceil_div(264, Hkv * B)));
   const int tps = odb::ceil_div(cap, splits);
   splits = odb::ceil_div(cap, tps);
-  launch_pdl(dec::verify_attn_kernel, dim3(splits, Hkv, B), dim3(dec::VTHREADS), dec::VSMEM, st, tk, tv, (const __nv_bfloat16*)q, ldq,
-             (const int*)pos, (float*)part_o, (float*)part_ml, Hkv, Smax, cap, tps, softmax_scale * 1.4426950408889634f, lg, n);
+  if (kinv != nullptr) {
+    static bool attr8 = false;
+    if (!attr8) {
+      cudaError_t e = cudaFuncSetAttribute(dec::verify_attn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dec::VSMEM8);
+      if (e != cudaSuccess) return (int)e;
+      attr8 = true;
+    }
+    CUtensorMap unused{};
+    launch_pdl(dec::verify_attn_kernel<true>, dim3(splits, Hkv, B), dim3(dec::VTHREADS), dec::VSMEM8, st, unused, unused,
+               (const __nv_bfloat16*)q, ldq, (const int*)pos, (float*)part_o, (float*)part_ml, Hkv, Smax, cap, tps,
+               softmax_scale * 1.4426950408889634f, lg, n, (const uint8_t*)kc, (const uint8_t*)vc, (const float*)kinv,
+               (const float*)vinv);
+  } else {
+    CUtensorMap tk, tv;
+    int rc;
+    const long long rows = (long long)B * Hkv * Smax;
+    if ((rc = make_tmap_2d(&tk, kc, rows, dec::D, dec::D * 2, dec::VB, dec::D, 2))) return rc;
+    if ((rc = make_tmap_2d(&tv, vc, rows, dec::D, dec::D * 2, dec::VB, dec::D, 2))) return rc;
+    static bool attr_set = false;
+    if (!attr_set) {
+      cudaError_t e = cudaFuncSetAttribute(dec::verify_attn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dec::VSMEM);
+      if (e != cudaSuccess) return (int)e;
+      attr_set = true;
+    }
+    launch_pdl(dec::verify_attn_kernel<false>, dim3(splits, Hkv, B), dim3(dec::VTHREADS), dec::VSMEM, st, tk, tv,
+               (const __nv_bfloat16*)q, ldq, (const int*)pos, (float*)part_o, (float*)part_ml, Hkv, Smax, cap, tps,
+               softmax_scale * 1.4426950408889634f, lg, n, (const uint8_t*)nullptr, (const uint8_t*)nullptr, (const float*)nullptr,
+               (const float*)nullptr);
+  }
   ODB_CHECK_LAST();
   launch_pdl(dec::verify_combine_kernel, dim3(Hq, n * B), dim3(dec::D), 0, st, (const float*)part_o, (const float*)part_ml,
              (const int*)pos, (__nv_bfloat16*)out, ldo, cap, tps * dec::VB, B);
@@ -1477,21 +1671,12 @@ ODB_EXPORT int odb_dec_beam_step(const void* part_ml, const void* cand_v, const 
   return 0;
 }
 
-// kv bf16 [L, 2, B*nb, Hkv, Smax, 64] (every layer's K and V of the beam rows, one allocation); table int32 [B*nb, Smax/128];
-// parent / pos int32 [B*nb] (pos: the next position to be written, equal over a prompt's beams).  See dec::beam_reorder_kernel.
+// kv [L, 2, B*nb, Hkv, Smax, 64] (every layer's K and V of the beam rows, one allocation; bf16, or e4m3 bytes with inv fp32
+// [L, 2, B*nb, Hkv, Smax], also one allocation); table int32 [B*nb, Smax/128]; parent / pos int32 [B*nb] (pos: the next
+// position to be written, equal over a prompt's beams).  See dec::beam_reorder_kernel.
 ODB_EXPORT int odb_dec_beam_reorder(void* kv, void* table, const void* parent, const void* pos, int B, int nb, int L, int Hkv, int Smax,
-                                    cudaStream_t st) {
+                                    void* inv, cudaStream_t st) {
   if (nb < 1 || nb > dec::MAX_BEAMS || Smax % dec::CH || Smax / dec::CH > dec::MAX_TABLE) return -1;
-  const int smem = nb * dec::CH * dec::D * 2;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(dec::beam_reorder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         dec::MAX_BEAMS * dec::CH * dec::D * 2);
-    if (e != cudaSuccess) return (int)e;
-    attr_set = true;
-  }
-  launch_pdl(dec::beam_reorder_kernel, dim3(L * 2 * Hkv, B), dim3(256), smem, st, (__nv_bfloat16*)kv, (int*)table, (const int*)parent,
-             (const int*)pos, nb, Hkv, Smax, Smax / dec::CH);
-  ODB_CHECK_LAST();
-  return 0;
+  if (inv != nullptr) return dec::launch_beam_reorder<uint8_t>(kv, inv, table, parent, pos, B, nb, L, Hkv, Smax, st);
+  return dec::launch_beam_reorder<__nv_bfloat16>(kv, nullptr, table, parent, pos, B, nb, L, Hkv, Smax, st);
 }

@@ -13,16 +13,13 @@
 //   quantize_rows : the same rule per ROW of a weight matrix (FP8 weight-only generation, ops/fp8w.py): one warp per row
 //          takes the row's amax, then writes q (e4m3), inv = 1 / scale and the dequantised bf16 row q * inv.  One launch
 //          covers a table of matrices (every projection of every layer).
-#include <cuda_fp8.h>
-#include <float.h>
-
 #include "common.cuh"
+#include "fp8_rows.cuh"
 
 using namespace odb;
 
 namespace {
 
-constexpr float kE4M3Max = 448.f, kE5M2Max = 57344.f;
 constexpr int kTile = 64;          // cast tile: 64 rows x 64 columns
 
 __device__ __forceinline__ uint32_t bf16_abs_bits_max(uint32_t acc, uint32_t w) {
@@ -51,22 +48,6 @@ __global__ void __launch_bounds__(256) amax_kernel(const uint4* __restrict__ x, 
     for (int w = 1; w < 8; ++w) m = max(m, sm[w]);
     atomicMax(slot, m);
   }
-}
-
-// scale = 2^e, e = floor(log2(fmax / amax)) clamped to [-126, 126]; returns false for a non-finite amax
-__device__ __forceinline__ bool fp8_scale(float amax, float fmax, float& scale) {
-  if (!(amax <= FLT_MAX)) { scale = 1.f; return false; }
-  if (amax == 0.f) { scale = 1.f; return true; }
-  const float r = fmax / amax;                                   // IEEE division (no fast-math in this build)
-  int e = isinf(r) ? 126 : (int)((__float_as_uint(r) >> 23) & 0xffu) - 127;
-  e = min(126, max(-126, e));
-  scale = __uint_as_float((uint32_t)(e + 127) << 23);
-  return true;
-}
-
-template <bool E5M2>
-__device__ __forceinline__ uint16_t cvt2(float a, float b) {
-  return __nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, E5M2 ? __NV_E5M2 : __NV_E4M3);
 }
 
 // One 64 x 64 tile per CTA.  Row-major: each thread converts 2 x 8 consecutive elements (16-byte load, 8-byte store).
@@ -151,8 +132,7 @@ __global__ void __launch_bounds__(256) quantize_rows_kernel(const long long* __r
     float d[8];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[k >> 1] >> (16 * (k & 1))), __NV_E4M3);
-      const float2 v = __half22float2(*reinterpret_cast<const __half2*>(&h));
+      const float2 v = e4m3x2_to_f2(w[k >> 1] >> (16 * (k & 1)));
       d[2 * k] = v.x * iv;
       d[2 * k + 1] = v.y * iv;
     }

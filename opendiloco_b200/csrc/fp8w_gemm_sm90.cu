@@ -19,9 +19,8 @@
 //   * Epilogue: inv[n] is applied in fp32 before the one bf16 rounding.  With the SwiGLU epilogue a tile holds 32 gate rows
 //     and the matching 32 up rows (N = 2I, I % 32 == 0) and also writes act = silu(g) * u from the bf16-rounded g, u, as the
 //     bf16 SwiGLU GEMM does (gemm_sm90.cu, kSwiGLU).
-#include <cuda_fp8.h>
-
 #include "common.cuh"
+#include "fp8_rows.cuh"
 
 using namespace odb;
 
@@ -45,12 +44,6 @@ struct Args {
   int* counters;                  // split-K arrival counters [tiles], zero between launches
   int M, N, K, I, splits;
 };
-
-__device__ __forceinline__ uint32_t e4m3x2_to_bf16x2(uint32_t v) {
-  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(v & 0xffffu), __NV_E4M3);
-  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
-  return f2_to_bf2(f.x, f.y);
-}
 
 __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"

@@ -33,6 +33,11 @@ FP8 weight-only mode, ``generate(fp8_weights=True)``: the layer programs take ev
 them (:mod:`~opendiloco_b200.models.fp8_weights`) rows of M <= 64 run the skinny e4m3 GEMM and wider ones the bf16 GEMM on
 the dequantised weights Ŵ.  Every graph key carries the mode, so switching it recaptures.
 
+FP8 KV cache, ``generate(fp8_kv_cache=True)``: the DecodeState holds K and V as e4m3 with one fp32 factor per (position,
+kv head) row (:mod:`~opendiloco_b200.ops.decode`); every writer quantises and every decode-time reader (the one-token step,
+the verify pass, beam steps) dequantises.  The flag is part of the DecodeState and BeamState keys, so toggling it
+reallocates the caches and recaptures; an assistant's own cache stays bf16.
+
 Nothing here goes through ``LlamaEngine.workspace`` or its captured training graphs: generating between training steps
 leaves the training buffers and graph untouched.
 """
@@ -47,6 +52,7 @@ import torch
 
 from ..ops import attention as A
 from ..ops import decode as DK
+from ..ops.fp8 import E4M3
 from ..ops import gemm as G
 from ..ops import kernels as K
 from ..ops import tc_gemm as TC
@@ -80,18 +86,25 @@ class _PrefillBuffers:
 
 
 class DecodeState:
-    """KV caches, decode buffers and device-side control scalars for B rows of up to Smax positions."""
+    """KV caches, decode buffers and device-side control scalars for B rows of up to Smax positions.  ``fp8_kv``: the caches
+    are e4m3 ``kv`` [L, 2, B, Hkv, Smax, D] with fp32 ``kv_inv`` [L, 2, B, Hkv, Smax] (each one allocation: beam search
+    reorders all of it); ``kinv`` / ``vinv`` are the per-layer views of ``kv_inv`` (None for a bf16 cache)."""
 
-    def __init__(self, cfg, B: int, Smax: int, device, dtype):
+    def __init__(self, cfg, B: int, Smax: int, device, dtype, fp8_kv: bool = False):
         L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         h, i, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
         e = lambda *shape: torch.empty(*shape, dtype=dtype, device=device)  # noqa: E731
         i32 = lambda: torch.zeros(B, dtype=torch.int32, device=device)      # noqa: E731
         self.cfg, self.B, self.Smax, self.device, self.dtype = cfg, B, Smax, torch.device(device), dtype
-        self.key = (B, Smax, str(device), dtype)
-        self.kv = torch.zeros(L, 2, B, Hkv, Smax, D, dtype=dtype, device=device)      # one allocation: beam search reorders all
+        self.key = (B, Smax, str(device), dtype, fp8_kv)
+        self.fp8_kv = fp8_kv
+        # one allocation: beam search reorders all
+        self.kv = torch.zeros(L, 2, B, Hkv, Smax, D, dtype=E4M3 if fp8_kv else dtype, device=device)
+        self.kv_inv = torch.zeros(L, 2, B, Hkv, Smax, dtype=torch.float32, device=device) if fp8_kv else None
         self.kc = [self.kv[l, 0] for l in range(L)]
         self.vc = [self.kv[l, 1] for l in range(L)]
+        self.kinv = [self.kv_inv[l, 0] if fp8_kv else None for l in range(L)]
+        self.vinv = [self.kv_inv[l, 1] if fp8_kv else None for l in range(L)]
         n_rope = _round_up(max(cfg.max_position_embeddings, Smax), 128)
         self.cos, self.sin = K.rope_tables(n_rope, D, cfg.rope_theta, device)
         # one-token-per-row buffers of the decode step
@@ -130,16 +143,16 @@ class DecodeState:
         self.fctl.copy_(fctl)
 
 
-def decode_state(model, B: int, Smax: int) -> DecodeState:
-    """The model's decode state for (B, Smax), allocated on first use; at most one is resident."""
+def decode_state(model, B: int, Smax: int, fp8_kv: bool = False) -> DecodeState:
+    """The model's decode state for (B, Smax, FP8 cache or not), allocated on first use; at most one is resident."""
     eng, ar = model.engine, model.arena
-    key = (B, Smax, str(ar.device), ar.compute_dtype)
+    key = (B, Smax, str(ar.device), ar.compute_dtype, fp8_kv)
     st = eng.decode_state
     if st is None or st.key != key:
         if eng.assisted_state is not None:           # its round graph reads the old caches: let them go
             eng.assisted_state.drop_graph()
         eng.decode_state = None                       # free the old caches before allocating the new ones
-        st = eng.decode_state = DecodeState(model.config, B, Smax, ar.device, ar.compute_dtype)
+        st = eng.decode_state = DecodeState(model.config, B, Smax, ar.device, ar.compute_dtype, fp8_kv)
     return st
 
 
@@ -148,7 +161,8 @@ def decode_state(model, B: int, Smax: int) -> DecodeState:
 def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, fp8=None) -> None:
     """ids [B, Sp]: prompts compacted to start at position 0 and right-padded; lens [B] real lengths.  Fills the caches,
     computes the logits at position lens[b]-1 and samples the first new token (st.pos ends at lens).  ``fp8``: the
-    model's FP8 weights (None: the arena weights)."""
+    model's FP8 weights (None: the arena weights).  An FP8 cache (st.fp8_kv) is filled with the quantised k|v rows; the
+    prompt's attention reads the in-flight bf16 q|k|v, so the first token does not depend on the cache format."""
     cfg, ar = model.config, model.arena
     B, Sp = ids.shape
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
@@ -162,7 +176,8 @@ def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, fp8=N
     st.hist[:, :n].copy_(ids[:, :n])
     pb.ids.copy_(ids.reshape(-1))
     delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
-                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, st.lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D), fp8=fp8)
+                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, st.lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, kinv=st.kinv[l],
+                                                            vinv=st.vinv[l]), fp8=fp8)
     # only the last real position of every row feeds the LM head: gather its residual and delta rows
     last = torch.arange(B, device=st.device, dtype=torch.int64) * Sp + st.lens.long() - 1
     K.embedding_fwd(last, pb.res, out=st.res)
@@ -259,13 +274,14 @@ def _layers(model, buf, ids: torch.Tensor, attend, fp8=None):
 
 def _one_token_layers(model, st: DecodeState, ids: torch.Tensor, table: torch.Tensor | None = None, fp8=None):
     """One token per row at st.pos: the decode layers with single-query RoPE+append and split-KV attention (through the
-    chunk table, if given)."""
+    chunk table, if given), on st's bf16 or FP8 cache."""
     cfg = model.config
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
 
     def attend(l, qkv, att):
-        DK.rope_append(qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D)
-        DK.attention(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.part_o, st.part_ml, table=table)
+        DK.rope_append(qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D, kinv=st.kinv[l], vinv=st.vinv[l])
+        DK.attention(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.part_o, st.part_ml, table=table, kinv=st.kinv[l],
+                     vinv=st.vinv[l])
 
     return _layers(model, st, ids, attend, fp8)
 
@@ -379,8 +395,9 @@ def _verify(model, tst: DecodeState, ast: AssistedState, fp8=None) -> None:
     n = ast.K + 1
 
     def attend(l, qkv, att):
-        DK.rope_append_multi(qkv, tst.cos, tst.sin, tst.pos, tst.kc[l], tst.vc[l], Hq, Hkv, D, n)
-        DK.verify_attention(qkv, tst.kc[l], tst.vc[l], tst.pos, att, Hq, Hkv, D, n, ast.part_o, ast.part_ml)
+        DK.rope_append_multi(qkv, tst.cos, tst.sin, tst.pos, tst.kc[l], tst.vc[l], Hq, Hkv, D, n, kinv=tst.kinv[l], vinv=tst.vinv[l])
+        DK.verify_attention(qkv, tst.kc[l], tst.vc[l], tst.pos, att, Hq, Hkv, D, n, ast.part_o, ast.part_ml, kinv=tst.kinv[l],
+                            vinv=tst.vinv[l])
 
     delta = _layers(model, ast, ast.tok, attend, fp8)
     K.rmsnorm_fwd(ast.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=ast.xn, rstd=ast.rstd, x_out=ast.res)
@@ -484,11 +501,12 @@ def _check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size, assistant_m
 
 
 def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int, Kp: int, controls: tuple, pad: int,
-                       eos: list[int], ngram: int = 2, fp8=None) -> torch.Tensor:
-    """Assisted generation with ``assistant``, or prompt lookup (n-grams up to ``ngram``) with ``assistant`` None."""
+                       eos: list[int], ngram: int = 2, fp8=None, fp8_kv: bool = False) -> torch.Tensor:
+    """Assisted generation with ``assistant``, or prompt lookup (n-grams up to ``ngram``) with ``assistant`` None.
+    ``fp8_kv``: the target's cache is FP8 (the draft's stays bf16)."""
     B = comp.shape[0]
     Smax = _round_up(P + max_new_tokens + Kp, 128)
-    tst = decode_state(model, B, Smax)
+    tst = decode_state(model, B, Smax, fp8_kv)
     ast = assisted_state(model, assistant, B, Kp, Smax)
     dst = ast.draft
     do_sample, temperature, top_k, top_p, seed = controls
@@ -528,13 +546,13 @@ class BeamState:
     rows (the model's ``decode_state`` is left alone), the selection state of ``ops.decode.beam_select``, the chunk table
     and selection partials of the kernel path, and the step graph."""
 
-    def __init__(self, cfg, B: int, nb: int, K: int, max_new: int, Smax: int, device, dtype):
+    def __init__(self, cfg, B: int, nb: int, K: int, max_new: int, Smax: int, device, dtype, fp8_kv: bool = False):
         rows = B * nb
         i32 = lambda *shape: torch.zeros(*shape, dtype=torch.int32, device=device)     # noqa: E731
         f32 = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=device)   # noqa: E731
         self.B, self.nb, self.K, self.max_new = B, nb, K, max_new
-        self.key = (B, nb, K, max_new, Smax, str(device), dtype)
-        self.dec = DecodeState(cfg, rows, Smax, device, dtype)
+        self.key = (B, nb, K, max_new, Smax, str(device), dtype, fp8_kv)
+        self.dec = DecodeState(cfg, rows, Smax, device, dtype, fp8_kv)
         self.run_score, self.fin_score = f32(rows), f32(rows)
         self.fin_flag, self.parent = i32(rows), i32(rows)
         self.run_seq, self.fin_seq = i32(2, rows, max_new), i32(2, rows, max_new)
@@ -577,14 +595,14 @@ class BeamState:
         return seq[:, :R].reshape(B * R, M).long(), self.fin_score.view(B, nb)[:, :R].reshape(B * R).clone()
 
 
-def beam_state(model, B: int, nb: int, K: int, max_new: int, Smax: int) -> BeamState:
-    """The model's beam-search state for these shapes, allocated on first use; at most one is resident."""
+def beam_state(model, B: int, nb: int, K: int, max_new: int, Smax: int, fp8_kv: bool = False) -> BeamState:
+    """The model's beam-search state for these shapes (and cache format), allocated on first use; at most one is resident."""
     eng, ar = model.engine, model.arena
-    key = (B, nb, K, max_new, Smax, str(ar.device), ar.compute_dtype)
+    key = (B, nb, K, max_new, Smax, str(ar.device), ar.compute_dtype, fp8_kv)
     bs = eng.beam_state
     if bs is None or bs.key != key:
         eng.beam_state = None                         # free the old buffers before allocating the new ones
-        bs = eng.beam_state = BeamState(model.config, B, nb, K, max_new, Smax, ar.device, ar.compute_dtype)
+        bs = eng.beam_state = BeamState(model.config, B, nb, K, max_new, Smax, ar.device, ar.compute_dtype, fp8_kv)
     return bs
 
 
@@ -600,8 +618,8 @@ def beam_prefill(model, bs: BeamState, ids: torch.Tensor, lens: torch.Tensor, fp
     st.pos.copy_(lens.repeat_interleave(nb) - 1)
     pb.ids.copy_(ids.reshape(-1))
     delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
-                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, row_stride=nb),
-                           fp8=fp8)
+                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, row_stride=nb,
+                                                            kinv=st.kinv[l], vinv=st.vinv[l]), fp8=fp8)
     last = (torch.arange(B, device=st.device, dtype=torch.int64) * Sp + lens.long() - 1).repeat_interleave(nb)
     K.embedding_fwd(last, pb.res, out=st.res)
     K.embedding_fwd(last, delta, out=st.proj)
@@ -614,7 +632,7 @@ def beam_select(bs: BeamState, length_penalty: float, early_stopping: int) -> No
     DK.beam_select(st.logits, st.ictl, bs.nb, bs.K, length_penalty, early_stopping, bs.max_new, bs.run_score, bs.fin_score,
                    bs.fin_flag, bs.run_seq, bs.fin_seq, bs.unsat, bs.done, bs.tstep, st.pos, st.ids, bs.parent, bs.part_ml,
                    bs.cand_v, bs.cand_i, fctl=st.fctl, prompt=bs.prompt, plens=bs.plens)
-    DK.beam_reorder(st.kv, bs.table, bs.parent, st.pos, bs.nb)
+    DK.beam_reorder(st.kv, bs.table, bs.parent, st.pos, bs.nb, inv=st.kv_inv)
 
 
 def _beam_step_eager(model, bs: BeamState, length_penalty: float, early_stopping: int, fp8=None) -> None:
@@ -649,10 +667,11 @@ def beam_step(model, bs: BeamState, length_penalty: float, early_stopping: int, 
 
 
 def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R: int, length_penalty: float, early_stopping,
-                   pad: int, eos: list[int], processors: tuple = (1.0, 0, 0), fp8=None) -> tuple[torch.Tensor, torch.Tensor]:
+                   pad: int, eos: list[int], processors: tuple = (1.0, 0, 0), fp8=None,
+                   fp8_kv: bool = False) -> tuple[torch.Tensor, torch.Tensor]:
     B, Sp = comp.shape
     es = DK.EARLY_STOPPING[early_stopping]
-    bs = beam_state(model, B, nb, DK.beams_to_keep(nb, len(eos)), max_new_tokens, Smax)
+    bs = beam_state(model, B, nb, DK.beams_to_keep(nb, len(eos)), max_new_tokens, Smax, fp8_kv)
     bs.dec.set_controls(False, 1.0, 0, 1.0, 0, pad, eos, *processors)
     bs.reset(pad)
     bs.prompt[:, :Sp].copy_(comp)
@@ -717,7 +736,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
              length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1,
              return_dict_in_generate: bool = False, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
              min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
-             max_matching_ngram_size: int | None = None, fp8_weights: bool = False) -> torch.Tensor | GenerateOutput:
+             max_matching_ngram_size: int | None = None, fp8_weights: bool = False,
+             fp8_kv_cache: bool = False) -> torch.Tensor | GenerateOutput:
     """See :meth:`LlamaForCausalLM.generate`."""
     cfg, ar = model.config, model.arena
     if ar.param_sharded:
@@ -743,6 +763,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
                           cfg.max_position_embeddings)
     processors = (float(repetition_penalty), no_repeat_ngram_size, min_new_tokens)
     W8.check_flag(fp8_weights)
+    if not isinstance(fp8_kv_cache, bool):
+        raise ValueError(f"fp8_kv_cache must be a bool, got {fp8_kv_cache!r}")
     dev = ar.device
     ids = input_ids.to(dev)
     if attention_mask is None:
@@ -768,16 +790,16 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     if assistant_model is not None or prompt_lookup_num_tokens is not None:
         K = num_assistant_tokens if assistant_model is not None else prompt_lookup_num_tokens
         new = _assisted_generate(model, assistant_model, comp, lens, P, max_new_tokens, K, (do_sample, temperature, top_k, top_p, seed),
-                                 pad, eos, ngram, fp8)
+                                 pad, eos, ngram, fp8, fp8_kv_cache)
         out = torch.cat([ids, new], dim=1)
         return GenerateOutput(out) if return_dict_in_generate else out
     Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))
     if num_beams > 1:
         new, scores = _beam_generate(model, comp, lens, Smax, max_new_tokens, num_beams, num_return_sequences, length_penalty,
-                                     early_stopping, pad, eos, processors, fp8)
+                                     early_stopping, pad, eos, processors, fp8, fp8_kv_cache)
         out = torch.cat([ids.repeat_interleave(num_return_sequences, dim=0), new], dim=1)
         return GenerateOutput(out, scores) if return_dict_in_generate else out
-    st = decode_state(model, B, Smax)
+    st = decode_state(model, B, Smax, fp8_kv_cache)
 
     st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, *processors)
     st.out.fill_(pad)

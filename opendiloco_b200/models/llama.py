@@ -748,7 +748,7 @@ class LlamaForCausalLM(nn.Module):
                  num_assistant_tokens: int = 4, num_beams: int = 1, length_penalty: float = 1.0, early_stopping=False,
                  num_return_sequences: int = 1, return_dict_in_generate: bool = False, repetition_penalty: float = 1.0,
                  no_repeat_ngram_size: int = 0, min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
-                 max_matching_ngram_size: int | None = None, fp8_weights: bool = False):
+                 max_matching_ngram_size: int | None = None, fp8_weights: bool = False, fp8_kv_cache: bool = False):
         """KV-cached text generation with HF ``generate`` keyword names.  Returns LongTensor [B, P + max_new_tokens]: the
         prompt as given, then the new tokens.
 
@@ -819,7 +819,19 @@ class LlamaForCausalLM(nn.Module):
         elsewhere (prefill, wider verify passes and beam steps); other precisions and devices run the reference path on
         Ŵ.  Works with every mode above; with ``assistant_model`` only this model is quantised.  While in use the e4m3 and
         dequantised copies take 1.5x the bf16 bytes of the projections (about 2.9 GB at the 1b preset), kept on the engine
-        for the next call; training state is not touched.  Raises ValueError when ``fp8_weights`` is not a bool."""
+        for the next call; training state is not touched.  Raises ValueError when ``fp8_weights`` is not a bool.
+
+        ``fp8_kv_cache=True`` keeps the KV cache in FP8: every K/V row written into the decode cache (one (position, kv
+        head) vector of ``head_dim`` values, the rotated k and the v the bf16 cache would store) is quantised to e4m3 with
+        one power-of-two scale per row by the rule of ``fp8_weights`` (ops/fp8w.py ``quantize_rows_ref``; a non-finite row
+        gives NaN bytes and factor), and stored as e4m3 [L, 2, B, Hkv, Smax, head_dim] plus an fp32 factor per row: 0.53x
+        the bf16 cache bytes at head_dim 64.  The result is exactly this program with every cache write followed by
+        replacing the written rows with their dequantised values q * inv: the prompt's own attention still reads its
+        in-flight bf16 q|k|v (so the first new token is unchanged), and every later read (the one-token steps, the verify
+        passes of assisted and prompt lookup decoding, beam steps, a token's own K/V included) sees the dequantised cache.
+        Works with every mode above and together with ``fp8_weights``; with ``assistant_model`` only this model's cache
+        is FP8.  ``False`` allocates and launches exactly what it did before.  Raises ValueError when ``fp8_kv_cache`` is
+        not a bool."""
         from .generation import generate
 
         return generate(self, input_ids, attention_mask=attention_mask, max_new_tokens=max_new_tokens, do_sample=do_sample,
@@ -829,7 +841,7 @@ class LlamaForCausalLM(nn.Module):
                         return_dict_in_generate=return_dict_in_generate, repetition_penalty=repetition_penalty,
                         no_repeat_ngram_size=no_repeat_ngram_size, min_new_tokens=min_new_tokens,
                         prompt_lookup_num_tokens=prompt_lookup_num_tokens, max_matching_ngram_size=max_matching_ngram_size,
-                        fp8_weights=fp8_weights)
+                        fp8_weights=fp8_weights, fp8_kv_cache=fp8_kv_cache)
 
     @torch.no_grad()
     def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None,

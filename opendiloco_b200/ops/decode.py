@@ -14,6 +14,14 @@ physical row ``table[r, c]`` (``attention``, ``beam_reorder``).
 
 Assisted generation scores n tokens per row in one pass.  Its buffers are slot-major: row ``j*B + b`` is token j of row
 b, at position ``pos[b] + j`` (``rope_append_multi``, ``verify_attention``, ``accept``).
+
+FP8 KV cache (``generate(fp8_kv_cache=True)``): K and V are e4m3 ``[B, Hkv, Smax, D]`` with fp32 ``kinv`` / ``vinv``
+``[B, Hkv, Smax]``, one power-of-two scale per (position, kv head) row by the per-row rule of :mod:`.fp8w`.  The writers
+(``rope_append``, ``rope_append_multi``, ``kv_fill``) quantise the rows the bf16 writers would store (``quantize_rows_ref``
+of the rotated k, and of v); the readers (``attention``, ``verify_attention``, ``gather_chunks``) see the dequantised cache
+Ĉ = ``dequantize_rows(q, inv)``, and ``beam_reorder`` moves inv with the bytes.  Every function takes the inv arrays as
+optional arguments: None is the bf16 cache.  Ĉ is a bf16 number for rows with amax >= 448 * 2^-125, so the kernels equal
+the bf16 kernels on Ĉ bit for bit, and the references dequantise and run the bf16 references.
 """
 from __future__ import annotations
 
@@ -23,21 +31,23 @@ import math
 import torch
 
 from .. import _lib
+from .fp8 import E4M3
+from .fp8w import dequantize_rows, quantize_rows_ref
 
 c_void_p, c_int, c_ll, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float
 _lib.register_optional("odb_dec_rope_append", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                               c_int, c_void_p])
+                                               c_int, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_kv_fill", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
-                                           c_void_p])
+                                           c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_attn_chunks", [c_int])
 _lib.register_optional("odb_dec_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_int,
-                                        c_int, c_int, c_int, c_float, c_void_p])
+                                        c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_sample", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                           c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p])
 _lib.register_optional("odb_dec_rope_append_multi", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                                     c_int, c_int, c_int, c_void_p])
+                                                     c_int, c_int, c_int, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_verify_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int,
-                                               c_int, c_int, c_int, c_int, c_float, c_void_p])
+                                               c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_accept", [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                           c_int, c_void_p])
@@ -49,7 +59,8 @@ _lib.register_optional("odb_dec_beam_topk", [c_void_p, c_ll, c_int, c_int, c_int
 _lib.register_optional("odb_dec_beam_step", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
                                              c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_void_p, c_void_p, c_int, c_void_p])
-_lib.register_optional("odb_dec_beam_reorder", [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p])
+_lib.register_optional("odb_dec_beam_reorder", [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                                c_void_p])
 
 MAX_EOS = 8
 # int64 control block of the sampler: do_sample, top_k, seed, pad_token_id, n_eos, eos ids, then the logits processors'
@@ -95,17 +106,53 @@ def attn_chunks(Smax: int) -> int:
     return int(_lib.cuda_lib().odb_dec_attn_chunks(Smax))
 
 
+# ------------------------------------------------------------------------------------------------ FP8 cache rows
+def _ptr(t: torch.Tensor | None):
+    return t.data_ptr() if t is not None else None
+
+
+def _check_fp8(kc: torch.Tensor, vc: torch.Tensor, kinv: torch.Tensor | None, vinv: torch.Tensor | None) -> None:
+    """The kernels' FP8 cache: e4m3 K / V with contiguous fp32 inv [B, Hkv, Smax], 16-byte aligned, Smax % 128 == 0."""
+    if kinv is None:
+        assert vinv is None
+        return
+    assert kc.dtype == E4M3 and vc.dtype == E4M3 and kinv.dtype == torch.float32 and vinv.dtype == torch.float32
+    assert kinv.is_contiguous() and vinv.is_contiguous() and kinv.shape == kc.shape[:-1] and vinv.shape == vc.shape[:-1]
+    assert kc.shape[2] % 128 == 0 and kinv.data_ptr() % 16 == 0 and vinv.data_ptr() % 16 == 0
+
+
+def dequantize_cache(cache: torch.Tensor, inv: torch.Tensor | None, dtype: torch.dtype) -> torch.Tensor:
+    """The cache as the attention reads it: Ĉ = q * inv (FP8 cache, [..., D] with inv [...]) or the cache itself."""
+    if inv is None:
+        return cache
+    D = cache.shape[-1]
+    return dequantize_rows(cache.reshape(-1, D), inv.reshape(-1), dtype).view(cache.shape)
+
+
+def _store_rows(cache: torch.Tensor, inv: torch.Tensor | None, index: tuple, x: torch.Tensor) -> None:
+    """cache[index] = x [..., D]; with an FP8 cache the rows of x are quantised (``quantize_rows_ref``) into the bytes of
+    cache[index] and inv[index]."""
+    if inv is None:
+        cache[index] = x
+        return
+    q, iv = quantize_rows_ref(x.reshape(-1, x.shape[-1]))
+    cache.view(torch.uint8)[index] = q.view(torch.uint8).view(x.shape)
+    inv[index] = iv.view(x.shape[:-1])
+
+
 # ------------------------------------------------------------------------------------------------ RoPE + append
 def rope_append(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, pos: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor,
-                Hq: int, Hkv: int, D: int) -> None:
-    """qkv [B, (Hq+2*Hkv)*D] (one token per row): rotate q (in place) and k at position pos[b]; k, v -> cache[b, :, pos[b]]."""
+                Hq: int, Hkv: int, D: int, kinv: torch.Tensor | None = None, vinv: torch.Tensor | None = None) -> None:
+    """qkv [B, (Hq+2*Hkv)*D] (one token per row): rotate q (in place) and k at position pos[b]; k, v -> cache[b, :, pos[b]]
+    (quantised with kinv / vinv: FP8 cache)."""
     B = qkv.shape[0]
     Smax = kc.shape[2]
     if usable(qkv, D, Hq, Hkv):
         assert qkv.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous() and pos.dtype == torch.int32
+        _check_fp8(kc, vc, kinv, vinv)
         _lib.check(_lib.cuda_lib().odb_dec_rope_append(qkv.data_ptr(), qkv.stride(0), cos.data_ptr(), sin.data_ptr(), pos.data_ptr(),
-                                                       kc.data_ptr(), vc.data_ptr(), B, Hq, Hkv, Smax, _lib.stream_ptr(qkv)),
-                   "dec_rope_append")
+                                                       kc.data_ptr(), vc.data_ptr(), B, Hq, Hkv, Smax, _ptr(kinv), _ptr(vinv),
+                                                       _lib.stream_ptr(qkv)), "dec_rope_append")
         _lib.count_launch()
         return
     half = D // 2
@@ -116,18 +163,21 @@ def rope_append(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, pos: to
     rot = torch.cat([a * c - b * s, b * c + a * s], dim=-1).to(qkv.dtype)
     qkv[:, : Hq * D] = rot[:, :Hq].reshape(B, Hq * D)
     rows = torch.arange(B, device=qkv.device)
-    kc[rows, :, p] = rot[:, Hq:]
-    vc[rows, :, p] = qkv[:, (Hq + Hkv) * D:].view(B, Hkv, D)
+    _store_rows(kc, kinv, (rows, slice(None), p), rot[:, Hq:])
+    _store_rows(vc, vinv, (rows, slice(None), p), qkv[:, (Hq + Hkv) * D:].view(B, Hkv, D))
 
 
 def kv_fill(qkv: torch.Tensor, lens: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, B: int, Sp: int, Hq: int, Hkv: int,
-            D: int, row_stride: int = 1) -> None:
-    """Prefill: rows s < lens[b] of the rotated packed projections qkv [B*Sp, row] -> cache[b * row_stride, :, s]."""
+            D: int, row_stride: int = 1, kinv: torch.Tensor | None = None, vinv: torch.Tensor | None = None) -> None:
+    """Prefill: rows s < lens[b] of the rotated packed projections qkv [B*Sp, row] -> cache[b * row_stride, :, s]
+    (quantised with kinv / vinv: FP8 cache)."""
     Smax = kc.shape[2]
     if usable(qkv, D, Hq, Hkv):
         assert qkv.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous() and lens.dtype == torch.int32
+        _check_fp8(kc, vc, kinv, vinv)
         _lib.check(_lib.cuda_lib().odb_dec_kv_fill(qkv.data_ptr(), qkv.stride(0), lens.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, Sp,
-                                                   Hq, Hkv, Smax, row_stride, _lib.stream_ptr(qkv)), "dec_kv_fill")
+                                                   Hq, Hkv, Smax, row_stride, _ptr(kinv), _ptr(vinv), _lib.stream_ptr(qkv)),
+                   "dec_kv_fill")
         _lib.count_launch()
         return
     n = min(Sp, Smax)
@@ -135,31 +185,41 @@ def kv_fill(qkv: torch.Tensor, lens: torch.Tensor, kc: torch.Tensor, vc: torch.T
     k = rows[..., Hq * D:(Hq + Hkv) * D].unflatten(-1, (Hkv, D)).transpose(1, 2)     # [B, Hkv, n, D]
     v = rows[..., (Hq + Hkv) * D:].unflatten(-1, (Hkv, D)).transpose(1, 2)
     keep = (torch.arange(n, device=qkv.device)[None, :] < lens.long()[:, None].to(qkv.device))[:, None, :, None]
-    kd, vd = kc[::row_stride], vc[::row_stride]
-    kd[:, :, :n] = torch.where(keep, k, kd[:, :, :n])
-    vd[:, :, :n] = torch.where(keep, v, vd[:, :, :n])
+    for cache, inv, x in ((kc, kinv, k), (vc, vinv, v)):
+        if inv is None:
+            d = cache[::row_stride]
+            d[:, :, :n] = torch.where(keep, x, d[:, :, :n])
+            continue
+        q, iv = quantize_rows_ref(x.reshape(-1, D))
+        d, di = cache.view(torch.uint8)[::row_stride], inv[::row_stride]
+        d[:, :, :n] = torch.where(keep, q.view(torch.uint8).view(x.shape), d[:, :, :n])
+        di[:, :, :n] = torch.where(keep[..., 0], iv.view(x.shape[:-1]), di[:, :, :n])
 
 
 # ------------------------------------------------------------------------------------------------ decode attention
 def attention(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, pos: torch.Tensor, out: torch.Tensor, Hq: int, Hkv: int, D: int,
-              part_o: torch.Tensor | None = None, part_ml: torch.Tensor | None = None, table: torch.Tensor | None = None) -> torch.Tensor:
+              part_o: torch.Tensor | None = None, part_ml: torch.Tensor | None = None, table: torch.Tensor | None = None,
+              kinv: torch.Tensor | None = None, vinv: torch.Tensor | None = None) -> torch.Tensor:
     """out[b, h*D:(h+1)*D] = softmax(q_bh . K[b, h//G, :pos[b]+1]^T / sqrt(D)) V[b, h//G, :pos[b]+1]  (one query per row).
 
     q: the first Hq*D columns of [B, row].  part_o fp32 [B, Hq, chunks, D] / part_ml fp32 [B, Hq, chunks, 2]: scratch of
     the split-KV kernel (``attn_chunks(Smax)`` chunks).  table: None, or the int32 chunk table [B, Smax / 128] (keys of
-    chunk c of row b are read from row table[b, c]; the reference gathers them, then attends)."""
+    chunk c of row b are read from row table[b, c]; the reference gathers them, then attends).  kinv / vinv: the FP8
+    cache's inv arrays (the reference attends over Ĉ)."""
     B = q.shape[0]
     Smax = kc.shape[2]
     if usable(q, D, Hq, Hkv):
         assert q.stride(1) == 1 and out.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous() and pos.dtype == torch.int32
+        _check_fp8(kc, vc, kinv, vinv)
         if table is not None:
             assert table.dtype == torch.int32 and table.is_contiguous() and table.shape == (B, attn_chunks(Smax)) and Smax % 128 == 0
         _lib.check(_lib.cuda_lib().odb_dec_attn(q.data_ptr(), q.stride(0), kc.data_ptr(), vc.data_ptr(), pos.data_ptr(), part_o.data_ptr(),
                                                 part_ml.data_ptr(), out.data_ptr(), out.stride(0),
                                                 table.data_ptr() if table is not None else None, B, Hq, Hkv, Smax,
-                                                1.0 / math.sqrt(D), _lib.stream_ptr(q)), "dec_attn")
+                                                1.0 / math.sqrt(D), _ptr(kinv), _ptr(vinv), _lib.stream_ptr(q)), "dec_attn")
         _lib.count_launch(2)
         return out
+    kc, vc = dequantize_cache(kc, kinv, q.dtype), dequantize_cache(vc, vinv, q.dtype)
     if table is not None:
         kc, vc = gather_chunks(kc, table), gather_chunks(vc, table)
     G = Hq // Hkv
@@ -172,8 +232,11 @@ def attention(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, pos: torch.Te
     return out
 
 
-def gather_chunks(cache: torch.Tensor, table: torch.Tensor) -> torch.Tensor:
-    """cache [rows, Hkv, Smax, D] read through the chunk table [rows, Smax / 128]: chunk c of row r from row table[r, c]."""
+def gather_chunks(cache: torch.Tensor, table: torch.Tensor, inv: torch.Tensor | None = None,
+                  dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """cache [rows, Hkv, Smax, D] read through the chunk table [rows, Smax / 128]: chunk c of row r from row table[r, c].
+    With ``inv`` (FP8 cache) the dequantised cache Ĉ in ``dtype`` is read."""
+    cache = dequantize_cache(cache, inv, dtype)
     rows, Hkv, Smax, D = cache.shape
     nch = table.shape[1]
     c5 = cache.view(rows, Hkv, nch, Smax // nch, D).transpose(1, 2)                   # [rows, nch, Hkv, 128, D]
@@ -183,15 +246,17 @@ def gather_chunks(cache: torch.Tensor, table: torch.Tensor) -> torch.Tensor:
 
 # ------------------------------------------------------------------------------------------------ assisted generation
 def rope_append_multi(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, pos: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor,
-                      Hq: int, Hkv: int, D: int, n: int) -> None:
-    """qkv [n*B, row] slot-major: rotate q (in place) and k of row j*B + b at position pos[b] + j; k, v -> cache[b, :, pos[b] + j]."""
+                      Hq: int, Hkv: int, D: int, n: int, kinv: torch.Tensor | None = None, vinv: torch.Tensor | None = None) -> None:
+    """qkv [n*B, row] slot-major: rotate q (in place) and k of row j*B + b at position pos[b] + j; k, v -> cache[b, :, pos[b] + j]
+    (quantised with kinv / vinv: FP8 cache)."""
     B = qkv.shape[0] // n
     Smax = kc.shape[2]
     if usable_verify(qkv, D, Hq, Hkv):
         assert qkv.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous() and pos.dtype == torch.int32
+        _check_fp8(kc, vc, kinv, vinv)
         _lib.check(_lib.cuda_lib().odb_dec_rope_append_multi(qkv.data_ptr(), qkv.stride(0), cos.data_ptr(), sin.data_ptr(),
                                                              pos.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, n, Hq, Hkv, Smax,
-                                                             _lib.stream_ptr(qkv)), "dec_rope_append_multi")
+                                                             _ptr(kinv), _ptr(vinv), _lib.stream_ptr(qkv)), "dec_rope_append_multi")
         _lib.count_launch()
         return
     half = D // 2
@@ -202,25 +267,29 @@ def rope_append_multi(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, p
     a, b = x[..., :half], x[..., half:]
     rot = torch.cat([a * c - b * s, b * c + a * s], dim=-1).to(qkv.dtype)
     qkv[:, : Hq * D] = rot[:, :Hq].reshape(n * B, Hq * D)
-    kc[rows, :, p] = rot[:, Hq:]
-    vc[rows, :, p] = qkv[:, (Hq + Hkv) * D:].view(n * B, Hkv, D)
+    _store_rows(kc, kinv, (rows, slice(None), p), rot[:, Hq:])
+    _store_rows(vc, vinv, (rows, slice(None), p), qkv[:, (Hq + Hkv) * D:].view(n * B, Hkv, D))
 
 
 def verify_attention(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, pos: torch.Tensor, out: torch.Tensor, Hq: int, Hkv: int,
-                     D: int, n: int, part_o: torch.Tensor | None = None, part_ml: torch.Tensor | None = None) -> torch.Tensor:
+                     D: int, n: int, part_o: torch.Tensor | None = None, part_ml: torch.Tensor | None = None,
+                     kinv: torch.Tensor | None = None, vinv: torch.Tensor | None = None) -> torch.Tensor:
     """Attention of n queries per row, slot-major: query row j*B + b attends keys 0 .. pos[b] + j of row b (causal inside
     the block).  part_o fp32 [n*B, Hq, verify_splits(Smax), D] / part_ml fp32 [n*B, Hq, verify_splits(Smax), 2]: scratch
-    of the split-KV kernel."""
+    of the split-KV kernel.  kinv / vinv: the FP8 cache's inv arrays (the reference attends over Ĉ)."""
     B = q.shape[0] // n
     Smax = kc.shape[2]
     if usable_verify(q, D, Hq, Hkv):
         assert n <= 8 and q.stride(1) == 1 and out.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous()
         assert pos.dtype == torch.int32 and part_o.shape[2] == verify_splits(Smax) and part_ml.shape[2] == verify_splits(Smax)
+        _check_fp8(kc, vc, kinv, vinv)
         _lib.check(_lib.cuda_lib().odb_dec_verify_attn(q.data_ptr(), q.stride(0), kc.data_ptr(), vc.data_ptr(), pos.data_ptr(),
                                                        part_o.data_ptr(), part_ml.data_ptr(), out.data_ptr(), out.stride(0), B, n, Hq,
-                                                       Hkv, Smax, 1.0 / math.sqrt(D), _lib.stream_ptr(q)), "dec_verify_attn")
+                                                       Hkv, Smax, 1.0 / math.sqrt(D), _ptr(kinv), _ptr(vinv), _lib.stream_ptr(q)),
+                   "dec_verify_attn")
         _lib.count_launch(2)
         return out
+    kc, vc = dequantize_cache(kc, kinv, q.dtype), dequantize_cache(vc, vinv, q.dtype)
     G = Hq // Hkv
     qf = q[:, : Hq * D].float().view(n, B, Hkv, G, D)
     att = torch.einsum("jbkgd,bksd->jbkgs", qf, kc.float()) / math.sqrt(D)
@@ -559,28 +628,35 @@ def beam_histories(prompt: torch.Tensor, plens: torch.Tensor, run_seq: torch.Ten
     return torch.where(col < (lens + t)[:, None], h, torch.full_like(h, -1))
 
 
-def beam_reorder(kv: torch.Tensor, table: torch.Tensor | None, parent: torch.Tensor, pos: torch.Tensor, num_beams: int) -> None:
+def beam_reorder(kv: torch.Tensor, table: torch.Tensor | None, parent: torch.Tensor, pos: torch.Tensor, num_beams: int,
+                 inv: torch.Tensor | None = None) -> None:
     """After a selection, make every beam row's cache the history of its parent row (int32 [rows], pos: the next position
-    to write, the same for all beams of a prompt).  kv: every layer's K and V of the beam rows, [L, 2, rows, Hkv, Smax, D].
+    to write, the same for all beams of a prompt).  kv: every layer's K and V of the beam rows, [L, 2, rows, Hkv, Smax, D];
+    inv: with an FP8 cache (e4m3 kv), its fp32 inv [L, 2, rows, Hkv, Smax], moved with the bytes.
 
     With a chunk table (the kernel path), complete 128-position chunks are shared: a child whose parent is another row
     takes the parent's table entries below pos // 128 and gets a copy of positions [128 * (pos // 128), pos) in its own
     row.  Without one, ``beam_reorder_reference`` moves whole rows."""
     if table is None:
-        beam_reorder_reference(kv, parent)
+        beam_reorder_reference(kv, parent, inv)
         return
     L, two, rows, Hkv, Smax, D = kv.shape
-    assert kv.is_cuda and kv.dtype == torch.bfloat16 and kv.is_contiguous() and two == 2 and D == 64 and rows % num_beams == 0
+    assert kv.is_cuda and kv.dtype == (torch.bfloat16 if inv is None else E4M3) and kv.is_contiguous() and two == 2 and D == 64
+    assert rows % num_beams == 0 and (inv is None or (inv.dtype == torch.float32 and inv.is_contiguous() and inv.shape == kv.shape[:-1]))
     assert table.shape == (rows, Smax // 128) and table.dtype == torch.int32 and parent.dtype == torch.int32 and pos.dtype == torch.int32
     _lib.check(_lib.cuda_lib().odb_dec_beam_reorder(kv.data_ptr(), table.data_ptr(), parent.data_ptr(), pos.data_ptr(), rows // num_beams,
-                                                    num_beams, L, Hkv, Smax, _lib.stream_ptr(kv)), "dec_beam_reorder")
+                                                    num_beams, L, Hkv, Smax, _ptr(inv), _lib.stream_ptr(kv)), "dec_beam_reorder")
     _lib.count_launch()
 
 
-def beam_reorder_reference(kv: torch.Tensor, parent: torch.Tensor) -> None:
-    """Physical reorder: row r of every layer's K and V becomes (a copy of) row parent[r].  The chunk table of
-    ``beam_reorder`` must read exactly like this."""
-    kv.copy_(kv.index_select(2, parent.long().to(kv.device)))
+def beam_reorder_reference(kv: torch.Tensor, parent: torch.Tensor, inv: torch.Tensor | None = None) -> None:
+    """Physical reorder: row r of every layer's K and V (and of an FP8 cache's inv) becomes (a copy of) row parent[r].  The
+    chunk table of ``beam_reorder`` must read exactly like this."""
+    idx = parent.long().to(kv.device)
+    raw = kv.view(torch.uint8) if kv.dtype == E4M3 else kv
+    raw.copy_(raw.index_select(2, idx))
+    if inv is not None:
+        inv.copy_(inv.index_select(2, idx))
 
 
 # ------------------------------------------------------------------------------------------------ sampler

@@ -117,6 +117,8 @@ def main(argv=None) -> None:
     ap.add_argument("--max-matching-ngram-size", type=int, default=None, help="prompt lookup: longest n-gram matched (default 2)")
     ap.add_argument("--fp8-weights", action="store_true",
                     help="quantise the decoder-layer projections to e4m3 (one scale per output row) and decode on them")
+    ap.add_argument("--fp8-kv-cache", action="store_true",
+                    help="keep the KV cache in e4m3 with one power-of-two scale per (position, kv head) row")
     a = ap.parse_args(argv)
     if a.assistant_model is None and a.assistant_checkpoint is not None:
         ap.error("--assistant-checkpoint needs --assistant-model")
@@ -156,7 +158,8 @@ def main(argv=None) -> None:
                          early_stopping=early_stopping, num_return_sequences=a.num_return_sequences, return_dict_in_generate=True,
                          repetition_penalty=a.repetition_penalty, no_repeat_ngram_size=a.no_repeat_ngram_size,
                          min_new_tokens=a.min_new_tokens, prompt_lookup_num_tokens=a.prompt_lookup_num_tokens,
-                         max_matching_ngram_size=a.max_matching_ngram_size, fp8_weights=a.fp8_weights)
+                         max_matching_ngram_size=a.max_matching_ngram_size, fp8_weights=a.fp8_weights,
+                         fp8_kv_cache=a.fp8_kv_cache)
     out = res.sequences.cpu()
     R = out.shape[0] // len(prompts)
     for i, p in enumerate(prompts):
