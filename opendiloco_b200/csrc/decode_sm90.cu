@@ -12,6 +12,8 @@
 //   odb_dec_beam_topk     beam search: per vocabulary split of a row, the (max, sum-exp) partial and the local top-K logits
 //   odb_dec_beam_step     beam search: one CTA per prompt merges the candidates and does HF's selection and bookkeeping
 //   odb_dec_beam_reorder  beam search: chunk-table update and partial-chunk K/V copy for beams that changed parent
+//   odb_dec_attn_group    multi-sample generation: split-KV decode attention that loads a chunk shared by sibling rows once
+//   odb_dec_fork          multi-sample generation: make the sibling rows of a prefilled prompt its children (chunk table)
 //
 // KV cache layout, per layer: K and V each [B, Hkv, Smax, 64] bf16, so the keys of one (row, kv head) are contiguous and a
 // chunk of them is ONE bulk copy.
@@ -186,58 +188,24 @@ struct AttSmem {
   static constexpr int BYTES = BAR_OFF + 16;
 };
 
+// The arithmetic of one partial: the G query heads of sQ (pre-scaled) against the n keys of sK / sV (and sKI / sVI) of
+// chunk c, written to part_o / part_ml of row b.  decode_attn_kernel and decode_attn_group_kernel both compute every
+// partial through this function, so their results are the same bits.  Ends with shared memory still being read (the
+// caller synchronises before overwriting it).
 template <int G, typename T>
-__global__ void __launch_bounds__(ATT_THREADS)
-decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const T* __restrict__ kc, const T* __restrict__ vc,
-                   const int* __restrict__ pos, float* __restrict__ part_o, float* __restrict__ part_ml, const int* __restrict__ table,
-                   int Hkv, int Smax, int nchunks, float scale_log2, const float* __restrict__ kinv, const float* __restrict__ vinv) {
+__device__ __forceinline__ void attn_chunk_partial(uint8_t* smem, int n, int b, int hk, int c, int Hkv, int nchunks,
+                                                   float* __restrict__ part_o, float* __restrict__ part_ml) {
   using L = AttSmem<G, T>;
   constexpr bool KV8 = sizeof(T) == 1;
-  extern __shared__ __align__(128) uint8_t smem[];
-  T* sK = reinterpret_cast<T*>(smem + L::K_OFF);
-  T* sV = reinterpret_cast<T*>(smem + L::V_OFF);
+  const T* sK = reinterpret_cast<const T*>(smem + L::K_OFF);
+  const T* sV = reinterpret_cast<const T*>(smem + L::V_OFF);
   const float* sKI = reinterpret_cast<const float*>(smem + L::KI_OFF);
   const float* sVI = reinterpret_cast<const float*>(smem + L::VI_OFF);
-  float* sQ = reinterpret_cast<float*>(smem + L::Q_OFF);
+  const float* sQ = reinterpret_cast<const float*>(smem + L::Q_OFF);
   float* sS = reinterpret_cast<float*>(smem + L::S_OFF);
   float* sR = reinterpret_cast<float*>(smem + L::R_OFF);
   float* sM = reinterpret_cast<float*>(smem + L::M_OFF);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
-
-  pdl_launch_dependents();
-  const int c = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  pdl_wait();
-  const int len = pos[b] + 1;
-  const int j0 = c * CH;
-  if (j0 >= len) return;                         // uniform over the CTA
-  const int n = min(CH, len - j0);
-  const int phys = table != nullptr ? table[b * nchunks + c] : b;
-  const long long kv_off = (((long long)phys * Hkv + hk) * Smax + j0) * D;
-  if (tid == 0) {
-    if constexpr (KV8) {
-      const long long i_off = ((long long)phys * Hkv + hk) * Smax + j0;
-      const uint32_t ib = (n * 4 + 15) & ~15;
-      mbar_arrive_expect_tx(bar, 2u * n * D + 2u * ib);
-      bulk_load_1d(sK, kc + kv_off, n * D, bar);
-      bulk_load_1d(sV, vc + kv_off, n * D, bar);
-      bulk_load_1d(smem + L::KI_OFF, kinv + i_off, ib, bar);
-      bulk_load_1d(smem + L::VI_OFF, vinv + i_off, ib, bar);
-    } else {
-      mbar_arrive_expect_tx(bar, 2u * n * D * 2);
-      bulk_load_1d(sK, kc + kv_off, n * D * 2, bar);
-      bulk_load_1d(sV, vc + kv_off, n * D * 2, bar);
-    }
-  }
-  const __nv_bfloat16* qrow = q + (long long)b * ldq + (long long)hk * G * D;
-  for (int i = tid; i < G * D; i += ATT_THREADS) sQ[i] = __bfloat162float(qrow[i]) * scale_log2;
-  __syncthreads();
-  mbar_wait(bar, 0);
 
   // ---- scores: thread = key; the 16-byte chunks of a key row are visited in a rotated order (no bank conflicts)
   {
@@ -324,6 +292,134 @@ decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const T* 
     float* ml = part_ml + (((long long)b * Hq + hk * G + tid) * nchunks + c) * 2;
     ml[0] = sM[2 * tid];
     ml[1] = sM[2 * tid + 1];
+  }
+}
+
+// Thread 0 of the CTA: bulk-copy keys [j0, j0 + n) of (physical row phys, kv head hk) into sK / sV (FP8 cache: also their two
+// inv runs, rounded up to 16 bytes, in bounds since Smax is a multiple of CH), completing on bar.
+template <int G, typename T>
+__device__ __forceinline__ void attn_chunk_load(uint8_t* smem, const T* __restrict__ kc, const T* __restrict__ vc,
+                                                const float* __restrict__ kinv, const float* __restrict__ vinv, int phys, int hk,
+                                                int Hkv, int Smax, int j0, int n, uint64_t* bar) {
+  using L = AttSmem<G, T>;
+  const long long kv_off = (((long long)phys * Hkv + hk) * Smax + j0) * D;
+  if constexpr (sizeof(T) == 1) {
+    const long long i_off = ((long long)phys * Hkv + hk) * Smax + j0;
+    const uint32_t ib = (n * 4 + 15) & ~15;
+    mbar_arrive_expect_tx(bar, 2u * n * D + 2u * ib);
+    bulk_load_1d(smem + L::K_OFF, kc + kv_off, n * D, bar);
+    bulk_load_1d(smem + L::V_OFF, vc + kv_off, n * D, bar);
+    bulk_load_1d(smem + L::KI_OFF, kinv + i_off, ib, bar);
+    bulk_load_1d(smem + L::VI_OFF, vinv + i_off, ib, bar);
+  } else {
+    mbar_arrive_expect_tx(bar, 2u * n * D * 2);
+    bulk_load_1d(smem + L::K_OFF, kc + kv_off, n * D * 2, bar);
+    bulk_load_1d(smem + L::V_OFF, vc + kv_off, n * D * 2, bar);
+  }
+}
+
+// The G query heads of kv head hk of row b -> sQ, pre-scaled by softmax_scale * log2(e).
+template <int G, typename T>
+__device__ __forceinline__ void attn_load_q(uint8_t* smem, const __nv_bfloat16* __restrict__ q, long long ldq, int b, int hk,
+                                            float scale_log2) {
+  float* sQ = reinterpret_cast<float*>(smem + AttSmem<G, T>::Q_OFF);
+  const __nv_bfloat16* qrow = q + (long long)b * ldq + (long long)hk * G * D;
+  for (int i = threadIdx.x; i < G * D; i += ATT_THREADS) sQ[i] = __bfloat162float(qrow[i]) * scale_log2;
+}
+
+template <int G, typename T>
+__global__ void __launch_bounds__(ATT_THREADS)
+decode_attn_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const T* __restrict__ kc, const T* __restrict__ vc,
+                   const int* __restrict__ pos, float* __restrict__ part_o, float* __restrict__ part_ml, const int* __restrict__ table,
+                   int Hkv, int Smax, int nchunks, float scale_log2, const float* __restrict__ kinv, const float* __restrict__ vinv) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + AttSmem<G, T>::BAR_OFF);
+  pdl_launch_dependents();
+  const int c = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
+  if (threadIdx.x == 0) {
+    mbar_init(bar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  const int len = pos[b] + 1;
+  const int j0 = c * CH;
+  if (j0 >= len) return;                         // uniform over the CTA
+  const int n = min(CH, len - j0);
+  const int phys = table != nullptr ? table[b * nchunks + c] : b;
+  if (threadIdx.x == 0) attn_chunk_load<G, T>(smem, kc, vc, kinv, vinv, phys, hk, Hkv, Smax, j0, n, bar);
+  attn_load_q<G, T>(smem, q, ldq, b, hk, scale_log2);
+  __syncthreads();
+  mbar_wait(bar, 0);
+  attn_chunk_partial<G, T>(smem, n, b, hk, c, Hkv, nchunks, part_o, part_ml);
+}
+
+// Sibling-grouped split-KV attention (multi-sample generation): rows p * ngrp .. p * ngrp + ngrp - 1 are the siblings of
+// prompt p and read their keys through the chunk table, as decode_attn_kernel does.  grid (ceil(Smax / CH), Hkv, P * splits),
+// block 128: CTA (c, hk, p * splits + s) serves siblings [s * per, min(ngrp, (s + 1) * per)) of prompt p, per =
+// ceil(ngrp / splits), one after the other.  A sibling whose table entry for chunk c names the physical row already in
+// shared memory, with at least its key count loaded, reuses that copy; otherwise the chunk is loaded again (after the
+// fork: the chunk holding the prompt's tail and every later one, which each row owns).  Each sibling's partial is
+// attn_chunk_partial on its own q, its own key count and the same bytes, so it is bit-identical to decode_attn_kernel's.
+// At least four resident CTAs (128 registers a thread): without a minimum, ptxas holds G = 8 to 64 registers and spills.
+template <int G, typename T>
+__global__ void __launch_bounds__(ATT_THREADS, 4)
+decode_attn_group_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const T* __restrict__ kc, const T* __restrict__ vc,
+                         const int* __restrict__ pos, float* __restrict__ part_o, float* __restrict__ part_ml,
+                         const int* __restrict__ table, int Hkv, int Smax, int nchunks, float scale_log2, const float* __restrict__ kinv,
+                         const float* __restrict__ vinv, int ngrp, int splits) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + AttSmem<G, T>::BAR_OFF);
+  pdl_launch_dependents();
+  const int c = blockIdx.x, hk = blockIdx.y, p = blockIdx.z / splits, s = blockIdx.z % splits;
+  const int per = ceil_div(ngrp, splits);
+  const int r0 = p * ngrp + s * per, r1 = p * ngrp + min(ngrp, (s + 1) * per);
+  if (threadIdx.x == 0) {
+    mbar_init(bar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  // The next sibling's q, position and table entry are loaded into registers while this sibling computes, so only the
+  // first sibling waits for them.  q is scaled exactly as attn_load_q does.
+  constexpr int QPT = (G * D + ATT_THREADS - 1) / ATT_THREADS;
+  float qn[QPT];
+  int pos_n = 0, phys_n = 0;
+  const int tid = threadIdx.x, j0 = c * CH;
+  auto fetch = [&](int r) {
+    pos_n = pos[r];
+    phys_n = table[r * nchunks + c];
+    const __nv_bfloat16* qrow = q + (long long)r * ldq + (long long)hk * G * D;
+#pragma unroll
+    for (int k = 0; k < QPT; ++k)
+      if (tid + k * ATT_THREADS < G * D) qn[k] = __bfloat162float(qrow[tid + k * ATT_THREADS]) * scale_log2;
+  };
+  float* sQ = reinterpret_cast<float*>(smem + AttSmem<G, T>::Q_OFF);
+  int cur = -1, cur_n = 0;
+  uint32_t phase = 0;
+  if (r0 < r1) fetch(r0);
+  for (int r = r0; r < r1; ++r) {
+    const int len = pos_n + 1, phys = phys_n;
+#pragma unroll
+    for (int k = 0; k < QPT; ++k)
+      if (tid + k * ATT_THREADS < G * D) sQ[tid + k * ATT_THREADS] = qn[k];
+    if (r + 1 < r1) fetch(r + 1);
+    if (j0 >= len) continue;                     // uniform over the CTA
+    const int n = min(CH, len - j0);
+    const bool load = phys != cur || n > cur_n;
+    if (load && tid == 0) {
+      fence_proxy_async_smem();                  // the previous sibling's reads of sK / sV come before the new copy
+      attn_chunk_load<G, T>(smem, kc, vc, kinv, vinv, phys, hk, Hkv, Smax, j0, n, bar);
+    }
+    __syncthreads();
+    if (load) {
+      mbar_wait(bar, phase);
+      phase ^= 1;
+      cur = phys;
+      cur_n = n;
+    }
+    attn_chunk_partial<G, T>(smem, n, r, hk, c, Hkv, nchunks, part_o, part_ml);
+    __syncthreads();                             // every read of this sibling's shared memory is done
   }
 }
 
@@ -1408,6 +1504,44 @@ beam_reorder_kernel(T* __restrict__ kv, int* __restrict__ table, const int* __re
   }
 }
 
+// ------------------------------------------------------------------------------------------------ multi-sample fork
+// grid (L * 2 * Hkv, B), block 256.  Prompt g's n rows g*n .. g*n + n - 1 after its prefill into row g*n, which holds
+// positions [0, p), p = len[g]: the children g*n + 1 .. take row g*n's table entries for the complete chunks c < p / CH
+// and get a copy of the partial chunk [CH * (p / CH), p) (FP8 cache: with its inv) in their own row; every other entry
+// of the n rows names the row itself.  (x, g) copies slab x / Hkv (a layer's K or V), kv head x % Hkv; the table is written
+// by the CTAs x = 0.  The source row is never a destination, so nothing is staged and n is unbounded.
+template <typename T>
+__global__ void __launch_bounds__(256)
+fork_kernel(T* __restrict__ kv, int* __restrict__ table, const int* __restrict__ len, int n, int Hkv, int Smax, int nchunks,
+            float* __restrict__ inv) {
+  constexpr int RV = D * (int)sizeof(T) / 16;    // 16-byte pieces per position
+  pdl_launch_dependents();
+  pdl_wait();
+  const int slab = blockIdx.x / Hkv, hk = blockIdx.x % Hkv, g = blockIdx.y, tid = threadIdx.x;
+  const long long rows = (long long)gridDim.y * n;
+  const int src = g * n, p = min(len[g], Smax), c = p / CH, m = (p - c * CH) * RV;
+  T* base = kv + (long long)slab * rows * Hkv * Smax * D;
+  const uint4* s4 = reinterpret_cast<const uint4*>(base + (((long long)src * Hkv + hk) * Smax + c * CH) * D);
+  for (int i = tid; i < (n - 1) * m; i += blockDim.x) {
+    const int j = 1 + i / m, e = i % m;
+    reinterpret_cast<uint4*>(base + (((long long)(src + j) * Hkv + hk) * Smax + c * CH) * D)[e] = s4[e];
+  }
+  if constexpr (sizeof(T) == 1) {
+    const int mi = p - c * CH;
+    float* ibase = inv + (long long)slab * rows * Hkv * Smax;
+    const float* isrc = ibase + ((long long)src * Hkv + hk) * Smax + c * CH;
+    for (int i = tid; i < (n - 1) * mi; i += blockDim.x) {
+      const int j = 1 + i / mi, e = i % mi;
+      ibase[((long long)(src + j) * Hkv + hk) * Smax + c * CH + e] = isrc[e];
+    }
+  }
+  if (blockIdx.x == 0)
+    for (int i = tid; i < n * nchunks; i += blockDim.x) {
+      const int j = i / nchunks, cc = i % nchunks;
+      table[(src + j) * nchunks + cc] = j > 0 && cc < c ? src : src + j;
+    }
+}
+
 template <int G, typename T>
 int launch_attn(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml, void* out,
                 long long ldo, const void* table, int B, int Hkv, int Smax, float scale, const void* kinv, const void* vinv,
@@ -1438,6 +1572,68 @@ int launch_attn_t(const void* q, long long ldq, const void* kc, const void* vc, 
     return launch_attn<G, uint8_t>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, scale, kinv, vinv, st);
   return launch_attn<G, __nv_bfloat16>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, scale, nullptr, nullptr,
                                        st);
+}
+
+// Siblings per CTA of decode_attn_group_kernel.  A CTA runs its siblings one after the other, so fewer siblings per CTA
+// buy parallelism with repeated loads of the shared chunks: at most max(1, 4 / G) siblings per CTA (the best of the splits
+// measured at G 1 and G 8, profiles/README.md), and more CTAs while the (chunk, kv head, prompt, split) grid would not
+// fill one wave of resident CTAs on the device.  splits > 0 forces the split (tests).
+template <int G, typename T>
+int attn_group_splits(int P, int ngrp, int Hkv, int nchunks) {
+  static int wave = 0;
+  if (wave == 0) {
+    int dev, sms, per_sm;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e == cudaSuccess)
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, decode_attn_group_kernel<G, T>, ATT_THREADS, AttSmem<G, T>::BYTES);
+    if (e != cudaSuccess) return -(int)e;
+    wave = sms * std::max(per_sm, 1);
+  }
+  const long long base = (long long)nchunks * Hkv * P;
+  const int per = std::max(1, 4 / G);
+  return (int)std::min<long long>(ngrp, std::max<long long>(ceil_div(ngrp, per), (wave + base - 1) / base));
+}
+
+template <int G, typename T>
+int launch_attn_group(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml,
+                      void* out, long long ldo, const void* table, int rows, int ngrp, int Hkv, int Smax, float scale,
+                      const void* kinv, const void* vinv, int splits, cudaStream_t st) {
+  static bool attr_set = false;
+  const int smem = AttSmem<G, T>::BYTES;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(decode_attn_group_kernel<G, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return (int)e;
+    attr_set = true;
+  }
+  const int nchunks = ceil_div(Smax, CH), P = rows / ngrp;
+  if (splits <= 0) splits = attn_group_splits<G, T>(P, ngrp, Hkv, nchunks);
+  if (splits <= 0) return -splits;
+  splits = ceil_div(ngrp, ceil_div(ngrp, std::min(splits, ngrp)));   // no CTA without a sibling
+  launch_pdl(decode_attn_group_kernel<G, T>, dim3(nchunks, Hkv, P * splits), dim3(ATT_THREADS), smem, st, (const __nv_bfloat16*)q,
+             ldq, (const T*)kc, (const T*)vc, (const int*)pos, (float*)part_o, (float*)part_ml, (const int*)table, Hkv, Smax, nchunks,
+             scale * 1.4426950408889634f, (const float*)kinv, (const float*)vinv, ngrp, splits);
+  ODB_CHECK_LAST();
+  launch_pdl(decode_combine_kernel, dim3(Hkv * G, rows), dim3(D), 0, st, (const float*)part_o, (const float*)part_ml, (const int*)pos,
+             (__nv_bfloat16*)out, ldo, nchunks);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+template <int G>
+int launch_attn_group_t(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml,
+                        void* out, long long ldo, const void* table, int rows, int ngrp, int Hkv, int Smax, float scale,
+                        const void* kinv, const void* vinv, int splits, cudaStream_t st) {
+  if (kinv != nullptr)
+    return launch_attn_group<G, uint8_t>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, scale, kinv,
+                                         vinv, splits, st);
+  return launch_attn_group<G, __nv_bfloat16>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, scale,
+                                             nullptr, nullptr, splits, st);
+}
+
+template <int G>
+int group_splits_t(bool kv8, int P, int ngrp, int Hkv, int nchunks) {
+  return kv8 ? attn_group_splits<G, uint8_t>(P, ngrp, Hkv, nchunks) : attn_group_splits<G, __nv_bfloat16>(P, ngrp, Hkv, nchunks);
 }
 
 template <typename T>
@@ -1510,6 +1706,48 @@ ODB_EXPORT int odb_dec_attn(const void* q, long long ldq, const void* kc, const 
     case 8: return dec::launch_attn_t<8>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, sc, kinv, vinv, st);
     default: return -2;                          // GQA groups of 1, 2, 4 or 8 query heads
   }
+}
+
+// Multi-sample decode attention: as odb_dec_attn with a chunk table (required), over rows = P * ngrp rows where rows
+// p * ngrp .. p * ngrp + ngrp - 1 are the siblings of prompt p; a chunk that siblings share through the table is loaded once
+// per CTA.  The partials and out are bit-identical to odb_dec_attn's with the same table.  splits: 0 lets the launcher
+// choose how many CTAs share a prompt's siblings (odb_dec_attn_group_splits; an FP8 cache at G = 1 runs odb_dec_attn through
+// the table, which measured faster there), > 0 forces the grouped kernel with that split.  See dec::decode_attn_group_kernel.
+ODB_EXPORT int odb_dec_attn_group(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o,
+                                  void* part_ml, void* out, long long ldo, const void* table, int rows, int ngrp, int Hq, int Hkv,
+                                  int Smax, float softmax_scale, const void* kinv, const void* vinv, int splits, cudaStream_t st) {
+  if (Hq % Hkv || ldq % 8 || ngrp < 1 || rows % ngrp || table == nullptr || (kinv != nullptr && Smax % dec::CH)) return -1;
+  const float sc = softmax_scale;
+  if (splits <= 0 && kinv != nullptr && Hq == Hkv)   // measured: an FP8 cache at G = 1 reads faster through the table path
+    return odb_dec_attn(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, Hq, Hkv, Smax, softmax_scale, kinv, vinv, st);
+  switch (Hq / Hkv) {
+    case 1: return dec::launch_attn_group_t<1>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, sc, kinv,
+                                                 vinv, splits, st);
+    case 2: return dec::launch_attn_group_t<2>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, sc, kinv,
+                                                 vinv, splits, st);
+    case 4: return dec::launch_attn_group_t<4>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, sc, kinv,
+                                                 vinv, splits, st);
+    case 8: return dec::launch_attn_group_t<8>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, sc, kinv,
+                                                 vinv, splits, st);
+    default: return -2;                          // GQA groups of 1, 2, 4 or 8 query heads
+  }
+}
+
+// The sibling split odb_dec_attn_group chooses for these shapes (CTAs per prompt and chunk; needs a device); 0: it runs
+// odb_dec_attn through the table instead; < 0: an error.
+ODB_EXPORT int odb_dec_attn_group_splits(int rows, int ngrp, int Hq, int Hkv, int Smax, int kv8) {
+  if (ngrp < 1 || rows % ngrp || Hq % Hkv) return -1;
+  if (kv8 && Hq == Hkv) return 0;
+  const int P = rows / ngrp, nch = odb::ceil_div(Smax, dec::CH);
+  int s;
+  switch (Hq / Hkv) {
+    case 1: s = dec::group_splits_t<1>(kv8 != 0, P, ngrp, Hkv, nch); break;
+    case 2: s = dec::group_splits_t<2>(kv8 != 0, P, ngrp, Hkv, nch); break;
+    case 4: s = dec::group_splits_t<4>(kv8 != 0, P, ngrp, Hkv, nch); break;
+    case 8: s = dec::group_splits_t<8>(kv8 != 0, P, ngrp, Hkv, nch); break;
+    default: return -2;
+  }
+  return s <= 0 ? s - 1 : odb::ceil_div(ngrp, odb::ceil_div(ngrp, s));
 }
 
 // logits [B, ld] bf16; ictl / fctl: see dec::sample_kernel; pos / gen / finished int32 [B]; out int64 [B, max_new];
@@ -1679,4 +1917,19 @@ ODB_EXPORT int odb_dec_beam_reorder(void* kv, void* table, const void* parent, c
   if (nb < 1 || nb > dec::MAX_BEAMS || Smax % dec::CH || Smax / dec::CH > dec::MAX_TABLE) return -1;
   if (inv != nullptr) return dec::launch_beam_reorder<uint8_t>(kv, inv, table, parent, pos, B, nb, L, Hkv, Smax, st);
   return dec::launch_beam_reorder<__nv_bfloat16>(kv, nullptr, table, parent, pos, B, nb, L, Hkv, Smax, st);
+}
+
+// kv [L, 2, B*n, Hkv, Smax, 64] (every layer's K and V, one allocation; bf16, or e4m3 bytes with inv fp32
+// [L, 2, B*n, Hkv, Smax], also one allocation); table int32 [B*n, Smax/128]; len int32 [B]: prompt g was prefilled into
+// row g*n, positions [0, len[g]).  Makes rows g*n + 1 .. g*n + n - 1 its children.  See dec::fork_kernel.
+ODB_EXPORT int odb_dec_fork(void* kv, void* table, const void* len, int B, int n, int L, int Hkv, int Smax, void* inv, cudaStream_t st) {
+  if (n < 1 || Smax % dec::CH) return -1;
+  if (inv != nullptr)
+    launch_pdl(dec::fork_kernel<uint8_t>, dim3(L * 2 * Hkv, B), dim3(256), 0, st, (uint8_t*)kv, (int*)table, (const int*)len, n, Hkv, Smax,
+               Smax / dec::CH, (float*)inv);
+  else
+    launch_pdl(dec::fork_kernel<__nv_bfloat16>, dim3(L * 2 * Hkv, B), dim3(256), 0, st, (__nv_bfloat16*)kv, (int*)table, (const int*)len,
+               n, Hkv, Smax, Smax / dec::CH, (float*)nullptr);
+  ODB_CHECK_LAST();
+  return 0;
 }

@@ -33,6 +33,12 @@ FP8 weight-only mode, ``generate(fp8_weights=True)``: the layer programs take ev
 them (:mod:`~opendiloco_b200.models.fp8_weights`) rows of M <= 64 run the skinny e4m3 GEMM and wider ones the bf16 GEMM on
 the dequantised weights Ŵ.  Every graph key carries the mode, so switching it recaptures.
 
+Multi-sample generation, ``generate(do_sample=True, num_return_sequences=n)``: n sibling rows per prompt (row p * n + j
+is sample j of prompt p) in a DecodeState of group n.  Each prompt is prefilled once, into row p * n; its last position's
+residual goes to all n rows, so the LM head and the sampler see exactly the rows of the repeated-prompt program.  A fork
+then points the siblings' chunk tables at row p * n for the prompt's complete 128-key chunks and copies the partial one
+into each child's own row; every decode step reads a shared chunk once for all siblings (``DK.attention_grouped``).
+
 FP8 KV cache, ``generate(fp8_kv_cache=True)``: the DecodeState holds K and V as e4m3 with one fp32 factor per (position,
 kv head) row (:mod:`~opendiloco_b200.ops.decode`); every writer quantises and every decode-time reader (the one-token step,
 the verify pass, beam steps) dequantises.  The flag is part of the DecodeState and BeamState keys, so toggling it
@@ -88,16 +94,18 @@ class _PrefillBuffers:
 class DecodeState:
     """KV caches, decode buffers and device-side control scalars for B rows of up to Smax positions.  ``fp8_kv``: the caches
     are e4m3 ``kv`` [L, 2, B, Hkv, Smax, D] with fp32 ``kv_inv`` [L, 2, B, Hkv, Smax] (each one allocation: beam search
-    reorders all of it); ``kinv`` / ``vinv`` are the per-layer views of ``kv_inv`` (None for a bf16 cache)."""
+    reorders all of it); ``kinv`` / ``vinv`` are the per-layer views of ``kv_inv`` (None for a bf16 cache).  ``group`` > 1:
+    multi-sample rows, ``group`` siblings per prompt, with the chunk table ``table`` int32 [B, Smax / 128] of the kernel
+    path (None otherwise, and for group 1)."""
 
-    def __init__(self, cfg, B: int, Smax: int, device, dtype, fp8_kv: bool = False):
+    def __init__(self, cfg, B: int, Smax: int, device, dtype, fp8_kv: bool = False, group: int = 1):
         L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         h, i, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
         e = lambda *shape: torch.empty(*shape, dtype=dtype, device=device)  # noqa: E731
         i32 = lambda: torch.zeros(B, dtype=torch.int32, device=device)      # noqa: E731
         self.cfg, self.B, self.Smax, self.device, self.dtype = cfg, B, Smax, torch.device(device), dtype
-        self.key = (B, Smax, str(device), dtype, fp8_kv)
-        self.fp8_kv = fp8_kv
+        self.key = (B, Smax, str(device), dtype, fp8_kv, group)
+        self.fp8_kv, self.group = fp8_kv, group
         # one allocation: beam search reorders all
         self.kv = torch.zeros(L, 2, B, Hkv, Smax, D, dtype=E4M3 if fp8_kv else dtype, device=device)
         self.kv_inv = torch.zeros(L, 2, B, Hkv, Smax, dtype=torch.float32, device=device) if fp8_kv else None
@@ -125,6 +133,7 @@ class DecodeState:
             nch = DK.attn_chunks(Smax)
             self.part_o = torch.empty(B, Hq, nch, D, dtype=torch.float32, device=device)
             self.part_ml = torch.empty(B, Hq, nch, 2, dtype=torch.float32, device=device)
+        self.table = torch.zeros(B, nch, dtype=torch.int32, device=device) if self.kernels and group > 1 else None
         self._prefill: _PrefillBuffers | None = None
         self.graph = None
         self.graph_key = None
@@ -143,16 +152,17 @@ class DecodeState:
         self.fctl.copy_(fctl)
 
 
-def decode_state(model, B: int, Smax: int, fp8_kv: bool = False) -> DecodeState:
-    """The model's decode state for (B, Smax, FP8 cache or not), allocated on first use; at most one is resident."""
+def decode_state(model, B: int, Smax: int, fp8_kv: bool = False, group: int = 1) -> DecodeState:
+    """The model's decode state for (B, Smax, FP8 cache or not, siblings per prompt), allocated on first use; at most one
+    is resident."""
     eng, ar = model.engine, model.arena
-    key = (B, Smax, str(ar.device), ar.compute_dtype, fp8_kv)
+    key = (B, Smax, str(ar.device), ar.compute_dtype, fp8_kv, group)
     st = eng.decode_state
     if st is None or st.key != key:
         if eng.assisted_state is not None:           # its round graph reads the old caches: let them go
             eng.assisted_state.drop_graph()
         eng.decode_state = None                       # free the old caches before allocating the new ones
-        st = eng.decode_state = DecodeState(model.config, B, Smax, ar.device, ar.compute_dtype, fp8_kv)
+        st = eng.decode_state = DecodeState(model.config, B, Smax, ar.device, ar.compute_dtype, fp8_kv, group)
     return st
 
 
@@ -182,6 +192,44 @@ def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, fp8=N
     last = torch.arange(B, device=st.device, dtype=torch.int64) * Sp + st.lens.long() - 1
     K.embedding_fwd(last, pb.res, out=st.res)
     K.embedding_fwd(last, delta, out=st.proj)
+    _head_and_sample(cfg, ar, st, st.proj)
+
+
+def _prefill_rows(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, stride: int, fp8=None) -> None:
+    """The layers over ids [B, Sp] (compacted prompts, real lengths lens [B]) once: prompt b fills cache row b * stride,
+    and its last position's residual and delta rows go to decode rows b * stride .. b * stride + stride - 1 (st.res,
+    st.proj), ready for the final norm and the LM head."""
+    cfg = model.config
+    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    B, Sp = ids.shape
+    pb = st.prefill_buffers(B * Sp)
+    pb.ids.copy_(ids.reshape(-1))
+    delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
+                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, row_stride=stride,
+                                                            kinv=st.kinv[l], vinv=st.vinv[l]), fp8=fp8)
+    last = (torch.arange(B, device=st.device, dtype=torch.int64) * Sp + lens.long() - 1).repeat_interleave(stride)
+    K.embedding_fwd(last, pb.res, out=st.res)
+    K.embedding_fwd(last, delta, out=st.proj)
+
+
+@torch.no_grad()
+def sample_prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, fp8=None) -> None:
+    """Multi-sample prefill: ids [B, Sp] compacted prompts, lens [B]; st has B * n rows, n = st.group.  The layers run on
+    the B prompts once, into rows p * n; the fork makes rows p * n + 1 .. its children (``DK.fork``: chunk table on the
+    kernel path, whole-row copies otherwise); the LM head and the sampler then run on all B * n rows, whose state (pos,
+    lens, history) is the repeated-prompt program's.  Samples the first token of every row (st.pos ends at lens)."""
+    cfg, ar = model.config, model.arena
+    n = st.group
+    Sp = ids.shape[1]
+    lr = lens.repeat_interleave(n)
+    st.lens.copy_(lr)
+    st.pos.copy_(lr - 1)
+    st.gen.zero_()
+    st.finished.zero_()
+    m = min(Sp, st.Smax)
+    st.hist[:, :m].copy_(ids[:, :m].repeat_interleave(n, dim=0))
+    _prefill_rows(model, st, ids, lens, n, fp8)
+    DK.fork(st.kv, st.table, lens, n, inv=st.kv_inv)
     _head_and_sample(cfg, ar, st, st.proj)
 
 
@@ -274,12 +322,17 @@ def _layers(model, buf, ids: torch.Tensor, attend, fp8=None):
 
 def _one_token_layers(model, st: DecodeState, ids: torch.Tensor, table: torch.Tensor | None = None, fp8=None):
     """One token per row at st.pos: the decode layers with single-query RoPE+append and split-KV attention (through the
-    chunk table, if given), on st's bf16 or FP8 cache."""
+    chunk table, if given), on st's bf16 or FP8 cache.  Multi-sample rows (st.group > 1) attend through st's own table
+    with the sibling-grouped attention."""
     cfg = model.config
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
 
     def attend(l, qkv, att):
         DK.rope_append(qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D, kinv=st.kinv[l], vinv=st.vinv[l])
+        if st.group > 1:
+            DK.attention_grouped(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.group, st.part_o, st.part_ml, table=st.table,
+                                 kinv=st.kinv[l], vinv=st.vinv[l])
+            return
         DK.attention(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.part_o, st.part_ml, table=table, kinv=st.kinv[l],
                      vinv=st.vinv[l])
 
@@ -299,13 +352,15 @@ def _step_eager(model, st: DecodeState, fp8=None) -> None:
 def step(model, st: DecodeState, graph: bool | None = None, fp8=None) -> None:
     """One decode step: consume st.ids at st.pos, sample the next token into st.ids / st.out.  With the kernels and
     ``graph`` (default: ``ODB_CUDA_GRAPH`` != 0) the first call runs eagerly (warm-up), the second captures the step and
-    every call replays it.  ``fp8``: the model's FP8 weights (None: the arena weights)."""
+    every call replays it.  ``fp8``: the model's FP8 weights (None: the arena weights).  Multi-sample rows (st.group > 1)
+    attend through st.table; the group and the table are part of the graph key."""
     if graph is None:
         graph = _use_graph()
     if not (graph and st.kernels):
         _step_eager(model, st, fp8)
         return
-    key = (model.arena.version, model.arena.shadow.data_ptr(), _fp8_key(fp8))
+    key = (model.arena.version, model.arena.shadow.data_ptr(), st.group, st.table.data_ptr() if st.table is not None else None,
+           _fp8_key(fp8))
     if st.graph is None or st.graph_key != key:
         if st.graph_key != ("warm",) + key:
             st.graph, st.graph_key = None, ("warm",) + key
@@ -536,7 +591,8 @@ MAX_BEAMS = 8
 @dataclass
 class GenerateOutput:
     """``generate(..., return_dict_in_generate=True)``: the sequences [B * num_return_sequences, P + max_new_tokens] and,
-    with beam search, the fp32 score of each (sum of its log-probabilities / generated_len ** length_penalty)."""
+    with beam search, the fp32 score of each (sum of its log-probabilities / generated_len ** length_penalty; None
+    otherwise, multi-sample generation included)."""
     sequences: torch.Tensor
     sequences_scores: torch.Tensor | None = None
 
@@ -610,20 +666,10 @@ def beam_state(model, B: int, nb: int, K: int, max_new: int, Smax: int, fp8_kv: 
 def beam_prefill(model, bs: BeamState, ids: torch.Tensor, lens: torch.Tensor, fp8=None) -> None:
     """ids [B, Sp] compacted prompts, lens [B]: the layers run on the B prompts once and fill the beam-0 row of each
     prompt; the last position's logits go to every beam row of the prompt (st.pos ends at lens - 1)."""
-    cfg, ar = model.config, model.arena
-    st, nb = bs.dec, bs.nb
-    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-    B, Sp = ids.shape
-    pb = st.prefill_buffers(B * Sp)
-    st.pos.copy_(lens.repeat_interleave(nb) - 1)
-    pb.ids.copy_(ids.reshape(-1))
-    delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
-                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, row_stride=nb,
-                                                            kinv=st.kinv[l], vinv=st.vinv[l]), fp8=fp8)
-    last = (torch.arange(B, device=st.device, dtype=torch.int64) * Sp + lens.long() - 1).repeat_interleave(nb)
-    K.embedding_fwd(last, pb.res, out=st.res)
-    K.embedding_fwd(last, delta, out=st.proj)
-    _head(cfg, ar, st, st.proj)
+    st = bs.dec
+    st.pos.copy_(lens.repeat_interleave(bs.nb) - 1)
+    _prefill_rows(model, st, ids, lens, bs.nb, fp8)
+    _head(model.config, model.arena, st, st.proj)
 
 
 def beam_select(bs: BeamState, length_penalty: float, early_stopping: int) -> None:
@@ -686,12 +732,19 @@ def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R
 
 
 def _check_beams(num_beams, num_return_sequences, do_sample: bool, assistant_model, early_stopping, vocab_size: int,
-                 n_eos: int) -> None:
+                 n_eos: int, prompt_lookup_num_tokens=None) -> None:
     if isinstance(num_beams, bool) or not isinstance(num_beams, int) or not 1 <= num_beams <= MAX_BEAMS:
         raise ValueError(f"num_beams must be an integer in [1, {MAX_BEAMS}], got {num_beams!r}")
-    if isinstance(num_return_sequences, bool) or not isinstance(num_return_sequences, int) \
-            or not 1 <= num_return_sequences <= num_beams:
+    if isinstance(num_return_sequences, bool) or not isinstance(num_return_sequences, int) or num_return_sequences < 1:
+        raise ValueError(f"num_return_sequences must be an integer >= 1, got {num_return_sequences!r}")
+    if num_beams > 1 and num_return_sequences > num_beams:
         raise ValueError(f"num_return_sequences must be an integer in [1, num_beams={num_beams}], got {num_return_sequences!r}")
+    if num_beams == 1 and num_return_sequences > 1:
+        if not do_sample:
+            raise ValueError(f"num_return_sequences={num_return_sequences} > 1 needs do_sample=True or num_beams >= "
+                             f"num_return_sequences: greedy decoding returns one sequence per prompt")
+        if assistant_model is not None or prompt_lookup_num_tokens is not None:
+            raise ValueError("num_return_sequences > 1 cannot be combined with assistant_model or prompt_lookup_num_tokens")
     if not (early_stopping is True or early_stopping is False or early_stopping == "never"):
         raise ValueError(f"early_stopping must be True, False or \"never\", got {early_stopping!r}")
     if num_beams > 1 and do_sample:
@@ -757,7 +810,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     if assistant_model is not None:
         _check_assistant(model, assistant_model, P, max_new_tokens, num_assistant_tokens)
     eos = _eos_list(cfg.eos_token_id if eos_token_id is None else eos_token_id)
-    _check_beams(num_beams, num_return_sequences, do_sample, assistant_model, early_stopping, cfg.vocab_size, len(eos))
+    _check_beams(num_beams, num_return_sequences, do_sample, assistant_model, early_stopping, cfg.vocab_size, len(eos),
+                 prompt_lookup_num_tokens)
     proc_on = _check_processors(repetition_penalty, no_repeat_ngram_size, min_new_tokens, assistant_model)
     ngram = _check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size, assistant_model, num_beams, proc_on, P, max_new_tokens,
                           cfg.max_position_embeddings)
@@ -799,11 +853,16 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
                                      early_stopping, pad, eos, processors, fp8, fp8_kv_cache)
         out = torch.cat([ids.repeat_interleave(num_return_sequences, dim=0), new], dim=1)
         return GenerateOutput(out, scores) if return_dict_in_generate else out
-    st = decode_state(model, B, Smax, fp8_kv_cache)
+    n = num_return_sequences
+    st = decode_state(model, B * n, Smax, fp8_kv_cache, n)
 
     st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, *processors)
     st.out.fill_(pad)
-    prefill(model, st, comp, lens, fp8)
+    if n > 1:
+        sample_prefill(model, st, comp, lens, fp8)
+        ids = ids.repeat_interleave(n, dim=0)
+    else:
+        prefill(model, st, comp, lens, fp8)
     for t in range(1, max_new_tokens):
         if eos and t % FINISHED_CHECK_EVERY == 0 and bool(st.finished.all()):
             break

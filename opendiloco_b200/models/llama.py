@@ -791,8 +791,8 @@ class LlamaForCausalLM(nn.Module):
         cache chunks of their history through a chunk table.  Those kernels take num_beams * ceil(vocab_size / 1024) <= 512
         and at most 32768 positions; beyond that the step runs on the PyTorch references without a graph, with a warning.
         Raises ValueError for ``num_beams`` outside [1, 8],
-        ``num_return_sequences`` outside [1, num_beams], an unknown ``early_stopping``, or ``do_sample=True`` or
-        ``assistant_model`` with ``num_beams`` > 1.
+        ``num_return_sequences`` outside [1, num_beams] with ``num_beams`` > 1, an unknown ``early_stopping``, or
+        ``do_sample=True`` or ``assistant_model`` with ``num_beams`` > 1.
 
         Logits processors, HF's, applied in HF's order to the fp32 value of each logit (greedy and sampling: before the
         temperature, top-k and top-p warpers) or log-prob (beam search), on greedy, sampling and beam search:
@@ -806,6 +806,16 @@ class LlamaForCausalLM(nn.Module):
         log-probs, as in HF.  The settings live in device memory: changing them replays the same CUDA graphs.  Raises
         ValueError for values outside those ranges, or for any of them on together with ``assistant_model`` (not supported
         yet).
+
+        ``num_return_sequences`` n > 1 with ``do_sample=True`` and ``num_beams == 1`` draws n independent samples per
+        prompt: ``[B * n, P + max_new_tokens]``, row ``b * n + j`` is prompt b as given, then its j-th sample; token for
+        token what ``generate(input_ids.repeat_interleave(n, 0), attention_mask=attention_mask.repeat_interleave(n, 0),
+        ...)`` returns with the same other arguments.  Each prompt is prefilled once; the n rows share its complete
+        128-position cache chunks through a chunk table, and bf16-mixed CUDA models decode them on an sm_90a attention
+        that loads a shared chunk once for several rows (the cache still holds B * n rows).  Works with the warpers, EOS,
+        the logits processors, ``fp8_weights`` and ``fp8_kv_cache``.  Raises ValueError for n > 1 with
+        ``do_sample=False`` and ``num_beams == 1``, or together with ``assistant_model`` or ``prompt_lookup_num_tokens``,
+        and for an n that is not an integer >= 1.
 
         ``return_dict_in_generate=True`` returns a ``GenerateOutput`` with ``sequences`` and ``sequences_scores`` (fp32
         [B * num_return_sequences]: each hypothesis's summed log-probabilities / generated_len ** length_penalty; None

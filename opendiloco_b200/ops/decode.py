@@ -12,6 +12,10 @@ Beam search keeps ``num_beams`` rows per prompt (row ``b * num_beams + j`` is be
 chunks between them: with a chunk table (int32 ``[rows, Smax / 128]``), keys ``[128 c, 128 c + 128)`` of row r live in
 physical row ``table[r, c]`` (``attention``, ``beam_reorder``).
 
+Multi-sample generation (``generate(do_sample=True, num_return_sequences=n)``) keeps n sibling rows per prompt (row
+``p * n + j`` is sample j of prompt p) in the same chunk-table layout: after ``fork`` the siblings read the prompt's complete
+chunks from row ``p * n``, and ``attention_grouped`` loads such a shared chunk once for all of them.
+
 Assisted generation scores n tokens per row in one pass.  Its buffers are slot-major: row ``j*B + b`` is token j of row
 b, at position ``pos[b] + j`` (``rope_append_multi``, ``verify_attention``, ``accept``).
 
@@ -61,6 +65,10 @@ _lib.register_optional("odb_dec_beam_step", [c_void_p, c_void_p, c_void_p, c_int
                                              c_void_p, c_void_p, c_void_p, c_int, c_void_p])
 _lib.register_optional("odb_dec_beam_reorder", [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                                 c_void_p])
+_lib.register_optional("odb_dec_attn_group", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p,
+                                              c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int, c_void_p])
+_lib.register_optional("odb_dec_attn_group_splits", [c_int, c_int, c_int, c_int, c_int, c_int])
+_lib.register_optional("odb_dec_fork", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p])
 
 MAX_EOS = 8
 # int64 control block of the sampler: do_sample, top_k, seed, pad_token_id, n_eos, eos ids, then the logits processors'
@@ -242,6 +250,75 @@ def gather_chunks(cache: torch.Tensor, table: torch.Tensor, inv: torch.Tensor | 
     c5 = cache.view(rows, Hkv, nch, Smax // nch, D).transpose(1, 2)                   # [rows, nch, Hkv, 128, D]
     g = c5[table.long().to(cache.device), torch.arange(nch, device=cache.device)[None, :]]
     return g.transpose(1, 2).reshape(rows, Hkv, Smax, D)
+
+
+# ------------------------------------------------------------------------------------------------ multi-sample generation
+def attention_grouped(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, pos: torch.Tensor, out: torch.Tensor, Hq: int, Hkv: int,
+                      D: int, group: int, part_o: torch.Tensor | None = None, part_ml: torch.Tensor | None = None,
+                      table: torch.Tensor | None = None, kinv: torch.Tensor | None = None, vinv: torch.Tensor | None = None,
+                      splits: int = 0) -> torch.Tensor:
+    """``attention`` over rows of ``group`` siblings (rows p * group .. p * group + group - 1 belong to prompt p), through
+    the chunk table: the kernel loads a chunk that siblings' table entries share once per CTA and computes every
+    sibling's partial from it with ``attention``'s arithmetic, so out and the partials are bit-identical to ``attention``
+    with the same table.  Siblings may sit at different positions.  ``splits``: 0 lets the launcher choose how many CTAs
+    share one prompt's siblings (``attn_group_splits``; with an FP8 cache at G = 1 it runs ``attention``'s kernel through
+    the table, which measured faster there); a positive value forces the grouped kernel with that split (tests).  The reference is
+    ``attention``'s (the table gather; table None reads every row's own cache)."""
+    rows = q.shape[0]
+    Smax = kc.shape[2]
+    if usable(q, D, Hq, Hkv):
+        assert table is not None and table.dtype == torch.int32 and table.is_contiguous() and table.shape == (rows, attn_chunks(Smax))
+        assert q.stride(1) == 1 and out.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous() and pos.dtype == torch.int32
+        assert group >= 1 and rows % group == 0 and Smax % 128 == 0 and splits >= 0
+        _check_fp8(kc, vc, kinv, vinv)
+        _lib.check(_lib.cuda_lib().odb_dec_attn_group(q.data_ptr(), q.stride(0), kc.data_ptr(), vc.data_ptr(), pos.data_ptr(),
+                                                      part_o.data_ptr(), part_ml.data_ptr(), out.data_ptr(), out.stride(0),
+                                                      table.data_ptr(), rows, group, Hq, Hkv, Smax, 1.0 / math.sqrt(D), _ptr(kinv),
+                                                      _ptr(vinv), splits, _lib.stream_ptr(q)), "dec_attn_group")
+        _lib.count_launch(2)
+        return out
+    return attention(q, kc, vc, pos, out, Hq, Hkv, D, part_o, part_ml, table=table, kinv=kinv, vinv=vinv)
+
+
+def attn_group_splits(rows: int, group: int, Hq: int, Hkv: int, Smax: int, fp8_kv: bool = False) -> int:
+    """How many CTAs ``attention_grouped`` gives the siblings of one prompt at these shapes: enough that each CTA runs at
+    most max(1, 4 / G) siblings (G = Hq / Hkv), and more, up to ``group``, while the (chunk, kv head, prompt, split) grid
+    would not fill one wave of resident CTAs on the current device; 0 for an FP8 cache at G = 1, where ``attention``'s kernel
+    runs through the table instead.  Needs the kernels and a device."""
+    s = int(_lib.cuda_lib().odb_dec_attn_group_splits(rows, group, Hq, Hkv, Smax, int(fp8_kv)))
+    if s < 0:
+        raise RuntimeError(f"odb_dec_attn_group_splits failed with code {s}")
+    return s
+
+
+def fork(kv: torch.Tensor, table: torch.Tensor | None, lens: torch.Tensor, group: int, inv: torch.Tensor | None = None) -> None:
+    """After prompt p was prefilled into row p * group (positions [0, lens[p]), lens int32 [P]), make rows p * group + 1 ..
+    p * group + group - 1 its children.  kv: every layer's K and V, [L, 2, P * group, Hkv, Smax, D]; inv: with an FP8 cache
+    (e4m3 kv), its fp32 inv [L, 2, P * group, Hkv, Smax].
+
+    With a chunk table (the kernel path; int32 [P * group, Smax / 128], fully rewritten) the children take row p * group's
+    entries for the complete chunks c < lens[p] // 128 and get a copy of the partial chunk [128 * (lens[p] // 128), lens[p])
+    (with its inv) in their own row; every other entry names the row itself.  Without one, ``fork_reference`` copies whole
+    rows."""
+    if table is None:
+        fork_reference(kv, group, inv)
+        return
+    L, two, rows, Hkv, Smax, D = kv.shape
+    assert kv.is_cuda and kv.dtype == (torch.bfloat16 if inv is None else E4M3) and kv.is_contiguous() and two == 2 and D == 64
+    assert inv is None or (inv.dtype == torch.float32 and inv.is_contiguous() and inv.shape == kv.shape[:-1])
+    assert group >= 1 and rows % group == 0 and lens.shape == (rows // group,) and lens.dtype == torch.int32 and lens.is_contiguous()
+    assert table.shape == (rows, Smax // 128) and table.dtype == torch.int32 and table.is_contiguous() and Smax % 128 == 0
+    _lib.check(_lib.cuda_lib().odb_dec_fork(kv.data_ptr(), table.data_ptr(), lens.data_ptr(), rows // group, group, L, Hkv, Smax,
+                                            _ptr(inv), _lib.stream_ptr(kv)), "dec_fork")
+    _lib.count_launch()
+
+
+def fork_reference(kv: torch.Tensor, group: int, inv: torch.Tensor | None = None) -> None:
+    """Physical fork: every row of a group becomes a copy of the group's first row, in every layer's K and V (and an FP8
+    cache's inv).  The chunk table of ``fork`` must read like this up to each prompt's length."""
+    rows = kv.shape[2]
+    parent = torch.arange(rows, dtype=torch.int32) // group * group
+    beam_reorder_reference(kv, parent, inv)
 
 
 # ------------------------------------------------------------------------------------------------ assisted generation

@@ -108,7 +108,8 @@ def main(argv=None) -> None:
     ap.add_argument("--length-penalty", type=float, default=1.0, help="beam search: hypothesis score = sum log p / length ** this")
     ap.add_argument("--early-stopping", choices=["true", "false", "never"], default="false",
                     help="beam search: HF's early_stopping (true, false or never)")
-    ap.add_argument("--num-return-sequences", type=int, default=1, help="beam search: hypotheses returned per prompt")
+    ap.add_argument("--num-return-sequences", type=int, default=1,
+                    help="beam search: hypotheses returned per prompt; with --do-sample: independent samples per prompt")
     ap.add_argument("--repetition-penalty", type=float, default=1.0, help="HF's repetition penalty on the row's history (1.0: off)")
     ap.add_argument("--no-repeat-ngram-size", type=int, default=0, help="no n-gram of this size occurs twice in a row (0: off)")
     ap.add_argument("--min-new-tokens", type=int, default=0, help="EOS is forbidden until this many new tokens (0: off)")
