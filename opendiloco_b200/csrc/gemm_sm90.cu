@@ -31,8 +31,9 @@
 //   kRoPE    : C is the packed qkv buffer; 64-column chunks are heads; chunks below `rope_cols` are rotated with the
 //              HF rotate-half convention using fp32 cos/sin tables (position = row % S)
 //   kLCEFwd  : fused linear-cross-entropy forward.  The accumulator holds a tile of LM-head logits z; the epilogue turns
-//              it into shifted exponentials e = exp(z - c_row) (c_row = the row's label logit, so sum_v e >= 1 and
-//              loss_row = log sum_v e), writes the tile's row sums into one partial plane per 256-column tile and
+//              it into shifted exponentials e = exp(z - c_row) (c_row = the row's label logit + 58 ln 2, so the label's
+//              e is exactly 2^-58 in bf16 and loss_row = log sum_v e + 58 ln 2; csrc/lce.cu), writes the tile's row sums
+//              into one partial plane per 256-column tile and
 //              (training only) stores bf16(e).  Logits are never written.
 //   kLCEdX   : dgrad of the LM head on the shifted exponentials: out = rowscale * acc - g * W[label]
 //   kLCEScore: scoring (evaluation) statistics of the LM head, per row and 256-column plane: the plane maximum m, its lowest
@@ -109,7 +110,7 @@ struct Params {
   const float* sin_t;
   int ks1, ks2;              // A split along K (A_MN = false) or along M (A_MN = true) into up to three tensors:
                              // blocks [0,ks1) from A, [ks1,ks2) from A1, [ks2,..) from A2 (0/0 = single tensor)
-  const float* row_shift;    // kLCEFwd: c_row [M] (label logit; 0 for ignored rows)
+  const float* row_shift;    // kLCEFwd: c_row [M] (label logit + 58 ln 2; 0 for ignored rows)
   float* partials;           // kLCEFwd: [num_n (+ num_n when want_sumsq)][M] partial row sums of exp(z - c)
   int want_sumsq;            // kLCEFwd: also accumulate sum z^2 into the second half of partials
   int store;                 // kLCEFwd: 1 = write bf16(e) to C (training) ; 0 = statistics only (evaluation)
@@ -551,7 +552,8 @@ __device__ __forceinline__ void mma_and_epilogue(const Params& p, const CUtensor
           for (int e = 0; e < 2; ++e) {
             float& v = acc[4 * i + 2 * h + e];
             const bool ok = col + e < p.N;
-            // clamp: a row whose label is > 69 nats below its best logit would overflow the fp32 row sum otherwise
+            // clamp at 2^100: a row whose label is > (100 + 58) ln 2 = 109.5 nats below its best logit saturates here
+            // instead of overflowing the fp32 row sum
             float x;
             asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(x) : "f"(fminf(fmaf(v, L2E, -shift[h]), 100.f)));
             psq[h] += ok ? v * v : 0.f;

@@ -207,16 +207,22 @@ ODB_EXPORT int odb_ce_fwd(const void* logits, const void* labels, int rows, int 
 //
 //   lce_prep       labels -> HF-shifted labels (position s predicts token s+1, last position ignored), n_valid,
 //                  gscale = loss_scale / max(n_valid, 1), loss_sum = 0             (replaces eight ATen launches)
-//   lce_label_dot  c[t] = x[t] . W[label[t]] + 40  (fp32)  - the shift of the exponentials, known BEFORE the GEMM, which is
-//                  what lets the GEMM epilogue emit exp(z - c) directly instead of logits: the label term of
-//                  sum_v exp(z_v - c) is exp(-40), so the row sum can never underflow, and loss_t = log(sum) + 40
+//   lce_label_dot  c[t] = x[t] . W[label[t]] + 58 ln 2  (fp32)  - the shift of the exponentials, known BEFORE the GEMM,
+//                  which is what lets the GEMM epilogue emit exp(z - c) directly instead of logits: the label term of
+//                  sum_v exp(z_v - c) is 2^-58, so the row sum can never underflow, and loss_t = log(sum) + 58 ln 2
 //   lce_finalize   per row: S = sum of the partial planes ; loss += log S ; rowscale = gscale / S ;
 //                  xs[t] = bf16(rowscale * x[t])   (B operand of the dW GEMM: dW = E^T xs - scatter)
-//                  dW[label[t]] -= gscale * x[t]   (the one-hot term of softmax - onehot, a vector red.add per row)
-// The shift is placed kLceShiftOffset nats ABOVE the label logit: the fp32 row sum then has head-room for best logits up to
-// ~69 + 40 = 109 nats above the label (the GEMM epilogue clamps the exponent at 2^100), while the label term itself,
-// exp(-40) = 4e-18, keeps the sum far from underflow.  loss_t = log(sum_v exp(z_v - c_t)) + kLceShiftOffset.
-constexpr float kLceShiftOffset = 40.f;
+//                  dW[label[t]] += -gscale * x[t] + 2^-58 (rowscale * x[t] - xs[t])   (the one-hot term, a vector red.add
+//                  per row, and the bf16 rounding of xs on the label's own product E_y xs[t], see below)
+// The shift is placed kLceShiftOffset = 58 ln 2 nats ABOVE the label logit: the fp32 row sum then has head-room for best
+// logits up to (100 + 58) ln 2 = 109.5 nats above the label (the GEMM epilogue clamps the exponent at 2^100), while the
+// label term keeps the sum far from underflow.  loss_t = log(sum_v exp(z_v - c_t)) + kLceShiftOffset.
+// The offset is a whole number of octaves so that the label's exponential is an exact power of two: the GEMM's z_y differs
+// from the label dot by ~1e-5 nats, far below half a bf16 ulp, so the stored E_y is exactly 2^-58 and the gradient GEMMs see
+// rowscale * E_y - gscale = gscale (p_y - 1) without a rounding bias.  (With an offset of 40, bf16(exp(-40)) is 0.17% above
+// exp(-40) on every row: the label's gradient changed sign once p_y > 0.9983, pushing confident predictions down.)
+constexpr float kLceShiftOffset = 40.2025365f;          // 58 ln 2
+constexpr float kLceLabelExp = 3.4694470e-18f;          // 2^-58: the label's exponential, exact in bf16
 
 __global__ void __launch_bounds__(1024) lce_prep_kernel(const long long* __restrict__ src, long long* __restrict__ dst, int B, int S,
                                                         float loss_scale, float* __restrict__ n_valid,
@@ -330,10 +336,18 @@ __global__ void __launch_bounds__(256) lce_finalize_kernel(const float* __restri
       unpack8(ld_nc_v4(xr + k), f);
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = f[j] * rs;
-      st_na_v4(xo + k, pack8(o));
+      const uint4 ob = pack8(o);
+      st_na_v4(xo + k, ob);
       if (dwr) {
-        red_add_f4(dwr + k * 8, make_float4(-gscale * f[0], -gscale * f[1], -gscale * f[2], -gscale * f[3]));
-        red_add_f4(dwr + k * 8 + 4, make_float4(-gscale * f[4], -gscale * f[5], -gscale * f[6], -gscale * f[7]));
+        // The dW GEMM adds E_y * xs[t] = 2^-58 bf16(rowscale x) to this row; -gscale x cancels most of it when p_y -> 1,
+        // which would leave the bf16 rounding of xs (2^-9 of p_y gscale x) as the result.  Adding 2^-58 (rowscale x - xs)
+        // here makes the label's own term exact to fp32: gscale (p_y - 1) x.
+        float r[8];
+        unpack8(ob, r);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) r[j] = fmaf(kLceLabelExp, o[j] - r[j], -gscale * f[j]);
+        red_add_f4(dwr + k * 8, make_float4(r[0], r[1], r[2], r[3]));
+        red_add_f4(dwr + k * 8 + 4, make_float4(r[4], r[5], r[6], r[7]));
       }
     }
   }

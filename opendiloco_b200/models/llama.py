@@ -331,15 +331,17 @@ class LlamaEngine:
     def _head_loss_fused(self, ws: _Workspace, w_lm: torch.Tensor, g_lm: torch.Tensor | None, want_norm: bool) -> None:
         """Fused linear-cross-entropy on the wgmma GEMM (SURVEY K7).  Per chunk of rows:
 
-          c_t   = x_t . W[y_t]                               (lce_label_dot: the label logit, 2 x T x h bytes)
+          c_t   = x_t . W[y_t] + 58 ln 2                     (lce_label_dot: the label logit, 2 x T x h bytes)
           E     = exp(X W^T - c)   + partial row sums        (ONE GEMM, epilogue in registers; bf16 E only when training)
-          S_t, loss_t = log S_t, rowscale_t = gscale / S_t, xs = rowscale * x, dW[y_t] -= gscale x_t     (lce_finalize)
+          S_t, loss_t = log S_t + 58 ln 2, rowscale_t = gscale / S_t, xs = rowscale * x, dW[y_t] -= gscale x_t  (lce_finalize)
           dX    = rowscale * (E W) - gscale W[y]             (dgrad GEMM, W read MN-major, normaliser + one-hot in the epilogue)
           dW   += E^T xs                                     (weight-gradient GEMM)
 
         softmax - onehot is never formed and there is no pass over a [T, V] tensor outside the three GEMMs: the shift c is
         known before the GEMM, so the exponentials can be emitted by its epilogue, and the per-row normaliser moves to
         the fp32 side of the two gradient GEMMs.  In evaluation (g_lm is None) nothing of size [T, V] is written at all.
+        The shift puts the label's exponential at exactly 2^-58 (a bf16 value), so rowscale * E_y - gscale is gscale (p_y - 1)
+        without a rounding bias even for a confidently predicted label (tests/test_loss_head_oracle_gpu.py).
         """
         T, h = ws.T, self.cfg.hidden_size
         V = w_lm.shape[0]

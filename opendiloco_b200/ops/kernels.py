@@ -261,8 +261,8 @@ def lce_prep(labels_in: torch.Tensor, labels_out: torch.Tensor, B: int, S: int, 
 
 
 def lce_label_dot(x: torch.Tensor, w: torch.Tensor, labels: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
-    """out[t] = x[t] . w[labels[t]] + 40 in fp32 (0 for ignored rows): the shift of the exponentials of the fused LCE
-    (40 nats of head-room above the label logit, see csrc/lce.cu)."""
+    """out[t] = x[t] . w[labels[t]] + 58 ln 2 in fp32 (0 for ignored rows): the shift of the exponentials of the fused LCE
+    (58 ln 2 nats above the label logit, so the label's exponential is exactly 2^-58; see csrc/lce.cu)."""
     T, h = x.shape
     if x.is_cuda and x.dtype == BF16:
         _lib.check(_lib.cuda_lib().odb_lce_label_dot(_p(x), x.stride(0), _p(w), w.stride(0), _p(labels), _p(out), T, h,
@@ -270,7 +270,7 @@ def lce_label_dot(x: torch.Tensor, w: torch.Tensor, labels: torch.Tensor, out: t
         _lib.count_launch()
     else:
         safe = labels.clamp(min=0)
-        out.copy_(((x.float() * w.float()[safe]).sum(-1) + 40.0) * (labels >= 0))
+        out.copy_(((x.float() * w.float()[safe]).sum(-1) + 58 * math.log(2.0)) * (labels >= 0))
     return out
 
 

@@ -2,6 +2,8 @@
 and ``beam_step_reference``, the sampling law on processed logits, the whole program against the references, graph
 replay, and properties of ``generate`` on a 150m-shaped model."""
 import re
+import subprocess
+import sys
 from pathlib import Path
 
 import numpy as np
@@ -422,6 +424,10 @@ def _gpu_kernels(fn):
 
 
 def test_steps_with_processors_launch_only_our_kernels():
+    _in_fresh_process("_steps_with_processors_launch_only_our_kernels")
+
+
+def _steps_with_processors_launch_only_our_kernels():
     cfg = _layer_cfg("1b_gqa_layer")
     model = LlamaForCausalLM(cfg, device="cuda", precision="bf16-mixed", seed=0)
     ours = _our_kernel_names()
@@ -477,3 +483,13 @@ def test_processors_do_not_disturb_training_or_decode_state():
     assert a.engine._graphs[key]["graph"] is g_obj
     for u, v in zip(la, lb):
         assert abs(u - v) <= 1e-5 * abs(v), (la, lb)
+
+
+def _in_fresh_process(fn: str) -> None:
+    """Run ``fn`` of this module in a new Python process and fail with its traceback if it fails.  Used by the tests that
+    read kernel names from the CUDA profiler: late in a long pytest process the profiler intermittently records no GPU
+    activity at all, while a fresh process records every launch."""
+    here = Path(__file__).resolve()
+    code = f"import sys; sys.path[:0] = [{str(here.parents[1])!r}, {str(here.parent)!r}]; import {here.stem}; {here.stem}.{fn}()"
+    res = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd=here.parents[1], timeout=900)
+    assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-6000:]
