@@ -1,10 +1,12 @@
 // Autoregressive decode kernels for sm_90a (bf16, head_dim 64, MHA + GQA): the pieces of a KV-cached generation step that
 // the training kernels do not cover.
 //
-//   odb_dec_rope_append   one new token per row: rotate q|k at the row's own position pos[b] (read from device memory, so a
-//                         captured graph stays valid at every step), write k and v into the layer's cache at (b, pos[b])
+//   odb_dec_rope_append   n new tokens per row (n = 1: the decode step; n > 1: an assisted round's verify pass): rotate q|k
+//                         of token j at the row's own position pos[b] + j (read from device memory, so a captured graph stays
+//                         valid at every step), write k and v into the layer's cache at (b, pos[b] + j)
 //   odb_dec_kv_fill       prefill: copy the (already rotated) k|v columns of the packed qkv rows into the cache
-//   odb_dec_attn          split-KV decode attention (flash-decoding) + a combine kernel
+//   odb_dec_attn          split-KV decode attention (flash-decoding) + the combine kernel that every split-KV attention
+//                         here (decode, grouped, verify) ends with
 //   odb_dec_sample        greedy / temperature + top-k + top-p sampler, one CTA per row, with HF's repetition penalty, n-gram
 //                         ban and min-new-tokens over the row's device-side token history when the control blocks ask
 //   odb_dec_accept        assisted generation / prompt lookup: speculative acceptance of one round's proposals
@@ -27,6 +29,7 @@
 
 #include <algorithm>
 #include <climits>
+#include <type_traits>
 
 #include "common.cuh"
 #include "fp8_rows.cuh"
@@ -109,25 +112,13 @@ __device__ __forceinline__ void rope_append_token(__nv_bfloat16* __restrict__ ro
   }
 }
 
-// grid B, block 256: one new token per row at the row's own position pos[b] (read from device memory, so a captured graph
-// stays valid at every step).
+// grid (B, n), block 256: n tokens per row, slot-major rows (row j*B + b is token j of sequence b, at position pos[b] + j);
+// n = 1 is the decode step.  pos is read from device memory, so a captured graph stays valid at every step.
 template <typename T>
 __global__ void __launch_bounds__(256)
 rope_append_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const float* __restrict__ cos_t, const float* __restrict__ sin_t,
                    const int* __restrict__ pos, T* __restrict__ kc, T* __restrict__ vc, int Hq, int Hkv, int Smax,
                    float* __restrict__ kinv, float* __restrict__ vinv) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int b = blockIdx.x;
-  rope_append_token(qkv + (long long)b * ld, pos[b], b, cos_t, sin_t, kc, vc, Hq, Hkv, Smax, kinv, vinv);
-}
-
-// grid (B, n), block 256: n tokens per row, slot-major rows (row j*B + b is token j of sequence b, at position pos[b] + j).
-template <typename T>
-__global__ void __launch_bounds__(256)
-rope_append_multi_kernel(__nv_bfloat16* __restrict__ qkv, long long ld, const float* __restrict__ cos_t,
-                         const float* __restrict__ sin_t, const int* __restrict__ pos, T* __restrict__ kc, T* __restrict__ vc, int Hq,
-                         int Hkv, int Smax, float* __restrict__ kinv, float* __restrict__ vinv) {
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x, j = blockIdx.y, B = gridDim.x;
@@ -423,15 +414,19 @@ decode_attn_group_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, con
   }
 }
 
-// grid (Hq, B), block 64: merge the chunks of (b, h) and write out[b, h*64 + d] (token-major: the o-proj GEMM's A operand).
+// The combine of every split-KV attention here.  grid (Hq, n*B), block 64: merge the splits of query row r = j*B + b
+// (slot-major, at position pos[b] + j; n = 1 for the decode kernels), head h, and write out[r, h*64 + d] (token-major: the
+// o-proj GEMM's A operand).  Split s covers keys [s*span, (s+1)*span) and has cap slots per (row, head); the splits holding
+// keys <= pos[b] + j each hold key s*span, so their max is finite.
 __global__ void __launch_bounds__(64)
-decode_combine_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml, const int* __restrict__ pos,
-                      __nv_bfloat16* __restrict__ out, long long ldo, int nchunks) {
+combine_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml, const int* __restrict__ pos,
+               __nv_bfloat16* __restrict__ out, long long ldo, int cap, int span, int B) {
   pdl_launch_dependents();
   pdl_wait();
-  const int h = blockIdx.x, b = blockIdx.y, Hq = gridDim.x, d = threadIdx.x;
-  const int used = ceil_div(pos[b] + 1, CH);
-  const long long base = ((long long)b * Hq + h) * nchunks;
+  const int h = blockIdx.x, r = blockIdx.y, Hq = gridDim.x, d = threadIdx.x;
+  const int b = r % B, j = r / B;
+  const int used = ceil_div(pos[b] + j + 1, span);
+  const long long base = ((long long)r * Hq + h) * cap;
   float M = -INFINITY;
   for (int c = 0; c < used; ++c) M = fmaxf(M, part_ml[(base + c) * 2]);
   float L = 0.f, acc = 0.f;
@@ -440,7 +435,7 @@ decode_combine_kernel(const float* __restrict__ part_o, const float* __restrict_
     L = fmaf(part_ml[(base + c) * 2 + 1], w, L);
     acc = fmaf(part_o[(base + c) * D + d], w, acc);
   }
-  out[(long long)b * ldo + h * D + d] = __float2bfloat16_rn(acc / L);
+  out[(long long)r * ldo + h * D + d] = __float2bfloat16_rn(acc / L);
 }
 
 // ------------------------------------------------------------------------------------------------ sampler
@@ -746,7 +741,7 @@ sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, con
 //               VSTAGES-deep full / empty mbarrier ring
 //   warps 0-3   one warpgroup: Q gathered into shared memory in the same swizzled layout, S = Q K^T on wgmma m64n64k16,
 //               causal mask + online softmax (exp2 domain) on the accumulators, O += P V with P as the register operand
-// Writes the unnormalised partial output and its (max, sum) per query row; verify_combine_kernel merges the splits.
+// Writes the unnormalised partial output and its (max, sum) per query row; combine_kernel merges the splits.
 //
 // FP8 cache (KV8): warp 4 bulk-copies each tile's e4m3 K and V [64 keys x 64 bytes] and their two inv runs into an FP8
 // stage of the ring; the warpgroup converts them (q * inv, exact in bf16) into ONE pair of bf16 K | V tiles in the same
@@ -943,28 +938,6 @@ verify_attn_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_cons
       part_ml[base * 2 + 1] = l[r];
     }
   }
-}
-
-// grid (Hq, n*B), block 64: merge the splits of query row r = j*B + b, head h (splits holding keys <= pos[b] + j; each
-// of them holds key s*span, so its max is finite).
-__global__ void __launch_bounds__(64)
-verify_combine_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml, const int* __restrict__ pos,
-                      __nv_bfloat16* __restrict__ out, long long ldo, int cap, int span, int B) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int h = blockIdx.x, r = blockIdx.y, Hq = gridDim.x, d = threadIdx.x;
-  const int b = r % B, j = r / B;
-  const int used = ceil_div(pos[b] + j + 1, span);
-  const long long base = ((long long)r * Hq + h) * cap;
-  float M = -INFINITY;
-  for (int c = 0; c < used; ++c) M = fmaxf(M, part_ml[(base + c) * 2]);
-  float L = 0.f, acc = 0.f;
-  for (int c = 0; c < used; ++c) {
-    const float w = exp2f(part_ml[(base + c) * 2] - M);
-    L = fmaf(part_ml[(base + c) * 2 + 1], w, L);
-    acc = fmaf(part_o[(base + c) * D + d], w, acc);
-  }
-  out[(long long)r * ldo + h * D + d] = __float2bfloat16_rn(acc / L);
 }
 
 // ------------------------------------------------------------------------------------------------ acceptance
@@ -1542,6 +1515,24 @@ fork_kernel(T* __restrict__ kv, int* __restrict__ table, const int* __restrict__
     }
 }
 
+// The GQA-group dispatch of the attention launchers: f(std::integral_constant<int, G>{}) for G = Hq / Hkv.
+template <class F>
+int with_group(int G, F&& f) {
+  switch (G) {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 8: return f(std::integral_constant<int, 8>{});
+    default: return -2;                          // GQA groups of 1, 2, 4 or 8 query heads
+  }
+}
+
+// The cache-type dispatch: f(T{}) with T = uint8_t for an FP8 cache (e4m3 bytes), __nv_bfloat16 for a bf16 one.
+template <class F>
+int with_cache(bool kv8, F&& f) {
+  return kv8 ? f(uint8_t{}) : f(__nv_bfloat16{});
+}
+
 template <int G, typename T>
 int launch_attn(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml, void* out,
                 long long ldo, const void* table, int B, int Hkv, int Smax, float scale, const void* kinv, const void* vinv,
@@ -1558,20 +1549,10 @@ int launch_attn(const void* q, long long ldq, const void* kc, const void* vc, co
              (const T*)kc, (const T*)vc, (const int*)pos, (float*)part_o, (float*)part_ml, (const int*)table, Hkv, Smax, nchunks,
              scale * 1.4426950408889634f, (const float*)kinv, (const float*)vinv);
   ODB_CHECK_LAST();
-  launch_pdl(decode_combine_kernel, dim3(Hkv * G, B), dim3(D), 0, st, (const float*)part_o, (const float*)part_ml, (const int*)pos,
-             (__nv_bfloat16*)out, ldo, nchunks);
+  launch_pdl(combine_kernel, dim3(Hkv * G, B), dim3(D), 0, st, (const float*)part_o, (const float*)part_ml, (const int*)pos,
+             (__nv_bfloat16*)out, ldo, nchunks, CH, B);
   ODB_CHECK_LAST();
   return 0;
-}
-
-template <int G>
-int launch_attn_t(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml, void* out,
-                  long long ldo, const void* table, int B, int Hkv, int Smax, float scale, const void* kinv, const void* vinv,
-                  cudaStream_t st) {
-  if (kinv != nullptr)
-    return launch_attn<G, uint8_t>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, scale, kinv, vinv, st);
-  return launch_attn<G, __nv_bfloat16>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, scale, nullptr, nullptr,
-                                       st);
 }
 
 // Siblings per CTA of decode_attn_group_kernel.  A CTA runs its siblings one after the other, so fewer siblings per CTA
@@ -1614,26 +1595,10 @@ int launch_attn_group(const void* q, long long ldq, const void* kc, const void* 
              ldq, (const T*)kc, (const T*)vc, (const int*)pos, (float*)part_o, (float*)part_ml, (const int*)table, Hkv, Smax, nchunks,
              scale * 1.4426950408889634f, (const float*)kinv, (const float*)vinv, ngrp, splits);
   ODB_CHECK_LAST();
-  launch_pdl(decode_combine_kernel, dim3(Hkv * G, rows), dim3(D), 0, st, (const float*)part_o, (const float*)part_ml, (const int*)pos,
-             (__nv_bfloat16*)out, ldo, nchunks);
+  launch_pdl(combine_kernel, dim3(Hkv * G, rows), dim3(D), 0, st, (const float*)part_o, (const float*)part_ml, (const int*)pos,
+             (__nv_bfloat16*)out, ldo, nchunks, CH, rows);
   ODB_CHECK_LAST();
   return 0;
-}
-
-template <int G>
-int launch_attn_group_t(const void* q, long long ldq, const void* kc, const void* vc, const void* pos, void* part_o, void* part_ml,
-                        void* out, long long ldo, const void* table, int rows, int ngrp, int Hkv, int Smax, float scale,
-                        const void* kinv, const void* vinv, int splits, cudaStream_t st) {
-  if (kinv != nullptr)
-    return launch_attn_group<G, uint8_t>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, scale, kinv,
-                                         vinv, splits, st);
-  return launch_attn_group<G, __nv_bfloat16>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, scale,
-                                             nullptr, nullptr, splits, st);
-}
-
-template <int G>
-int group_splits_t(bool kv8, int P, int ngrp, int Hkv, int nchunks) {
-  return kv8 ? attn_group_splits<G, uint8_t>(P, ngrp, Hkv, nchunks) : attn_group_splits<G, __nv_bfloat16>(P, ngrp, Hkv, nchunks);
 }
 
 template <typename T>
@@ -1659,33 +1624,31 @@ int launch_beam_reorder(void* kv, void* inv, void* table, const void* parent, co
 // Every cache argument below is either bf16 (kinv = vinv = nullptr) or an FP8 cache: e4m3 bytes of the same shape plus fp32
 // kinv / vinv [B, Hkv, Smax] (16-byte aligned, Smax a multiple of 128), written and read as described at the top of the file.
 
-// qkv [B, ld] bf16 (one token per row); cos/sin fp32 [max_pos, 32]; pos int32 [B]; kc/vc [B, Hkv, Smax, 64]
+// qkv [n*B, ld] bf16, slot-major (row j*B + b: token j of sequence b, at position pos[b] + j; n = 1: one token per row);
+// cos/sin fp32 [max_pos, 32]; pos int32 [B]; kc/vc [B, Hkv, Smax, 64]
 ODB_EXPORT int odb_dec_rope_append(void* qkv, long long ld, const void* cos_t, const void* sin_t, const void* pos, void* kc, void* vc,
-                                   int B, int Hq, int Hkv, int Smax, void* kinv, void* vinv, cudaStream_t st) {
-  if (ld % 2) return -1;
-  if (kinv != nullptr)
-    launch_pdl(dec::rope_append_kernel<uint8_t>, dim3(B), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t,
-               (const float*)sin_t, (const int*)pos, (uint8_t*)kc, (uint8_t*)vc, Hq, Hkv, Smax, (float*)kinv, (float*)vinv);
-  else
-    launch_pdl(dec::rope_append_kernel<__nv_bfloat16>, dim3(B), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t,
-               (const float*)sin_t, (const int*)pos, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, Hq, Hkv, Smax, (float*)nullptr,
-               (float*)nullptr);
-  ODB_CHECK_LAST();
-  return 0;
+                                   int B, int n, int Hq, int Hkv, int Smax, void* kinv, void* vinv, cudaStream_t st) {
+  if (ld % 2 || n < 1) return -1;
+  return dec::with_cache(kinv != nullptr, [&](auto t) {
+    using T = decltype(t);
+    launch_pdl(dec::rope_append_kernel<T>, dim3(B, n), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t,
+               (const float*)sin_t, (const int*)pos, (T*)kc, (T*)vc, Hq, Hkv, Smax, (float*)kinv, (float*)vinv);
+    ODB_CHECK_LAST();
+    return 0;
+  });
 }
 
 // qkv [B*Sp, ld] bf16 (rotated prefill projections); len int32 [B]: rows s < len[b] are copied into cache row b * row_stride
 ODB_EXPORT int odb_dec_kv_fill(const void* qkv, long long ld, const void* len, void* kc, void* vc, int B, int Sp, int Hq, int Hkv,
                                int Smax, int row_stride, void* kinv, void* vinv, cudaStream_t st) {
   if (ld % 8 || row_stride < 1) return -1;
-  if (kinv != nullptr)
-    launch_pdl(dec::kv_fill_kernel<uint8_t>, dim3(Sp, B), dim3(128), 0, st, (const __nv_bfloat16*)qkv, ld, (const int*)len,
-               (uint8_t*)kc, (uint8_t*)vc, Sp, Hq, Hkv, Smax, row_stride, (float*)kinv, (float*)vinv);
-  else
-    launch_pdl(dec::kv_fill_kernel<__nv_bfloat16>, dim3(Sp, B), dim3(128), 0, st, (const __nv_bfloat16*)qkv, ld, (const int*)len,
-               (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, Sp, Hq, Hkv, Smax, row_stride, (float*)nullptr, (float*)nullptr);
-  ODB_CHECK_LAST();
-  return 0;
+  return dec::with_cache(kinv != nullptr, [&](auto t) {
+    using T = decltype(t);
+    launch_pdl(dec::kv_fill_kernel<T>, dim3(Sp, B), dim3(128), 0, st, (const __nv_bfloat16*)qkv, ld, (const int*)len, (T*)kc, (T*)vc,
+               Sp, Hq, Hkv, Smax, row_stride, (float*)kinv, (float*)vinv);
+    ODB_CHECK_LAST();
+    return 0;
+  });
 }
 
 // Number of key chunks of the split-KV attention for a cache of Smax positions (sizes the partial buffers).
@@ -1698,14 +1661,12 @@ ODB_EXPORT int odb_dec_attn(const void* q, long long ldq, const void* kc, const 
                             void* out, long long ldo, const void* table, int B, int Hq, int Hkv, int Smax, float softmax_scale,
                             const void* kinv, const void* vinv, cudaStream_t st) {
   if (Hq % Hkv || ldq % 8 || (kinv != nullptr && Smax % dec::CH)) return -1;
-  const float sc = softmax_scale;
-  switch (Hq / Hkv) {
-    case 1: return dec::launch_attn_t<1>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, sc, kinv, vinv, st);
-    case 2: return dec::launch_attn_t<2>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, sc, kinv, vinv, st);
-    case 4: return dec::launch_attn_t<4>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, sc, kinv, vinv, st);
-    case 8: return dec::launch_attn_t<8>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax, sc, kinv, vinv, st);
-    default: return -2;                          // GQA groups of 1, 2, 4 or 8 query heads
-  }
+  return dec::with_group(Hq / Hkv, [&](auto g) {
+    return dec::with_cache(kinv != nullptr, [&](auto t) {
+      return dec::launch_attn<decltype(g)::value, decltype(t)>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, B, Hkv, Smax,
+                                                               softmax_scale, kinv, vinv, st);
+    });
+  });
 }
 
 // Multi-sample decode attention: as odb_dec_attn with a chunk table (required), over rows = P * ngrp rows where rows
@@ -1717,20 +1678,14 @@ ODB_EXPORT int odb_dec_attn_group(const void* q, long long ldq, const void* kc, 
                                   void* part_ml, void* out, long long ldo, const void* table, int rows, int ngrp, int Hq, int Hkv,
                                   int Smax, float softmax_scale, const void* kinv, const void* vinv, int splits, cudaStream_t st) {
   if (Hq % Hkv || ldq % 8 || ngrp < 1 || rows % ngrp || table == nullptr || (kinv != nullptr && Smax % dec::CH)) return -1;
-  const float sc = softmax_scale;
   if (splits <= 0 && kinv != nullptr && Hq == Hkv)   // measured: an FP8 cache at G = 1 reads faster through the table path
     return odb_dec_attn(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, Hq, Hkv, Smax, softmax_scale, kinv, vinv, st);
-  switch (Hq / Hkv) {
-    case 1: return dec::launch_attn_group_t<1>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, sc, kinv,
-                                                 vinv, splits, st);
-    case 2: return dec::launch_attn_group_t<2>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, sc, kinv,
-                                                 vinv, splits, st);
-    case 4: return dec::launch_attn_group_t<4>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, sc, kinv,
-                                                 vinv, splits, st);
-    case 8: return dec::launch_attn_group_t<8>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp, Hkv, Smax, sc, kinv,
-                                                 vinv, splits, st);
-    default: return -2;                          // GQA groups of 1, 2, 4 or 8 query heads
-  }
+  return dec::with_group(Hq / Hkv, [&](auto g) {
+    return dec::with_cache(kinv != nullptr, [&](auto t) {
+      return dec::launch_attn_group<decltype(g)::value, decltype(t)>(q, ldq, kc, vc, pos, part_o, part_ml, out, ldo, table, rows, ngrp,
+                                                                     Hkv, Smax, softmax_scale, kinv, vinv, splits, st);
+    });
+  });
 }
 
 // The sibling split odb_dec_attn_group chooses for these shapes (CTAs per prompt and chunk; needs a device); 0: it runs
@@ -1739,14 +1694,12 @@ ODB_EXPORT int odb_dec_attn_group_splits(int rows, int ngrp, int Hq, int Hkv, in
   if (ngrp < 1 || rows % ngrp || Hq % Hkv) return -1;
   if (kv8 && Hq == Hkv) return 0;
   const int P = rows / ngrp, nch = odb::ceil_div(Smax, dec::CH);
-  int s;
-  switch (Hq / Hkv) {
-    case 1: s = dec::group_splits_t<1>(kv8 != 0, P, ngrp, Hkv, nch); break;
-    case 2: s = dec::group_splits_t<2>(kv8 != 0, P, ngrp, Hkv, nch); break;
-    case 4: s = dec::group_splits_t<4>(kv8 != 0, P, ngrp, Hkv, nch); break;
-    case 8: s = dec::group_splits_t<8>(kv8 != 0, P, ngrp, Hkv, nch); break;
-    default: return -2;
-  }
+  int s = 0;
+  const int rc = dec::with_group(Hq / Hkv, [&](auto g) {
+    s = dec::with_cache(kv8 != 0, [&](auto t) { return dec::attn_group_splits<decltype(g)::value, decltype(t)>(P, ngrp, Hkv, nch); });
+    return 0;
+  });
+  if (rc) return rc;
   return s <= 0 ? s - 1 : odb::ceil_div(ngrp, odb::ceil_div(ngrp, s));
 }
 
@@ -1767,22 +1720,6 @@ ODB_EXPORT int odb_dec_sample(const void* logits, long long ld, int V, const voi
   launch_pdl(dec::sample_kernel, dim3(B), dim3(dec::SAMPLE_THREADS), smem, st, (const __nv_bfloat16*)logits, ld, V,
              (const long long*)ictl, (const float*)fctl, (int*)pos, (int*)gen, (int*)finished, (long long*)out, max_new,
              (long long*)ids_next, (int*)hist, ldh, (unsigned*)scratch);
-  ODB_CHECK_LAST();
-  return 0;
-}
-
-// qkv [n*B, ld] bf16, slot-major (row j*B + b: token j of sequence b, at position pos[b] + j); cos/sin fp32 [max_pos, 32];
-// pos int32 [B]; kc/vc [B, Hkv, Smax, 64] bf16
-ODB_EXPORT int odb_dec_rope_append_multi(void* qkv, long long ld, const void* cos_t, const void* sin_t, const void* pos, void* kc,
-                                         void* vc, int B, int n, int Hq, int Hkv, int Smax, void* kinv, void* vinv, cudaStream_t st) {
-  if (ld % 2 || n < 1) return -1;
-  if (kinv != nullptr)
-    launch_pdl(dec::rope_append_multi_kernel<uint8_t>, dim3(B, n), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld, (const float*)cos_t,
-               (const float*)sin_t, (const int*)pos, (uint8_t*)kc, (uint8_t*)vc, Hq, Hkv, Smax, (float*)kinv, (float*)vinv);
-  else
-    launch_pdl(dec::rope_append_multi_kernel<__nv_bfloat16>, dim3(B, n), dim3(256), 0, st, (__nv_bfloat16*)qkv, ld,
-               (const float*)cos_t, (const float*)sin_t, (const int*)pos, (__nv_bfloat16*)kc, (__nv_bfloat16*)vc, Hq, Hkv, Smax,
-               (float*)nullptr, (float*)nullptr);
   ODB_CHECK_LAST();
   return 0;
 }
@@ -1832,7 +1769,7 @@ ODB_EXPORT int odb_dec_verify_attn(const void* q, long long ldq, const void* kc,
                (const float*)nullptr);
   }
   ODB_CHECK_LAST();
-  launch_pdl(dec::verify_combine_kernel, dim3(Hq, n * B), dim3(dec::D), 0, st, (const float*)part_o, (const float*)part_ml,
+  launch_pdl(dec::combine_kernel, dim3(Hq, n * B), dim3(dec::D), 0, st, (const float*)part_o, (const float*)part_ml,
              (const int*)pos, (__nv_bfloat16*)out, ldo, cap, tps * dec::VB, B);
   ODB_CHECK_LAST();
   return 0;
@@ -1915,8 +1852,9 @@ ODB_EXPORT int odb_dec_beam_step(const void* part_ml, const void* cand_v, const 
 ODB_EXPORT int odb_dec_beam_reorder(void* kv, void* table, const void* parent, const void* pos, int B, int nb, int L, int Hkv, int Smax,
                                     void* inv, cudaStream_t st) {
   if (nb < 1 || nb > dec::MAX_BEAMS || Smax % dec::CH || Smax / dec::CH > dec::MAX_TABLE) return -1;
-  if (inv != nullptr) return dec::launch_beam_reorder<uint8_t>(kv, inv, table, parent, pos, B, nb, L, Hkv, Smax, st);
-  return dec::launch_beam_reorder<__nv_bfloat16>(kv, nullptr, table, parent, pos, B, nb, L, Hkv, Smax, st);
+  return dec::with_cache(inv != nullptr, [&](auto t) {
+    return dec::launch_beam_reorder<decltype(t)>(kv, inv, table, parent, pos, B, nb, L, Hkv, Smax, st);
+  });
 }
 
 // kv [L, 2, B*n, Hkv, Smax, 64] (every layer's K and V, one allocation; bf16, or e4m3 bytes with inv fp32
@@ -1924,12 +1862,11 @@ ODB_EXPORT int odb_dec_beam_reorder(void* kv, void* table, const void* parent, c
 // row g*n, positions [0, len[g]).  Makes rows g*n + 1 .. g*n + n - 1 its children.  See dec::fork_kernel.
 ODB_EXPORT int odb_dec_fork(void* kv, void* table, const void* len, int B, int n, int L, int Hkv, int Smax, void* inv, cudaStream_t st) {
   if (n < 1 || Smax % dec::CH) return -1;
-  if (inv != nullptr)
-    launch_pdl(dec::fork_kernel<uint8_t>, dim3(L * 2 * Hkv, B), dim3(256), 0, st, (uint8_t*)kv, (int*)table, (const int*)len, n, Hkv, Smax,
+  return dec::with_cache(inv != nullptr, [&](auto t) {
+    using T = decltype(t);
+    launch_pdl(dec::fork_kernel<T>, dim3(L * 2 * Hkv, B), dim3(256), 0, st, (T*)kv, (int*)table, (const int*)len, n, Hkv, Smax,
                Smax / dec::CH, (float*)inv);
-  else
-    launch_pdl(dec::fork_kernel<__nv_bfloat16>, dim3(L * 2 * Hkv, B), dim3(256), 0, st, (__nv_bfloat16*)kv, (int*)table, (const int*)len,
-               n, Hkv, Smax, Smax / dec::CH, (float*)nullptr);
-  ODB_CHECK_LAST();
-  return 0;
+    ODB_CHECK_LAST();
+    return 0;
+  });
 }

@@ -1,14 +1,17 @@
 """KV-cached autoregressive generation for :class:`~opendiloco_b200.models.llama.LlamaForCausalLM`.
 
-Prefill runs the prompt through the training layer program (fused QKV+RoPE GEMM, the causal attention forward, the
-SwiGLU GEMM) on buffers of this module's own, copies k|v into per-layer caches and samples the first token.  Every later
-token is one decode step over ``[B, ·]`` buffers:
+Every pass over the model is one layer program (``_layers``) on rows of this module's own (``Rows``):
 
-    embedding -> per layer: rmsnorm -> QKV GEMM -> rope+append -> split-KV attention -> o-proj -> rmsnorm(+residual)
-              -> gate|up SwiGLU GEMM -> down -> final norm -> LM head -> sampler
+    embedding -> per layer: rmsnorm -> attend -> o-proj -> rmsnorm(+residual) -> gate|up SwiGLU GEMM -> down
+
+Only ``attend`` differs.  Prefill (and ``score``) runs the fused QKV+RoPE GEMM, copies k|v into per-layer caches and runs
+the causal attention forward; the decode step runs the QKV GEMM, RoPE+append at each row's position and split-KV
+attention over the cache; the verify pass of assisted generation does the same for several tokens per row.  The final
+norm and the LM head (``_head``) then feed the sampler.
 
 All the per-step scalars (positions, step counters, finished flags, sampler settings) live in device memory, so the step
-is captured once into a CUDA graph and replayed (``ODB_CUDA_GRAPH=0``: eager launches).  CUDA bf16 models run the
+is captured once into a CUDA graph and replayed (``ODB_CUDA_GRAPH=0``: eager launches); the decode step, the assisted
+round and the beam step share the warm-up / capture / replay protocol (``_graphed``).  CUDA bf16 models run the
 kernels of ``csrc/decode_sm90.cu`` and the training GEMMs; other precisions and devices run the same program on the
 PyTorch references of :mod:`opendiloco_b200.ops`.
 
@@ -28,7 +31,7 @@ decode layers, the LM head, the selection kernels and the cache reorder.  All be
 so every 128-key chunk behind the current one is immutable history: a beam that continues another row takes that row's
 chunks through a per-row chunk table and copies only the current partial chunk.
 
-FP8 weight-only mode, ``generate(fp8_weights=True)``: the layer programs take every projection weight from one helper
+FP8 weight-only mode, ``generate(fp8_weights=True)``: the layer program takes every projection weight from one helper
 (``_proj``, ``_weight``, ``_mlp``).  Without FP8 weights it returns the arena weight and launches what it always did; with
 them (:mod:`~opendiloco_b200.models.fp8_weights`) rows of M <= 64 run the skinny e4m3 GEMM and wider ones the bf16 GEMM on
 the dequantised weights Ŵ.  Every graph key carries the mode, so switching it recaptures.
@@ -50,7 +53,6 @@ leaves the training buffers and graph untouched.
 from __future__ import annotations
 
 import math
-import os
 import warnings
 from dataclasses import dataclass
 
@@ -63,6 +65,7 @@ from ..ops import gemm as G
 from ..ops import kernels as K
 from ..ops import tc_gemm as TC
 from . import fp8_weights as W8
+from .llama import _use_graph
 
 FINISHED_CHECK_EVERY = 16           # decode steps between host checks of "every row has finished"
 ASSISTED_CHECK_EVERY = 4            # assisted rounds between host checks (a round emits 1 .. K+1 tokens per row)
@@ -74,37 +77,64 @@ def _round_up(x: int, m: int) -> int:
     return (x + m - 1) // m * m
 
 
-def _use_graph() -> bool:
-    return os.environ.get("ODB_CUDA_GRAPH", "1") == "1"
+def _resident(model, attr: str, key: tuple, make):
+    """The engine's state ``attr`` if its key is ``key``, else a new one from make(); at most one is resident (the old one is
+    freed before make() allocates)."""
+    eng = model.engine
+    st = getattr(eng, attr)
+    if st is None or st.key != key:
+        setattr(eng, attr, None)
+        st = make()
+        st.key = key
+        setattr(eng, attr, st)
+    return st
 
 
-class _PrefillBuffers:
-    """Transient [B*Sp, ·] activations of one prefill (no per-layer saved activations)."""
+def _graphed(holder, key: tuple, device, run) -> None:
+    """run() through holder's CUDA graph (holder.graph, holder.graph_key): the first call with a new key runs it eagerly
+    (warm-up), the next one captures it and every later call replays it."""
+    if holder.graph is None or holder.graph_key != key:
+        if holder.graph_key != ("warm",) + key:
+            holder.graph, holder.graph_key = None, ("warm",) + key
+            run()
+            return
+        torch.cuda.synchronize(device)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, capture_error_mode="thread_local"):
+            run()
+        holder.graph, holder.graph_key = g, key
+    holder.graph.replay()
 
-    def __init__(self, cfg, T: int, device, dtype):
+
+class Rows:
+    """The activations of T rows of the layer program (``_layers``), one token per row: token ids, residual, normed rows,
+    projection outputs, q|k|v, gate|up and SwiGLU rows.  ``att``: also the attention output (decode step, verify pass);
+    prefill and scoring take theirs from the attention forward."""
+
+    def __init__(self, cfg, T: int, device, dtype, att: bool = False):
         e = lambda *shape: torch.empty(*shape, dtype=dtype, device=device)  # noqa: E731
         h, i = cfg.hidden_size, cfg.intermediate_size
         self.T = T
-        self.ids = torch.empty(T, dtype=torch.int64, device=device)
+        self.ids = torch.zeros(T, dtype=torch.int64, device=device)
         self.res, self.xn, self.proj = e(T, h), e(T, h), e(T, h)
         self.rstd = torch.empty(T, dtype=torch.float32, device=device)
         self.qkv, self.gu, self.act = e(T, cfg.qkv_dim), e(T, 2 * i), e(T, i)
+        self.att = e(T, cfg.q_dim) if att else None
 
 
-class DecodeState:
-    """KV caches, decode buffers and device-side control scalars for B rows of up to Smax positions.  ``fp8_kv``: the caches
-    are e4m3 ``kv`` [L, 2, B, Hkv, Smax, D] with fp32 ``kv_inv`` [L, 2, B, Hkv, Smax] (each one allocation: beam search
-    reorders all of it); ``kinv`` / ``vinv`` are the per-layer views of ``kv_inv`` (None for a bf16 cache).  ``group`` > 1:
-    multi-sample rows, ``group`` siblings per prompt, with the chunk table ``table`` int32 [B, Smax / 128] of the kernel
-    path (None otherwise, and for group 1)."""
+class DecodeState(Rows):
+    """KV caches, the one-token rows of the decode step and device-side control scalars for B rows of up to Smax positions.
+    ``fp8_kv``: the caches are e4m3 ``kv`` [L, 2, B, Hkv, Smax, D] with fp32 ``kv_inv`` [L, 2, B, Hkv, Smax] (each one
+    allocation: beam search reorders all of it); ``kinv`` / ``vinv`` are the per-layer views of ``kv_inv`` (None for a bf16
+    cache).  ``group`` > 1: multi-sample rows, ``group`` siblings per prompt, with the chunk table ``table`` int32 [B, Smax /
+    128] of the kernel path (None otherwise, and for group 1)."""
 
     def __init__(self, cfg, B: int, Smax: int, device, dtype, fp8_kv: bool = False, group: int = 1):
+        super().__init__(cfg, B, device, dtype, att=True)
         L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-        h, i, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
-        e = lambda *shape: torch.empty(*shape, dtype=dtype, device=device)  # noqa: E731
+        V = cfg.vocab_size
         i32 = lambda: torch.zeros(B, dtype=torch.int32, device=device)      # noqa: E731
         self.cfg, self.B, self.Smax, self.device, self.dtype = cfg, B, Smax, torch.device(device), dtype
-        self.key = (B, Smax, str(device), dtype, fp8_kv, group)
         self.fp8_kv, self.group = fp8_kv, group
         # one allocation: beam search reorders all
         self.kv = torch.zeros(L, 2, B, Hkv, Smax, D, dtype=E4M3 if fp8_kv else dtype, device=device)
@@ -115,12 +145,7 @@ class DecodeState:
         self.vinv = [self.kv_inv[l, 1] if fp8_kv else None for l in range(L)]
         n_rope = _round_up(max(cfg.max_position_embeddings, Smax), 128)
         self.cos, self.sin = K.rope_tables(n_rope, D, cfg.rope_theta, device)
-        # one-token-per-row buffers of the decode step
-        self.ids = torch.zeros(B, dtype=torch.int64, device=device)
-        self.res, self.xn, self.proj = e(B, h), e(B, h), e(B, h)
-        self.rstd = torch.empty(B, dtype=torch.float32, device=device)
-        self.qkv, self.att, self.gu, self.act = e(B, cfg.qkv_dim), e(B, cfg.q_dim), e(B, 2 * i), e(B, i)
-        self.logits = e(B, V)
+        self.logits = torch.empty(B, V, dtype=dtype, device=device)
         self.pos, self.gen, self.finished, self.lens = i32(), i32(), i32(), i32()
         self.out = torch.zeros(B, Smax, dtype=torch.int64, device=device)
         self.ictl, self.fctl = DK.make_controls(False, 1.0, 0, 1.0, 0, 0, [], device)
@@ -134,14 +159,15 @@ class DecodeState:
             self.part_o = torch.empty(B, Hq, nch, D, dtype=torch.float32, device=device)
             self.part_ml = torch.empty(B, Hq, nch, 2, dtype=torch.float32, device=device)
         self.table = torch.zeros(B, nch, dtype=torch.int32, device=device) if self.kernels and group > 1 else None
-        self._prefill: _PrefillBuffers | None = None
+        self._prefill: Rows | None = None
         self.graph = None
         self.graph_key = None
 
-    def prefill_buffers(self, T: int) -> _PrefillBuffers:
+    def prefill_rows(self, T: int) -> Rows:
+        """The [T = B*Sp] rows of a prefill, kept for the next prefill of the same size."""
         if self._prefill is None or self._prefill.T != T:
             self._prefill = None                      # free the old buffers before allocating the new ones
-            self._prefill = _PrefillBuffers(self.cfg, T, self.device, self.dtype)
+            self._prefill = Rows(self.cfg, T, self.device, self.dtype)
         return self._prefill
 
     def set_controls(self, do_sample: bool, temperature: float, top_k: int, top_p: float, seed: int, pad: int, eos: list[int],
@@ -156,111 +182,54 @@ def decode_state(model, B: int, Smax: int, fp8_kv: bool = False, group: int = 1)
     """The model's decode state for (B, Smax, FP8 cache or not, siblings per prompt), allocated on first use; at most one
     is resident."""
     eng, ar = model.engine, model.arena
-    key = (B, Smax, str(ar.device), ar.compute_dtype, fp8_kv, group)
-    st = eng.decode_state
-    if st is None or st.key != key:
+
+    def make():
         if eng.assisted_state is not None:           # its round graph reads the old caches: let them go
             eng.assisted_state.drop_graph()
-        eng.decode_state = None                       # free the old caches before allocating the new ones
-        st = eng.decode_state = DecodeState(model.config, B, Smax, ar.device, ar.compute_dtype, fp8_kv, group)
-    return st
+        return DecodeState(model.config, B, Smax, ar.device, ar.compute_dtype, fp8_kv, group)
+
+    return _resident(model, "decode_state", (B, Smax, str(ar.device), ar.compute_dtype, fp8_kv, group), make)
 
 
-# ------------------------------------------------------------------------------------------------ prefill
-@torch.no_grad()
-def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, fp8=None) -> None:
-    """ids [B, Sp]: prompts compacted to start at position 0 and right-padded; lens [B] real lengths.  Fills the caches,
-    computes the logits at position lens[b]-1 and samples the first new token (st.pos ends at lens).  ``fp8``: the
-    model's FP8 weights (None: the arena weights).  An FP8 cache (st.fp8_kv) is filled with the quantised k|v rows; the
-    prompt's attention reads the in-flight bf16 q|k|v, so the first token does not depend on the cache format."""
+# ------------------------------------------------------------------------------------------------ layer program
+def _layers(model, buf: Rows, ids: torch.Tensor, attend, fp8=None):
+    """The forward layer program over the rows of ``buf``: embedding of ids, then per layer rmsnorm -> ``attend(l)`` (the
+    attention output of the normed rows buf.xn: QKV GEMM, RoPE, cache writes, attention) -> o-proj -> rmsnorm(+residual)
+    -> SwiGLU GEMM -> down.  Returns the last layer's output delta; the residual before it is in buf.res."""
     cfg, ar = model.config, model.arena
-    B, Sp = ids.shape
-    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-    T = B * Sp
-    pb = st.prefill_buffers(T)
-    st.lens.copy_(lens)
-    st.pos.copy_(lens - 1)
-    st.gen.zero_()
-    st.finished.zero_()
-    n = min(Sp, st.Smax)
-    st.hist[:, :n].copy_(ids[:, :n])
-    pb.ids.copy_(ids.reshape(-1))
-    delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
-                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, st.lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, kinv=st.kinv[l],
-                                                            vinv=st.vinv[l]), fp8=fp8)
-    # only the last real position of every row feeds the LM head: gather its residual and delta rows
-    last = torch.arange(B, device=st.device, dtype=torch.int64) * Sp + st.lens.long() - 1
-    K.embedding_fwd(last, pb.res, out=st.res)
-    K.embedding_fwd(last, delta, out=st.proj)
-    _head_and_sample(cfg, ar, st, st.proj)
-
-
-def _prefill_rows(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, stride: int, fp8=None) -> None:
-    """The layers over ids [B, Sp] (compacted prompts, real lengths lens [B]) once: prompt b fills cache row b * stride,
-    and its last position's residual and delta rows go to decode rows b * stride .. b * stride + stride - 1 (st.res,
-    st.proj), ready for the final norm and the LM head."""
-    cfg = model.config
-    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-    B, Sp = ids.shape
-    pb = st.prefill_buffers(B * Sp)
-    pb.ids.copy_(ids.reshape(-1))
-    delta = forward_layers(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels,
-                           on_qkv=lambda l, qkv: DK.kv_fill(qkv, lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, row_stride=stride,
-                                                            kinv=st.kinv[l], vinv=st.vinv[l]), fp8=fp8)
-    last = (torch.arange(B, device=st.device, dtype=torch.int64) * Sp + lens.long() - 1).repeat_interleave(stride)
-    K.embedding_fwd(last, pb.res, out=st.res)
-    K.embedding_fwd(last, delta, out=st.proj)
-
-
-@torch.no_grad()
-def sample_prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, fp8=None) -> None:
-    """Multi-sample prefill: ids [B, Sp] compacted prompts, lens [B]; st has B * n rows, n = st.group.  The layers run on
-    the B prompts once, into rows p * n; the fork makes rows p * n + 1 .. its children (``DK.fork``: chunk table on the
-    kernel path, whole-row copies otherwise); the LM head and the sampler then run on all B * n rows, whose state (pos,
-    lens, history) is the repeated-prompt program's.  Samples the first token of every row (st.pos ends at lens)."""
-    cfg, ar = model.config, model.arena
-    n = st.group
-    Sp = ids.shape[1]
-    lr = lens.repeat_interleave(n)
-    st.lens.copy_(lr)
-    st.pos.copy_(lr - 1)
-    st.gen.zero_()
-    st.finished.zero_()
-    m = min(Sp, st.Smax)
-    st.hist[:, :m].copy_(ids[:, :m].repeat_interleave(n, dim=0))
-    _prefill_rows(model, st, ids, lens, n, fp8)
-    DK.fork(st.kv, st.table, lens, n, inv=st.kv_inv)
-    _head_and_sample(cfg, ar, st, st.proj)
-
-
-def forward_layers(model, pb: _PrefillBuffers, B: int, Sp: int, cos, sin, fused_rope: bool, on_qkv=None, fp8=None):
-    """The forward-only layer program over pb.ids [B*Sp] (rows start at position 0; causal attention keeps right padding
-    from reaching real positions): embedding, then per layer rmsnorm -> QKV(+RoPE) GEMM -> attention -> o-proj ->
-    rmsnorm(+residual) -> SwiGLU GEMM -> down.  ``on_qkv(l, qkv)`` sees the rotated projections of layer l.  Returns the
-    last layer's output delta; the residual before it is in pb.res."""
-    cfg, ar = model.config, model.arena
-    L, Hq, Hkv, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     eps = cfg.rms_norm_eps
-    K.embedding_fwd(pb.ids, ar.w("model.embed_tokens.weight"), out=pb.res)
+    K.embedding_fwd(ids, ar.w("model.embed_tokens.weight"), out=buf.res)
     delta = None
-    for l in range(L):
+    for l in range(cfg.num_hidden_layers):
         p = f"model.layers.{l}."
-        K.rmsnorm_fwd(pb.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
-        w_qkv = _weight(ar, fp8, "qkv", l)
-        if fused_rope and TC.usable(pb.xn, w_qkv):
-            TC.linear_qkv_rope(pb.xn, w_qkv, pb.qkv, cos, sin, Sp, (Hq + Hkv) * D)
-        else:
-            _proj(ar, fp8, "qkv", l, pb.xn, pb.qkv)
-            K.rope_(pb.qkv, cos, sin, Sp, Hq + Hkv, D)
-        if on_qkv is not None:
-            on_qkv(l, pb.qkv)
-        att, _ = A.attention_fwd(pb.qkv, B, Sp, Hq, Hkv, D)
-        _proj(ar, fp8, "o", l, att, pb.proj)
-        K.rmsnorm_fwd(pb.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=pb.proj, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
-        _mlp(cfg, ar, l, pb.xn, pb.gu, pb.act, fp8)
-        _proj(ar, fp8, "down", l, pb.act, pb.proj)
-        delta = pb.proj
+        K.rmsnorm_fwd(buf.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=buf.xn, rstd=buf.rstd, x_out=buf.res)
+        _proj(ar, fp8, "o", l, attend(l), buf.proj)
+        K.rmsnorm_fwd(buf.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=buf.proj, out=buf.xn, rstd=buf.rstd, x_out=buf.res)
+        _mlp(cfg, ar, l, buf.xn, buf.gu, buf.act, fp8)
+        _proj(ar, fp8, "down", l, buf.act, buf.proj)
+        delta = buf.proj
     return delta
+
+
+def _prompt_attend(model, buf: Rows, B: int, Sp: int, cos, sin, fused_rope: bool, fp8=None, fill=None):
+    """The ``attend`` of prefill and scoring over B rows of Sp positions each, starting at position 0 (causal attention
+    keeps right padding from reaching real positions): QKV(+RoPE) GEMM, ``fill(l, qkv)`` (the cache fill) on the rotated
+    projections, causal attention forward."""
+    cfg, ar = model.config, model.arena
+    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+
+    def attend(l):
+        w_qkv = _weight(ar, fp8, "qkv", l)
+        if fused_rope and TC.usable(buf.xn, w_qkv):
+            TC.linear_qkv_rope(buf.xn, w_qkv, buf.qkv, cos, sin, Sp, (Hq + Hkv) * D)
+        else:
+            _proj(ar, fp8, "qkv", l, buf.xn, buf.qkv)
+            K.rope_(buf.qkv, cos, sin, Sp, Hq + Hkv, D)
+        if fill is not None:
+            fill(l, buf.qkv)
+        return A.attention_fwd(buf.qkv, B, Sp, Hq, Hkv, D)[0]
+
+    return attend
 
 
 def _weight(ar, fp8, kind: str, l: int) -> torch.Tensor:
@@ -288,53 +257,83 @@ def _mlp(cfg, ar, l: int, xn, gu, act, fp8=None) -> None:
         K.swiglu_fwd(gu, out=act)
 
 
-def _head(cfg, ar, st: DecodeState, delta) -> None:
-    K.rmsnorm_fwd(st.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=st.xn, rstd=st.rstd, x_out=st.res)
-    G.mm_nt(st.xn, ar.w("lm_head.weight"), out=st.logits)
+def _head(model, buf: Rows, delta, logits) -> None:
+    """The final RMSNorm of buf's rows (residual + delta) and the LM-head GEMM into logits."""
+    cfg, ar = model.config, model.arena
+    K.rmsnorm_fwd(buf.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=buf.xn, rstd=buf.rstd, x_out=buf.res)
+    G.mm_nt(buf.xn, ar.w("lm_head.weight"), out=logits)
 
 
-def _head_and_sample(cfg, ar, st: DecodeState, delta) -> None:
-    _head(cfg, ar, st, delta)
+def _head_and_sample(model, st: DecodeState, delta) -> None:
+    _head(model, st, delta, st.logits)
     DK.sample(st.logits, st.ictl, st.fctl, st.pos, st.gen, st.finished, st.out, st.ids, st.hist, st.proc_scratch)
 
 
+# ------------------------------------------------------------------------------------------------ prefill
+@torch.no_grad()
+def prefill(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, fp8=None) -> None:
+    """ids [B, Sp]: prompts compacted to start at position 0 and right-padded; lens [B] real lengths; st has B * n rows,
+    n = st.group.  The layers run on the B prompts once, prompt p filling cache row p * n; with n > 1 the fork makes rows
+    p * n + 1 .. its children (``DK.fork``: chunk table on the kernel path, whole-row copies otherwise) and every row's
+    state (pos, lens, history) is the repeated-prompt program's.  Computes the logits at position lens[p] - 1 of every row
+    and samples the first token (st.pos ends at lens).  ``fp8``: the model's FP8 weights (None: the arena weights).  An
+    FP8 cache (st.fp8_kv) is filled with the quantised k|v rows; the prompt's attention reads the in-flight bf16 q|k|v, so
+    the first token does not depend on the cache format."""
+    n, Sp = st.group, ids.shape[1]
+    lr = lens.repeat_interleave(n) if n > 1 else lens
+    st.lens.copy_(lr)
+    st.pos.copy_(lr - 1)
+    st.gen.zero_()
+    st.finished.zero_()
+    m = min(Sp, st.Smax)
+    st.hist[:, :m].copy_(ids[:, :m].repeat_interleave(n, dim=0) if n > 1 else ids[:, :m])
+    # one sample per prompt reads the lengths from st.lens, the device copy of lens
+    _prefill_rows(model, st, ids, lens if n > 1 else st.lens, n, fp8)
+    if n > 1:
+        DK.fork(st.kv, st.table, lens, n, inv=st.kv_inv)
+    _head_and_sample(model, st, st.proj)
+
+
+def _prefill_rows(model, st: DecodeState, ids: torch.Tensor, lens: torch.Tensor, stride: int, fp8=None) -> None:
+    """The layers over ids [B, Sp] (compacted prompts, real lengths lens [B]) once: prompt b fills cache row b * stride,
+    and its last position's residual and delta rows go to decode rows b * stride .. b * stride + stride - 1 (st.res,
+    st.proj), ready for the final norm and the LM head."""
+    cfg = model.config
+    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    B, Sp = ids.shape
+    pb = st.prefill_rows(B * Sp)
+    pb.ids.copy_(ids.reshape(-1))
+
+    def fill(l, qkv):
+        DK.kv_fill(qkv, lens, st.kc[l], st.vc[l], B, Sp, Hq, Hkv, D, row_stride=stride, kinv=st.kinv[l], vinv=st.vinv[l])
+
+    delta = _layers(model, pb, pb.ids, _prompt_attend(model, pb, B, Sp, st.cos[:Sp], st.sin[:Sp], st.kernels, fp8, fill), fp8)
+    # only the last real position of every prompt feeds the LM head: gather its residual and delta rows
+    last = torch.arange(B, device=st.device, dtype=torch.int64) * Sp + lens.long() - 1
+    if stride > 1:
+        last = last.repeat_interleave(stride)
+    K.embedding_fwd(last, pb.res, out=st.res)
+    K.embedding_fwd(last, delta, out=st.proj)
+
+
 # ------------------------------------------------------------------------------------------------ decode step
-def _layers(model, buf, ids: torch.Tensor, attend, fp8=None):
-    """The decode layer program over the rows of ``buf`` (a DecodeState or AssistedState): embedding of ids, then per layer
-    rmsnorm -> QKV GEMM -> ``attend(l, qkv, att)`` (RoPE, cache append, attention) -> o-proj -> rmsnorm(+residual) ->
-    SwiGLU GEMM -> down.  Returns the last layer's output delta; the residual before it is in buf.res."""
-    cfg, ar = model.config, model.arena
-    eps = cfg.rms_norm_eps
-    K.embedding_fwd(ids, ar.w("model.embed_tokens.weight"), out=buf.res)
-    delta = None
-    for l in range(cfg.num_hidden_layers):
-        p = f"model.layers.{l}."
-        K.rmsnorm_fwd(buf.res, ar.w(p + "input_layernorm.weight"), eps, delta=delta, out=buf.xn, rstd=buf.rstd, x_out=buf.res)
-        _proj(ar, fp8, "qkv", l, buf.xn, buf.qkv)
-        attend(l, buf.qkv, buf.att)
-        _proj(ar, fp8, "o", l, buf.att, buf.proj)
-        K.rmsnorm_fwd(buf.res, ar.w(p + "post_attention_layernorm.weight"), eps, delta=buf.proj, out=buf.xn, rstd=buf.rstd, x_out=buf.res)
-        _mlp(cfg, ar, l, buf.xn, buf.gu, buf.act, fp8)
-        _proj(ar, fp8, "down", l, buf.act, buf.proj)
-        delta = buf.proj
-    return delta
-
-
 def _one_token_layers(model, st: DecodeState, ids: torch.Tensor, table: torch.Tensor | None = None, fp8=None):
     """One token per row at st.pos: the decode layers with single-query RoPE+append and split-KV attention (through the
     chunk table, if given), on st's bf16 or FP8 cache.  Multi-sample rows (st.group > 1) attend through st's own table
     with the sibling-grouped attention."""
-    cfg = model.config
+    cfg, ar = model.config, model.arena
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
 
-    def attend(l, qkv, att):
-        DK.rope_append(qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D, kinv=st.kinv[l], vinv=st.vinv[l])
+    def attend(l):
+        _proj(ar, fp8, "qkv", l, st.xn, st.qkv)
+        DK.rope_append(st.qkv, st.cos, st.sin, st.pos, st.kc[l], st.vc[l], Hq, Hkv, D, kinv=st.kinv[l], vinv=st.vinv[l])
         if st.group > 1:
-            DK.attention_grouped(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.group, st.part_o, st.part_ml, table=st.table,
-                                 kinv=st.kinv[l], vinv=st.vinv[l])
-            return
-        DK.attention(qkv, st.kc[l], st.vc[l], st.pos, att, Hq, Hkv, D, st.part_o, st.part_ml, table=table, kinv=st.kinv[l],
-                     vinv=st.vinv[l])
+            DK.attention_grouped(st.qkv, st.kc[l], st.vc[l], st.pos, st.att, Hq, Hkv, D, st.group, st.part_o, st.part_ml,
+                                 table=st.table, kinv=st.kinv[l], vinv=st.vinv[l])
+        else:
+            DK.attention(st.qkv, st.kc[l], st.vc[l], st.pos, st.att, Hq, Hkv, D, st.part_o, st.part_ml, table=table,
+                         kinv=st.kinv[l], vinv=st.vinv[l])
+        return st.att
 
     return _layers(model, st, ids, attend, fp8)
 
@@ -345,7 +344,7 @@ def _fp8_key(fp8):
 
 def _step_eager(model, st: DecodeState, fp8=None) -> None:
     delta = _one_token_layers(model, st, st.ids, fp8=fp8)
-    _head_and_sample(model.config, model.arena, st, delta)
+    _head_and_sample(model, st, delta)
 
 
 @torch.no_grad()
@@ -361,41 +360,28 @@ def step(model, st: DecodeState, graph: bool | None = None, fp8=None) -> None:
         return
     key = (model.arena.version, model.arena.shadow.data_ptr(), st.group, st.table.data_ptr() if st.table is not None else None,
            _fp8_key(fp8))
-    if st.graph is None or st.graph_key != key:
-        if st.graph_key != ("warm",) + key:
-            st.graph, st.graph_key = None, ("warm",) + key
-            _step_eager(model, st, fp8)
-            return
-        torch.cuda.synchronize(st.device)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, capture_error_mode="thread_local"):
-            _step_eager(model, st, fp8)
-        st.graph, st.graph_key = g, key
-    st.graph.replay()
+    _graphed(st, key, st.device, lambda: _step_eager(model, st, fp8))
 
 
 # ------------------------------------------------------------------------------------------------ assisted generation
-class AssistedState:
-    """The target's buffers of assisted generation over B rows with K proposals: the multi-token verify pass over
-    (K+1)*B slot-major rows (row j*B + b is slot j of row b), the draft's proposal logits, the draft's own DecodeState
-    (so a model can draft for itself, and the assistant's ``decode_state`` is left alone) and the round graph.  The
-    target's caches, positions and outputs stay in its DecodeState.
+class AssistedState(Rows):
+    """The target's buffers of assisted generation over B rows with K proposals: the rows of the multi-token verify pass,
+    (K+1)*B slot-major rows (row j*B + b is slot j of row b; ``ids`` slot 0 holds the last token, slots 1..K the
+    proposals), the draft's proposal logits, the draft's own DecodeState (so a model can draft for itself, and the
+    assistant's ``decode_state`` is left alone) and the round graph.  The target's caches, positions and outputs stay in
+    its DecodeState.
 
     With ``dcfg`` None (prompt lookup) there is no draft: no draft DecodeState and no proposal logits; the proposals
     come from the target's token history, and ``cnt`` / ``proposed`` count each row's candidates."""
 
     def __init__(self, cfg, dcfg, B: int, K: int, Smax: int, device, dtype):
-        h, i, V, D = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size, cfg.head_dim
+        V, D = cfg.vocab_size, cfg.head_dim
         T = (K + 1) * B
-        e = lambda *shape: torch.empty(*shape, dtype=dtype, device=device)  # noqa: E731
-        self.B, self.K, self.key = B, K, (B, K, Smax, str(device), dtype, _shape(dcfg) if dcfg is not None else None)
+        self.B, self.K = B, K
         self.draft = DecodeState(dcfg, B, Smax, device, dtype) if dcfg is not None else None
-        self.tok = torch.zeros(T, dtype=torch.int64, device=device)          # slot 0: last token; 1..K: proposals
-        self.res, self.xn, self.proj = e(T, h), e(T, h), e(T, h)
-        self.rstd = torch.empty(T, dtype=torch.float32, device=device)
-        self.qkv, self.att, self.gu, self.act = e(T, cfg.qkv_dim), e(T, cfg.q_dim), e(T, 2 * i), e(T, i)
-        self.plog = e(T, V)
-        self.qlog = e(K * B, V) if dcfg is not None else None
+        super().__init__(cfg, T, device, dtype, att=True)
+        self.plog = torch.empty(T, V, dtype=dtype, device=device)
+        self.qlog = torch.empty(K * B, V, dtype=dtype, device=device) if dcfg is not None else None
         self.stats = torch.zeros(B, 2, dtype=torch.int64, device=device)     # per row: rounds taken part in, accepted
         self.cnt = torch.zeros(B, dtype=torch.int32, device=device)          # prompt lookup: this round's candidates per row
         self.proposed = torch.zeros(B, dtype=torch.int64, device=device)     # prompt lookup: candidates proposed per row
@@ -433,52 +419,47 @@ def _shape(cfg) -> tuple:
 def assisted_state(model, assistant, B: int, K: int, Smax: int) -> AssistedState:
     """The model's assisted-generation state for (assistant shapes, B, K, Smax), allocated on first use; at most one is
     resident, on the target's engine.  ``assistant`` None: the draft-less state of prompt lookup."""
-    eng, ar = model.engine, model.arena
+    ar = model.arena
     dcfg = assistant.config if assistant is not None else None
     key = (B, K, Smax, str(ar.device), ar.compute_dtype, _shape(dcfg) if dcfg is not None else None)
-    st = eng.assisted_state
-    if st is None or st.key != key:
-        eng.assisted_state = None                     # free the old buffers before allocating the new ones
-        st = eng.assisted_state = AssistedState(model.config, dcfg, B, K, Smax, ar.device, ar.compute_dtype)
-    return st
+    return _resident(model, "assisted_state", key, lambda: AssistedState(model.config, dcfg, B, K, Smax, ar.device, ar.compute_dtype))
 
 
 def _verify(model, tst: DecodeState, ast: AssistedState, fp8=None) -> None:
-    """The target scores ast.tok (slot j at tst.pos + j) in one pass: logits of every slot -> ast.plog."""
+    """The target scores ast.ids (slot j at tst.pos + j) in one pass: logits of every slot -> ast.plog."""
     cfg, ar = model.config, model.arena
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     n = ast.K + 1
 
-    def attend(l, qkv, att):
-        DK.rope_append_multi(qkv, tst.cos, tst.sin, tst.pos, tst.kc[l], tst.vc[l], Hq, Hkv, D, n, kinv=tst.kinv[l], vinv=tst.vinv[l])
-        DK.verify_attention(qkv, tst.kc[l], tst.vc[l], tst.pos, att, Hq, Hkv, D, n, ast.part_o, ast.part_ml, kinv=tst.kinv[l],
-                            vinv=tst.vinv[l])
+    def attend(l):
+        _proj(ar, fp8, "qkv", l, ast.xn, ast.qkv)
+        DK.rope_append_multi(ast.qkv, tst.cos, tst.sin, tst.pos, tst.kc[l], tst.vc[l], Hq, Hkv, D, n, kinv=tst.kinv[l],
+                             vinv=tst.vinv[l])
+        DK.verify_attention(ast.qkv, tst.kc[l], tst.vc[l], tst.pos, ast.att, Hq, Hkv, D, n, ast.part_o, ast.part_ml,
+                            kinv=tst.kinv[l], vinv=tst.vinv[l])
+        return ast.att
 
-    delta = _layers(model, ast, ast.tok, attend, fp8)
-    K.rmsnorm_fwd(ast.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=ast.xn, rstd=ast.rstd, x_out=ast.res)
-    G.mm_nt(ast.xn, ar.w("lm_head.weight"), out=ast.plog)
+    _head(model, ast, _layers(model, ast, ast.ids, attend, fp8), ast.plog)
 
 
 def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: int, ngram: int, fp8=None) -> None:
     if draft is None:                                 # prompt lookup: proposals from the history, point-mass acceptance
-        DK.lookup_propose(tst.hist, tst.pos, tst.finished, tst.ictl, ast.tok, ast.cnt, ast.proposed, ngram)
+        DK.lookup_propose(tst.hist, tst.pos, tst.finished, tst.ictl, ast.ids, ast.cnt, ast.proposed, ngram)
         _verify(target, tst, ast, fp8)
-        DK.accept(ast.plog, None, tst.ictl, tst.fctl, ast.tok, tst.pos, tst.gen, tst.finished, tst.out, max_new, None, ast.stats,
+        DK.accept(ast.plog, None, tst.ictl, tst.fctl, ast.ids, tst.pos, tst.gen, tst.finished, tst.out, max_new, None, ast.stats,
                   cnt=ast.cnt, hist=tst.hist)
         return
     B, Kp, dst = ast.B, ast.K, ast.draft
-    dcfg, dar = draft.config, draft.arena
     for i in range(Kp + 1):
         # draft step i consumes slot i at dst.pos; steps 0..K-1 propose slot i+1, step K only writes d_K into the cache
-        delta = _one_token_layers(draft, dst, ast.tok[i * B:(i + 1) * B])
+        delta = _one_token_layers(draft, dst, ast.ids[i * B:(i + 1) * B])
         if i == Kp:
             break
         q = ast.qlog[i * B:(i + 1) * B]
-        K.rmsnorm_fwd(dst.res, dar.w("model.norm.weight"), dcfg.rms_norm_eps, delta=delta, out=dst.xn, rstd=dst.rstd, x_out=dst.res)
-        G.mm_nt(dst.xn, dar.w("lm_head.weight"), out=q)
-        DK.sample(q, dst.ictl, dst.fctl, dst.pos, dst.gen, dst.finished, dst.out, ast.tok[(i + 1) * B:(i + 2) * B])
+        _head(draft, dst, delta, q)
+        DK.sample(q, dst.ictl, dst.fctl, dst.pos, dst.gen, dst.finished, dst.out, ast.ids[(i + 1) * B:(i + 2) * B])
     _verify(target, tst, ast, fp8)                    # the draft above runs on its own weights
-    DK.accept(ast.plog, ast.qlog, tst.ictl, tst.fctl, ast.tok, tst.pos, tst.gen, tst.finished, tst.out, max_new, dst.pos, ast.stats)
+    DK.accept(ast.plog, ast.qlog, tst.ictl, tst.fctl, ast.ids, tst.pos, tst.gen, tst.finished, tst.out, max_new, dst.pos, ast.stats)
 
 
 @torch.no_grad()
@@ -496,17 +477,8 @@ def assisted_round(target, draft, tst: DecodeState, ast: AssistedState, max_new:
         return
     proposer = (draft.arena.version, draft.arena.shadow.data_ptr()) if draft is not None else ("lookup", ngram)
     key = (target.arena.version, target.arena.shadow.data_ptr(), *proposer, id(tst), max_new, _fp8_key(fp8))
-    if ast.graph is None or ast.graph_key != key:
-        if ast.graph_key != ("warm",) + key:
-            ast.graph, ast.graph_key, ast.graph_target = None, ("warm",) + key, tst
-            _round_eager(target, draft, tst, ast, max_new, ngram, fp8)
-            return
-        torch.cuda.synchronize(tst.device)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, capture_error_mode="thread_local"):
-            _round_eager(target, draft, tst, ast, max_new, ngram, fp8)
-        ast.graph, ast.graph_key = g, key
-    ast.graph.replay()
+    ast.graph_target = tst                            # id(tst) is in the key: keep tst alive while a graph may read it
+    _graphed(ast, key, tst.device, lambda: _round_eager(target, draft, tst, ast, max_new, ngram, fp8))
 
 
 def _check_assistant(model, assistant, P: int, max_new_tokens: int, num_assistant_tokens) -> None:
@@ -574,7 +546,7 @@ def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int
         prefill(assistant, dst, comp, lens)
         dst.finished.zero_()                          # the draft never stops by itself; its position follows the target's
         dst.pos.copy_(tst.pos)
-    ast.tok[:B].copy_(tst.ids)
+    ast.ids[:B].copy_(tst.ids)
     ast.stats.zero_()
     ast.proposed.zero_()
     for r in range(max_new_tokens - 1):               # every round emits >= 1 token per unfinished row
@@ -607,7 +579,6 @@ class BeamState:
         i32 = lambda *shape: torch.zeros(*shape, dtype=torch.int32, device=device)     # noqa: E731
         f32 = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=device)   # noqa: E731
         self.B, self.nb, self.K, self.max_new = B, nb, K, max_new
-        self.key = (B, nb, K, max_new, Smax, str(device), dtype, fp8_kv)
         self.dec = DecodeState(cfg, rows, Smax, device, dtype, fp8_kv)
         self.run_score, self.fin_score = f32(rows), f32(rows)
         self.fin_flag, self.parent = i32(rows), i32(rows)
@@ -653,13 +624,10 @@ class BeamState:
 
 def beam_state(model, B: int, nb: int, K: int, max_new: int, Smax: int, fp8_kv: bool = False) -> BeamState:
     """The model's beam-search state for these shapes (and cache format), allocated on first use; at most one is resident."""
-    eng, ar = model.engine, model.arena
+    ar = model.arena
     key = (B, nb, K, max_new, Smax, str(ar.device), ar.compute_dtype, fp8_kv)
-    bs = eng.beam_state
-    if bs is None or bs.key != key:
-        eng.beam_state = None                         # free the old buffers before allocating the new ones
-        bs = eng.beam_state = BeamState(model.config, B, nb, K, max_new, Smax, ar.device, ar.compute_dtype, fp8_kv)
-    return bs
+    return _resident(model, "beam_state", key,
+                     lambda: BeamState(model.config, B, nb, K, max_new, Smax, ar.device, ar.compute_dtype, fp8_kv))
 
 
 @torch.no_grad()
@@ -669,7 +637,7 @@ def beam_prefill(model, bs: BeamState, ids: torch.Tensor, lens: torch.Tensor, fp
     st = bs.dec
     st.pos.copy_(lens.repeat_interleave(bs.nb) - 1)
     _prefill_rows(model, st, ids, lens, bs.nb, fp8)
-    _head(model.config, model.arena, st, st.proj)
+    _head(model, st, st.proj, st.logits)
 
 
 def beam_select(bs: BeamState, length_penalty: float, early_stopping: int) -> None:
@@ -684,7 +652,7 @@ def beam_select(bs: BeamState, length_penalty: float, early_stopping: int) -> No
 def _beam_step_eager(model, bs: BeamState, length_penalty: float, early_stopping: int, fp8=None) -> None:
     st = bs.dec
     delta = _one_token_layers(model, st, st.ids, bs.table, fp8)
-    _head(model.config, model.arena, st, delta)
+    _head(model, st, delta, st.logits)
     beam_select(bs, length_penalty, early_stopping)
 
 
@@ -699,17 +667,7 @@ def beam_step(model, bs: BeamState, length_penalty: float, early_stopping: int, 
         _beam_step_eager(model, bs, length_penalty, early_stopping, fp8)
         return
     key = (model.arena.version, model.arena.shadow.data_ptr(), float(length_penalty), int(early_stopping), _fp8_key(fp8))
-    if bs.graph is None or bs.graph_key != key:
-        if bs.graph_key != ("warm",) + key:
-            bs.graph, bs.graph_key = None, ("warm",) + key
-            _beam_step_eager(model, bs, length_penalty, early_stopping, fp8)
-            return
-        torch.cuda.synchronize(bs.dec.device)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, capture_error_mode="thread_local"):
-            _beam_step_eager(model, bs, length_penalty, early_stopping, fp8)
-        bs.graph, bs.graph_key = g, key
-    bs.graph.replay()
+    _graphed(bs, key, bs.dec.device, lambda: _beam_step_eager(model, bs, length_penalty, early_stopping, fp8))
 
 
 def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R: int, length_penalty: float, early_stopping,
@@ -858,11 +816,9 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
 
     st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, *processors)
     st.out.fill_(pad)
+    prefill(model, st, comp, lens, fp8)
     if n > 1:
-        sample_prefill(model, st, comp, lens, fp8)
         ids = ids.repeat_interleave(n, dim=0)
-    else:
-        prefill(model, st, comp, lens, fp8)
     for t in range(1, max_new_tokens):
         if eos and t % FINISHED_CHECK_EVERY == 0 and bool(st.finished.all()):
             break

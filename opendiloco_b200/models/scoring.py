@@ -1,8 +1,9 @@
 """Per-token log-likelihood scoring for :class:`~opendiloco_b200.models.llama.LlamaForCausalLM` (``model.score``).
 
 Every row is compacted to start at position 0 and the batch is right-padded (to a multiple of 128 on the kernels), then
-runs the forward-only layer program of prefill (:func:`~opendiloco_b200.models.generation.forward_layers`); causal
-attention keeps the right padding away from the real positions.  The final-norm rows that predict a target are gathered
+runs generation's layer program with prefill's attention (QKV(+RoPE) GEMM and the causal attention forward,
+:func:`~opendiloco_b200.models.generation._prompt_attend`); causal attention keeps the right padding away from the real
+positions.  The final-norm rows that predict a target are gathered
 in output order and go through the LM head in chunks of at most ``SCORE_CHUNK`` rows:
 
     tc_gemm.lce_score           per 256-column plane: max, lowest argmax, sum exp(z - max), and the label logit
@@ -24,7 +25,7 @@ import torch
 from ..ops import kernels as K
 from ..ops import tc_gemm as TC
 from . import fp8_weights as W8
-from .generation import _PrefillBuffers, _round_up, forward_layers
+from .generation import Rows, _layers, _prompt_attend, _resident, _round_up
 
 SCORE_CHUNK = 32768                 # LM-head rows per scoring GEMM on the kernels
 REFERENCE_CHUNK = 4096              # the reference materialises an fp32 [rows, V] logits chunk
@@ -42,9 +43,8 @@ class ScoreState:
     statistics of one LM-head chunk."""
 
     def __init__(self, cfg, B: int, Sp: int, S: int, device, dtype, kernels: bool):
-        self.key = (B, Sp, S, str(device), dtype, kernels)
         n = B * S
-        self.pb = _PrefillBuffers(cfg, B * Sp, device, dtype)
+        self.pb = Rows(cfg, B * Sp, device, dtype)
         self.cos, self.sin = K.rope_tables(Sp, cfg.head_dim, cfg.rope_theta, device)
         self.xg = torch.empty(n, cfg.hidden_size, dtype=dtype, device=device)
         self.gidx = torch.empty(n, dtype=torch.int64, device=device)
@@ -58,13 +58,9 @@ class ScoreState:
 
 def score_state(model, B: int, Sp: int, S: int, kernels: bool) -> ScoreState:
     """The model's scoring state for this shape, allocated on first use; at most one is resident."""
-    eng, ar = model.engine, model.arena
-    key = (B, Sp, S, str(ar.device), ar.compute_dtype, kernels)
-    st = eng.score_state
-    if st is None or st.key != key:
-        eng.score_state = None                        # free the old buffers before allocating the new ones
-        st = eng.score_state = ScoreState(model.config, B, Sp, S, ar.device, ar.compute_dtype, kernels)
-    return st
+    ar = model.arena
+    return _resident(model, "score_state", (B, Sp, S, str(ar.device), ar.compute_dtype, kernels),
+                     lambda: ScoreState(model.config, B, Sp, S, ar.device, ar.compute_dtype, kernels))
 
 
 def _plan(cfg, input_ids, attention_mask, labels, kernels: bool):
@@ -131,7 +127,7 @@ def score(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = 
     pb.ids.copy_(comp.reshape(-1))
     st.gidx.copy_(gidx)
     st.labels.copy_(lab)
-    delta = forward_layers(model, pb, B, Sp, st.cos, st.sin, kernels, fp8=fp8)
+    delta = _layers(model, pb, pb.ids, _prompt_attend(model, pb, B, Sp, st.cos, st.sin, kernels, fp8), fp8)
     K.rmsnorm_fwd(pb.res, ar.w("model.norm.weight"), cfg.rms_norm_eps, delta=delta, out=pb.xn, rstd=pb.rstd, x_out=pb.res)
     K.embedding_fwd(st.gidx, pb.xn, out=st.xg)        # the row that predicts each output slot, in output order
     n = B * S

@@ -40,7 +40,7 @@ from .fp8w import dequantize_rows, quantize_rows_ref
 
 c_void_p, c_int, c_ll, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float
 _lib.register_optional("odb_dec_rope_append", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                               c_int, c_void_p, c_void_p, c_void_p])
+                                               c_int, c_int, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_kv_fill", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                            c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_attn_chunks", [c_int])
@@ -48,8 +48,6 @@ _lib.register_optional("odb_dec_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_vo
                                         c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_sample", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                           c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p])
-_lib.register_optional("odb_dec_rope_append_multi", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                                     c_int, c_int, c_int, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_verify_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int,
                                                c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_accept", [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -91,7 +89,7 @@ def usable(t: torch.Tensor, head_dim: int, Hq: int = 1, Hkv: int = 1) -> bool:
 def usable_verify(t: torch.Tensor, head_dim: int, Hq: int = 1, Hkv: int = 1) -> bool:
     """``usable`` plus the assisted-generation kernels (multi-token RoPE+append, verify attention, acceptance)."""
     return (usable(t, head_dim, Hq, Hkv) and _lib.has_symbol("odb_dec_verify_attn") and _lib.has_symbol("odb_dec_accept")
-            and _lib.has_symbol("odb_dec_rope_append_multi"))
+            and _lib.has_symbol("odb_dec_rope_append"))
 
 
 def usable_beam(t: torch.Tensor, head_dim: int, Hq: int, Hkv: int, V: int, num_beams: int, Smax: int) -> bool:
@@ -152,27 +150,8 @@ def _store_rows(cache: torch.Tensor, inv: torch.Tensor | None, index: tuple, x: 
 def rope_append(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, pos: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor,
                 Hq: int, Hkv: int, D: int, kinv: torch.Tensor | None = None, vinv: torch.Tensor | None = None) -> None:
     """qkv [B, (Hq+2*Hkv)*D] (one token per row): rotate q (in place) and k at position pos[b]; k, v -> cache[b, :, pos[b]]
-    (quantised with kinv / vinv: FP8 cache)."""
-    B = qkv.shape[0]
-    Smax = kc.shape[2]
-    if usable(qkv, D, Hq, Hkv):
-        assert qkv.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous() and pos.dtype == torch.int32
-        _check_fp8(kc, vc, kinv, vinv)
-        _lib.check(_lib.cuda_lib().odb_dec_rope_append(qkv.data_ptr(), qkv.stride(0), cos.data_ptr(), sin.data_ptr(), pos.data_ptr(),
-                                                       kc.data_ptr(), vc.data_ptr(), B, Hq, Hkv, Smax, _ptr(kinv), _ptr(vinv),
-                                                       _lib.stream_ptr(qkv)), "dec_rope_append")
-        _lib.count_launch()
-        return
-    half = D // 2
-    p = pos.long()
-    c, s = cos[p][:, None, :], sin[p][:, None, :]                     # [B, 1, D/2]
-    x = qkv[:, : (Hq + Hkv) * D].float().view(B, Hq + Hkv, D)
-    a, b = x[..., :half], x[..., half:]
-    rot = torch.cat([a * c - b * s, b * c + a * s], dim=-1).to(qkv.dtype)
-    qkv[:, : Hq * D] = rot[:, :Hq].reshape(B, Hq * D)
-    rows = torch.arange(B, device=qkv.device)
-    _store_rows(kc, kinv, (rows, slice(None), p), rot[:, Hq:])
-    _store_rows(vc, vinv, (rows, slice(None), p), qkv[:, (Hq + Hkv) * D:].view(B, Hkv, D))
+    (quantised with kinv / vinv: FP8 cache).  ``rope_append_multi`` with n = 1."""
+    _rope_append(qkv, cos, sin, pos, kc, vc, Hq, Hkv, D, 1, kinv, vinv, usable(qkv, D, Hq, Hkv))
 
 
 def kv_fill(qkv: torch.Tensor, lens: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, B: int, Sp: int, Hq: int, Hkv: int,
@@ -326,14 +305,19 @@ def rope_append_multi(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, p
                       Hq: int, Hkv: int, D: int, n: int, kinv: torch.Tensor | None = None, vinv: torch.Tensor | None = None) -> None:
     """qkv [n*B, row] slot-major: rotate q (in place) and k of row j*B + b at position pos[b] + j; k, v -> cache[b, :, pos[b] + j]
     (quantised with kinv / vinv: FP8 cache)."""
+    _rope_append(qkv, cos, sin, pos, kc, vc, Hq, Hkv, D, n, kinv, vinv, usable_verify(qkv, D, Hq, Hkv))
+
+
+def _rope_append(qkv, cos, sin, pos, kc, vc, Hq: int, Hkv: int, D: int, n: int, kinv, vinv, kernel: bool) -> None:
+    """The body of both: ``rope_append_kernel`` on grid (B, n) when ``kernel``, else the reference."""
     B = qkv.shape[0] // n
     Smax = kc.shape[2]
-    if usable_verify(qkv, D, Hq, Hkv):
+    if kernel:
         assert qkv.stride(1) == 1 and kc.is_contiguous() and vc.is_contiguous() and pos.dtype == torch.int32
         _check_fp8(kc, vc, kinv, vinv)
-        _lib.check(_lib.cuda_lib().odb_dec_rope_append_multi(qkv.data_ptr(), qkv.stride(0), cos.data_ptr(), sin.data_ptr(),
-                                                             pos.data_ptr(), kc.data_ptr(), vc.data_ptr(), B, n, Hq, Hkv, Smax,
-                                                             _ptr(kinv), _ptr(vinv), _lib.stream_ptr(qkv)), "dec_rope_append_multi")
+        _lib.check(_lib.cuda_lib().odb_dec_rope_append(qkv.data_ptr(), qkv.stride(0), cos.data_ptr(), sin.data_ptr(), pos.data_ptr(),
+                                                       kc.data_ptr(), vc.data_ptr(), B, n, Hq, Hkv, Smax, _ptr(kinv), _ptr(vinv),
+                                                       _lib.stream_ptr(qkv)), "dec_rope_append")
         _lib.count_launch()
         return
     half = D // 2

@@ -255,7 +255,7 @@ def test_round_is_one_graph_of_our_kernels():
     """Three rounds are three graph launches and no kernel launch, and the GPU runs only our kernels.  The profiler runs
     in a process of its own, so tracing graph replays leaves no profiler state behind for other tests."""
     ours = _our_kernel_names()
-    assert {"verify_attn_kernel", "verify_combine_kernel", "accept_kernel", "rope_append_multi_kernel"} <= ours
+    assert {"verify_attn_kernel", "combine_kernel", "accept_kernel", "rope_append_kernel"} <= ours
     env = dict(os.environ, ODB_CUDA_GRAPH="1")
     res = subprocess.run([sys.executable, "-c", _PROFILE_ROUNDS], capture_output=True, text=True, env=env, cwd=ROOT, timeout=600)
     assert res.returncode == 0, res.stderr[-4000:]
