@@ -7,8 +7,9 @@
 //   odb_dec_kv_fill       prefill: copy the (already rotated) k|v columns of the packed qkv rows into the cache
 //   odb_dec_attn          split-KV decode attention (flash-decoding) + the combine kernel that every split-KV attention
 //                         here (decode, grouped, verify) ends with
-//   odb_dec_sample        greedy / temperature + top-k + top-p sampler, one CTA per row, with HF's repetition penalty, n-gram
-//                         ban and min-new-tokens over the row's device-side token history when the control blocks ask
+//   odb_dec_sample        greedy / temperature + top-k + top-p + min-p sampler, one CTA per row, with HF's sequence bias,
+//                         repetition penalty, n-gram ban, bad words, min-length and min-new-tokens over the row's device-side
+//                         token history when the control blocks ask
 //   odb_dec_accept        assisted generation / prompt lookup: speculative acceptance of one round's proposals
 //   odb_dec_lookup_propose  prompt lookup: each row's proposals from an earlier occurrence of its last n-gram
 //   odb_dec_beam_topk     beam search: per vocabulary split of a row, the (max, sum-exp) partial and the local top-K logits
@@ -440,17 +441,76 @@ combine_kernel(const float* __restrict__ part_o, const float* __restrict__ part_
 
 // ------------------------------------------------------------------------------------------------ sampler
 // ictl (int64, device): [0] do_sample, [1] top_k, [2] seed, [3] pad_token_id, [4] number of EOS ids (<= 8), [5..12] EOS ids,
-//                       [13] no_repeat_ngram_size, [14] min_new_tokens
-// fctl (fp32, device):  [0] temperature, [1] top_p, [2] repetition_penalty
+//                       [13] no_repeat_ngram_size, [14] min_new_tokens, [15] min_length, [16] entries of the sequence table
+// fctl (fp32, device):  [0] temperature, [1] top_p, [2] repetition_penalty, [3] min_p
 constexpr int SAMPLE_THREADS = 1024;
 constexpr int MAX_EOS = 8;
-constexpr int CTL_NGRAM = 13, CTL_MIN_NEW = 14;
+constexpr int CTL_NGRAM = 13, CTL_MIN_NEW = 14, CTL_MIN_LEN = 15, CTL_N_SEQ = 16;
+constexpr int MAX_SEQS = 1024;                   // entries of a sequence table (sequence_bias + bad_words_ids)
 
 // ------------------------------------------------------------------------------------------------ logits processors
-// HF's repetition penalty, n-gram ban and min-new-tokens, applied to the fp32 value of each logit (sampler) or log-prob
-// (beam search).  The settings live in the control blocks, so a captured graph serves every value, "off" included.
+// HF's sequence bias, repetition penalty, n-gram ban, bad words, min-length and min-new-tokens, applied to the fp32 value of
+// each logit (sampler) or log-prob (beam search).  The settings live in the control blocks and the sequence table, so a
+// captured graph serves every value, "off" included.
 __device__ __forceinline__ bool processors_on(const long long* __restrict__ ictl, const float* __restrict__ fctl) {
-  return fctl[2] != 1.f || ictl[CTL_NGRAM] > 0 || (ictl[CTL_MIN_NEW] > 0 && ictl[4] > 0);
+  return fctl[2] != 1.f || ictl[CTL_NGRAM] > 0 || ((ictl[CTL_MIN_NEW] > 0 || ictl[CTL_MIN_LEN] > 0) && ictl[4] > 0) ||
+         ictl[CTL_N_SEQ] > 0;
+}
+
+// The sequence table of sequence_bias and bad_words_ids (ops/decode.py SeqTable): entry e is ids[off[e], off[e + 1]),
+// kind[e] 0 (a bias of bias[e] on its last token) or 1 (a ban of its last token); n = ictl[CTL_N_SEQ] entries.  The
+// bias entries come in HF's summation order: the length-1 sequences first, then the longer ones in dict order.
+struct SeqTable {
+  const int* off;                                // [MAX_SEQS + 1], then kind [MAX_SEQS], then the ids
+  const float* bias;
+  int n;
+  __device__ __forceinline__ const int* kind() const { return off + MAX_SEQS + 1; }
+  __device__ __forceinline__ const int* ids() const { return off + 2 * MAX_SEQS + 1; }
+  __device__ __forceinline__ int last(int e) const { return ids()[off[e + 1] - 1]; }
+};
+
+// Entry e matches the history h (HF's SequenceBiasLogitsProcessor rule): a length-1 sequence always; a longer one of length
+// n when L >= n and the history ends with its first n - 1 tokens.
+template <class H>
+__device__ __forceinline__ bool seq_match(const SeqTable& tab, int e, const H& h) {
+  const int o = tab.off[e], n = tab.off[e + 1] - o;
+  if (n == 1) return true;
+  if (h.L < n) return false;
+  const int* q = tab.ids() + o;
+  const int s = h.L - n + 1;
+  for (int k = 0; k < n - 1; ++k)
+    if (h[s + k] != q[k]) return false;
+  return true;
+}
+
+// Marks the table's matches whose last token lies in [lo, hi): a matched ban sets its bit of ban; a matched bias sets bit
+// e of matched (shared, MAX_SEQS / 32 words, zero on entry) and the token's bit of biased (when not null).  The caller
+// synchronises.
+template <class H>
+__device__ void mark_sequences(const SeqTable& tab, const H& h, int lo, int hi, unsigned* ban, unsigned* biased, unsigned* matched) {
+  for (int e = threadIdx.x; e < tab.n; e += blockDim.x) {
+    const int v = tab.last(e);
+    if (v < lo || v >= hi || !seq_match(tab, e, h)) continue;
+    if (tab.kind()[e] != 0) {
+      atomicOr(ban + ((v - lo) >> 5), 1u << ((v - lo) & 31));
+    } else {
+      atomicOr(matched + (e >> 5), 1u << (e & 31));
+      if (biased != nullptr) atomicOr(biased + ((v - lo) >> 5), 1u << ((v - lo) & 31));
+    }
+  }
+}
+
+// After mark_sequences: for the matched bias entry e, whether it is the first matched one of its token, and then the sum
+// of the matched biases of that token in table order, starting from 0 (HF's fp32 order, so the result is its bit pattern).
+// last (optional): the entries' last tokens staged in shared memory, so the scans read no global memory per entry.
+__device__ __forceinline__ bool seq_bias_sum(const SeqTable& tab, const unsigned* matched, const int* last, int e, int v, float& sum) {
+  for (int f = 0; f < e; ++f)
+    if (((matched[f >> 5] >> (f & 31)) & 1u) && (last != nullptr ? last[f] : tab.last(f)) == v) return false;
+  float s = 0.f;
+  for (int f = e; f < tab.n; ++f)
+    if (((matched[f >> 5] >> (f & 31)) & 1u) && (last != nullptr ? last[f] : tab.last(f)) == v) s = __fadd_rn(s, tab.bias[f]);
+  sum = s;
+  return true;
 }
 
 // HF's RepetitionPenaltyLogitsProcessor on one value.
@@ -502,14 +562,17 @@ struct RawLogit {
   const __nv_bfloat16* row;
   __device__ __forceinline__ float operator()(int i) const { return __bfloat162float(row[i]); }
 };
+// With a sequence table, bias (not null) is the row's summed bias per token (0 where none, as HF's); the bias comes first.
 struct ProcessedLogit {
   const __nv_bfloat16* row;
   const unsigned* pen;
   const unsigned* ban;
   float p;
+  const float* bias;
   __device__ __forceinline__ float operator()(int i) const {
     float x = __bfloat162float(row[i]);
     const unsigned bit = 1u << (i & 31);
+    if (bias != nullptr) x = __fadd_rn(x, __ldcg(bias + i));
     if (__ldcg(pen + (i >> 5)) & bit) x = penalise(x, p);
     if (__ldcg(ban + (i >> 5)) & bit) x = -INFINITY;
     return x;
@@ -585,10 +648,11 @@ __device__ __forceinline__ float warped_weight(float x, float temp, float mx) {
   return exp2f((x / temp - mx) * 1.4426950408889634f);
 }
 
-// HF warper order: temperature, then top-k, then top-p.  Fills e[i] with the kept weights (0 elsewhere) and returns the
-// threshold T on the weight's bit pattern: token i is kept iff bits(warped_weight(x_i)) >= T.  mx = max logit / temp.
+// HF warper order: temperature, then top-k, then top-p, then min-p.  Fills e[i] with the kept weights (0 elsewhere) and
+// returns the threshold T on the weight's bit pattern: token i is kept iff bits(warped_weight(x_i)) >= T.  mx = max logit
+// / temp, so the top weight is 1 and min-p (keep p_i >= min_p * p_max) keeps e_i >= min_p: one more bit-pattern threshold.
 template <class Load>
-__device__ uint32_t warp_weights(Load x, int V, float temp, int top_k, float top_p, float mx, float* e, float* red) {
+__device__ uint32_t warp_weights(Load x, int V, float temp, int top_k, float top_p, float min_p, float mx, float* e, float* red) {
   const int tid = threadIdx.x;
   uint32_t T = 0;
   for (int i = tid; i < V; i += blockDim.x) e[i] = warped_weight(x(i), temp, mx);
@@ -609,11 +673,18 @@ __device__ uint32_t warp_weights(Load x, int V, float temp, int top_k, float top
     __syncthreads();
     T = max(T, t);
   }
+  if (min_p > 0.f) {
+    const uint32_t t = __float_as_uint(min_p);
+    for (int i = tid; i < V; i += blockDim.x)
+      if (__float_as_uint(e[i]) < t) e[i] = 0.f;
+    __syncthreads();
+    T = max(T, t);
+  }
   return T;
 }
-__device__ uint32_t warp_weights(const __nv_bfloat16* __restrict__ row, int V, float temp, int top_k, float top_p, float mx, float* e,
-                                 float* red) {
-  return warp_weights(RawLogit{row}, V, temp, top_k, top_p, mx, e, red);
+__device__ uint32_t warp_weights(const __nv_bfloat16* __restrict__ row, int V, float temp, int top_k, float top_p, float min_p, float mx,
+                                 float* e, float* red) {
+  return warp_weights(RawLogit{row}, V, temp, top_k, top_p, min_p, mx, e, red);
 }
 
 // Inverse CDF in index order over the weights e[0, V): u in (0, 1] picks the token; `fallback` when rounding leaves r
@@ -674,7 +745,7 @@ __device__ int pick_token(Load x, int V, const long long* __restrict__ ictl, con
   int tok = best.i;
   if (do_sample && top_k != 1 && (!finite_only || best.v > -INFINITY)) {
     const float temp = fctl[0], top_p = fctl[1];
-    warp_weights(x, V, temp, top_k, top_p, best.v / temp, e, red);
+    warp_weights(x, V, temp, top_k, top_p, fctl[3], best.v / temp, e, red);
     curandStatePhilox4_32_10_t rng;
     curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)g, &rng);
     tok = draw_index(e, V, curand_uniform(&rng), best.i, red, tok_sm);   // u in (0, 1]
@@ -682,18 +753,39 @@ __device__ int pick_token(Load x, int V, const long long* __restrict__ ictl, con
   return tok;
 }
 
+// The sampler's sequence-table pass over a whole row: stage the entries' last tokens in last_sm, mark the matches (bans
+// into ban), and store each biased token's summed bias in the row's zeroed bias.  Out of line, so its registers do not
+// add to sample_kernel's.  Ends with a barrier.
+__device__ __noinline__ void sample_sequences(const SeqTable tab, const History hh, int V, unsigned* ban, unsigned* matched, int* last_sm,
+                                              float* bias) {
+  for (int i = threadIdx.x; i < tab.n; i += blockDim.x) last_sm[i] = tab.last(i);
+  mark_sequences(tab, hh, 0, V, ban, nullptr, matched);
+  __syncthreads();
+  for (int i = threadIdx.x; i < tab.n; i += blockDim.x) {
+    float sum;
+    if (((matched[i >> 5] >> (i & 31)) & 1u) && seq_bias_sum(tab, matched, last_sm, i, last_sm[i], sum)) bias[last_sm[i]] = sum;
+  }
+  __syncthreads();
+}
+
 // With a history (hist int32 [B, ldh]: row b's tokens at positions 0 .. pos[b]), the logits processors run when the control
 // blocks turn them on: the row's bitmaps (scratch [B][2][nw] words, nw = ceil(V / 32): penalised, banned) are cleared and
 // marked, and the token is picked from the processed values.  The emitted token is appended at hist[b, pos[b] + 1].
+// With a sequence table (tab_off not null, ictl[CTL_N_SEQ] > 0), seq_scratch fp32 [B][V] (zero when the kernel starts, and
+// again when it ends) takes the row's summed bias at the matched tokens, which are set back to 0 once the token is
+// picked: the clearing costs one store per matched table entry, not a pass over V.
 __global__ void __launch_bounds__(SAMPLE_THREADS)
 sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const long long* __restrict__ ictl,
               const float* __restrict__ fctl, int* __restrict__ pos, int* __restrict__ gen, int* __restrict__ finished,
               long long* __restrict__ out, int max_new, long long* __restrict__ ids_next, int* __restrict__ hist, int ldh,
-              unsigned* __restrict__ scratch) {
+              unsigned* __restrict__ scratch, const int* __restrict__ tab_off, const float* __restrict__ tab_bias,
+              float* __restrict__ seq_scratch) {
   extern __shared__ __align__(16) float e[];     // [V] exp(x - max) of the kept tokens, 0 elsewhere
   __shared__ float red[33];
   __shared__ ArgMax am[32];
   __shared__ int tok_sm;
+  __shared__ unsigned matched[MAX_SEQS / 32];
+  __shared__ int last_sm[MAX_SEQS];
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x, tid = threadIdx.x;
@@ -703,13 +795,23 @@ sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, con
     const int nw = ceil_div(V, 32), L = pos[b] + 1, g = gen[b];
     unsigned* pen = scratch + (long long)b * 2 * nw;
     unsigned* ban = pen + nw;
+    const SeqTable tab{tab_off, tab_bias, tab_off != nullptr ? (int)min(ictl[CTL_N_SEQ], (long long)MAX_SEQS) : 0};
+    float* bias = tab.n > 0 ? seq_scratch + (long long)b * V : nullptr;
     for (int i = tid; i < 2 * nw; i += blockDim.x) pen[i] = 0u;
+    for (int i = tid; i < MAX_SEQS / 32; i += blockDim.x) matched[i] = 0u;
     __syncthreads();
     const float p = fctl[2];
     const int* h = hist + (long long)b * ldh;
-    mark_history(History{h, h, L, L}, 0, V, p != 1.f, (int)ictl[CTL_NGRAM], g < ictl[CTL_MIN_NEW], ictl, pen, ban);
+    const History hh{h, h, L, L};
+    mark_history(hh, 0, V, p != 1.f, (int)ictl[CTL_NGRAM], g < ictl[CTL_MIN_NEW] || L < ictl[CTL_MIN_LEN], ictl, pen, ban);
+    if (bias != nullptr) sample_sequences(tab, hh, V, ban, matched, last_sm, bias);
     __syncthreads();
-    tok = pick_token(ProcessedLogit{row, pen, ban, p}, V, ictl, fctl, b, g, true, e, red, am, &tok_sm);
+    tok = pick_token(ProcessedLogit{row, pen, ban, p, bias}, V, ictl, fctl, b, g, true, e, red, am, &tok_sm);
+    if (bias != nullptr) {
+      __syncthreads();                           // every read of bias is done
+      for (int i = tid; i < tab.n; i += blockDim.x)
+        if ((matched[i >> 5] >> (i & 31)) & 1u) bias[last_sm[i]] = 0.f;
+    }
   } else {
     tok = pick_token(RawLogit{row}, V, ictl, fctl, b, gen[b], false, e, red, am, &tok_sm);
   }
@@ -979,7 +1081,7 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
   }
   const bool greedy = !(ictl[0] != 0 && ictl[1] != 1);
   const int top_k = (int)ictl[1];
-  const float temp = fctl[0], top_p = fctl[1];
+  const float temp = fctl[0], top_p = fctl[1], min_p = fctl[3];
   const int g0 = gen[b];
   const int c = cnt != nullptr ? min(max(cnt[b], 0), K) : K;   // candidates of this row
   int n_acc = 0, t_new = 0;
@@ -996,7 +1098,7 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
       break;
     }
     const float mxp = pm.v / temp;
-    const uint32_t Tp = warp_weights(prow, V, temp, top_k, top_p, mxp, e, red);
+    const uint32_t Tp = warp_weights(prow, V, temp, top_k, top_p, min_p, mxp, e, red);
     curandStatePhilox4_32_10_t rng;
     curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)g0 * 16ull + 2ull * i, &rng);
     const float u_acc = curand_uniform(&rng), u_draw = curand_uniform(&rng);    // (0, 1]
@@ -1025,7 +1127,7 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
     }
     const __nv_bfloat16* qrow = qlog + ((long long)i * B + b) * ldq;
     const ArgMax qm = block_argmax(qrow, V, am);   // starts with a barrier: every thread has read e[d]
-    warp_weights(qrow, V, temp, top_k, top_p, qm.v / temp, e, red);
+    warp_weights(qrow, V, temp, top_k, top_p, min_p, qm.v / temp, e, red);
     float zq = 0.f;
     for (int v = tid; v < V; v += blockDim.x) zq += e[v];
     zq = block_sum(zq, red);
@@ -1169,14 +1271,22 @@ __device__ __forceinline__ void split_topk(const float* key, unsigned avail, int
 // token's log-prob (z - lse) * p is monotone in z within the penalised tokens, but not against the others, so the split
 // gives two lists: cand[..][0..K) the best of the unpenalised tokens, with the banned ones (any class) as -inf, and
 // cand[..][K..2K) the best of the penalised tokens that are not banned, by their raw logits.  beam_step maps and merges them.
+//
+// With a sequence table (tab_off not null, ictl[CTL_N_SEQ] > 0), a biased token (z - lse + bias, then maybe penalised) is
+// monotone with neither list, so the biased tokens that are not banned leave both lists.  The split owns the table entries
+// whose last token it holds, and writes slot [r][e] of each: for the first matched bias entry of a token, the token (with
+// SLOT_PEN when it is penalised), its raw logit and its summed bias (seq_bias_sum); -1 for every other entry.  Every slot
+// below ictl[CTL_N_SEQ] is written every step, so nothing needs clearing; beam_step scores the slots exactly.
+constexpr int SLOT_PEN = 1 << 30;
 __global__ void __launch_bounds__(TOPK_THREADS)
 beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, int K, int ck, float* __restrict__ part_ml,
                  float* __restrict__ cand_v, int* __restrict__ cand_i, const long long* __restrict__ ictl, const float* __restrict__ fctl,
                  const int* __restrict__ prompt, int ldp, const int* __restrict__ plens, const int* __restrict__ run_seq,
-                 const int* __restrict__ tstep, int nb, int max_new) {
+                 const int* __restrict__ tstep, int nb, int max_new, const int* __restrict__ tab_off, const float* __restrict__ tab_bias,
+                 int* __restrict__ slot_i, float2* __restrict__ slot_v) {
   __shared__ float red[33];
   __shared__ ArgMax am[32];
-  __shared__ unsigned pen_sm[TOPK_SPLIT / 32], ban_sm[TOPK_SPLIT / 32];
+  __shared__ unsigned pen_sm[TOPK_SPLIT / 32], ban_sm[TOPK_SPLIT / 32], bsd_sm[TOPK_SPLIT / 32], matched[MAX_SEQS / 32];
   pdl_launch_dependents();
   pdl_wait();
   const int s = blockIdx.x, r = blockIdx.y, ns = gridDim.x, tid = threadIdx.x;
@@ -1213,18 +1323,36 @@ beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, 
   }
   // ---- processors: this split's bits of the row's penalised and banned tokens
   const int g = r / nb, t = tstep[g], rows = gridDim.y;
-  for (int i = tid; i < TOPK_SPLIT / 32; i += TOPK_THREADS) pen_sm[i] = ban_sm[i] = 0u;
+  const SeqTable tab{tab_off, tab_bias, tab_off != nullptr ? (int)min(ictl[CTL_N_SEQ], (long long)MAX_SEQS) : 0};
+  for (int i = tid; i < TOPK_SPLIT / 32; i += TOPK_THREADS) pen_sm[i] = ban_sm[i] = bsd_sm[i] = 0u;
+  for (int i = tid; i < MAX_SEQS / 32; i += TOPK_THREADS) matched[i] = 0u;
   __syncthreads();
   const float p = fctl[2];
   const History h{prompt + (long long)g * ldp, run_seq + ((long long)(t & 1) * rows + r) * max_new, plens[g], plens[g] + t};
-  mark_history(h, base, base + TOPK_SPLIT, p != 1.f, (int)ictl[CTL_NGRAM], t < ictl[CTL_MIN_NEW], ictl, pen_sm, ban_sm);
+  mark_history(h, base, base + TOPK_SPLIT, p != 1.f, (int)ictl[CTL_NGRAM], t < ictl[CTL_MIN_NEW] || h.L < ictl[CTL_MIN_LEN], ictl,
+               pen_sm, ban_sm);
+  if (tab.n > 0) mark_sequences(tab, h, base, base + TOPK_SPLIT, ban_sm, bsd_sm, matched);
   __syncthreads();
+  for (int e = tid; e < tab.n; e += TOPK_THREADS) {
+    const int v = tab.last(e);
+    if (v < base || v >= base + TOPK_SPLIT) continue;
+    const int j = v - base;
+    float sum;
+    int si = -1;
+    if (((matched[e >> 5] >> (e & 31)) & 1u) && !((ban_sm[j >> 5] >> (j & 31)) & 1u) && seq_bias_sum(tab, matched, nullptr, e, v, sum)) {
+      const float z = __bfloat162float(row[v]);
+      si = v | (((pen_sm[j >> 5] >> (j & 31)) & 1u) ? SLOT_PEN : 0);
+      slot_v[(long long)r * MAX_SEQS + e] = make_float2(z == z ? z : -INFINITY, sum);
+    }
+    slot_i[(long long)r * MAX_SEQS + e] = si;
+  }
   unsigned in_pen = 0u;
 #pragma unroll
   for (int e = 0; e < TOPK_PER; ++e) {
     const int j = e * TOPK_THREADS + tid;
     const unsigned bit = 1u << (j & 31);
     if (ban_sm[j >> 5] & bit) x[e] = -INFINITY;
+    else if (bsd_sm[j >> 5] & bit) valid &= ~(1u << e);       // scored by beam_step from its slot
     else if (pen_sm[j >> 5] & bit) in_pen |= 1u << e;
   }
   in_pen &= valid;
@@ -1247,12 +1375,16 @@ beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, 
 // += 1, and the finished scores, flags and histories.  A prompt that is done is left untouched (parents = itself).
 // Candidate rows hold ck entries.  With the logits processors on (fctl not null; see beam_topk_kernel) each thread also
 // owns the split's penalised list, scored penalise(logit - lse, p) + run_score, and offers the better of its two heads.
+// With a sequence table (slot_i not null, ictl[CTL_N_SEQ] = n > 0) thread l also owns the slots l, l + 512, ... of the
+// prompt's nb * n (beam, entry) slots: each valid one is a candidate scored (logit - lse) + bias, penalised when marked,
+// + run_score; the thread offers the best of its untaken ones too.
 __global__ void __launch_bounds__(STEP_THREADS)
 beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ cand_v, const int* __restrict__ cand_i, int ns, int V,
                  int nb, int K, int ck, const long long* __restrict__ ictl, const float* __restrict__ fctl, float length_penalty,
                  int early_stopping, int max_new, float* __restrict__ run_score, float* __restrict__ fin_score, int* __restrict__ fin_flag,
                  int* __restrict__ run_seq, int* __restrict__ fin_seq, int* __restrict__ unsat, int* __restrict__ done,
-                 int* __restrict__ tstep, int* __restrict__ pos, long long* __restrict__ ids_next, int* __restrict__ parent) {
+                 int* __restrict__ tstep, int* __restrict__ pos, long long* __restrict__ ids_next, int* __restrict__ parent,
+                 const int* __restrict__ slot_i, const float2* __restrict__ slot_v) {
   __shared__ ArgMax am[32];
   __shared__ float lse[MAX_BEAMS];
   __shared__ float sel_v[MAX_KEEP], fcand[MAX_KEEP];
@@ -1287,10 +1419,12 @@ beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ ca
   const int nl = nb * ns, jb = tid / ns, sp = tid % ns;
   const bool two = fctl != nullptr && processors_on(ictl, fctl);
   const float pen = two ? fctl[2] : 1.f;
+  const int nseq = two && slot_i != nullptr ? (int)min(ictl[CTL_N_SEQ], (long long)MAX_SEQS) : 0;
   int head = 0, head2 = 0;
+  unsigned taken3 = 0u;                          // bit m: slot tid + m * STEP_THREADS was selected (nb * nseq <= 16 * 512)
   for (int k = 0; k < K; ++k) {
     ArgMax c{-INFINITY, INT_MAX};
-    bool second = false;
+    int src = 0;                                 // 0: first list, 1: penalised list, 2 + m: slot m of this thread
     if (tid < nl) {
       const long long at = ((long long)(row0 + jb) * ns + sp) * ck;
       if (head < K) {
@@ -1303,14 +1437,30 @@ beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ ca
           const ArgMax c2{penalise(cand_v[at + K + head2] - lse[jb], pen) + run_score[row0 + jb], jb * V + ci};
           if (argmax_merge(c, c2).i == c2.i) {
             c = c2;
-            second = true;
+            src = 1;
           }
         }
       }
     }
+    for (int m = 0, q = tid; q < nb * nseq; ++m, q += STEP_THREADS) {
+      if ((taken3 >> m) & 1u) continue;
+      const int jq = q / nseq;
+      const long long at = (long long)(row0 + jq) * MAX_SEQS + q % nseq;
+      const int si = slot_i[at];
+      if (si < 0) continue;
+      const float2 zb = slot_v[at];
+      float v = __fadd_rn(zb.x - lse[jq], zb.y);
+      if (si & SLOT_PEN) v = penalise(v, pen);
+      const ArgMax c3{v + run_score[row0 + jq], jq * V + (si & (SLOT_PEN - 1))};
+      if (argmax_merge(c, c3).i == c3.i) {
+        c = c3;
+        src = 2 + m;
+      }
+    }
     const ArgMax w = block_reduce_argmax(c, am);
-    if (tid < nl && c.i != INT_MAX && w.i == c.i) {           // beam * V + token is unique to one list
-      if (second) ++head2;
+    if (c.i != INT_MAX && w.i == c.i) {          // beam * V + token is unique to one list or slot
+      if (src >= 2) taken3 |= 1u << (src - 2);
+      else if (src == 1) ++head2;
       else ++head;
     }
     if (tid == 0) {
@@ -1707,8 +1857,9 @@ ODB_EXPORT int odb_dec_attn_group_splits(int rows, int ngrp, int Hq, int Hkv, in
 // ids_next int64 [B]; hist: nullptr (no logits processors), or int32 [B, ldh] with scratch int32 [B, 2 * ceil(V / 32)].
 // The vocabulary lives in shared memory as fp32: V <= 56000.
 ODB_EXPORT int odb_dec_sample(const void* logits, long long ld, int V, const void* ictl, const void* fctl, void* pos, void* gen,
-                              void* finished, void* out, int max_new, void* ids_next, void* hist, int ldh, void* scratch, int B,
-                              cudaStream_t st) {
+                              void* finished, void* out, int max_new, void* ids_next, void* hist, int ldh, void* scratch,
+                              const void* tab_off, const void* tab_bias, void* seq_scratch, int B, cudaStream_t st) {
+  if (tab_off != nullptr && (hist == nullptr || tab_bias == nullptr || seq_scratch == nullptr)) return -1;
   const int smem = V * 4;
   if (smem > 224000) return -1;
   static int attr = 0;
@@ -1719,7 +1870,8 @@ ODB_EXPORT int odb_dec_sample(const void* logits, long long ld, int V, const voi
   }
   launch_pdl(dec::sample_kernel, dim3(B), dim3(dec::SAMPLE_THREADS), smem, st, (const __nv_bfloat16*)logits, ld, V,
              (const long long*)ictl, (const float*)fctl, (int*)pos, (int*)gen, (int*)finished, (long long*)out, max_new,
-             (long long*)ids_next, (int*)hist, ldh, (unsigned*)scratch);
+             (long long*)ids_next, (int*)hist, ldh, (unsigned*)scratch, (const int*)tab_off, (const float*)tab_bias,
+             (float*)seq_scratch);
   ODB_CHECK_LAST();
   return 0;
 }
@@ -1816,11 +1968,14 @@ ODB_EXPORT int odb_dec_beam_splits(int V) { return odb::ceil_div(V, dec::TOPK_SP
 // plens / tstep int32 [rows / nb] and run_seq int32 [2, rows, max_new] (see dec::beam_topk_kernel).
 ODB_EXPORT int odb_dec_beam_topk(const void* logits, long long ld, int V, int K, int ck, void* part_ml, void* cand_v, void* cand_i,
                                  const void* ictl, const void* fctl, const void* prompt, int ldp, const void* plens, const void* run_seq,
-                                 const void* tstep, int nb, int max_new, int rows, cudaStream_t st) {
+                                 const void* tstep, int nb, int max_new, int rows, const void* tab_off, const void* tab_bias, void* slot_i,
+                                 void* slot_v, cudaStream_t st) {
   if (K < 1 || K > dec::MAX_KEEP || V < K || ck < K || (fctl != nullptr && (ck < 2 * K || nb < 1 || rows % nb))) return -1;
+  if (tab_off != nullptr && (fctl == nullptr || tab_bias == nullptr || slot_i == nullptr || slot_v == nullptr)) return -1;
   launch_pdl(dec::beam_topk_kernel, dim3(odb::ceil_div(V, dec::TOPK_SPLIT), rows), dim3(dec::TOPK_THREADS), 0, st,
              (const __nv_bfloat16*)logits, ld, V, K, ck, (float*)part_ml, (float*)cand_v, (int*)cand_i, (const long long*)ictl,
-             (const float*)fctl, (const int*)prompt, ldp, (const int*)plens, (const int*)run_seq, (const int*)tstep, nb, max_new);
+             (const float*)fctl, (const int*)prompt, ldp, (const int*)plens, (const int*)run_seq, (const int*)tstep, nb, max_new,
+             (const int*)tab_off, (const float*)tab_bias, (int*)slot_i, (float2*)slot_v);
   ODB_CHECK_LAST();
   return 0;
 }
@@ -1832,7 +1987,7 @@ ODB_EXPORT int odb_dec_beam_topk(const void* logits, long long ld, int V, int K,
 ODB_EXPORT int odb_dec_beam_step(const void* part_ml, const void* cand_v, const void* cand_i, int V, int nb, int K, int ck,
                                  const void* ictl, const void* fctl, float length_penalty, int early_stopping, int max_new, void* run_score,
                                  void* fin_score, void* fin_flag, void* run_seq, void* fin_seq, void* unsat, void* done, void* tstep,
-                                 void* pos, void* ids_next, void* parent, int B, cudaStream_t st) {
+                                 void* pos, void* ids_next, void* parent, const void* slot_i, const void* slot_v, int B, cudaStream_t st) {
   const int ns = odb::ceil_div(V, dec::TOPK_SPLIT);
   if (nb < 1 || nb > dec::MAX_BEAMS || K < 1 || K > dec::MAX_KEEP || nb * ns > dec::STEP_THREADS || early_stopping < 0 ||
       early_stopping > 2 || max_new < 1 || ck < K || (fctl != nullptr && ck < 2 * K))
@@ -1841,7 +1996,7 @@ ODB_EXPORT int odb_dec_beam_step(const void* part_ml, const void* cand_v, const 
              (const int*)cand_i, ns, V, nb, K, ck, (const long long*)ictl, (const float*)fctl, length_penalty, early_stopping, max_new,
              (float*)run_score,
              (float*)fin_score, (int*)fin_flag, (int*)run_seq, (int*)fin_seq, (int*)unsat, (int*)done, (int*)tstep, (int*)pos,
-             (long long*)ids_next, (int*)parent);
+             (long long*)ids_next, (int*)parent, (const int*)slot_i, (const float2*)slot_v);
   ODB_CHECK_LAST();
   return 0;
 }

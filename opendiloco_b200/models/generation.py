@@ -152,6 +152,9 @@ class DecodeState(Rows):
         # token histories of the logits processors: the real prompt tokens, then the generated ones (the sampler appends)
         self.hist = torch.zeros(B, Smax, dtype=torch.int32, device=device)
         self.proc_scratch = torch.zeros(B, 2 * ((V + 31) // 32), dtype=torch.int32, device=device)
+        # sequence_bias / bad_words_ids: the fixed-capacity table and the sampler's zeroed bias rows, allocated on first use
+        self.seq: DK.SeqTable | None = None
+        self.seq_scratch: torch.Tensor | None = None
         self.kernels = DK.usable(self.res, D, Hq, Hkv)
         self.part_o = self.part_ml = None
         if self.kernels:
@@ -171,9 +174,18 @@ class DecodeState(Rows):
         return self._prefill
 
     def set_controls(self, do_sample: bool, temperature: float, top_k: int, top_p: float, seed: int, pad: int, eos: list[int],
-                     repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_new_tokens: int = 0):
+                     repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_new_tokens: int = 0, min_length: int = 0,
+                     min_p: float = 0.0, entries: list | None = None):
+        """The control blocks, and the sequence table's ``entries`` (``DK.sequence_entries``; None or empty: none).  The
+        table and the sampler's bias rows are allocated the first time there are entries and rewritten in place after."""
+        entries = entries or []
+        if entries and self.seq is None:
+            self.seq = DK.SeqTable(self.device)
+            self.seq_scratch = torch.zeros(self.B, self.cfg.vocab_size, dtype=torch.float32, device=self.device)
+        if self.seq is not None:
+            self.seq.set(entries)
         ictl, fctl = DK.make_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, "cpu", repetition_penalty,
-                                      no_repeat_ngram_size, min_new_tokens)
+                                      no_repeat_ngram_size, min_new_tokens, min_length, min_p, len(entries))
         self.ictl.copy_(ictl)
         self.fctl.copy_(fctl)
 
@@ -266,7 +278,8 @@ def _head(model, buf: Rows, delta, logits) -> None:
 
 def _head_and_sample(model, st: DecodeState, delta) -> None:
     _head(model, st, delta, st.logits)
-    DK.sample(st.logits, st.ictl, st.fctl, st.pos, st.gen, st.finished, st.out, st.ids, st.hist, st.proc_scratch)
+    DK.sample(st.logits, st.ictl, st.fctl, st.pos, st.gen, st.finished, st.out, st.ids, st.hist, st.proc_scratch, st.seq,
+              st.seq_scratch)
 
 
 # ------------------------------------------------------------------------------------------------ prefill
@@ -352,14 +365,15 @@ def step(model, st: DecodeState, graph: bool | None = None, fp8=None) -> None:
     """One decode step: consume st.ids at st.pos, sample the next token into st.ids / st.out.  With the kernels and
     ``graph`` (default: ``ODB_CUDA_GRAPH`` != 0) the first call runs eagerly (warm-up), the second captures the step and
     every call replays it.  ``fp8``: the model's FP8 weights (None: the arena weights).  Multi-sample rows (st.group > 1)
-    attend through st.table; the group and the table are part of the graph key."""
+    attend through st.table; the group and the table are part of the graph key, and so is whether the state has a sequence
+    table (its entries and sizes are not: the graph reads them from device memory)."""
     if graph is None:
         graph = _use_graph()
     if not (graph and st.kernels):
         _step_eager(model, st, fp8)
         return
     key = (model.arena.version, model.arena.shadow.data_ptr(), st.group, st.table.data_ptr() if st.table is not None else None,
-           _fp8_key(fp8))
+           st.seq is not None, _fp8_key(fp8))
     _graphed(st, key, st.device, lambda: _step_eager(model, st, fp8))
 
 
@@ -528,18 +542,19 @@ def _check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size, assistant_m
 
 
 def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int, Kp: int, controls: tuple, pad: int,
-                       eos: list[int], ngram: int = 2, fp8=None, fp8_kv: bool = False) -> torch.Tensor:
+                       eos: list[int], ngram: int = 2, fp8=None, fp8_kv: bool = False, min_p: float = 0.0) -> torch.Tensor:
     """Assisted generation with ``assistant``, or prompt lookup (n-grams up to ``ngram``) with ``assistant`` None.
-    ``fp8_kv``: the target's cache is FP8 (the draft's stays bf16)."""
+    ``fp8_kv``: the target's cache is FP8 (the draft's stays bf16).  ``min_p`` goes to both control blocks: the acceptance
+    computes q with the target's, so the draft must draw from the same warped law."""
     B = comp.shape[0]
     Smax = _round_up(P + max_new_tokens + Kp, 128)
     tst = decode_state(model, B, Smax, fp8_kv)
     ast = assisted_state(model, assistant, B, Kp, Smax)
     dst = ast.draft
     do_sample, temperature, top_k, top_p, seed = controls
-    tst.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos)
+    tst.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, min_p=min_p)
     if dst is not None:
-        dst.set_controls(do_sample, temperature, top_k, top_p, seed ^ DRAFT_SEED_XOR, 0, [])
+        dst.set_controls(do_sample, temperature, top_k, top_p, seed ^ DRAFT_SEED_XOR, 0, [], min_p=min_p)
     tst.out.fill_(pad)
     prefill(model, tst, comp, lens, fp8)              # also leaves each row's history in tst.hist
     if dst is not None:
@@ -598,6 +613,7 @@ class BeamState:
             self.part_ml = f32(rows, nsp, 2)
             # two lists of K per split: the unpenalised and the penalised tokens (the second one only with the processors on)
             self.cand_v, self.cand_i = f32(rows, nsp, 2 * K), i32(rows, nsp, 2 * K)
+        self.slot_i = self.slot_v = None             # the biased tokens of sequence_bias (kernels), with the table
         self.graph = None
         self.graph_key = None
 
@@ -645,7 +661,8 @@ def beam_select(bs: BeamState, length_penalty: float, early_stopping: int) -> No
     st = bs.dec
     DK.beam_select(st.logits, st.ictl, bs.nb, bs.K, length_penalty, early_stopping, bs.max_new, bs.run_score, bs.fin_score,
                    bs.fin_flag, bs.run_seq, bs.fin_seq, bs.unsat, bs.done, bs.tstep, st.pos, st.ids, bs.parent, bs.part_ml,
-                   bs.cand_v, bs.cand_i, fctl=st.fctl, prompt=bs.prompt, plens=bs.plens)
+                   bs.cand_v, bs.cand_i, fctl=st.fctl, prompt=bs.prompt, plens=bs.plens, table=st.seq, slot_i=bs.slot_i,
+                   slot_v=bs.slot_v)
     DK.beam_reorder(st.kv, bs.table, bs.parent, st.pos, bs.nb, inv=st.kv_inv)
 
 
@@ -666,17 +683,22 @@ def beam_step(model, bs: BeamState, length_penalty: float, early_stopping: int, 
     if not (graph and bs.kernels):
         _beam_step_eager(model, bs, length_penalty, early_stopping, fp8)
         return
-    key = (model.arena.version, model.arena.shadow.data_ptr(), float(length_penalty), int(early_stopping), _fp8_key(fp8))
+    key = (model.arena.version, model.arena.shadow.data_ptr(), float(length_penalty), int(early_stopping), bs.dec.seq is not None,
+           _fp8_key(fp8))
     _graphed(bs, key, bs.dec.device, lambda: _beam_step_eager(model, bs, length_penalty, early_stopping, fp8))
 
 
 def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R: int, length_penalty: float, early_stopping,
                    pad: int, eos: list[int], processors: tuple = (1.0, 0, 0), fp8=None,
-                   fp8_kv: bool = False) -> tuple[torch.Tensor, torch.Tensor]:
+                   fp8_kv: bool = False, min_length: int = 0, entries: list | None = None) -> tuple[torch.Tensor, torch.Tensor]:
     B, Sp = comp.shape
     es = DK.EARLY_STOPPING[early_stopping]
     bs = beam_state(model, B, nb, DK.beams_to_keep(nb, len(eos)), max_new_tokens, Smax, fp8_kv)
-    bs.dec.set_controls(False, 1.0, 0, 1.0, 0, pad, eos, *processors)
+    bs.dec.set_controls(False, 1.0, 0, 1.0, 0, pad, eos, *processors, min_length=min_length, entries=entries)
+    if bs.kernels and bs.dec.seq is not None and bs.slot_i is None:
+        rows = bs.B * bs.nb
+        bs.slot_i = torch.zeros(rows, DK.MAX_SEQS, dtype=torch.int32, device=bs.dec.device)
+        bs.slot_v = torch.zeros(rows, DK.MAX_SEQS, 2, dtype=torch.float32, device=bs.dec.device)
     bs.reset(pad)
     bs.prompt[:, :Sp].copy_(comp)
     bs.plens.copy_(lens)
@@ -714,8 +736,18 @@ def _check_beams(num_beams, num_return_sequences, do_sample: bool, assistant_mod
                          f"{DK.beams_to_keep(num_beams, n_eos)} tokens, the model has {vocab_size}")
 
 
-def _check_processors(repetition_penalty, no_repeat_ngram_size, min_new_tokens, assistant_model) -> bool:
-    """Validates the logits-processor arguments (HF's terms); True when one of them is on."""
+def _check_processors(repetition_penalty, no_repeat_ngram_size, min_new_tokens, assistant_model, min_length=0, min_p=None,
+                      sequence_processors: bool = False, prompt_lookup: bool = False) -> bool:
+    """Validates the logits-processor arguments (HF's terms) and min_p; True when one of the processors is on.
+    ``sequence_processors``: sequence_bias or bad_words_ids has entries (checked by ``DK.sequence_entries``)."""
+    if isinstance(min_length, bool) or not isinstance(min_length, int) or min_length < 0:
+        raise ValueError(f"min_length must be an integer >= 0 (0: off), got {min_length!r}")
+    if min_p is not None and (isinstance(min_p, bool) or not isinstance(min_p, (int, float)) or not 0 <= min_p <= 1):
+        raise ValueError(f"min_p must be a float in [0, 1] (None or 0: off), got {min_p!r}")
+    if sequence_processors or min_length > 0:
+        for on, name in ((assistant_model is not None, "assistant_model"), (prompt_lookup, "prompt_lookup_num_tokens")):
+            if on:
+                raise ValueError(f"sequence_bias, bad_words_ids and min_length are not supported yet together with {name}")
     if isinstance(repetition_penalty, bool) or not isinstance(repetition_penalty, (int, float)) \
             or not math.isfinite(repetition_penalty) or not repetition_penalty > 0:
         raise ValueError(f"repetition_penalty must be a finite float > 0 (1.0: off), got {repetition_penalty!r}")
@@ -748,7 +780,8 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
              return_dict_in_generate: bool = False, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
              min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
              max_matching_ngram_size: int | None = None, fp8_weights: bool = False,
-             fp8_kv_cache: bool = False) -> torch.Tensor | GenerateOutput:
+             fp8_kv_cache: bool = False, sequence_bias=None, bad_words_ids=None, min_length: int = 0,
+             min_p: float | None = None) -> torch.Tensor | GenerateOutput:
     """See :meth:`LlamaForCausalLM.generate`."""
     cfg, ar = model.config, model.arena
     if ar.param_sharded:
@@ -770,7 +803,10 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     eos = _eos_list(cfg.eos_token_id if eos_token_id is None else eos_token_id)
     _check_beams(num_beams, num_return_sequences, do_sample, assistant_model, early_stopping, cfg.vocab_size, len(eos),
                  prompt_lookup_num_tokens)
-    proc_on = _check_processors(repetition_penalty, no_repeat_ngram_size, min_new_tokens, assistant_model)
+    entries = DK.sequence_entries(sequence_bias, bad_words_ids, eos, cfg.vocab_size)
+    proc_on = _check_processors(repetition_penalty, no_repeat_ngram_size, min_new_tokens, assistant_model, min_length, min_p,
+                                bool(entries), prompt_lookup_num_tokens is not None)
+    min_p = float(min_p or 0.0) if do_sample else 0.0          # a warper: off unless sampling, as in HF
     ngram = _check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size, assistant_model, num_beams, proc_on, P, max_new_tokens,
                           cfg.max_position_embeddings)
     processors = (float(repetition_penalty), no_repeat_ngram_size, min_new_tokens)
@@ -802,19 +838,20 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     if assistant_model is not None or prompt_lookup_num_tokens is not None:
         K = num_assistant_tokens if assistant_model is not None else prompt_lookup_num_tokens
         new = _assisted_generate(model, assistant_model, comp, lens, P, max_new_tokens, K, (do_sample, temperature, top_k, top_p, seed),
-                                 pad, eos, ngram, fp8, fp8_kv_cache)
+                                 pad, eos, ngram, fp8, fp8_kv_cache, min_p)
         out = torch.cat([ids, new], dim=1)
         return GenerateOutput(out) if return_dict_in_generate else out
     Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))
     if num_beams > 1:
         new, scores = _beam_generate(model, comp, lens, Smax, max_new_tokens, num_beams, num_return_sequences, length_penalty,
-                                     early_stopping, pad, eos, processors, fp8, fp8_kv_cache)
+                                     early_stopping, pad, eos, processors, fp8, fp8_kv_cache, min_length, entries)
         out = torch.cat([ids.repeat_interleave(num_return_sequences, dim=0), new], dim=1)
         return GenerateOutput(out, scores) if return_dict_in_generate else out
     n = num_return_sequences
     st = decode_state(model, B * n, Smax, fp8_kv_cache, n)
 
-    st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, *processors)
+    st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, *processors, min_length=min_length, min_p=min_p,
+                    entries=entries)
     st.out.fill_(pad)
     prefill(model, st, comp, lens, fp8)
     if n > 1:

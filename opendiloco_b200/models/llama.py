@@ -750,12 +750,16 @@ class LlamaForCausalLM(nn.Module):
                  num_assistant_tokens: int = 4, num_beams: int = 1, length_penalty: float = 1.0, early_stopping=False,
                  num_return_sequences: int = 1, return_dict_in_generate: bool = False, repetition_penalty: float = 1.0,
                  no_repeat_ngram_size: int = 0, min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
-                 max_matching_ngram_size: int | None = None, fp8_weights: bool = False, fp8_kv_cache: bool = False):
+                 max_matching_ngram_size: int | None = None, fp8_weights: bool = False, fp8_kv_cache: bool = False,
+                 sequence_bias=None, bad_words_ids=None, min_length: int = 0, min_p: float | None = None):
         """KV-cached text generation with HF ``generate`` keyword names.  Returns LongTensor [B, P + max_new_tokens]: the
         prompt as given, then the new tokens.
 
         Prompts may be left-padded with an ``attention_mask``.  ``do_sample=False`` is greedy (ties to the lowest id);
-        otherwise temperature, top-k (0 = off) and top-p are applied in HF's order and tokens are drawn with ``seed``.
+        otherwise temperature, top-k (0 = off), top-p and ``min_p`` (in [0, 1]; None or 0 is off: keep the tokens whose
+        probability is at least min_p times the largest) are applied in HF's order and tokens are drawn with ``seed``.
+        ``min_p`` is a warper, so it does nothing without ``do_sample`` (greedy, beam search) and works with
+        ``assistant_model`` and ``prompt_lookup_num_tokens``, whose acceptance applies it to both distributions.
         ``eos_token_id`` (int or list) defaults to ``config.eos_token_id``; after a row emits it, the row is filled with
         ``pad_token_id`` (default: the first EOS id).  Reads the current compute weights.  bf16-mixed CUDA models run the
         decode kernels (csrc/decode_sm90.cu) with the step replayed from a CUDA graph; other precisions and devices run the
@@ -797,17 +801,24 @@ class LlamaForCausalLM(nn.Module):
         ``do_sample=True`` or ``assistant_model`` with ``num_beams`` > 1.
 
         Logits processors, HF's, applied in HF's order to the fp32 value of each logit (greedy and sampling: before the
-        temperature, top-k and top-p warpers) or log-prob (beam search), on greedy, sampling and beam search:
-        ``repetition_penalty`` (a finite float > 0; 1.0 is off) divides the positive and multiplies the negative values of
-        every token in the row's history, once per distinct token; ``no_repeat_ngram_size`` n (0..64; 0 is off) forbids
-        any n-gram from occurring twice in the history; ``min_new_tokens`` (0 is off) forbids every EOS id until that many
-        tokens have been generated (nothing without EOS ids).  A row's history is its real prompt tokens followed by its
+        temperature, top-k, top-p and min-p warpers) or log-prob (beam search), on greedy, sampling and beam search:
+        ``sequence_bias`` (HF's dict ``{tuple(ids): bias}`` or list ``[[ids], bias]``) adds a bias to the last token of a
+        sequence: always for one id, and for a longer sequence when the history ends with its other ids (and is at least
+        as long as the sequence); biases of one token are summed in HF's order (the length-1 one first, then dict order);
+        ``repetition_penalty`` (a finite float > 0; 1.0 is off) then divides the positive and multiplies the negative values
+        of every token in the row's history, once per distinct token; ``no_repeat_ngram_size`` n (0..64; 0 is off) forbids
+        any n-gram from occurring twice in the history; ``bad_words_ids`` (a list of id lists) forbids the last id of each
+        sequence by the matching rule of ``sequence_bias`` (single ids equal to an EOS id are dropped, as in HF);
+        ``min_length`` (0 is off) forbids every EOS id while the history (prompt included) is shorter than it;
+        ``min_new_tokens`` (0 is off) forbids every EOS id until that many tokens have been generated (nothing without EOS
+        ids).  Sequences have 1..64 ids in [0, vocab_size); ``sequence_bias`` and ``bad_words_ids`` hold at most 1024
+        sequences and 16384 ids together, and a bias may be -inf (a ban) but not NaN or +inf.  A row's history is its real prompt tokens followed by its
         generated tokens (beam search: the beam's own running sequence).  Unlike HF, the padding of a left-padded batch is
         not part of the history, so every row generates what it would alone.  A greedy row whose values are all -inf
         emits token 0; a sampled one its processed argmax.  With beam search, ``sequences_scores`` sum the processed
-        log-probs, as in HF.  The settings live in device memory: changing them replays the same CUDA graphs.  Raises
-        ValueError for values outside those ranges, or for any of them on together with ``assistant_model`` (not supported
-        yet).
+        log-probs, as in HF.  The settings live in device memory (the sequences in a fixed-capacity table): changing them
+        replays the same CUDA graphs.  Raises ValueError for values outside those ranges, or for any of them on together
+        with ``assistant_model`` or ``prompt_lookup_num_tokens`` (not supported yet).
 
         ``num_return_sequences`` n > 1 with ``do_sample=True`` and ``num_beams == 1`` draws n independent samples per
         prompt: ``[B * n, P + max_new_tokens]``, row ``b * n + j`` is prompt b as given, then its j-th sample; token for
@@ -853,7 +864,8 @@ class LlamaForCausalLM(nn.Module):
                         return_dict_in_generate=return_dict_in_generate, repetition_penalty=repetition_penalty,
                         no_repeat_ngram_size=no_repeat_ngram_size, min_new_tokens=min_new_tokens,
                         prompt_lookup_num_tokens=prompt_lookup_num_tokens, max_matching_ngram_size=max_matching_ngram_size,
-                        fp8_weights=fp8_weights, fp8_kv_cache=fp8_kv_cache)
+                        fp8_weights=fp8_weights, fp8_kv_cache=fp8_kv_cache, sequence_bias=sequence_bias,
+                        bad_words_ids=bad_words_ids, min_length=min_length, min_p=min_p)
 
     @torch.no_grad()
     def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None,

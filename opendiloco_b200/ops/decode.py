@@ -47,7 +47,7 @@ _lib.register_optional("odb_dec_attn_chunks", [c_int])
 _lib.register_optional("odb_dec_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_int,
                                         c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_sample", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                          c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p])
+                                          c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p])
 _lib.register_optional("odb_dec_verify_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int,
                                                c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_accept", [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -57,10 +57,11 @@ _lib.register_optional("odb_dec_lookup_propose", [c_void_p, c_int, c_void_p, c_v
                                                   c_int, c_int, c_void_p])
 _lib.register_optional("odb_dec_beam_splits", [c_int])
 _lib.register_optional("odb_dec_beam_topk", [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                             c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p])
+                                             c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_beam_step", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
                                              c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                             c_void_p, c_void_p, c_void_p, c_int, c_void_p])
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p])
 _lib.register_optional("odb_dec_beam_reorder", [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                                 c_void_p])
 _lib.register_optional("odb_dec_attn_group", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p,
@@ -70,14 +71,20 @@ _lib.register_optional("odb_dec_fork", [c_void_p, c_void_p, c_void_p, c_int, c_i
 
 MAX_EOS = 8
 # int64 control block of the sampler: do_sample, top_k, seed, pad_token_id, n_eos, eos ids, then the logits processors'
-# no_repeat_ngram_size and min_new_tokens.  fp32 block: temperature, top_p, repetition_penalty.
+# no_repeat_ngram_size, min_new_tokens, min_length and the number of sequence-table entries.  fp32 block: temperature,
+# top_p, repetition_penalty, min_p.
 CTL_DO_SAMPLE, CTL_TOP_K, CTL_SEED, CTL_PAD, CTL_N_EOS, CTL_EOS = range(6)
 CTL_NGRAM = CTL_EOS + MAX_EOS
 CTL_MIN_NEW = CTL_NGRAM + 1
-CTL_SIZE = CTL_MIN_NEW + 1
-FCTL_TEMPERATURE, FCTL_TOP_P, FCTL_PENALTY = range(3)
-MAX_NGRAM = 64                    # the largest no_repeat_ngram_size generate() takes
+CTL_MIN_LEN = CTL_MIN_NEW + 1
+CTL_N_SEQ = CTL_MIN_LEN + 1
+CTL_SIZE = CTL_N_SEQ + 1
+FCTL_TEMPERATURE, FCTL_TOP_P, FCTL_PENALTY, FCTL_MIN_P = range(4)
+MAX_NGRAM = 64                    # the largest no_repeat_ngram_size generate() takes (and the longest table sequence)
 MAX_SAMPLE_VOCAB = 56000          # the sampler keeps one fp32 per vocabulary entry in shared memory
+MAX_SEQS = 1024                   # sequence table: sequence_bias + bad_words_ids entries ...
+MAX_SEQ_IDS = 16384               # ... and their ids in all
+SEQ_BIAS, SEQ_BAN = 0, 1          # kinds of table entries
 
 
 def usable(t: torch.Tensor, head_dim: int, Hq: int = 1, Hkv: int = 1) -> bool:
@@ -372,7 +379,7 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor | None, ictl: torch.Tensor, fc
 
     Greedy (ictl do_sample = 0, or top_k = 1): accept the longest prefix where d_i is the target's argmax, then emit the
     argmax at the first mismatch (or the bonus argmax after d_K).  Sampling: p and q are both distributions after the
-    sampler's warpers; d_i is accepted with probability min(1, p(d_i) / q(d_i)); the first rejection draws from
+    sampler's warpers (min_p included, with the same fctl for both); d_i is accepted with probability min(1, p(d_i) / q(d_i)); the first rejection draws from
     normalise(max(0, p - q)); K acceptances draw the bonus token from p_{K+1}.
 
     The emitted tokens go to out[b, gen[b]..] (a row stops after an EOS id or at max_new tokens; later tokens are never
@@ -407,7 +414,9 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor | None, ictl: torch.Tensor, fc
         _lib.count_launch()
         return
     c = ictl.tolist()
-    temperature, top_p = (float(v) for v in fctl.tolist()[:2])
+    fc = fctl.tolist()
+    temperature, top_p = fc[FCTL_TEMPERATURE], fc[FCTL_TOP_P]
+    min_p = fc[FCTL_MIN_P] if len(fc) > FCTL_MIN_P else 0.0
     greedy = not (c[CTL_DO_SAMPLE] and c[CTL_TOP_K] != 1)
     eos = set(c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]])
     p_all = plog.float().view(K + 1, B, V)
@@ -429,8 +438,9 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor | None, ictl: torch.Tensor, fc
             t_new = am[n_acc]
         else:
             rng = torch.Generator(device="cpu").manual_seed((int(c[CTL_SEED]) * 1000003 + b * 7919 + g0) & ((1 << 63) - 1))
-            p = torch.softmax(warp_logits(p_all[:, b].cpu(), temperature, c[CTL_TOP_K], top_p), dim=-1)          # [K+1, V]
-            q = torch.softmax(warp_logits(q_all[:, b].cpu(), temperature, c[CTL_TOP_K], top_p), dim=-1) if q_all is not None else None
+            p = torch.softmax(warp_logits(p_all[:, b].cpu(), temperature, c[CTL_TOP_K], top_p, min_p), dim=-1)          # [K+1, V]
+            q = (torch.softmax(warp_logits(q_all[:, b].cpu(), temperature, c[CTL_TOP_K], top_p, min_p), dim=-1)
+                 if q_all is not None else None)
             while n_acc < n_cand:
                 d = drafts[n_acc]
                 u = float(torch.rand((), generator=rng))
@@ -538,7 +548,8 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
                 fin_seq: torch.Tensor, unsat: torch.Tensor, done: torch.Tensor, tstep: torch.Tensor, pos: torch.Tensor,
                 ids_next: torch.Tensor, parent: torch.Tensor, part_ml: torch.Tensor | None = None, cand_v: torch.Tensor | None = None,
                 cand_i: torch.Tensor | None = None, fctl: torch.Tensor | None = None, prompt: torch.Tensor | None = None,
-                plens: torch.Tensor | None = None) -> None:
+                plens: torch.Tensor | None = None, table: SeqTable | None = None, slot_i: torch.Tensor | None = None,
+                slot_v: torch.Tensor | None = None) -> None:
     """One step of deterministic beam search (transformers' ``_beam_search`` with do_sample=False) over logits
     [B * num_beams, V] (row b * num_beams + j: beam j of prompt b).
 
@@ -561,11 +572,17 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
     rules (not renormalised), then + run_score.  Beam row r of prompt b has the history ``prompt[b, :plens[b]]`` followed
     by ``run_seq[t & 1, r, :t]`` and has generated t tokens; at step 0 that is the prompt alone.  Scores are then sums of
     processed log-probs.  The kernel path needs ck >= 2K: beam_topk lists each split's best unpenalised and best penalised
-    tokens apart, and beam_step maps both to processed scores and merges them."""
+    tokens apart, and beam_step maps both to processed scores and merges them.
+
+    ``table``: the ``SeqTable`` of sequence_bias / bad_words_ids.  On the kernel path its biased tokens are monotone with
+    neither list, so beam_topk writes each row's matched, unbanned biased tokens to slots (slot_i int32 / slot_v fp32
+    [rows, MAX_SEQS] / [rows, MAX_SEQS, 2]: token, then raw logit and summed bias) and beam_step scores them exactly and
+    merges them with the lists."""
     proc = (fctl is not None and prompt is not None and plens is not None)
     if part_ml is None:
         beam_step_reference(logits, ictl, num_beams, K, length_penalty, early_stopping, max_new, run_score, fin_score, fin_flag, run_seq,
-                            fin_seq, unsat, done, tstep, pos, ids_next, parent, fctl=fctl if proc else None, prompt=prompt, plens=plens)
+                            fin_seq, unsat, done, tstep, pos, ids_next, parent, fctl=fctl if proc else None, prompt=prompt, plens=plens,
+                            table=table)
         return
     rows, V = logits.shape
     ck = cand_v.shape[2]
@@ -576,17 +593,24 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
     if proc:
         assert prompt.dtype == torch.int32 and prompt.is_contiguous() and prompt.shape[0] == rows // num_beams
         assert plens.dtype == torch.int32 and fctl.dtype == torch.float32
+    tab = proc and table is not None
+    if tab:
+        assert slot_i.shape == (rows, MAX_SEQS) and slot_i.dtype == torch.int32 and slot_i.is_contiguous()
+        assert slot_v.shape == (rows, MAX_SEQS, 2) and slot_v.dtype == torch.float32 and slot_v.is_contiguous()
     st = _lib.stream_ptr(logits)
     fp = fctl.data_ptr() if proc else None
     _lib.check(_lib.cuda_lib().odb_dec_beam_topk(logits.data_ptr(), logits.stride(0), V, K, ck, part_ml.data_ptr(), cand_v.data_ptr(),
                                                  cand_i.data_ptr(), ictl.data_ptr(), fp, prompt.data_ptr() if proc else None,
                                                  prompt.shape[1] if proc else 0, plens.data_ptr() if proc else None, run_seq.data_ptr(),
-                                                 tstep.data_ptr(), num_beams, max_new, rows, st), "dec_beam_topk")
+                                                 tstep.data_ptr(), num_beams, max_new, rows, table.ints.data_ptr() if tab else None,
+                                                 table.bias.data_ptr() if tab else None, slot_i.data_ptr() if tab else None,
+                                                 slot_v.data_ptr() if tab else None, st), "dec_beam_topk")
     _lib.check(_lib.cuda_lib().odb_dec_beam_step(part_ml.data_ptr(), cand_v.data_ptr(), cand_i.data_ptr(), V, num_beams, K, ck,
                                                  ictl.data_ptr(), fp, float(length_penalty), int(early_stopping), max_new,
                                                  run_score.data_ptr(), fin_score.data_ptr(), fin_flag.data_ptr(), run_seq.data_ptr(),
                                                  fin_seq.data_ptr(), unsat.data_ptr(), done.data_ptr(), tstep.data_ptr(), pos.data_ptr(),
-                                                 ids_next.data_ptr(), parent.data_ptr(), rows // num_beams, st), "dec_beam_step")
+                                                 ids_next.data_ptr(), parent.data_ptr(), slot_i.data_ptr() if tab else None,
+                                                 slot_v.data_ptr() if tab else None, rows // num_beams, st), "dec_beam_step")
     _lib.count_launch(2)
 
 
@@ -594,7 +618,7 @@ def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int
                         max_new: int, run_score: torch.Tensor, fin_score: torch.Tensor, fin_flag: torch.Tensor, run_seq: torch.Tensor,
                         fin_seq: torch.Tensor, unsat: torch.Tensor, done: torch.Tensor, tstep: torch.Tensor, pos: torch.Tensor,
                         ids_next: torch.Tensor, parent: torch.Tensor, fctl: torch.Tensor | None = None,
-                        prompt: torch.Tensor | None = None, plens: torch.Tensor | None = None) -> None:
+                        prompt: torch.Tensor | None = None, plens: torch.Tensor | None = None, table: SeqTable | None = None) -> None:
     """``beam_select`` in PyTorch: transformers' ``_get_top_k_continuations``, ``_get_running_beams_for_next_iteration``,
     ``_update_finished_beams`` and ``_check_early_stop_heuristic`` over [B, num_beams, ...], with stable sorts for the
     tie rule (-inf ties included: the lower beam * V + token).  With fctl / prompt / plens, the logits processors as
@@ -615,7 +639,8 @@ def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int
     if prompt is not None and plens is not None and processors_on(c, fc):
         tr = t.to(dev).repeat_interleave(nb)
         logp = process_logits_reference(logp, beam_histories(prompt, plens, run_seq, tstep, nb), plens.long().to(dev).repeat_interleave(nb) + tr,
-                                        tr, fc[FCTL_PENALTY], c[CTL_NGRAM], c[CTL_MIN_NEW], c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]])
+                                        tr, fc[FCTL_PENALTY], c[CTL_NGRAM], c[CTL_MIN_NEW], c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]],
+                                        _table_entries(table, c), c[CTL_MIN_LEN])
     logp = logp.view(B, nb, V) + run_score.view(B, nb, 1)
     idx = top(logp.view(B, nb * V), K)
     vals = logp.view(B, nb * V).gather(1, idx)
@@ -722,31 +747,132 @@ def beam_reorder_reference(kv: torch.Tensor, parent: torch.Tensor, inv: torch.Te
 
 # ------------------------------------------------------------------------------------------------ sampler
 def make_controls(do_sample: bool, temperature: float, top_k: int, top_p: float, seed: int, pad: int, eos: list[int], device,
-                  repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_new_tokens: int = 0):
-    """(ictl int64 [CTL_SIZE], fctl fp32 [3]) for ``sample`` and ``beam_select``.  The logits processors are off at their
-    defaults (penalty 1.0, n-gram size 0, min_new_tokens 0)."""
+                  repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_new_tokens: int = 0, min_length: int = 0,
+                  min_p: float = 0.0, n_seq: int = 0):
+    """(ictl int64 [CTL_SIZE], fctl fp32 [4]) for ``sample``, ``accept`` and ``beam_select``.  The logits processors are
+    off at their defaults (penalty 1.0, n-gram size 0, min_new_tokens 0, min_length 0, no sequence-table entries: n_seq
+    counts the entries of the state's ``SeqTable``), and so is min_p (0)."""
     if len(eos) > MAX_EOS:
         raise ValueError(f"at most {MAX_EOS} EOS ids are supported, got {len(eos)}")
     ictl = [int(do_sample), int(top_k), int(seed) & ((1 << 63) - 1), int(pad), len(eos)] + list(eos) + [0] * (MAX_EOS - len(eos))
-    ictl += [int(no_repeat_ngram_size), int(min_new_tokens)]
+    ictl += [int(no_repeat_ngram_size), int(min_new_tokens), int(min_length), int(n_seq)]
     return (torch.tensor(ictl, dtype=torch.int64, device=device),
-            torch.tensor([float(temperature), float(top_p), float(repetition_penalty)], dtype=torch.float32, device=device))
+            torch.tensor([float(temperature), float(top_p), float(repetition_penalty), float(min_p)], dtype=torch.float32,
+                         device=device))
 
 
 def processors_on(ictl: list[int], fctl: list[float]) -> bool:
     """The control blocks (as lists) turn a logits processor on (the kernels' test, on the same fields)."""
-    return (len(fctl) > FCTL_PENALTY and len(ictl) > CTL_MIN_NEW
-            and (fctl[FCTL_PENALTY] != 1.0 or ictl[CTL_NGRAM] > 0 or (ictl[CTL_MIN_NEW] > 0 and ictl[CTL_N_EOS] > 0)))
+    return (len(fctl) > FCTL_PENALTY and len(ictl) > CTL_N_SEQ
+            and (fctl[FCTL_PENALTY] != 1.0 or ictl[CTL_NGRAM] > 0 or ictl[CTL_N_SEQ] > 0
+                 or ((ictl[CTL_MIN_NEW] > 0 or ictl[CTL_MIN_LEN] > 0) and ictl[CTL_N_EOS] > 0)))
+
+
+def _check_sequence(seq, vocab_size: int, what: str) -> tuple[int, ...]:
+    if not isinstance(seq, (list, tuple)) or not seq:
+        raise ValueError(f"{what}: every sequence must be a non-empty list of token ids, got {seq!r}")
+    if len(seq) > MAX_NGRAM:
+        raise ValueError(f"{what}: sequences of at most {MAX_NGRAM} ids are supported, got one of {len(seq)}")
+    for t in seq:
+        if isinstance(t, bool) or not isinstance(t, int) or not 0 <= t < vocab_size:
+            raise ValueError(f"{what}: token ids must be integers in [0, {vocab_size}), got {t!r} in {seq!r}")
+    return tuple(int(t) for t in seq)
+
+
+def sequence_entries(sequence_bias, bad_words_ids, eos: list[int], vocab_size: int) -> list[tuple[tuple[int, ...], float, int]]:
+    """The entries (ids, bias, kind) of a ``SeqTable`` for generate()'s ``sequence_bias`` (HF's dict ``{tuple(ids): bias}``
+    or list ``[[ids], bias]`` form; later duplicates of the list form win, as HF's conversion to a dict) and
+    ``bad_words_ids`` (a list of id lists; single-token entries equal to an EOS id are dropped, as HF drops them).  The
+    bias entries come first, in HF's summation order: the length-1 sequences, then the longer ones, each in dict order.
+    Raises ValueError for ids outside [0, vocab_size), empty or over-long (> MAX_NGRAM) sequences, a NaN or +inf bias, and
+    more than MAX_SEQS entries or MAX_SEQ_IDS ids in all."""
+    entries = []
+    if sequence_bias is not None:
+        if isinstance(sequence_bias, dict):
+            items = list(sequence_bias.items())
+        elif isinstance(sequence_bias, (list, tuple)):
+            for it in sequence_bias:
+                if not (isinstance(it, (list, tuple)) and len(it) == 2 and isinstance(it[0], (list, tuple))):
+                    raise ValueError(f"sequence_bias: the list form is [[ids], bias] per entry, got {it!r}")
+            items = list({tuple(it[0]): it[1] for it in sequence_bias}.items())
+        else:
+            raise ValueError(f"sequence_bias must be a dict {{tuple(ids): bias}} or a list of [[ids], bias], got {sequence_bias!r}")
+        seqs = []
+        for ids, b in items:
+            ids = _check_sequence(list(ids) if isinstance(ids, tuple) else ids, vocab_size, "sequence_bias")
+            if isinstance(b, bool) or not isinstance(b, (int, float)) or math.isnan(b) or b == math.inf:
+                raise ValueError(f"sequence_bias: a bias must be a float that is not NaN or +inf (-inf bans), got {b!r}")
+            seqs.append((ids, float(b)))
+        entries += [(i, b, SEQ_BIAS) for i, b in seqs if len(i) == 1] + [(i, b, SEQ_BIAS) for i, b in seqs if len(i) > 1]
+    if bad_words_ids is not None:
+        if not isinstance(bad_words_ids, (list, tuple)):
+            raise ValueError(f"bad_words_ids must be a list of lists of token ids, got {bad_words_ids!r}")
+        for w in bad_words_ids:
+            ids = _check_sequence(w, vocab_size, "bad_words_ids")
+            if len(ids) == 1 and ids[0] in eos:
+                continue
+            entries.append((ids, -math.inf, SEQ_BAN))
+    if len(entries) > MAX_SEQS or sum(len(e[0]) for e in entries) > MAX_SEQ_IDS:
+        raise ValueError(f"sequence_bias and bad_words_ids take at most {MAX_SEQS} sequences and {MAX_SEQ_IDS} ids together, "
+                         f"got {len(entries)} and {sum(len(e[0]) for e in entries)}")
+    return entries
+
+
+class SeqTable:
+    """The fixed-capacity device table of ``sequence_entries``: int32 ``ints`` = offsets [MAX_SEQS + 1] | kinds [MAX_SEQS]
+    | ids [MAX_SEQ_IDS] (entry e is ids[off[e], off[e + 1])) and fp32 ``bias`` [MAX_SEQS]; ``entries`` keeps the host
+    copy the references read.  ``set`` rewrites it in place, so graphs that read it replay with any entries; the number in
+    use is the control block's CTL_N_SEQ."""
+
+    def __init__(self, device):
+        self.ints = torch.zeros(2 * MAX_SEQS + 1 + MAX_SEQ_IDS, dtype=torch.int32, device=device)
+        self.bias = torch.zeros(MAX_SEQS, dtype=torch.float32, device=device)
+        self.entries: list = []
+
+    def set(self, entries: list) -> None:
+        if entries == self.entries:
+            return
+        assert len(entries) <= MAX_SEQS and sum(len(e[0]) for e in entries) <= MAX_SEQ_IDS
+        ints = torch.zeros(self.ints.shape, dtype=torch.int32)
+        off = [0]
+        for ids, _, _ in entries:
+            off.append(off[-1] + len(ids))
+        ints[:len(off)] = torch.tensor(off, dtype=torch.int32)
+        ints[MAX_SEQS + 1:MAX_SEQS + 1 + len(entries)] = torch.tensor([k for _, _, k in entries], dtype=torch.int32)
+        ints[2 * MAX_SEQS + 1:2 * MAX_SEQS + 1 + off[-1]] = torch.tensor([t for ids, _, _ in entries for t in ids], dtype=torch.int32)
+        bias = torch.zeros(MAX_SEQS, dtype=torch.float32)
+        bias[:len(entries)] = torch.tensor([b for _, b, _ in entries], dtype=torch.float32)
+        self.ints.copy_(ints)
+        self.bias.copy_(bias)
+        self.entries = list(entries)
+
+
+def _table_entries(table: SeqTable | None, ictl: list[int]) -> list:
+    return table.entries[:ictl[CTL_N_SEQ]] if table is not None and len(ictl) > CTL_N_SEQ else []
+
+
+def _seq_matches(h: torch.Tensor, L: torch.Tensor, ids: tuple[int, ...]) -> torch.Tensor:
+    """[rows] bool: the histories h[r, :L[r]] end with ids[:-1] and L >= len(ids) (always true for one id)."""
+    k = len(ids)
+    if k == 1:
+        return torch.ones(h.shape[0], dtype=torch.bool, device=h.device)
+    q = (L[:, None] - k + 1 + torch.arange(k - 1, device=h.device)[None, :]).clamp(0, h.shape[1] - 1)
+    return (L >= k) & (h.gather(1, q) == torch.tensor(ids[:-1], dtype=h.dtype, device=h.device)[None, :]).all(dim=1)
 
 
 def process_logits_reference(x: torch.Tensor, histories: torch.Tensor, lens: torch.Tensor, n_generated: torch.Tensor, penalty: float,
-                             n: int, min_new: int, eos: list[int]) -> torch.Tensor:
+                             n: int, min_new: int, eos: list[int], seqs: list = (), min_len: int = 0) -> torch.Tensor:
     """HF's logits processors, in HF's order, on fp32 values x [rows, V]; returns a new tensor.  Row r's history is
     histories[r, :lens[r]] (int, [rows, S]); n_generated[r] counts the tokens it has generated.
 
+    - Sequence bias (the SEQ_BIAS entries of ``seqs``, ``sequence_entries``): a length-1 sequence adds its bias to its
+      token; a longer one adds it to its last token when the history (of length L >= its length) ends with its other
+      tokens.  The biases of a token are summed from 0 in table order, then added to x once.
     - Repetition penalty (``penalty`` != 1): every distinct token of the history gets ``x < 0 ? x * p : x / p``, once.
     - N-gram ban (``n`` > 0): with h the history and L its length, if L + 1 >= n, every start s <= L - n with
       ``h[s .. s+n-2] == h[L-n+1 .. L-1]`` bans ``h[s+n-1]`` (-inf); matches may overlap, and n = 1 bans the whole history.
+    - Bad words (the SEQ_BAN entries of ``seqs``): the last token of a sequence that matches as above gets -inf.
+    - Min length: while L < ``min_len``, every id of ``eos`` gets -inf.
     - Min new tokens: while n_generated < ``min_new``, every id of ``eos`` gets -inf.
 
     HF passes the padded ``input_ids``, so for left-padded prompts it also counts the padding ids; here a history holds only
@@ -758,6 +884,12 @@ def process_logits_reference(x: torch.Tensor, histories: torch.Tensor, lens: tor
     L = lens.to(dev).long()
     col = torch.arange(S, device=dev)[None, :]
     x = x.clone()
+    if any(k == SEQ_BIAS for _, _, k in seqs):
+        bias = torch.zeros(rows, V, dtype=torch.float32, device=dev)
+        for ids, b, k in seqs:
+            if k == SEQ_BIAS:
+                bias[:, ids[-1]] += torch.where(_seq_matches(h, L, ids), torch.tensor(b, device=dev), torch.tensor(0.0, device=dev))
+        x = x + bias
     if penalty != 1.0:
         tok = torch.where((col < L[:, None]) & (h >= 0) & (h < V), h, torch.full_like(h, V))
         seen = torch.zeros(rows, V + 1, dtype=torch.bool, device=dev).scatter_(1, tok, True)[:, :V]
@@ -772,19 +904,25 @@ def process_logits_reference(x: torch.Tensor, histories: torch.Tensor, lens: tor
         follower = win[:, :, n - 1]
         follower = torch.where(match & (follower >= 0) & (follower < V), follower, torch.full_like(follower, V))
         ban.scatter_(1, follower, True)
-    if min_new > 0 and eos:
-        early = n_generated.to(dev).long() < min_new
+    for ids, _, k in seqs:
+        if k == SEQ_BAN:
+            ban[:, ids[-1]] |= _seq_matches(h, L, ids)
+    if eos and (min_new > 0 or min_len > 0):
+        early = (n_generated.to(dev).long() < min_new) | (L < min_len)
         ban[:, torch.tensor(eos, dtype=torch.long, device=dev)] |= early[:, None]
     return x.masked_fill(ban[:, :V], float("-inf"))
 
 
 def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: torch.Tensor, gen: torch.Tensor, finished: torch.Tensor,
-           out: torch.Tensor, ids_next: torch.Tensor, hist: torch.Tensor | None = None, scratch: torch.Tensor | None = None) -> None:
+           out: torch.Tensor, ids_next: torch.Tensor, hist: torch.Tensor | None = None, scratch: torch.Tensor | None = None,
+           table: SeqTable | None = None, seq_scratch: torch.Tensor | None = None) -> None:
     """Pick one token per row of logits [B, V] and write it to out[b, gen[b]] and ids_next[b]; then gen += 1, pos += 1.
 
     Greedy (ictl do_sample = 0, or top_k = 1): argmax, ties to the lowest index.  Sampling: logits / temperature, keep the
     top_k largest (0 = all; ties with the k-th value are kept), keep the smallest set of largest probabilities whose mass
-    reaches top_p (every token tied with the smallest kept one is kept too), draw from the rest.  A row that has produced an EOS id emits ``pad`` from then on (``finished``).
+    reaches top_p (every token tied with the smallest kept one is kept too), keep the tokens whose probability is at least
+    min_p times the largest (fctl min_p > 0), draw from the rest.  A row that has produced an EOS id emits ``pad`` from then
+    on (``finished``).
     CUDA draws use Philox keyed by (seed, row, gen[b]); the reference draws from a torch generator seeded by (seed, step),
     so the two paths give different (equally distributed) samples for the same seed.
 
@@ -794,38 +932,45 @@ def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: to
     rules in fp32 (history length pos[b] + 1, gen[b] tokens generated), and greedy and sampling work on the processed
     values, which are never rounded back to bf16.  A row whose processed values are all -inf emits token 0 greedily; a
     sampled row with no finite value emits its processed argmax.  The kernel keeps two bitmaps per row in scratch (int32
-    [B, 2 * ceil(V / 32)])."""
+    [B, 2 * ceil(V / 32)]).  ``table``: the ``SeqTable`` of sequence_bias / bad_words_ids (its first ictl CTL_N_SEQ
+    entries apply); the kernel then needs ``seq_scratch``, fp32 [B, V] of zeros, which it leaves zero."""
     B, V = logits.shape
     if logits.is_cuda and logits.dtype == torch.bfloat16 and _lib.has_symbol("odb_dec_sample"):
         assert logits.stride(1) == 1 and V <= MAX_SAMPLE_VOCAB and out.is_contiguous()
         if hist is not None:
             assert hist.dtype == torch.int32 and hist.is_contiguous() and hist.shape[0] == B
             assert scratch is not None and scratch.is_contiguous() and scratch.numel() >= B * 2 * ((V + 31) // 32)
+        tab = table is not None and hist is not None
+        if tab:
+            assert seq_scratch is not None and seq_scratch.dtype == torch.float32 and seq_scratch.is_contiguous()
+            assert seq_scratch.numel() >= B * V
         _lib.check(_lib.cuda_lib().odb_dec_sample(logits.data_ptr(), logits.stride(0), V, ictl.data_ptr(), fctl.data_ptr(), pos.data_ptr(),
                                                   gen.data_ptr(), finished.data_ptr(), out.data_ptr(), out.shape[1],
                                                   ids_next.data_ptr(), hist.data_ptr() if hist is not None else None,
                                                   hist.shape[1] if hist is not None else 0,
-                                                  scratch.data_ptr() if hist is not None else None, B, _lib.stream_ptr(logits)),
+                                                  scratch.data_ptr() if hist is not None else None,
+                                                  table.ints.data_ptr() if tab else None, table.bias.data_ptr() if tab else None,
+                                                  seq_scratch.data_ptr() if tab else None, B, _lib.stream_ptr(logits)),
                    "dec_sample")
         _lib.count_launch()
         return
     c = ictl.tolist()
     fc = fctl.tolist()
-    temperature, top_p = fc[FCTL_TEMPERATURE], fc[FCTL_TOP_P]
+    temperature, top_p, min_p = fc[FCTL_TEMPERATURE], fc[FCTL_TOP_P], fc[FCTL_MIN_P]
     x = logits.float()
     proc = hist is not None and processors_on(c, fc)
     if proc:
         x = process_logits_reference(x, hist, pos.long() + 1, gen, fc[FCTL_PENALTY], c[CTL_NGRAM], c[CTL_MIN_NEW],
-                                     c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]])
+                                     c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]], _table_entries(table, c), c[CTL_MIN_LEN])
     tok = x.argmax(dim=-1)
     if c[CTL_DO_SAMPLE] and c[CTL_TOP_K] != 1:
         if proc:
             ok = torch.isfinite(x.max(dim=-1).values)
             drawn = _sample_reference(torch.where(ok[:, None], x, torch.zeros_like(x)), temperature, c[CTL_TOP_K], top_p, c[CTL_SEED],
-                                      int(gen.min()))
+                                      int(gen.min()), min_p)
             tok = torch.where(ok, drawn, tok)
         else:
-            tok = _sample_reference(x, temperature, c[CTL_TOP_K], top_p, c[CTL_SEED], int(gen.min()))
+            tok = _sample_reference(x, temperature, c[CTL_TOP_K], top_p, c[CTL_SEED], int(gen.min()), min_p)
     fin = finished.bool()
     tok = torch.where(fin, torch.full_like(tok, c[CTL_PAD]), tok)
     g = gen.long()
@@ -843,8 +988,9 @@ def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: to
     finished.copy_((fin | torch.isin(tok, eos)).to(finished.dtype))
 
 
-def warp_logits(x: torch.Tensor, temperature: float, top_k: int, top_p: float) -> torch.Tensor:
-    """HF's logits warpers in HF's order (temperature, top-k, top-p) on fp32 logits [B, V]; removed entries are -inf."""
+def warp_logits(x: torch.Tensor, temperature: float, top_k: int, top_p: float, min_p: float = 0.0) -> torch.Tensor:
+    """HF's logits warpers in HF's order (temperature, top-k, top-p, min-p) on fp32 logits [B, V]; removed entries are
+    -inf.  Min-p (> 0) removes the tokens whose probability is below min_p times the largest one (never the largest)."""
     x = x / temperature
     if 0 < top_k < x.shape[-1]:
         kth = torch.topk(x, top_k, dim=-1).values[..., -1:]
@@ -855,10 +1001,16 @@ def warp_logits(x: torch.Tensor, temperature: float, top_k: int, top_p: float) -
         remove = cum <= (1 - top_p)
         remove[..., -1:] = False
         x = x.masked_fill(remove.scatter(-1, idx, remove), float("-inf"))
+    if min_p > 0:
+        probs = torch.softmax(x, dim=-1)
+        remove = probs < min_p * probs.amax(dim=-1, keepdim=True)
+        remove.scatter_(-1, torch.topk(probs, 1, dim=-1).indices, False)
+        x = x.masked_fill(remove, float("-inf"))
     return x
 
 
-def _sample_reference(x: torch.Tensor, temperature: float, top_k: int, top_p: float, seed: int, step: int) -> torch.Tensor:
-    probs = torch.softmax(warp_logits(x, temperature, top_k, top_p), dim=-1)
+def _sample_reference(x: torch.Tensor, temperature: float, top_k: int, top_p: float, seed: int, step: int,
+                      min_p: float = 0.0) -> torch.Tensor:
+    probs = torch.softmax(warp_logits(x, temperature, top_k, top_p, min_p), dim=-1)
     gen = torch.Generator(device=x.device).manual_seed((int(seed) * 1000003 + int(step)) & ((1 << 63) - 1))
     return torch.multinomial(probs, 1, generator=gen)[:, 0]

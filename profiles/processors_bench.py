@@ -4,6 +4,11 @@ Presets with random weights, B in {1, 8, 64}, prompts of 128 and 1024 tokens, EO
 
     python profiles/processors_bench.py                          # the sweep, one JSON line per configuration
     python profiles/processors_bench.py --models 150m --batches 8 --prompts 128
+    python profiles/processors_bench.py --processors sequence   # sequence_bias, bad_words_ids and min_length instead
+
+``--processors sequence`` times 200 ``bad_words_ids`` of 1-4 random ids, 50 ``sequence_bias`` entries of 1-3 ids and
+``min_length=64`` (a sequence table of 250 entries, matched against every row's history each step) instead of the
+repetition controls; the rows and their columns are the same.
 
 ms/token is the time of one whole ``generate`` call (prefill included; minimum over --reps calls, host clock around a
 device synchronise) over its new tokens; each mode is timed after a warm-up call of the same mode and shape, and off
@@ -29,6 +34,15 @@ from opendiloco_b200.models.llama import LlamaForCausalLM  # noqa: E402
 
 PROC = dict(no_repeat_ngram_size=3, repetition_penalty=1.2)
 OFF = dict(no_repeat_ngram_size=0, repetition_penalty=1.0)
+
+
+def sequence_processors(V: int, seed: int = 0) -> dict:
+    """200 bad words of 1-4 ids, 50 sequence biases of 1-3 ids and min_length 64, drawn from a fixed seed."""
+    g = torch.Generator().manual_seed(seed)
+    ids = lambda n: torch.randint(3, V, (n,), generator=g).tolist()   # noqa: E731
+    bad = [ids(1 + i % 4) for i in range(200)]
+    bias = {tuple(ids(1 + i % 3)): float(torch.randn((), generator=g) * 2) for i in range(50)}
+    return dict(bad_words_ids=bad, sequence_bias=bias, min_length=64)
 
 
 def timed_call(fn) -> float:
@@ -61,6 +75,8 @@ def main() -> None:
     ap.add_argument("--num-beams", type=int, default=4)
     ap.add_argument("--reps", type=int, default=2)
     ap.add_argument("--profile-steps", type=int, default=20)
+    ap.add_argument("--processors", choices=["repetition", "sequence"], default="repetition",
+                    help="repetition: no_repeat_ngram_size=3, repetition_penalty=1.2; sequence: see the module docstring")
     ap.add_argument("--out", default=None, help="also append the JSON lines to this file")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "processors_bench needs a GPU"
@@ -76,21 +92,25 @@ def main() -> None:
     for name in a.models.split(","):
         model = LlamaForCausalLM(LlamaConfig.from_pretrained(name), device="cuda", precision="bf16-mixed", seed=0).eval()
         V = model.config.vocab_size
+        on = PROC if a.processors == "repetition" else sequence_processors(V)
+        off = OFF if a.processors == "repetition" else {}
         for P in (int(x) for x in a.prompts.split(",")):
             for B in (int(x) for x in a.batches.split(",")):
                 ids = torch.randint(3, V, (B, P), generator=torch.Generator().manual_seed(B + P)).cuda()
                 row = {"model": name, "B": B, "prompt": P, "new_tokens": a.new_tokens, "num_beams": a.num_beams, "reps": a.reps}
+                if a.processors != "repetition":
+                    row["processors"] = a.processors
                 for mode, extra in (("greedy", {}), ("beam", dict(num_beams=a.num_beams))):
                     kw = dict(max_new_tokens=a.new_tokens, eos_token_id=[], **extra)
                     t = {"off": [], "on": []}
-                    for s, p in (("off", OFF), ("on", PROC)):
+                    for s, p in (("off", off), ("on", on)):
                         model.generate(ids, **kw, **p)                         # warm-up: caches and step graph of this shape
                     for _ in range(a.reps):
-                        for s, p in (("off", OFF), ("on", PROC)):
+                        for s, p in (("off", off), ("on", on)):
                             t[s].append(timed_call(lambda: model.generate(ids, **kw, **p)))
                     for s in ("off", "on"):
                         row[f"{mode}_ms_per_token_{s}"] = round(1e3 * min(t[s]) / a.new_tokens, 3)
-                    for s, p in (("off", OFF), ("on", PROC)):
+                    for s, p in (("off", off), ("on", on)):
                         model.generate(ids, **dict(kw, max_new_tokens=a.new_tokens // 2), **p)   # leaves the state mid-run
                         if mode == "greedy":
                             st = model.engine.decode_state

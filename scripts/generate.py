@@ -59,6 +59,26 @@ def load_checkpoint_weights(model: LlamaForCausalLM, ckpt_dir: str, weights: str
     model.arena.sync_shadow()
 
 
+def parse_bad_words(text: str | None) -> list[list[int]] | None:
+    """"12 13;99" -> [[12, 13], [99]]."""
+    if text is None:
+        return None
+    return [[int(t) for t in seq.split()] for seq in text.split(";") if seq.strip()]
+
+
+def parse_sequence_bias(text: str | None) -> dict[tuple[int, ...], float] | None:
+    """"12 13:-2.5;99:1.0" -> {(12, 13): -2.5, (99,): 1.0}."""
+    if text is None:
+        return None
+    out = {}
+    for item in text.split(";"):
+        if not item.strip():
+            continue
+        ids, _, bias = item.rpartition(":")
+        out[tuple(int(t) for t in ids.split())] = float(bias)
+    return out
+
+
 def add_model_args(ap: argparse.ArgumentParser) -> None:
     """The options that choose the model and its weights (shared with scripts/evaluate.py)."""
     ap.add_argument("--model", required=True, help="HF model directory or preset name (150m, 1b, ...)")
@@ -120,6 +140,10 @@ def main(argv=None) -> None:
                     help="quantise the decoder-layer projections to e4m3 (one scale per output row) and decode on them")
     ap.add_argument("--fp8-kv-cache", action="store_true",
                     help="keep the KV cache in e4m3 with one power-of-two scale per (position, kv head) row")
+    ap.add_argument("--bad-words-ids", default=None, help='sequences that must not be generated, e.g. "12 13;99"')
+    ap.add_argument("--sequence-bias", default=None, help='bias of the last id of each sequence, e.g. "12 13:-2.5;99:1.0"')
+    ap.add_argument("--min-length", type=int, default=0, help="EOS is forbidden while prompt + new tokens are shorter (0: off)")
+    ap.add_argument("--min-p", type=float, default=None, help="sampling: keep tokens with p >= min_p * p_max (off by default)")
     a = ap.parse_args(argv)
     if a.assistant_model is None and a.assistant_checkpoint is not None:
         ap.error("--assistant-checkpoint needs --assistant-model")
@@ -160,7 +184,8 @@ def main(argv=None) -> None:
                          repetition_penalty=a.repetition_penalty, no_repeat_ngram_size=a.no_repeat_ngram_size,
                          min_new_tokens=a.min_new_tokens, prompt_lookup_num_tokens=a.prompt_lookup_num_tokens,
                          max_matching_ngram_size=a.max_matching_ngram_size, fp8_weights=a.fp8_weights,
-                         fp8_kv_cache=a.fp8_kv_cache)
+                         fp8_kv_cache=a.fp8_kv_cache, bad_words_ids=parse_bad_words(a.bad_words_ids),
+                         sequence_bias=parse_sequence_bias(a.sequence_bias), min_length=a.min_length, min_p=a.min_p)
     out = res.sequences.cpu()
     R = out.shape[0] // len(prompts)
     for i, p in enumerate(prompts):
