@@ -734,21 +734,53 @@ __device__ int draw_index(const float* e, int V, float u, int fallback, float* r
   return *tok_sm;
 }
 
-// One row's token from its values x(i): the argmax (greedy, and the reference point of the exponentials), or a draw from
-// the warped weights.  finite_only: a row with no finite value keeps its argmax instead of drawing.
+// generate(output_scores / output_logits): where one emitted token's score row (fp32) and raw logits (bf16) go; either
+// may be null.
+struct ScoreOut {
+  float* score;
+  __nv_bfloat16* logit;
+};
+constexpr int SCORE_RAW = 0, SCORE_WARPED = 1, SCORE_ARGMAX = 2;
+
+// One score row, HF's: SCORE_RAW the values x(i) (greedy: the processed logits); SCORE_WARPED x(i) / temp where
+// bits(warped_weight(x(i))) >= T (warp_weights' kept set, which is exactly the set a draw picks from) and -inf elsewhere;
+// SCORE_ARGMAX x(top) / temp at the argmax alone (top_k = 1, or a row with no finite value).  The raw logits are copied.
+// Out of line, so the pass adds no registers to its callers.
 template <class Load>
-__device__ int pick_token(Load x, int V, const long long* __restrict__ ictl, const float* __restrict__ fctl, int b, int g,
-                          bool finite_only, float* e, float* red, ArgMax* am, int* tok_sm) {
+__device__ __noinline__ void store_scores(Load x, const __nv_bfloat16* __restrict__ row, int V, int mode, float temp, float mx,
+                                          uint32_t T, int top, ScoreOut so) {
+  for (int i = threadIdx.x; i < V; i += blockDim.x) {
+    if (so.logit != nullptr) so.logit[i] = row[i];
+    if (so.score == nullptr) continue;
+    const float v = x(i);
+    float s = v;
+    if (mode == SCORE_WARPED) s = __float_as_uint(warped_weight(v, temp, mx)) >= T ? __fdiv_rn(v, temp) : -INFINITY;
+    else if (mode == SCORE_ARGMAX) s = i == top ? __fdiv_rn(v, temp) : -INFINITY;
+    so.score[i] = s;
+  }
+}
+
+// One row's token from its values x(i): the argmax (greedy, and the reference point of the exponentials), or a draw from
+// the warped weights.  finite_only: a row with no finite value keeps its argmax instead of drawing.  so (either pointer
+// may be null): the row's score row and raw logits (row), from the same values and threshold the pick uses.
+template <class Load>
+__device__ int pick_token(Load x, const __nv_bfloat16* __restrict__ row, int V, const long long* __restrict__ ictl,
+                          const float* __restrict__ fctl, int b, int g, bool finite_only, float* e, float* red, ArgMax* am, int* tok_sm,
+                          ScoreOut so) {
   const ArgMax best = block_argmax(x, V, am);
   const bool do_sample = ictl[0] != 0;
   const int top_k = (int)ictl[1];
+  const float temp = fctl[0];
   int tok = best.i;
   if (do_sample && top_k != 1 && (!finite_only || best.v > -INFINITY)) {
-    const float temp = fctl[0], top_p = fctl[1];
-    warp_weights(x, V, temp, top_k, top_p, fctl[3], best.v / temp, e, red);
+    const float mx = best.v / temp;
+    const uint32_t T = warp_weights(x, V, temp, top_k, fctl[1], fctl[3], mx, e, red);
     curandStatePhilox4_32_10_t rng;
     curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)g, &rng);
     tok = draw_index(e, V, curand_uniform(&rng), best.i, red, tok_sm);   // u in (0, 1]
+    if (so.score != nullptr || so.logit != nullptr) store_scores(x, row, V, SCORE_WARPED, temp, mx, T, tok, so);
+  } else if (so.score != nullptr || so.logit != nullptr) {
+    store_scores(x, row, V, do_sample ? SCORE_ARGMAX : SCORE_RAW, temp, 0.f, 0u, best.i, so);
   }
   return tok;
 }
@@ -774,12 +806,14 @@ __device__ __noinline__ void sample_sequences(const SeqTable tab, const History 
 // With a sequence table (tab_off not null, ictl[CTL_N_SEQ] > 0), seq_scratch fp32 [B][V] (zero when the kernel starts, and
 // again when it ends) takes the row's summed bias at the matched tokens, which are set back to 0 once the token is
 // picked: the clearing costs one store per matched table entry, not a pass over V.
+// score_out / logit_out (generate(output_scores / output_logits), each may be null): [score_cols, B, V]; a row that is not
+// finished writes its score row (store_scores: the values and threshold of its pick) and raw logits at column gen[b].
 __global__ void __launch_bounds__(SAMPLE_THREADS)
 sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const long long* __restrict__ ictl,
               const float* __restrict__ fctl, int* __restrict__ pos, int* __restrict__ gen, int* __restrict__ finished,
               long long* __restrict__ out, int max_new, long long* __restrict__ ids_next, int* __restrict__ hist, int ldh,
               unsigned* __restrict__ scratch, const int* __restrict__ tab_off, const float* __restrict__ tab_bias,
-              float* __restrict__ seq_scratch) {
+              float* __restrict__ seq_scratch, float* __restrict__ score_out, __nv_bfloat16* __restrict__ logit_out, int score_cols) {
   extern __shared__ __align__(16) float e[];     // [V] exp(x - max) of the kept tokens, 0 elsewhere
   __shared__ float red[33];
   __shared__ ArgMax am[32];
@@ -790,6 +824,12 @@ sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, con
   pdl_wait();
   const int b = blockIdx.x, tid = threadIdx.x;
   const __nv_bfloat16* row = logits + (long long)b * ld;
+  ScoreOut so{nullptr, nullptr};
+  if (!finished[b] && gen[b] < score_cols) {     // a live row's column gen[b] of the [score_cols, B, V] score / logit buffers
+    const long long at = ((long long)gen[b] * gridDim.x + b) * V;
+    if (score_out != nullptr) so.score = score_out + at;
+    if (logit_out != nullptr) so.logit = logit_out + at;
+  }
   int tok;
   if (hist != nullptr && processors_on(ictl, fctl)) {
     const int nw = ceil_div(V, 32), L = pos[b] + 1, g = gen[b];
@@ -806,14 +846,14 @@ sample_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, con
     mark_history(hh, 0, V, p != 1.f, (int)ictl[CTL_NGRAM], g < ictl[CTL_MIN_NEW] || L < ictl[CTL_MIN_LEN], ictl, pen, ban);
     if (bias != nullptr) sample_sequences(tab, hh, V, ban, matched, last_sm, bias);
     __syncthreads();
-    tok = pick_token(ProcessedLogit{row, pen, ban, p, bias}, V, ictl, fctl, b, g, true, e, red, am, &tok_sm);
+    tok = pick_token(ProcessedLogit{row, pen, ban, p, bias}, row, V, ictl, fctl, b, g, true, e, red, am, &tok_sm, so);
     if (bias != nullptr) {
       __syncthreads();                           // every read of bias is done
       for (int i = tid; i < tab.n; i += blockDim.x)
         if ((matched[i >> 5] >> (i & 31)) & 1u) bias[last_sm[i]] = 0.f;
     }
   } else {
-    tok = pick_token(RawLogit{row}, V, ictl, fctl, b, gen[b], false, e, red, am, &tok_sm);
+    tok = pick_token(RawLogit{row}, row, V, ictl, fctl, b, gen[b], false, e, red, am, &tok_sm, so);
   }
   if (tid == 0) {
     const int g = gen[b];
@@ -1061,13 +1101,15 @@ verify_attn_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_cons
 // with no candidate left (slot cnt[b], the bonus slot when cnt[b] = K) draw from p_{cnt[b]}.  The same Philox keys.
 // hist (int32 [B, ldh], nullptr in assisted mode): every emitted token is appended at hist[b, pos[b] + 1 ...], so
 // hist[b, :pos[b] + 1] stays the row's history.  draft_pos may be nullptr.
+// score_out / logit_out (generate(output_scores / output_logits), each may be null): [max_new, B, V]; every slot that emits
+// a token writes, at the token's column, its p row's score row (store_scores, with warp_weights' threshold) and raw logits.
 // One CTA per SM (the fp32 vocabulary fills shared memory): asking for it lets ptxas go past 32 registers without spilling.
 __global__ void __launch_bounds__(SAMPLE_THREADS, 1)
 accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_bfloat16* __restrict__ qlog, long long ldq, int V,
               int K, const long long* __restrict__ ictl, const float* __restrict__ fctl, long long* __restrict__ tok,
               int* __restrict__ pos, int* __restrict__ gen, int* __restrict__ finished, long long* __restrict__ out, int ld_out,
               int max_new, int* __restrict__ draft_pos, long long* __restrict__ stats, const int* __restrict__ cnt,
-              int* __restrict__ hist, int ldh) {
+              int* __restrict__ hist, int ldh, float* __restrict__ score_out, __nv_bfloat16* __restrict__ logit_out) {
   extern __shared__ __align__(16) float e[];
   __shared__ float red[33];
   __shared__ ArgMax am[32];
@@ -1085,11 +1127,23 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
   const int g0 = gen[b];
   const int c = cnt != nullptr ? min(max(cnt[b], 0), K) : K;   // candidates of this row
   int n_acc = 0, t_new = 0;
+  bool stopped = false;                          // an accepted proposal before slot i is an EOS id
   for (int i = 0; i <= c; ++i) {
     const __nv_bfloat16* prow = plog + ((long long)i * B + b) * ldp;
     const ArgMax pm = block_argmax(prow, V, am);
     const long long d = i < c ? tok[(long long)(i + 1) * B + b] : -1;
+    // every slot the loop reaches emits one token; it lands in column g0 + i unless an EOS id came first
+    if (i > 0)
+      for (int k = 0; k < (int)min(ictl[4], (long long)MAX_EOS); ++k) stopped |= tok[(long long)i * B + b] == ictl[5 + k];
+    ScoreOut so{nullptr, nullptr};
+    if (!stopped && g0 + i < max_new) {
+      const long long at = ((long long)(g0 + i) * B + b) * V;
+      if (score_out != nullptr) so.score = score_out + at;
+      if (logit_out != nullptr) so.logit = logit_out + at;
+    }
     if (greedy) {
+      if (so.score != nullptr || so.logit != nullptr)
+        store_scores(RawLogit{prow}, prow, V, ictl[0] != 0 ? SCORE_ARGMAX : SCORE_RAW, temp, 0.f, 0u, pm.i, so);
       if (d == pm.i) {
         ++n_acc;
         continue;
@@ -1099,6 +1153,7 @@ accept_kernel(const __nv_bfloat16* __restrict__ plog, long long ldp, const __nv_
     }
     const float mxp = pm.v / temp;
     const uint32_t Tp = warp_weights(prow, V, temp, top_k, top_p, min_p, mxp, e, red);
+    if (so.score != nullptr || so.logit != nullptr) store_scores(RawLogit{prow}, prow, V, SCORE_WARPED, temp, mxp, Tp, 0, so);
     curandStatePhilox4_32_10_t rng;
     curand_init((unsigned long long)ictl[2], (unsigned long long)b, (unsigned long long)g0 * 16ull + 2ull * i, &rng);
     const float u_acc = curand_uniform(&rng), u_draw = curand_uniform(&rng);    // (0, 1]
@@ -1360,6 +1415,46 @@ beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, 
   split_topk(x, in_pen, base, K, am, cand_v + rs * ck + K, cand_i + rs * ck + K);
 }
 
+// generate(output_scores=True): the beam indices [2][rows][max_new] (int32, -1 past a hypothesis' end), double-buffered
+// and gathered through the same sources as run_seq / fin_seq; a candidate's entry at t is its parent's global row.  Out of
+// line, so beam_step keeps its registers.
+__device__ __noinline__ void beam_indices_step(int* __restrict__ run_bi, int* __restrict__ fin_bi, int row0, int nb, int t, long long M,
+                                               long long rows, int V, const int* sel_f, const int* run_src, const int* fin_src) {
+  const int* rsrc = run_bi + (t & 1) * rows * M;
+  int* rdst = run_bi + ((t & 1) ^ 1) * rows * M;
+  const int* fsrc = fin_bi + (t & 1) * rows * M;
+  int* fdst = fin_bi + ((t & 1) ^ 1) * rows * M;
+  const int n = t + 1;
+  for (int i = threadIdx.x; i < nb * n; i += blockDim.x) {
+    const int j = i / n, c = i % n;
+    const int f = sel_f[run_src[j]];
+    rdst[(row0 + j) * M + c] = c < t ? rsrc[(row0 + f / V) * M + c] : row0 + f / V;
+    const int m = fin_src[j];
+    int v;
+    if (m < nb) {
+      v = fsrc[(row0 + m) * M + c];
+    } else {
+      const int fk = sel_f[m - nb];
+      v = c < t ? rsrc[(row0 + fk / V) * M + c] : row0 + fk / V;
+    }
+    fdst[(row0 + j) * M + c] = v;
+  }
+}
+
+// The log-sum-exp of one beam row from its beam_topk partials ml [ns][2], computed by one whole warp (every lane gets it).
+// beam_step and beam_scores both call it, so the scores equal the selection's values bit for bit.
+__device__ __forceinline__ float beam_row_lse(const float* __restrict__ ml, int ns) {
+  const int lane = threadIdx.x & 31;
+  float m = -INFINITY;
+  for (int s = lane; s < ns; s += 32) m = fmaxf(m, ml[2 * s]);
+  m = warp_max(m);
+  float z = 0.f;
+  for (int s = lane; s < ns; s += 32)
+    if (ml[2 * s] > -INFINITY) z += ml[2 * s + 1] * expf(ml[2 * s] - m);
+  z = warp_sum(z);
+  return m + logf(z);
+}
+
 // One CTA per prompt g, whose beams are rows g*nb .. g*nb + nb-1.  One step of HF's beam search (t = tokens generated so
 // far, tstep[g]):
 //   c. score = logit - lse(row) + run_score(row); the K best over all beams (ties: lower beam * V + token), by a K-way
@@ -1384,7 +1479,7 @@ beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ ca
                  int early_stopping, int max_new, float* __restrict__ run_score, float* __restrict__ fin_score, int* __restrict__ fin_flag,
                  int* __restrict__ run_seq, int* __restrict__ fin_seq, int* __restrict__ unsat, int* __restrict__ done,
                  int* __restrict__ tstep, int* __restrict__ pos, long long* __restrict__ ids_next, int* __restrict__ parent,
-                 const int* __restrict__ slot_i, const float2* __restrict__ slot_v) {
+                 const int* __restrict__ slot_i, const float2* __restrict__ slot_v, int* __restrict__ run_bi, int* __restrict__ fin_bi) {
   __shared__ ArgMax am[32];
   __shared__ float lse[MAX_BEAMS];
   __shared__ float sel_v[MAX_KEEP], fcand[MAX_KEEP];
@@ -1403,15 +1498,8 @@ beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ ca
 
   // ---- log-sum-exp of each beam row from the split partials: warp j takes row j
   if (warp < nb) {
-    const float* ml = part_ml + (long long)(row0 + warp) * ns * 2;
-    float m = -INFINITY;
-    for (int s = lane; s < ns; s += 32) m = fmaxf(m, ml[2 * s]);
-    m = warp_max(m);
-    float z = 0.f;
-    for (int s = lane; s < ns; s += 32)
-      if (ml[2 * s] > -INFINITY) z += ml[2 * s + 1] * expf(ml[2 * s] - m);
-    z = warp_sum(z);
-    if (lane == 0) lse[warp] = m + logf(z);
+    const float l = beam_row_lse(part_ml + (long long)(row0 + warp) * ns * 2, ns);
+    if (lane == 0) lse[warp] = l;
   }
   __syncthreads();
 
@@ -1558,6 +1646,7 @@ beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ ca
     }
     fdst[(row0 + j) * M + c] = v;
   }
+  if (run_bi != nullptr) beam_indices_step(run_bi, fin_bi, row0, nb, t, M, rows, V, sel_f, run_src, fin_src);
   if (tid < nb) {
     const int f = sel_f[run_src[tid]];
     run_score[row0 + tid] = new_rs[tid];
@@ -1568,6 +1657,68 @@ beam_step_kernel(const float* __restrict__ part_ml, const float* __restrict__ ca
     fin_flag[row0 + tid] = new_ff[tid];
   }
   if (tid == 0) tstep[g] = t + 1;
+}
+
+// generate(num_beams > 1, output_scores / output_logits): HF's per-step log_probs of every beam row, launched between
+// beam_topk and beam_step.  grid (splits, rows), block 128, split s of row r as in beam_topk.  For a prompt g that is not
+// done, column t = tstep[g] of score_out fp32 [max_new, rows, V] gets, per token, the value beam_step ranks before it adds
+// the running score: z - lse (lse from the partials, as beam_step computes it), + the token's summed sequence bias, then
+// penalise() when the token is in the history, -inf when banned (the same device helpers and bitmaps as beam_topk; z NaN
+// counts as -inf).  logit_out bf16 [max_new, rows, V] gets the raw logits.  Either may be nullptr.
+__global__ void __launch_bounds__(TOPK_THREADS)
+beam_scores_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V, const float* __restrict__ part_ml,
+                   const long long* __restrict__ ictl, const float* __restrict__ fctl, const int* __restrict__ prompt, int ldp,
+                   const int* __restrict__ plens, const int* __restrict__ run_seq, const int* __restrict__ tstep,
+                   const int* __restrict__ done, int nb, int max_new, const int* __restrict__ tab_off,
+                   const float* __restrict__ tab_bias, float* __restrict__ score_out, __nv_bfloat16* __restrict__ logit_out) {
+  __shared__ unsigned pen_sm[TOPK_SPLIT / 32], ban_sm[TOPK_SPLIT / 32], bsd_sm[TOPK_SPLIT / 32], matched[MAX_SEQS / 32];
+  __shared__ float bias_sm[TOPK_SPLIT];
+  __shared__ float lse;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int s = blockIdx.x, r = blockIdx.y, ns = gridDim.x, rows = gridDim.y, tid = threadIdx.x;
+  const int g = r / nb, t = tstep[g], base = s * TOPK_SPLIT;
+  if (done[g] || t >= max_new) return;
+  const __nv_bfloat16* row = logits + (long long)r * ld;
+  const long long at = ((long long)t * rows + r) * V;
+  const bool proc = fctl != nullptr && processors_on(ictl, fctl);
+  for (int i = tid; i < TOPK_SPLIT / 32; i += TOPK_THREADS) pen_sm[i] = ban_sm[i] = bsd_sm[i] = 0u;
+  for (int i = tid; i < MAX_SEQS / 32; i += TOPK_THREADS) matched[i] = 0u;
+  if (tid < 32) {
+    const float l = beam_row_lse(part_ml + (long long)r * ns * 2, ns);
+    if (tid == 0) lse = l;
+  }
+  __syncthreads();
+  const float p = proc ? fctl[2] : 1.f;
+  if (proc) {
+    const SeqTable tab{tab_off, tab_bias, tab_off != nullptr ? (int)min(ictl[CTL_N_SEQ], (long long)MAX_SEQS) : 0};
+    const History h{prompt + (long long)g * ldp, run_seq + ((long long)(t & 1) * rows + r) * max_new, plens[g], plens[g] + t};
+    mark_history(h, base, base + TOPK_SPLIT, p != 1.f, (int)ictl[CTL_NGRAM], t < ictl[CTL_MIN_NEW] || h.L < ictl[CTL_MIN_LEN], ictl,
+                 pen_sm, ban_sm);
+    if (tab.n > 0) mark_sequences(tab, h, base, base + TOPK_SPLIT, ban_sm, bsd_sm, matched);
+    __syncthreads();
+    for (int e = tid; e < tab.n; e += TOPK_THREADS) {
+      const int v = tab.last(e);
+      float sum;
+      if (v >= base && v < base + TOPK_SPLIT && ((matched[e >> 5] >> (e & 31)) & 1u) && seq_bias_sum(tab, matched, nullptr, e, v, sum))
+        bias_sm[v - base] = sum;
+    }
+    __syncthreads();
+  }
+  for (int j = tid; j < TOPK_SPLIT; j += TOPK_THREADS) {
+    const int i = base + j;
+    if (i >= V) break;
+    const __nv_bfloat16 raw = row[i];
+    if (logit_out != nullptr) logit_out[at + i] = raw;
+    if (score_out == nullptr) continue;
+    const float z = __bfloat162float(raw);
+    float v = (z == z ? z : -INFINITY) - lse;
+    const unsigned bit = 1u << (j & 31);
+    if (bsd_sm[j >> 5] & bit) v = __fadd_rn(v, bias_sm[j]);
+    if (pen_sm[j >> 5] & bit) v = penalise(v, p);
+    if (ban_sm[j >> 5] & bit) v = -INFINITY;
+    score_out[at + i] = v;
+  }
 }
 
 // grid (L * 2 * Hkv, B), block 256, dynamic shared memory nb * CH * 64 * 2 bytes.  kv [L][2][rows][Hkv][Smax][64]: CTA
@@ -1855,10 +2006,12 @@ ODB_EXPORT int odb_dec_attn_group_splits(int rows, int ngrp, int Hq, int Hkv, in
 
 // logits [B, ld] bf16; ictl / fctl: see dec::sample_kernel; pos / gen / finished int32 [B]; out int64 [B, max_new];
 // ids_next int64 [B]; hist: nullptr (no logits processors), or int32 [B, ldh] with scratch int32 [B, 2 * ceil(V / 32)].
-// The vocabulary lives in shared memory as fp32: V <= 56000.
+// score_out fp32 / logit_out bf16 [score_cols, B, V] (each may be nullptr): a live row's score row and raw logits at column
+// gen[b] < score_cols (see dec::store_scores).  The vocabulary lives in shared memory as fp32: V <= 56000.
 ODB_EXPORT int odb_dec_sample(const void* logits, long long ld, int V, const void* ictl, const void* fctl, void* pos, void* gen,
                               void* finished, void* out, int max_new, void* ids_next, void* hist, int ldh, void* scratch,
-                              const void* tab_off, const void* tab_bias, void* seq_scratch, int B, cudaStream_t st) {
+                              const void* tab_off, const void* tab_bias, void* seq_scratch, void* score_out, void* logit_out,
+                              int score_cols, int B, cudaStream_t st) {
   if (tab_off != nullptr && (hist == nullptr || tab_bias == nullptr || seq_scratch == nullptr)) return -1;
   const int smem = V * 4;
   if (smem > 224000) return -1;
@@ -1871,7 +2024,7 @@ ODB_EXPORT int odb_dec_sample(const void* logits, long long ld, int V, const voi
   launch_pdl(dec::sample_kernel, dim3(B), dim3(dec::SAMPLE_THREADS), smem, st, (const __nv_bfloat16*)logits, ld, V,
              (const long long*)ictl, (const float*)fctl, (int*)pos, (int*)gen, (int*)finished, (long long*)out, max_new,
              (long long*)ids_next, (int*)hist, ldh, (unsigned*)scratch, (const int*)tab_off, (const float*)tab_bias,
-             (float*)seq_scratch);
+             (float*)seq_scratch, (float*)score_out, (__nv_bfloat16*)logit_out, score_cols);
   ODB_CHECK_LAST();
   return 0;
 }
@@ -1930,10 +2083,12 @@ ODB_EXPORT int odb_dec_verify_attn(const void* q, long long ldq, const void* kc,
 // plog [(K+1)*B, ldp] / qlog [K*B, ldq] bf16 slot-major; tok int64 [(K+1)*B]; ictl / fctl: see dec::sample_kernel; pos / gen /
 // finished / draft_pos int32 [B]; out int64 [B, ld_out]; stats int64 [B, 2].  V <= 56000 (fp32 vocabulary in shared memory).
 // Point-mass mode (prompt lookup): qlog nullptr, cnt int32 [B] candidate counts, hist int32 [B, ldh] (or nullptr), draft_pos
-// may be nullptr.  See dec::accept_kernel.
+// may be nullptr.  score_out fp32 / logit_out bf16 [max_new, B, V] (each may be nullptr): the score row and raw logits of
+// the slot that emitted each token, at its column.  See dec::accept_kernel.
 ODB_EXPORT int odb_dec_accept(const void* plog, long long ldp, const void* qlog, long long ldq, int V, int K, const void* ictl,
                               const void* fctl, void* tok, void* pos, void* gen, void* finished, void* out, int ld_out, int max_new,
-                              void* draft_pos, void* stats, const void* cnt, void* hist, int ldh, int B, cudaStream_t st) {
+                              void* draft_pos, void* stats, const void* cnt, void* hist, int ldh, void* score_out, void* logit_out,
+                              int B, cudaStream_t st) {
   const int smem = V * 4;
   if (smem > 224000 || K < 1 || K > 7 || (qlog == nullptr && cnt == nullptr)) return -1;
   static int attr = 0;
@@ -1944,7 +2099,8 @@ ODB_EXPORT int odb_dec_accept(const void* plog, long long ldp, const void* qlog,
   }
   launch_pdl(dec::accept_kernel, dim3(B), dim3(dec::SAMPLE_THREADS), smem, st, (const __nv_bfloat16*)plog, ldp,
              (const __nv_bfloat16*)qlog, ldq, V, K, (const long long*)ictl, (const float*)fctl, (long long*)tok, (int*)pos, (int*)gen,
-             (int*)finished, (long long*)out, ld_out, max_new, (int*)draft_pos, (long long*)stats, (const int*)cnt, (int*)hist, ldh);
+             (int*)finished, (long long*)out, ld_out, max_new, (int*)draft_pos, (long long*)stats, (const int*)cnt, (int*)hist, ldh,
+             (float*)score_out, (__nv_bfloat16*)logit_out);
   ODB_CHECK_LAST();
   return 0;
 }
@@ -1987,7 +2143,8 @@ ODB_EXPORT int odb_dec_beam_topk(const void* logits, long long ld, int V, int K,
 ODB_EXPORT int odb_dec_beam_step(const void* part_ml, const void* cand_v, const void* cand_i, int V, int nb, int K, int ck,
                                  const void* ictl, const void* fctl, float length_penalty, int early_stopping, int max_new, void* run_score,
                                  void* fin_score, void* fin_flag, void* run_seq, void* fin_seq, void* unsat, void* done, void* tstep,
-                                 void* pos, void* ids_next, void* parent, const void* slot_i, const void* slot_v, int B, cudaStream_t st) {
+                                 void* pos, void* ids_next, void* parent, const void* slot_i, const void* slot_v, void* run_bi, void* fin_bi,
+                                 int B, cudaStream_t st) {
   const int ns = odb::ceil_div(V, dec::TOPK_SPLIT);
   if (nb < 1 || nb > dec::MAX_BEAMS || K < 1 || K > dec::MAX_KEEP || nb * ns > dec::STEP_THREADS || early_stopping < 0 ||
       early_stopping > 2 || max_new < 1 || ck < K || (fctl != nullptr && ck < 2 * K))
@@ -1996,7 +2153,23 @@ ODB_EXPORT int odb_dec_beam_step(const void* part_ml, const void* cand_v, const 
              (const int*)cand_i, ns, V, nb, K, ck, (const long long*)ictl, (const float*)fctl, length_penalty, early_stopping, max_new,
              (float*)run_score,
              (float*)fin_score, (int*)fin_flag, (int*)run_seq, (int*)fin_seq, (int*)unsat, (int*)done, (int*)tstep, (int*)pos,
-             (long long*)ids_next, (int*)parent, (const int*)slot_i, (const float2*)slot_v);
+             (long long*)ids_next, (int*)parent, (const int*)slot_i, (const float2*)slot_v, (int*)run_bi, (int*)fin_bi);
+  ODB_CHECK_LAST();
+  return 0;
+}
+
+// Between beam_topk and beam_step, with its arguments: score_out fp32 / logit_out bf16 [max_new, rows, V] (either may be
+// nullptr).  See dec::beam_scores_kernel.
+ODB_EXPORT int odb_dec_beam_scores(const void* logits, long long ld, int V, const void* part_ml, const void* ictl, const void* fctl,
+                                   const void* prompt, int ldp, const void* plens, const void* run_seq, const void* tstep, const void* done,
+                                   int nb, int max_new, int rows, const void* tab_off, const void* tab_bias, void* score_out,
+                                   void* logit_out, cudaStream_t st) {
+  if (nb < 1 || rows % nb || max_new < 1 || (fctl != nullptr && (prompt == nullptr || plens == nullptr))) return -1;
+  if (tab_off != nullptr && (fctl == nullptr || tab_bias == nullptr)) return -1;
+  launch_pdl(dec::beam_scores_kernel, dim3(odb::ceil_div(V, dec::TOPK_SPLIT), rows), dim3(dec::TOPK_THREADS), 0, st,
+             (const __nv_bfloat16*)logits, ld, V, (const float*)part_ml, (const long long*)ictl, (const float*)fctl, (const int*)prompt,
+             ldp, (const int*)plens, (const int*)run_seq, (const int*)tstep, (const int*)done, nb, max_new, (const int*)tab_off,
+             (const float*)tab_bias, (float*)score_out, (__nv_bfloat16*)logit_out);
   ODB_CHECK_LAST();
   return 0;
 }

@@ -162,6 +162,8 @@ class DecodeState(Rows):
             self.part_o = torch.empty(B, Hq, nch, D, dtype=torch.float32, device=device)
             self.part_ml = torch.empty(B, Hq, nch, 2, dtype=torch.float32, device=device)
         self.table = torch.zeros(B, nch, dtype=torch.int32, device=device) if self.kernels and group > 1 else None
+        self.score_buf: torch.Tensor | None = None   # generate(output_scores / output_logits): see set_outputs
+        self.logit_buf: torch.Tensor | None = None
         self._prefill: Rows | None = None
         self.graph = None
         self.graph_key = None
@@ -188,6 +190,30 @@ class DecodeState(Rows):
                                       no_repeat_ngram_size, min_new_tokens, min_length, min_p, len(entries))
         self.ictl.copy_(ictl)
         self.fctl.copy_(fctl)
+
+
+def set_outputs(holder, rows: int, V: int, max_new: int, scores: bool, logits: bool, pad: int, dtype) -> None:
+    """generate(return_dict_in_generate=True, output_scores / output_logits): holder.score_buf fp32 and holder.logit_buf
+    (the compute dtype) [max_new, rows, V], one [rows, V] row block per generated position, each allocated only when its
+    flag is on (rows * max_new * V * (4 + 2) bytes with both: about 790 MB at 8 rows, 512 tokens and V = 32000) and kept
+    for the next call of the same shape, so its CUDA graphs replay.  Both are filled with the padding row (-inf, 0 at
+    ``pad``) here, outside any graph; the sampler, the acceptance and the beam selection overwrite the columns a live row
+    emits.  A flag that is off frees its buffer."""
+    for attr, on, dt in (("score_buf", scores, torch.float32), ("logit_buf", logits, dtype)):
+        buf = getattr(holder, attr)
+        if not on or (buf is not None and buf.shape != (max_new, rows, V)):
+            setattr(holder, attr, None)
+            buf = None
+        if on:
+            if buf is None:
+                buf = torch.empty(max_new, rows, V, dtype=dt, device=holder.device)
+                setattr(holder, attr, buf)
+            DK.padding_rows(buf, pad)
+
+
+def _out_key(holder) -> tuple:
+    """The score / logit buffers a graph writes (part of every graph key, like the sequence table)."""
+    return tuple(None if b is None else (b.data_ptr(), tuple(b.shape)) for b in (holder.score_buf, holder.logit_buf))
 
 
 def decode_state(model, B: int, Smax: int, fp8_kv: bool = False, group: int = 1) -> DecodeState:
@@ -279,7 +305,7 @@ def _head(model, buf: Rows, delta, logits) -> None:
 def _head_and_sample(model, st: DecodeState, delta) -> None:
     _head(model, st, delta, st.logits)
     DK.sample(st.logits, st.ictl, st.fctl, st.pos, st.gen, st.finished, st.out, st.ids, st.hist, st.proc_scratch, st.seq,
-              st.seq_scratch)
+              st.seq_scratch, st.score_buf, st.logit_buf)
 
 
 # ------------------------------------------------------------------------------------------------ prefill
@@ -373,7 +399,7 @@ def step(model, st: DecodeState, graph: bool | None = None, fp8=None) -> None:
         _step_eager(model, st, fp8)
         return
     key = (model.arena.version, model.arena.shadow.data_ptr(), st.group, st.table.data_ptr() if st.table is not None else None,
-           st.seq is not None, _fp8_key(fp8))
+           st.seq is not None, _out_key(st), _fp8_key(fp8))
     _graphed(st, key, st.device, lambda: _step_eager(model, st, fp8))
 
 
@@ -461,7 +487,7 @@ def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: i
         DK.lookup_propose(tst.hist, tst.pos, tst.finished, tst.ictl, ast.ids, ast.cnt, ast.proposed, ngram)
         _verify(target, tst, ast, fp8)
         DK.accept(ast.plog, None, tst.ictl, tst.fctl, ast.ids, tst.pos, tst.gen, tst.finished, tst.out, max_new, None, ast.stats,
-                  cnt=ast.cnt, hist=tst.hist)
+                  cnt=ast.cnt, hist=tst.hist, score_out=tst.score_buf, logit_out=tst.logit_buf)
         return
     B, Kp, dst = ast.B, ast.K, ast.draft
     for i in range(Kp + 1):
@@ -473,7 +499,8 @@ def _round_eager(target, draft, tst: DecodeState, ast: AssistedState, max_new: i
         _head(draft, dst, delta, q)
         DK.sample(q, dst.ictl, dst.fctl, dst.pos, dst.gen, dst.finished, dst.out, ast.ids[(i + 1) * B:(i + 2) * B])
     _verify(target, tst, ast, fp8)                    # the draft above runs on its own weights
-    DK.accept(ast.plog, ast.qlog, tst.ictl, tst.fctl, ast.ids, tst.pos, tst.gen, tst.finished, tst.out, max_new, dst.pos, ast.stats)
+    DK.accept(ast.plog, ast.qlog, tst.ictl, tst.fctl, ast.ids, tst.pos, tst.gen, tst.finished, tst.out, max_new, dst.pos, ast.stats,
+              score_out=tst.score_buf, logit_out=tst.logit_buf)
 
 
 @torch.no_grad()
@@ -490,7 +517,7 @@ def assisted_round(target, draft, tst: DecodeState, ast: AssistedState, max_new:
         _round_eager(target, draft, tst, ast, max_new, ngram, fp8)
         return
     proposer = (draft.arena.version, draft.arena.shadow.data_ptr()) if draft is not None else ("lookup", ngram)
-    key = (target.arena.version, target.arena.shadow.data_ptr(), *proposer, id(tst), max_new, _fp8_key(fp8))
+    key = (target.arena.version, target.arena.shadow.data_ptr(), *proposer, id(tst), max_new, _out_key(tst), _fp8_key(fp8))
     ast.graph_target = tst                            # id(tst) is in the key: keep tst alive while a graph may read it
     _graphed(ast, key, tst.device, lambda: _round_eager(target, draft, tst, ast, max_new, ngram, fp8))
 
@@ -542,8 +569,10 @@ def _check_lookup(prompt_lookup_num_tokens, max_matching_ngram_size, assistant_m
 
 
 def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int, Kp: int, controls: tuple, pad: int,
-                       eos: list[int], ngram: int = 2, fp8=None, fp8_kv: bool = False, min_p: float = 0.0) -> torch.Tensor:
+                       eos: list[int], ngram: int = 2, fp8=None, fp8_kv: bool = False, min_p: float = 0.0,
+                       outputs: tuple = (False, False)) -> tuple[torch.Tensor, DecodeState]:
     """Assisted generation with ``assistant``, or prompt lookup (n-grams up to ``ngram``) with ``assistant`` None.
+    Returns the new tokens and the target's DecodeState (``outputs``: its score / logit buffers, ``set_outputs``).
     ``fp8_kv``: the target's cache is FP8 (the draft's stays bf16).  ``min_p`` goes to both control blocks: the acceptance
     computes q with the target's, so the draft must draw from the same warped law."""
     B = comp.shape[0]
@@ -553,6 +582,7 @@ def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int
     dst = ast.draft
     do_sample, temperature, top_k, top_p, seed = controls
     tst.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, min_p=min_p)
+    set_outputs(tst, B, model.config.vocab_size, max_new_tokens, *outputs, pad, tst.dtype)
     if dst is not None:
         dst.set_controls(do_sample, temperature, top_k, top_p, seed ^ DRAFT_SEED_XOR, 0, [], min_p=min_p)
     tst.out.fill_(pad)
@@ -568,7 +598,7 @@ def _assisted_generate(model, assistant, comp, lens, P: int, max_new_tokens: int
         if r % ASSISTED_CHECK_EVERY == 0 and bool(tst.finished.all()):
             break
         assisted_round(model, assistant, tst, ast, max_new_tokens, ngram=ngram, fp8=fp8)
-    return tst.out[:, :max_new_tokens].clone()
+    return tst.out[:, :max_new_tokens].clone(), tst
 
 
 # ------------------------------------------------------------------------------------------------ beam search
@@ -579,9 +609,17 @@ MAX_BEAMS = 8
 class GenerateOutput:
     """``generate(..., return_dict_in_generate=True)``: the sequences [B * num_return_sequences, P + max_new_tokens] and,
     with beam search, the fp32 score of each (sum of its log-probabilities / generated_len ** length_penalty; None
-    otherwise, multi-sample generation included)."""
+    otherwise, multi-sample generation included).
+
+    With ``output_scores=True`` / ``output_logits=True``: ``scores`` / ``logits``, tuples of max_new_tokens fp32 tensors
+    [rows, V] (rows: the sequences' rows; beam search: B * num_beams running beams), and with beam search ``beam_indices``
+    (int64 [B * num_return_sequences, max_new_tokens]: the running row that emitted each token, -1 after the hypothesis
+    ends).  None when not asked for."""
     sequences: torch.Tensor
     sequences_scores: torch.Tensor | None = None
+    scores: tuple[torch.Tensor, ...] | None = None
+    logits: tuple[torch.Tensor, ...] | None = None
+    beam_indices: torch.Tensor | None = None
 
 
 class BeamState:
@@ -614,6 +652,9 @@ class BeamState:
             # two lists of K per split: the unpenalised and the penalised tokens (the second one only with the processors on)
             self.cand_v, self.cand_i = f32(rows, nsp, 2 * K), i32(rows, nsp, 2 * K)
         self.slot_i = self.slot_v = None             # the biased tokens of sequence_bias (kernels), with the table
+        self.score_buf = self.logit_buf = None       # output_scores / output_logits (set_outputs), with the beam indices
+        self.run_bi = self.fin_bi = None
+        self.device = self.dec.device
         self.graph = None
         self.graph_key = None
 
@@ -627,15 +668,31 @@ class BeamState:
         self.unsat.fill_(1)
         self.done.zero_()
         self.tstep.zero_()
+        if self.run_bi is not None:
+            self.run_bi.fill_(-1)
+            self.fin_bi.fill_(-1)
         if self.table is not None:
             self.table.copy_(torch.arange(self.table.shape[0], dtype=torch.int32, device=self.table.device)[:, None].expand_as(self.table))
 
-    def results(self, R: int) -> tuple[torch.Tensor, torch.Tensor]:
-        """The R best finished hypotheses of every prompt: tokens int64 [B * R, max_new] and scores fp32 [B * R]."""
+    def set_outputs(self, scores: bool, logits: bool, pad: int) -> None:
+        """The score / logit buffers of ``set_outputs`` over the running rows, and the beam indices with either."""
+        rows, cfg = self.B * self.nb, self.dec.cfg
+        set_outputs(self, rows, cfg.vocab_size, self.max_new, scores, logits, pad, self.dec.dtype)
+        if not (scores or logits):
+            self.run_bi = self.fin_bi = None
+        elif self.run_bi is None:
+            self.run_bi = torch.full((2, rows, self.max_new), -1, dtype=torch.int32, device=self.device)
+            self.fin_bi = torch.full((2, rows, self.max_new), -1, dtype=torch.int32, device=self.device)
+
+    def results(self, R: int) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor | None]:
+        """The R best finished hypotheses of every prompt: tokens int64 [B * R, max_new], scores fp32 [B * R] and, when kept,
+        their beam indices int64 [B * R, max_new] (else None)."""
         B, nb, M = self.B, self.nb, self.max_new
         par = self.tstep.long() & 1                  # each prompt's latest history buffer
-        seq = self.fin_seq.view(2, B, nb, M)[par, torch.arange(B, device=par.device)]
-        return seq[:, :R].reshape(B * R, M).long(), self.fin_score.view(B, nb)[:, :R].reshape(B * R).clone()
+        ar = torch.arange(B, device=par.device)
+        seq = self.fin_seq.view(2, B, nb, M)[par, ar]
+        bi = self.fin_bi.view(2, B, nb, M)[par, ar][:, :R].reshape(B * R, M).long() if self.fin_bi is not None else None
+        return seq[:, :R].reshape(B * R, M).long(), self.fin_score.view(B, nb)[:, :R].reshape(B * R).clone(), bi
 
 
 def beam_state(model, B: int, nb: int, K: int, max_new: int, Smax: int, fp8_kv: bool = False) -> BeamState:
@@ -662,7 +719,7 @@ def beam_select(bs: BeamState, length_penalty: float, early_stopping: int) -> No
     DK.beam_select(st.logits, st.ictl, bs.nb, bs.K, length_penalty, early_stopping, bs.max_new, bs.run_score, bs.fin_score,
                    bs.fin_flag, bs.run_seq, bs.fin_seq, bs.unsat, bs.done, bs.tstep, st.pos, st.ids, bs.parent, bs.part_ml,
                    bs.cand_v, bs.cand_i, fctl=st.fctl, prompt=bs.prompt, plens=bs.plens, table=st.seq, slot_i=bs.slot_i,
-                   slot_v=bs.slot_v)
+                   slot_v=bs.slot_v, score_out=bs.score_buf, logit_out=bs.logit_buf, run_bi=bs.run_bi, fin_bi=bs.fin_bi)
     DK.beam_reorder(st.kv, bs.table, bs.parent, st.pos, bs.nb, inv=st.kv_inv)
 
 
@@ -684,13 +741,14 @@ def beam_step(model, bs: BeamState, length_penalty: float, early_stopping: int, 
         _beam_step_eager(model, bs, length_penalty, early_stopping, fp8)
         return
     key = (model.arena.version, model.arena.shadow.data_ptr(), float(length_penalty), int(early_stopping), bs.dec.seq is not None,
-           _fp8_key(fp8))
+           _out_key(bs), bs.run_bi.data_ptr() if bs.run_bi is not None else None, _fp8_key(fp8))
     _graphed(bs, key, bs.dec.device, lambda: _beam_step_eager(model, bs, length_penalty, early_stopping, fp8))
 
 
 def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R: int, length_penalty: float, early_stopping,
                    pad: int, eos: list[int], processors: tuple = (1.0, 0, 0), fp8=None,
-                   fp8_kv: bool = False, min_length: int = 0, entries: list | None = None) -> tuple[torch.Tensor, torch.Tensor]:
+                   fp8_kv: bool = False, min_length: int = 0, entries: list | None = None,
+                   outputs: tuple = (False, False)) -> tuple[BeamState, tuple]:
     B, Sp = comp.shape
     es = DK.EARLY_STOPPING[early_stopping]
     bs = beam_state(model, B, nb, DK.beams_to_keep(nb, len(eos)), max_new_tokens, Smax, fp8_kv)
@@ -699,6 +757,7 @@ def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R
         rows = bs.B * bs.nb
         bs.slot_i = torch.zeros(rows, DK.MAX_SEQS, dtype=torch.int32, device=bs.dec.device)
         bs.slot_v = torch.zeros(rows, DK.MAX_SEQS, 2, dtype=torch.float32, device=bs.dec.device)
+    bs.set_outputs(*outputs, pad)
     bs.reset(pad)
     bs.prompt[:, :Sp].copy_(comp)
     bs.plens.copy_(lens)
@@ -708,7 +767,7 @@ def _beam_generate(model, comp, lens, Smax: int, max_new_tokens: int, nb: int, R
         if t % FINISHED_CHECK_EVERY == 0 and bool(bs.done.all()):
             break
         beam_step(model, bs, length_penalty, es, fp8=fp8)
-    return bs.results(R)
+    return bs, bs.results(R)
 
 
 def _check_beams(num_beams, num_return_sequences, do_sample: bool, assistant_model, early_stopping, vocab_size: int,
@@ -781,7 +840,7 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
              min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
              max_matching_ngram_size: int | None = None, fp8_weights: bool = False,
              fp8_kv_cache: bool = False, sequence_bias=None, bad_words_ids=None, min_length: int = 0,
-             min_p: float | None = None) -> torch.Tensor | GenerateOutput:
+             min_p: float | None = None, output_scores: bool = False, output_logits: bool = False) -> torch.Tensor | GenerateOutput:
     """See :meth:`LlamaForCausalLM.generate`."""
     cfg, ar = model.config, model.arena
     if ar.param_sharded:
@@ -813,6 +872,10 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     W8.check_flag(fp8_weights)
     if not isinstance(fp8_kv_cache, bool):
         raise ValueError(f"fp8_kv_cache must be a bool, got {fp8_kv_cache!r}")
+    for name, flag in (("output_scores", output_scores), ("output_logits", output_logits)):
+        if not isinstance(flag, bool):
+            raise ValueError(f"{name} must be a bool, got {flag!r}")
+    outputs = (output_scores and return_dict_in_generate, output_logits and return_dict_in_generate)   # as in HF
     dev = ar.device
     ids = input_ids.to(dev)
     if attention_mask is None:
@@ -837,21 +900,22 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
     fp8 = W8.fp8_weights(model) if fp8_weights else None
     if assistant_model is not None or prompt_lookup_num_tokens is not None:
         K = num_assistant_tokens if assistant_model is not None else prompt_lookup_num_tokens
-        new = _assisted_generate(model, assistant_model, comp, lens, P, max_new_tokens, K, (do_sample, temperature, top_k, top_p, seed),
-                                 pad, eos, ngram, fp8, fp8_kv_cache, min_p)
+        new, tst = _assisted_generate(model, assistant_model, comp, lens, P, max_new_tokens, K,
+                                      (do_sample, temperature, top_k, top_p, seed), pad, eos, ngram, fp8, fp8_kv_cache, min_p, outputs)
         out = torch.cat([ids, new], dim=1)
-        return GenerateOutput(out) if return_dict_in_generate else out
+        return GenerateOutput(out, None, *_step_outputs(tst)) if return_dict_in_generate else out
     Smax = min(_round_up(P + max_new_tokens, 128), _round_up(cfg.max_position_embeddings, 128))
     if num_beams > 1:
-        new, scores = _beam_generate(model, comp, lens, Smax, max_new_tokens, num_beams, num_return_sequences, length_penalty,
-                                     early_stopping, pad, eos, processors, fp8, fp8_kv_cache, min_length, entries)
+        bs, (new, scores, bi) = _beam_generate(model, comp, lens, Smax, max_new_tokens, num_beams, num_return_sequences, length_penalty,
+                                               early_stopping, pad, eos, processors, fp8, fp8_kv_cache, min_length, entries, outputs)
         out = torch.cat([ids.repeat_interleave(num_return_sequences, dim=0), new], dim=1)
-        return GenerateOutput(out, scores) if return_dict_in_generate else out
+        return GenerateOutput(out, scores, *_step_outputs(bs), bi) if return_dict_in_generate else out
     n = num_return_sequences
     st = decode_state(model, B * n, Smax, fp8_kv_cache, n)
 
     st.set_controls(do_sample, temperature, top_k, top_p, seed, pad, eos, *processors, min_length=min_length, min_p=min_p,
                     entries=entries)
+    set_outputs(st, B * n, cfg.vocab_size, max_new_tokens, *outputs, pad, st.dtype)
     st.out.fill_(pad)
     prefill(model, st, comp, lens, fp8)
     if n > 1:
@@ -861,4 +925,11 @@ def generate(model, input_ids: torch.Tensor, attention_mask: torch.Tensor | None
             break
         step(model, st, fp8=fp8)
     out = torch.cat([ids, st.out[:, :max_new_tokens].clone()], dim=1)
-    return GenerateOutput(out) if return_dict_in_generate else out
+    return GenerateOutput(out, None, *_step_outputs(st)) if return_dict_in_generate else out
+
+
+def _step_outputs(holder) -> tuple:
+    """(scores, logits) of GenerateOutput from holder's buffers (``set_outputs``): copies, so the resident buffers serve the
+    next call; each entry is one contiguous [rows, V] fp32 step."""
+    return tuple(None if b is None else b.float().unbind(0) if b.dtype != torch.float32 else b.clone().unbind(0)
+                 for b in (holder.score_buf, holder.logit_buf))

@@ -751,7 +751,8 @@ class LlamaForCausalLM(nn.Module):
                  num_return_sequences: int = 1, return_dict_in_generate: bool = False, repetition_penalty: float = 1.0,
                  no_repeat_ngram_size: int = 0, min_new_tokens: int = 0, prompt_lookup_num_tokens: int | None = None,
                  max_matching_ngram_size: int | None = None, fp8_weights: bool = False, fp8_kv_cache: bool = False,
-                 sequence_bias=None, bad_words_ids=None, min_length: int = 0, min_p: float | None = None):
+                 sequence_bias=None, bad_words_ids=None, min_length: int = 0, min_p: float | None = None,
+                 output_scores: bool = False, output_logits: bool = False):
         """KV-cached text generation with HF ``generate`` keyword names.  Returns LongTensor [B, P + max_new_tokens]: the
         prompt as given, then the new tokens.
 
@@ -834,6 +835,23 @@ class LlamaForCausalLM(nn.Module):
         [B * num_return_sequences]: each hypothesis's summed log-probabilities / generated_len ** length_penalty; None
         without beam search).
 
+        ``output_scores=True`` / ``output_logits=True`` (bools; ignored without ``return_dict_in_generate``, as in HF) add
+        ``scores`` / ``logits`` to it: tuples of ``max_new_tokens`` fp32 tensors ``[rows, vocab_size]``, one per generated
+        position, and with beam search ``beam_indices`` (int64 [B * num_return_sequences, max_new_tokens]: the running row
+        ``b * num_beams + j`` that emitted each token of the hypothesis, -1 after it ends).  ``logits`` are the raw logits
+        (the compute dtype's values, exactly).  ``scores`` follow HF per mode: greedy, the processed logits the argmax is
+        taken of (the logits processors applied, bans as -inf); sampling and multi-sample, those divided by ``temperature``
+        with -inf outside the set the token is drawn from (top-k, top-p and min-p; ``top_k=1`` keeps the argmax alone); beam
+        search, the processed log_softmax of every running beam row (B * num_beams rows, in that step's order, without the
+        running score); assisted and prompt lookup decoding, the target's processed and warped row of the slot that
+        emitted each token.  ``compute_transition_scores`` turns them into per-token scores.  One deviation from HF: a
+        column where a row (beam search: a prompt) had already finished holds a padding row, -inf everywhere and 0 at
+        ``pad_token_id``, where HF keeps computing rows for finished sequences; so the tuples always have
+        ``max_new_tokens`` entries and padding scores 0 in ``compute_transition_scores``.  The rows are written by the
+        sm_90a sampler, acceptance and beam kernels into device buffers of rows * max_new_tokens * vocab_size * 6 bytes
+        (about 790 MB at 8 rows, 512 tokens and 32000 ids), kept for the next call of the same shape; with both flags off
+        nothing is allocated or launched for them.  Raises ValueError when either is not a bool.
+
         ``fp8_weights=True`` generates with FP8 weight-only quantisation: at the start of the call the q|k|v, o, gate|up
         and down projections of every decoder layer are quantised to e4m3 with one power-of-two scale per output row
         (ops/fp8w.py); the embedding, the norms and the LM head stay in the compute dtype.  The result is the model with
@@ -865,7 +883,35 @@ class LlamaForCausalLM(nn.Module):
                         no_repeat_ngram_size=no_repeat_ngram_size, min_new_tokens=min_new_tokens,
                         prompt_lookup_num_tokens=prompt_lookup_num_tokens, max_matching_ngram_size=max_matching_ngram_size,
                         fp8_weights=fp8_weights, fp8_kv_cache=fp8_kv_cache, sequence_bias=sequence_bias,
-                        bad_words_ids=bad_words_ids, min_length=min_length, min_p=min_p)
+                        bad_words_ids=bad_words_ids, min_length=min_length, min_p=min_p, output_scores=output_scores,
+                        output_logits=output_logits)
+
+    def compute_transition_scores(self, sequences: torch.Tensor, scores: tuple, beam_indices: torch.Tensor | None = None,
+                                  normalize_logits: bool = False) -> torch.Tensor:
+        """HF's ``compute_transition_scores``: the score of each generated token, [rows, generated length], from
+        ``generate(..., return_dict_in_generate=True, output_scores=True)``'s ``sequences``, ``scores`` and (beam search)
+        ``beam_indices``.  ``normalize_logits`` applies log_softmax to every score row first (per-token log-probabilities
+        of sampled or greedy output).  Positions with a negative beam index score 0, and so do padding rows of finished
+        sequences (their padding token has score 0).  Returns as many columns as the longest hypothesis (beam search) or
+        ``len(scores)``.  The generated tokens are the last ``len(scores)`` columns of ``sequences``, as ``generate``
+        returns them (always ``max_new_tokens`` wide); HF instead counts back from the end of sequences trimmed to the
+        longest hypothesis, which would take the trailing padding here.  Plain torch on the scores' device."""
+        V = self.config.vocab_size
+        if beam_indices is None:
+            beam_indices = torch.arange(scores[0].shape[0], device=sequences.device).view(-1, 1).expand(-1, len(scores))
+        stacked = torch.stack(scores).reshape(len(scores), -1).transpose(0, 1)
+        if normalize_logits:
+            stacked = torch.log_softmax(stacked.reshape(-1, V, stacked.shape[-1]), dim=1).reshape(-1, stacked.shape[-1])
+        mask = beam_indices < 0
+        n = int((~mask).long().sum(-1).max())
+        beam_indices = beam_indices.clone()[:, :n]
+        mask = mask[:, :n]
+        beam_indices[mask] = 0
+        start = sequences.shape[-1] - len(scores)              # the first generated column
+        idx = sequences[:, start:start + n].to(stacked.device) + beam_indices.to(stacked.device) * V
+        out = stacked.gather(0, idx)
+        out[mask.to(out.device)] = 0
+        return out
 
     @torch.no_grad()
     def score(self, input_ids: torch.Tensor, attention_mask: torch.Tensor | None = None, labels: torch.Tensor | None = None,

@@ -47,12 +47,13 @@ _lib.register_optional("odb_dec_attn_chunks", [c_int])
 _lib.register_optional("odb_dec_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_int,
                                         c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_sample", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                          c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p])
+                                          c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                          c_int, c_void_p])
 _lib.register_optional("odb_dec_verify_attn", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int,
                                                c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_accept", [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                          c_int, c_void_p])
+                                          c_void_p, c_void_p, c_int, c_void_p])
 _lib.register_optional("odb_dec_lookup_propose", [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                                   c_int, c_int, c_void_p])
 _lib.register_optional("odb_dec_beam_splits", [c_int])
@@ -61,7 +62,9 @@ _lib.register_optional("odb_dec_beam_topk", [c_void_p, c_ll, c_int, c_int, c_int
                                              c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_beam_step", [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
                                              c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p])
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p])
+_lib.register_optional("odb_dec_beam_scores", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                               c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p])
 _lib.register_optional("odb_dec_beam_reorder", [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                                 c_void_p])
 _lib.register_optional("odb_dec_attn_group", [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p,
@@ -371,7 +374,8 @@ def verify_attention(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, pos: t
 
 def accept(plog: torch.Tensor, qlog: torch.Tensor | None, ictl: torch.Tensor, fctl: torch.Tensor, tok: torch.Tensor, pos: torch.Tensor,
            gen: torch.Tensor, finished: torch.Tensor, out: torch.Tensor, max_new: int, draft_pos: torch.Tensor | None,
-           stats: torch.Tensor, cnt: torch.Tensor | None = None, hist: torch.Tensor | None = None) -> None:
+           stats: torch.Tensor, cnt: torch.Tensor | None = None, hist: torch.Tensor | None = None,
+           score_out: torch.Tensor | None = None, logit_out: torch.Tensor | None = None) -> None:
     """The acceptance step of one assisted round (speculative sampling; Leviathan et al. 2023, Chen et al. 2023).
 
     plog [(K+1)*B, V]: the target's logits, slot-major, slot i predicting the token at pos[b] + i + 1; qlog [K*B, V]: the
@@ -394,7 +398,11 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor | None, ictl: torch.Tensor, fc
     removed and renormalised; with no candidate left (slot cnt[b]) the token is drawn from p_{cnt[b]}.  This is the law of
     drawing from p and keeping the candidate while the draw equals it.  hist (int32 [B, S], or None): every emitted token
     is appended at hist[b, pos[b] + 1 ...] (positions < S), so hist[b, :pos[b] + 1] stays the row's history.  draft_pos
-    may be None."""
+    may be None.
+
+    ``score_out`` fp32 / ``logit_out`` [max_new, B, V], each optional: every emitted token writes, at its column of out,
+    the score row (``score_rows``: greedy the raw values, sampling the warped p row it was accepted or drawn against) and
+    the logits of the slot that produced it."""
     B = pos.shape[0]
     K = plog.shape[0] // B - 1
     V = plog.shape[1]
@@ -404,13 +412,14 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor | None, ictl: torch.Tensor, fc
         assert qlog is None or (qlog.stride(1) == 1 and qlog.shape[0] == K * B)
         assert cnt is None or (cnt.dtype == torch.int32 and cnt.is_contiguous())
         assert hist is None or (hist.dtype == torch.int32 and hist.is_contiguous() and hist.shape[0] == B)
+        assert _check_outputs(score_out, logit_out, B, V) in (0, max_new)
         _lib.check(_lib.cuda_lib().odb_dec_accept(plog.data_ptr(), plog.stride(0), qlog.data_ptr() if qlog is not None else None,
                                                   qlog.stride(0) if qlog is not None else 0, V, K, ictl.data_ptr(), fctl.data_ptr(),
                                                   tok.data_ptr(), pos.data_ptr(), gen.data_ptr(), finished.data_ptr(), out.data_ptr(),
                                                   out.shape[1], max_new, draft_pos.data_ptr() if draft_pos is not None else None,
                                                   stats.data_ptr(), cnt.data_ptr() if cnt is not None else None,
                                                   hist.data_ptr() if hist is not None else None, hist.shape[1] if hist is not None else 0,
-                                                  B, _lib.stream_ptr(plog)), "dec_accept")
+                                                  _ptr(score_out), _ptr(logit_out), B, _lib.stream_ptr(plog)), "dec_accept")
         _lib.count_launch()
         return
     c = ictl.tolist()
@@ -462,6 +471,10 @@ def accept(plog: torch.Tensor, qlog: torch.Tensor | None, ictl: torch.Tensor, fc
             if fin or g >= max_new:
                 break
             out[b, g] = x
+            if score_out is not None:
+                score_out[g, b] = score_rows(p_all[g - g0, b][None], c, fc)[0].to(score_out.device)
+            if logit_out is not None:
+                logit_out[g, b] = plog.view(K + 1, B, V)[g - g0, b]
             if hist is not None and int(pos[b]) + 1 + g - g0 < hist.shape[1]:
                 hist[b, int(pos[b]) + 1 + g - g0] = x
             g += 1
@@ -549,7 +562,8 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
                 ids_next: torch.Tensor, parent: torch.Tensor, part_ml: torch.Tensor | None = None, cand_v: torch.Tensor | None = None,
                 cand_i: torch.Tensor | None = None, fctl: torch.Tensor | None = None, prompt: torch.Tensor | None = None,
                 plens: torch.Tensor | None = None, table: SeqTable | None = None, slot_i: torch.Tensor | None = None,
-                slot_v: torch.Tensor | None = None) -> None:
+                slot_v: torch.Tensor | None = None, score_out: torch.Tensor | None = None, logit_out: torch.Tensor | None = None,
+                run_bi: torch.Tensor | None = None, fin_bi: torch.Tensor | None = None) -> None:
     """One step of deterministic beam search (transformers' ``_beam_search`` with do_sample=False) over logits
     [B * num_beams, V] (row b * num_beams + j: beam j of prompt b).
 
@@ -577,12 +591,18 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
     ``table``: the ``SeqTable`` of sequence_bias / bad_words_ids.  On the kernel path its biased tokens are monotone with
     neither list, so beam_topk writes each row's matched, unbanned biased tokens to slots (slot_i int32 / slot_v fp32
     [rows, MAX_SEQS] / [rows, MAX_SEQS, 2]: token, then raw logit and summed bias) and beam_step scores them exactly and
-    merges them with the lists."""
+    merges them with the lists.
+
+    generate's ``output_scores`` / ``output_logits`` (each optional, for prompts not yet done): ``score_out`` fp32 [max_new,
+    rows, V] takes, at column t, every beam row's processed log-probs (HF's ``log_probs``: the values ranked before the
+    running score is added; the kernel path launches ``beam_scores_kernel`` for them), ``logit_out`` [max_new, rows, V]
+    the logits.  ``run_bi`` / ``fin_bi`` (int32 [2, rows, max_new], -1 where nothing was emitted) are the beam indices of
+    the running and finished hypotheses, kept like run_seq / fin_seq: entry t is the global row whose token t it is."""
     proc = (fctl is not None and prompt is not None and plens is not None)
     if part_ml is None:
         beam_step_reference(logits, ictl, num_beams, K, length_penalty, early_stopping, max_new, run_score, fin_score, fin_flag, run_seq,
                             fin_seq, unsat, done, tstep, pos, ids_next, parent, fctl=fctl if proc else None, prompt=prompt, plens=plens,
-                            table=table)
+                            table=table, score_out=score_out, logit_out=logit_out, run_bi=run_bi, fin_bi=fin_bi)
         return
     rows, V = logits.shape
     ck = cand_v.shape[2]
@@ -597,6 +617,9 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
     if tab:
         assert slot_i.shape == (rows, MAX_SEQS) and slot_i.dtype == torch.int32 and slot_i.is_contiguous()
         assert slot_v.shape == (rows, MAX_SEQS, 2) and slot_v.dtype == torch.float32 and slot_v.is_contiguous()
+    assert _check_outputs(score_out, logit_out, rows, V) in (0, max_new)
+    assert (run_bi is None) == (fin_bi is None) and (run_bi is None or (run_bi.shape == run_seq.shape and run_bi.dtype == torch.int32
+                                                                         and fin_bi.shape == run_seq.shape and fin_bi.dtype == torch.int32))
     st = _lib.stream_ptr(logits)
     fp = fctl.data_ptr() if proc else None
     _lib.check(_lib.cuda_lib().odb_dec_beam_topk(logits.data_ptr(), logits.stride(0), V, K, ck, part_ml.data_ptr(), cand_v.data_ptr(),
@@ -605,12 +628,21 @@ def beam_select(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int, K: int
                                                  tstep.data_ptr(), num_beams, max_new, rows, table.ints.data_ptr() if tab else None,
                                                  table.bias.data_ptr() if tab else None, slot_i.data_ptr() if tab else None,
                                                  slot_v.data_ptr() if tab else None, st), "dec_beam_topk")
+    if score_out is not None or logit_out is not None:
+        _lib.check(_lib.cuda_lib().odb_dec_beam_scores(logits.data_ptr(), logits.stride(0), V, part_ml.data_ptr(), ictl.data_ptr(), fp,
+                                                       prompt.data_ptr() if proc else None, prompt.shape[1] if proc else 0,
+                                                       plens.data_ptr() if proc else None, run_seq.data_ptr(), tstep.data_ptr(),
+                                                       done.data_ptr(), num_beams, max_new, rows, table.ints.data_ptr() if tab else None,
+                                                       table.bias.data_ptr() if tab else None, _ptr(score_out), _ptr(logit_out), st),
+                   "dec_beam_scores")
+        _lib.count_launch()
     _lib.check(_lib.cuda_lib().odb_dec_beam_step(part_ml.data_ptr(), cand_v.data_ptr(), cand_i.data_ptr(), V, num_beams, K, ck,
                                                  ictl.data_ptr(), fp, float(length_penalty), int(early_stopping), max_new,
                                                  run_score.data_ptr(), fin_score.data_ptr(), fin_flag.data_ptr(), run_seq.data_ptr(),
                                                  fin_seq.data_ptr(), unsat.data_ptr(), done.data_ptr(), tstep.data_ptr(), pos.data_ptr(),
                                                  ids_next.data_ptr(), parent.data_ptr(), slot_i.data_ptr() if tab else None,
-                                                 slot_v.data_ptr() if tab else None, rows // num_beams, st), "dec_beam_step")
+                                                 slot_v.data_ptr() if tab else None, _ptr(run_bi), _ptr(fin_bi), rows // num_beams, st),
+               "dec_beam_step")
     _lib.count_launch(2)
 
 
@@ -618,7 +650,9 @@ def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int
                         max_new: int, run_score: torch.Tensor, fin_score: torch.Tensor, fin_flag: torch.Tensor, run_seq: torch.Tensor,
                         fin_seq: torch.Tensor, unsat: torch.Tensor, done: torch.Tensor, tstep: torch.Tensor, pos: torch.Tensor,
                         ids_next: torch.Tensor, parent: torch.Tensor, fctl: torch.Tensor | None = None,
-                        prompt: torch.Tensor | None = None, plens: torch.Tensor | None = None, table: SeqTable | None = None) -> None:
+                        prompt: torch.Tensor | None = None, plens: torch.Tensor | None = None, table: SeqTable | None = None,
+                        score_out: torch.Tensor | None = None, logit_out: torch.Tensor | None = None,
+                        run_bi: torch.Tensor | None = None, fin_bi: torch.Tensor | None = None) -> None:
     """``beam_select`` in PyTorch: transformers' ``_get_top_k_continuations``, ``_get_running_beams_for_next_iteration``,
     ``_update_finished_beams`` and ``_check_early_stop_heuristic`` over [B, num_beams, ...], with stable sorts for the
     tie rule (-inf ties included: the lower beam * V + token).  With fctl / prompt / plens, the logits processors as
@@ -641,6 +675,12 @@ def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int
         logp = process_logits_reference(logp, beam_histories(prompt, plens, run_seq, tstep, nb), plens.long().to(dev).repeat_interleave(nb) + tr,
                                         tr, fc[FCTL_PENALTY], c[CTL_NGRAM], c[CTL_MIN_NEW], c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]],
                                         _table_entries(table, c), c[CTL_MIN_LEN])
+    lr = live.repeat_interleave(nb)
+    col = t.to(dev).repeat_interleave(nb)[lr]
+    if score_out is not None:
+        score_out[col, lr.nonzero()[:, 0]] = logp[lr]
+    if logit_out is not None:
+        logit_out[col, lr.nonzero()[:, 0]] = logits.to(dev)[lr]
     logp = logp.view(B, nb, V) + run_score.view(B, nb, 1)
     idx = top(logp.view(B, nb * V), K)
     vals = logp.view(B, nb * V).gather(1, idx)
@@ -673,6 +713,13 @@ def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int
     cand = torch.where(torch.arange(M, device=dev)[None, None, :] == t[:, None, None], tok[:, :, None].to(cand.dtype), cand)
     new_run = cand.gather(1, rsel[:, :, None].expand(B, nb, M))
     new_fin = torch.cat([fin_all[par, ar], cand], dim=1).gather(1, msel[:, :, None].expand(B, nb, M))
+    if run_bi is not None:                       # the same gathers, with the candidate's global parent row at t
+        rbi, fbi = run_bi.view(2, B, nb, M), fin_bi.view(2, B, nb, M)
+        cbi = rbi[par, ar].gather(1, beam[:, :, None].expand(B, K, M))
+        cbi = torch.where(torch.arange(M, device=dev)[None, None, :] == t[:, None, None], (ar[:, None] * nb + beam)[:, :, None].to(cbi.dtype),
+                          cbi)
+        new_rbi = cbi.gather(1, rsel[:, :, None].expand(B, nb, M))
+        new_fbi = torch.cat([fbi[par, ar], cbi], dim=1).gather(1, msel[:, :, None].expand(B, nb, M))
     # g. early-stop heuristic
     best_len = [max_new if (early_stopping == 2 and length_penalty > 0) else x + 1 for x in ts]
     bden = torch.tensor([float(n ** float(length_penalty)) for n in best_len], dtype=torch.float32, device=dev)
@@ -681,9 +728,11 @@ def beam_step_reference(logits: torch.Tensor, ictl: torch.Tensor, num_beams: int
     new_unsat = (unsat != 0) & (best_possible > worst).any(dim=1)
     new_done = ~new_unsat | ((early_stopping == 1) & new_ff.all(dim=1)) | last[:, 0]
     # write back the prompts that were not done
-    lr = live.repeat_interleave(nb)
     run_all[1 - par[live], ar[live]] = new_run[live]
     fin_all[1 - par[live], ar[live]] = new_fin[live]
+    if run_bi is not None:
+        rbi[1 - par[live], ar[live]] = new_rbi[live]
+        fbi[1 - par[live], ar[live]] = new_fbi[live]
     run_score.copy_(torch.where(lr, new_rs.reshape(-1), run_score))
     fin_score.copy_(torch.where(lr, new_fs.reshape(-1), fin_score))
     fin_flag.copy_(torch.where(lr, new_ff.reshape(-1).to(fin_flag.dtype), fin_flag))
@@ -915,7 +964,8 @@ def process_logits_reference(x: torch.Tensor, histories: torch.Tensor, lens: tor
 
 def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: torch.Tensor, gen: torch.Tensor, finished: torch.Tensor,
            out: torch.Tensor, ids_next: torch.Tensor, hist: torch.Tensor | None = None, scratch: torch.Tensor | None = None,
-           table: SeqTable | None = None, seq_scratch: torch.Tensor | None = None) -> None:
+           table: SeqTable | None = None, seq_scratch: torch.Tensor | None = None, score_out: torch.Tensor | None = None,
+           logit_out: torch.Tensor | None = None) -> None:
     """Pick one token per row of logits [B, V] and write it to out[b, gen[b]] and ids_next[b]; then gen += 1, pos += 1.
 
     Greedy (ictl do_sample = 0, or top_k = 1): argmax, ties to the lowest index.  Sampling: logits / temperature, keep the
@@ -933,7 +983,11 @@ def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: to
     values, which are never rounded back to bf16.  A row whose processed values are all -inf emits token 0 greedily; a
     sampled row with no finite value emits its processed argmax.  The kernel keeps two bitmaps per row in scratch (int32
     [B, 2 * ceil(V / 32)]).  ``table``: the ``SeqTable`` of sequence_bias / bad_words_ids (its first ictl CTL_N_SEQ
-    entries apply); the kernel then needs ``seq_scratch``, fp32 [B, V] of zeros, which it leaves zero."""
+    entries apply); the kernel then needs ``seq_scratch``, fp32 [B, V] of zeros, which it leaves zero.
+
+    ``score_out`` fp32 / ``logit_out`` (the logits' dtype) [M, B, V], each optional (generate's ``output_scores`` /
+    ``output_logits``): a row that is not finished, with gen[b] < M, writes its score row (``score_rows``) and its logits
+    to column gen[b].  Other columns are left alone."""
     B, V = logits.shape
     if logits.is_cuda and logits.dtype == torch.bfloat16 and _lib.has_symbol("odb_dec_sample"):
         assert logits.stride(1) == 1 and V <= MAX_SAMPLE_VOCAB and out.is_contiguous()
@@ -944,13 +998,15 @@ def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: to
         if tab:
             assert seq_scratch is not None and seq_scratch.dtype == torch.float32 and seq_scratch.is_contiguous()
             assert seq_scratch.numel() >= B * V
+        cols = _check_outputs(score_out, logit_out, B, V)
         _lib.check(_lib.cuda_lib().odb_dec_sample(logits.data_ptr(), logits.stride(0), V, ictl.data_ptr(), fctl.data_ptr(), pos.data_ptr(),
                                                   gen.data_ptr(), finished.data_ptr(), out.data_ptr(), out.shape[1],
                                                   ids_next.data_ptr(), hist.data_ptr() if hist is not None else None,
                                                   hist.shape[1] if hist is not None else 0,
                                                   scratch.data_ptr() if hist is not None else None,
                                                   table.ints.data_ptr() if tab else None, table.bias.data_ptr() if tab else None,
-                                                  seq_scratch.data_ptr() if tab else None, B, _lib.stream_ptr(logits)),
+                                                  seq_scratch.data_ptr() if tab else None, _ptr(score_out), _ptr(logit_out), cols,
+                                                  B, _lib.stream_ptr(logits)),
                    "dec_sample")
         _lib.count_launch()
         return
@@ -972,9 +1028,15 @@ def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: to
         else:
             tok = _sample_reference(x, temperature, c[CTL_TOP_K], top_p, c[CTL_SEED], int(gen.min()), min_p)
     fin = finished.bool()
-    tok = torch.where(fin, torch.full_like(tok, c[CTL_PAD]), tok)
     g = gen.long()
     rows = torch.arange(B, device=logits.device)
+    if score_out is not None or logit_out is not None:
+        live = ~fin & (g < (score_out if score_out is not None else logit_out).shape[0])
+        if score_out is not None:
+            score_out[g[live], rows[live]] = score_rows(x, c, fc)[live].to(score_out.device)
+        if logit_out is not None:
+            logit_out[g[live], rows[live]] = logits[live]
+    tok = torch.where(fin, torch.full_like(tok, c[CTL_PAD]), tok)
     inside = g < out.shape[1]
     out[rows[inside], g[inside]] = tok[inside]
     ids_next.copy_(tok)
@@ -986,6 +1048,37 @@ def sample(logits: torch.Tensor, ictl: torch.Tensor, fctl: torch.Tensor, pos: to
     pos.add_(1)
     eos = torch.tensor(c[CTL_EOS:CTL_EOS + c[CTL_N_EOS]], dtype=torch.int64, device=logits.device)
     finished.copy_((fin | torch.isin(tok, eos)).to(finished.dtype))
+
+
+def score_rows(x: torch.Tensor, ictl: list[int], fctl: list[float]) -> torch.Tensor:
+    """HF's score rows of the values x [rows, V] fp32 a sampler or an acceptance picks from (the logits after the logits
+    processors): greedy, x itself; sampling, ``warp_logits`` (x / temperature, -inf outside the kept set); sampling with
+    top_k = 1, x / temperature at the argmax alone (-inf elsewhere)."""
+    if not ictl[CTL_DO_SAMPLE]:
+        return x
+    temperature = fctl[FCTL_TEMPERATURE]
+    if ictl[CTL_TOP_K] == 1:
+        top = x.argmax(dim=-1, keepdim=True)
+        return torch.full_like(x, float("-inf")).scatter(-1, top, x.gather(-1, top) / temperature)
+    return warp_logits(x, temperature, ictl[CTL_TOP_K], fctl[FCTL_TOP_P], fctl[FCTL_MIN_P])
+
+
+def padding_rows(buf: torch.Tensor, pad: int) -> torch.Tensor:
+    """Fills a score or logit buffer [..., V] with the padding row of generate's outputs: -inf everywhere, 0 at ``pad``
+    (a column where a row had already finished)."""
+    buf.fill_(float("-inf"))
+    buf[..., pad] = 0.0
+    return buf
+
+
+def _check_outputs(score_out: torch.Tensor | None, logit_out: torch.Tensor | None, rows: int, V: int) -> int:
+    """The kernels' score / logit buffers: contiguous [M, rows, V], fp32 / bf16, the same M; returns M (0: none)."""
+    cols = 0
+    for t, dt in ((score_out, torch.float32), (logit_out, torch.bfloat16)):
+        if t is not None:
+            assert t.dtype == dt and t.is_contiguous() and t.dim() == 3 and t.shape[1:] == (rows, V) and cols in (0, t.shape[0])
+            cols = t.shape[0]
+    return cols
 
 
 def warp_logits(x: torch.Tensor, temperature: float, top_k: int, top_p: float, min_p: float = 0.0) -> torch.Tensor:

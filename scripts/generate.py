@@ -144,6 +144,8 @@ def main(argv=None) -> None:
     ap.add_argument("--sequence-bias", default=None, help='bias of the last id of each sequence, e.g. "12 13:-2.5;99:1.0"')
     ap.add_argument("--min-length", type=int, default=0, help="EOS is forbidden while prompt + new tokens are shorter (0: off)")
     ap.add_argument("--min-p", type=float, default=None, help="sampling: keep tokens with p >= min_p * p_max (off by default)")
+    ap.add_argument("--print-logprobs", action="store_true",
+                    help="print each generated token with its log-probability (compute_transition_scores, normalize_logits=True)")
     a = ap.parse_args(argv)
     if a.assistant_model is None and a.assistant_checkpoint is not None:
         ap.error("--assistant-checkpoint needs --assistant-model")
@@ -185,8 +187,11 @@ def main(argv=None) -> None:
                          min_new_tokens=a.min_new_tokens, prompt_lookup_num_tokens=a.prompt_lookup_num_tokens,
                          max_matching_ngram_size=a.max_matching_ngram_size, fp8_weights=a.fp8_weights,
                          fp8_kv_cache=a.fp8_kv_cache, bad_words_ids=parse_bad_words(a.bad_words_ids),
-                         sequence_bias=parse_sequence_bias(a.sequence_bias), min_length=a.min_length, min_p=a.min_p)
+                         sequence_bias=parse_sequence_bias(a.sequence_bias), min_length=a.min_length, min_p=a.min_p,
+                         output_scores=a.print_logprobs)
     out = res.sequences.cpu()
+    logprobs = (model.compute_transition_scores(res.sequences, res.scores, res.beam_indices, normalize_logits=True).cpu()
+                if a.print_logprobs else None)
     R = out.shape[0] // len(prompts)
     for i, p in enumerate(prompts):
         for r in range(R):
@@ -194,6 +199,9 @@ def main(argv=None) -> None:
             if res.sequences_scores is not None:
                 print(f"score: {float(res.sequences_scores[i * R + r]):.6f}")
             print("ids:", " ".join(str(t) for t in p + new))
+            if logprobs is not None:                 # beam search: the hypothesis' own tokens, EOS included
+                n = int((res.beam_indices[i * R + r] >= 0).sum()) if res.beam_indices is not None else len(new)
+                print("logprobs:", " ".join(f"{t}:{float(lp):.4f}" for t, lp in zip(new[:n], logprobs[i * R + r, :n].tolist())))
             if tok is not None:
                 print("text:", tok.decode(p + new, skip_special_tokens=True))
     if assistant is not None:
