@@ -38,7 +38,7 @@ _CUDA_SIGS: dict[str, list] = {
     "odb_ce_fwd": [c_void_p, c_void_p, c_int, c_int, c_ll, c_void_p, c_void_p],
     "odb_grad_sqnorm": [c_void_p, c_ll, c_void_p, c_void_p, c_void_p],
     "odb_adamw_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_int, c_void_p,
-                       c_void_p, c_int, c_void_p],
+                       c_void_p, c_void_p, c_int, c_void_p],
     "odb_pseudo_grad": [c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p],
     "odb_nesterov_outer": [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_ll, c_float, c_float, c_int,
                            c_float, c_void_p],

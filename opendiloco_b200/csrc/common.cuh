@@ -129,6 +129,32 @@ __device__ __forceinline__ float block_max(float v, float* sm) {
   return sm[32];
 }
 
+// ---------------------------------------------------------------- AdamW bias corrections (adamw_step, adamw_segments, ZeRO step)
+// hp[5], hp[6] hold 1 - beta^t for the host's step count t = hp[13], computed by the host in double.  A step that a
+// non-finite gradient skipped (GradScaler) is not an update, so the corrections must use t minus the steps skipped so far.
+// That count lives on the device, in two int slots `skipped` (nullable: no skip accounting): a launch reads slot t & 1 and
+// writes slot (t + 1) & 1, which only the next step reads, so readers and the writer never share a slot and the host
+// never has to read the verdict.  After a skip the corrections are recomputed in double from beta = hp[1] + hp[14]
+// (resp. hp[2] + hp[15]): the fp32 slot plus the residual of the host's double.
+constexpr int kHpStep = 13, kHpB1Lo = 14, kHpB2Lo = 15;
+__device__ __forceinline__ void adamw_bias_corrections(const float* hp, const int* skipped, float& bc1, float& bc2) {
+  bc1 = hp[5];
+  bc2 = hp[6];
+  if (skipped == nullptr) return;
+  const int t = (int)hp[kHpStep];
+  const int s = skipped[t & 1];
+  if (s == 0) return;
+  const double b1 = (double)hp[1] + (double)hp[kHpB1Lo], b2 = (double)hp[2] + (double)hp[kHpB2Lo];
+  bc1 = (float)(1.0 - pow(b1, (double)(t - s)));
+  bc2 = (float)(1.0 - pow(b2, (double)(t - s)));
+}
+// one thread of the launch carries the count forward: skipped[(t + 1) & 1] = skipped[t & 1] + (this step skipped)
+__device__ __forceinline__ void adamw_count_skip(const float* hp, int* skipped, bool skip) {
+  if (skipped == nullptr || blockIdx.x != 0 || threadIdx.x != 0) return;
+  const int t = (int)hp[kHpStep];
+  skipped[(t + 1) & 1] = skipped[t & 1] + (skip ? 1 : 0);
+}
+
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // Every kernel of the micro-step raises `launch_dependents` on entry and executes `griddepcontrol.wait` before its first
 // global-memory access; launched with the programmatic-serialization attribute, the NEXT kernel's CTAs are scheduled as soon

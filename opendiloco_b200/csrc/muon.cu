@@ -24,7 +24,8 @@ using namespace odb;
 namespace {
 
 // hp slots shared with adamw_step (optim.cu) + the Muon group's own
-constexpr int HP_LR = 0, HP_B1 = 1, HP_B2 = 2, HP_EPS = 3, HP_WD = 4, HP_BC1 = 5, HP_BC2 = 6, HP_MAXNORM = 7, HP_INVSCALE = 8;
+// (slots 5, 6 and 13-15 are read by adamw_bias_corrections, common.cuh)
+constexpr int HP_LR = 0, HP_B1 = 1, HP_B2 = 2, HP_EPS = 3, HP_WD = 4, HP_MAXNORM = 7, HP_INVSCALE = 8;
 constexpr int HP_MLR = 9, HP_MOM = 10, HP_MWD = 11, HP_NESTEROV = 12;
 constexpr int kTile = 32;
 constexpr int kTableCols = 8;   // matrix table row: flat offset, rows, cols, transposed, chunk0, chunk1, scratch offset, adjust (f32 bits)
@@ -155,12 +156,16 @@ __global__ void __launch_bounds__(256) adamw_segments_kernel(float* __restrict__
                                                              float* __restrict__ v, __nv_bfloat16* __restrict__ shadow,
                                                              const long long* __restrict__ chunks, const float* __restrict__ hp,
                                                              const float* __restrict__ gpart, int n_gpart,
-                                                             const int* __restrict__ found_inf, int zero_grad) {
+                                                             const int* __restrict__ found_inf, int* __restrict__ skipped,
+                                                             int zero_grad) {
   __shared__ float sm[33];
   const float coef = clip_coef(hp, gpart, n_gpart, sm, nullptr, nullptr);
   const bool skip = found_inf != nullptr && *found_inf != 0;
+  adamw_count_skip(hp, skipped, skip);
   const float lr = hp[HP_LR], b1 = hp[HP_B1], b2 = hp[HP_B2], eps = hp[HP_EPS], wd = hp[HP_WD];
-  const float step_size = lr / hp[HP_BC1], sqrt_bc2 = sqrtf(hp[HP_BC2]), decay = 1.f - lr * wd;
+  float bc1, bc2;
+  adamw_bias_corrections(hp, skipped, bc1, bc2);
+  const float step_size = lr / bc1, sqrt_bc2 = sqrtf(bc2), decay = 1.f - lr * wd;
   const long long start = chunks[2 * blockIdx.x], len = chunks[2 * blockIdx.x + 1];
   if (start % 4 == 0 && len % 4 == 0) {               // 16-byte aligned chunk: the float4 body of adamw_step
     for (long long i = start + 4 * threadIdx.x; i < start + len; i += 4 * blockDim.x) {
@@ -246,12 +251,12 @@ ODB_EXPORT int odb_muon_apply(void* p, void* g, void* shadow, const void* table,
 }
 
 ODB_EXPORT int odb_adamw_segments(void* p, void* g, void* m, void* v, void* shadow, const void* chunks, int n_chunks,
-                                  const void* hp, const void* gpart, int n_gpart, const void* found_inf, int zero_grad,
-                                  cudaStream_t st) {
+                                  const void* hp, const void* gpart, int n_gpart, const void* found_inf, void* skipped,
+                                  int zero_grad, cudaStream_t st) {
   if (n_chunks <= 0) return -1;
   adamw_segments_kernel<<<n_chunks, 256, 0, st>>>((float*)p, (float*)g, (float*)m, (float*)v, (__nv_bfloat16*)shadow,
                                                   (const long long*)chunks, (const float*)hp, (const float*)gpart, n_gpart,
-                                                  (const int*)found_inf, zero_grad);
+                                                  (const int*)found_inf, (int*)skipped, zero_grad);
   ODB_CHECK_LAST();
   return 0;
 }

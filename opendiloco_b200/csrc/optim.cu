@@ -42,14 +42,16 @@ __global__ void __launch_bounds__(256) adamw_step_kernel(float* __restrict__ p, 
                                                          __nv_bfloat16* __restrict__ shadow, long long n4,
                                                          const float* __restrict__ hp, const float* __restrict__ partials,
                                                          int n_partials, const int* __restrict__ found_inf,
-                                                         float* __restrict__ out_stats) {
+                                                         int* __restrict__ skipped, float* __restrict__ out_stats) {
   __shared__ float sm[33];
   // every CTA re-reduces the (<= 2048) partials: deterministic, no atomics, no extra launch
   float s = 0.f;
   for (int i = threadIdx.x; i < n_partials; i += blockDim.x) s += partials[i];
   s = block_sum(s, sm);
-  const float lr = hp[0], b1 = hp[1], b2 = hp[2], eps = hp[3], wd = hp[4], bc1 = hp[5], bc2 = hp[6];
+  const float lr = hp[0], b1 = hp[1], b2 = hp[2], eps = hp[3], wd = hp[4];
   const float max_norm = hp[7], inv_scale = hp[8];
+  float bc1, bc2;
+  adamw_bias_corrections(hp, skipped, bc1, bc2);
   const float gnorm = sqrtf(s) * inv_scale;
   float coef = inv_scale;
   float clip = 1.f;
@@ -60,6 +62,7 @@ __global__ void __launch_bounds__(256) adamw_step_kernel(float* __restrict__ p, 
   if (blockIdx.x == 0 && threadIdx.x == 0 && out_stats) { out_stats[0] = gnorm; out_stats[1] = clip; }
   // GradScaler semantics: skip the update (but still zero the grads) when a non-finite gradient was found
   const bool skip = (found_inf != nullptr) && (*found_inf != 0);
+  adamw_count_skip(hp, skipped, skip);
   const float step_size = lr / bc1;
   const float sqrt_bc2 = sqrtf(bc2);
   const float decay = 1.f - lr * wd;
@@ -168,14 +171,14 @@ ODB_EXPORT int odb_grad_sqnorm(const void* g, long long n, void* partials, void*
 }
 
 ODB_EXPORT int odb_adamw_step(void* p, void* g, void* m, void* v, void* shadow, long long n, const void* hp,
-                              const void* partials, int n_partials, const void* found_inf, void* out_stats,
-                              int zero_grad, cudaStream_t st) {
+                              const void* partials, int n_partials, const void* found_inf, void* skipped,
+                              void* out_stats, int zero_grad, cudaStream_t st) {
   if (n % 4) return -1;
   const int grid = flat_grid(n / 4, 256, 8);
 #define ODB_ADAMW(WS, ZG)                                                                                         \
   adamw_step_kernel<WS, ZG><<<grid, 256, 0, st>>>((float*)p, (float*)g, (float*)m, (float*)v, (__nv_bfloat16*)shadow, \
                                                   n / 4, (const float*)hp, (const float*)partials, n_partials,      \
-                                                  (const int*)found_inf, (float*)out_stats)
+                                                  (const int*)found_inf, (int*)skipped, (float*)out_stats)
   if (shadow && zero_grad) ODB_ADAMW(true, true);
   else if (shadow) ODB_ADAMW(true, false);
   else if (zero_grad) ODB_ADAMW(false, true);

@@ -6,7 +6,7 @@
 //   bucket8    : arbitrary sorted borders (quantile codec), binary search in shared memory
 //   lookup dequant (+ optional accumulate) : out (+)= alpha * table[q]   - the reduce stage of the butterfly averages
 //                                            N dequantised parts in fp32 without materialising them
-//   bucket stats: per-code sum and count (shared-memory histogram) -> code book of bucket means
+//   bucket stats: per-code fp32 sum and int32 count (shared-memory histogram) -> code book of bucket means
 #include "common.cuh"
 
 using namespace odb;
@@ -81,18 +81,20 @@ __global__ void __launch_bounds__(256) quant_bucket8_kernel(const float* __restr
 
 // ---------------------------------------------------------------------------------------- code-book statistics
 __global__ void __launch_bounds__(256) bucket_stats_kernel(const float* __restrict__ x, const uint8_t* __restrict__ q,
-                                                           long long n, float* __restrict__ sums, float* __restrict__ counts) {
-  __shared__ float s_sum[256], s_cnt[256];
+                                                           long long n, float* __restrict__ sums, int* __restrict__ counts) {
+  // counts are integers: an fp32 count stops being exact past 2^24 members, which one bucket of a large part can hold
+  __shared__ float s_sum[256];
+  __shared__ int s_cnt[256];
   s_sum[threadIdx.x] = 0.f;
-  s_cnt[threadIdx.x] = 0.f;
+  s_cnt[threadIdx.x] = 0;
   __syncthreads();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const int c = q[i];
     atomicAdd(&s_sum[c], x[i]);
-    atomicAdd(&s_cnt[c], 1.f);
+    atomicAdd(&s_cnt[c], 1);
   }
   __syncthreads();
-  if (s_cnt[threadIdx.x] > 0.f) {
+  if (s_cnt[threadIdx.x] > 0) {
     atomicAdd(&sums[threadIdx.x], s_sum[threadIdx.x]);
     atomicAdd(&counts[threadIdx.x], s_cnt[threadIdx.x]);
   }
@@ -145,7 +147,7 @@ ODB_EXPORT int odb_quant_bucket8(const void* x, void* q, long long n, const void
 }
 ODB_EXPORT int odb_bucket_stats(const void* x, const void* q, long long n, void* sums, void* counts, cudaStream_t st) {
   if (n == 0) return 0;
-  bucket_stats_kernel<<<qgrid(n), 256, 0, st>>>((const float*)x, (const uint8_t*)q, n, (float*)sums, (float*)counts);
+  bucket_stats_kernel<<<qgrid(n), 256, 0, st>>>((const float*)x, (const uint8_t*)q, n, (float*)sums, (int*)counts);
   ODB_CHECK_LAST();
   return 0;
 }

@@ -99,7 +99,8 @@ __global__ void __launch_bounds__(512) zero_step_kernel(float* __restrict__ p, f
                                                         PeerPtrs flags, PeerPtrs xchg, int rank, int world, long long n,
                                                         const float* __restrict__ hp, float* __restrict__ partials,
                                                         float* __restrict__ bcast, int check_inf, int* __restrict__ found_inf,
-                                                        float* __restrict__ out_stats, unsigned seq, int* timeout_flag) {
+                                                        int* __restrict__ skipped, float* __restrict__ out_stats, unsigned seq,
+                                                        int* timeout_flag) {
   cg::grid_group grid = cg::this_grid();
   __shared__ float sm[33];
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -166,8 +167,10 @@ __global__ void __launch_bounds__(512) zero_step_kernel(float* __restrict__ p, f
   if (*reinterpret_cast<volatile int*>(timeout_flag)) return;
 
   // ---------------- phase 2: clip + AdamW on my slab, multicast the bf16 weights, zero the gradient arena
-  const float lr = hp[0], b1 = hp[1], b2 = hp[2], eps = hp[3], wd = hp[4], bc1 = hp[5], bc2 = hp[6];
+  const float lr = hp[0], b1 = hp[1], b2 = hp[2], eps = hp[3], wd = hp[4];
   const float max_norm = hp[7], inv_scale = hp[8];
+  float bc1, bc2;
+  adamw_bias_corrections(hp, skipped, bc1, bc2);
   const float gnorm = sqrtf(ld_volatile_f32(bcast)) * inv_scale;
   float coef = inv_scale, clip = 1.f;
   if (max_norm > 0.f) {
@@ -176,6 +179,7 @@ __global__ void __launch_bounds__(512) zero_step_kernel(float* __restrict__ p, f
   }
   if (blockIdx.x == 0 && threadIdx.x == 0 && out_stats) { out_stats[0] = gnorm; out_stats[1] = clip; }
   const bool skip = check_inf && (ld_volatile_f32(bcast + 1) != 0.f);
+  adamw_count_skip(hp, skipped, skip);
   const float step_size = lr / bc1, sqrt_bc2 = sqrtf(bc2), decay = 1.f - lr * wd;
   // two float4 (= 8 weights = one 16-byte bf16 vector) per thread iteration; the slab is a multiple of 8 elements
   const long long slab8 = slab4 / 2, lo8 = (long long)rank * slab8;
@@ -223,11 +227,12 @@ __global__ void __launch_bounds__(512) zero_step_kernel(float* __restrict__ p, f
 // p / m / v: this rank's slab (n / world elements).  grad_local / grad_mc: the full fp32 gradient arena in its symmetric
 // window and the multicast alias.  shadow: multicast alias of the bf16 compute-weight arena (shadow_mode 1), this rank's
 // bf16 shard (shadow_mode 2, FULL_SHARD) or null (shadow_mode 0: fp32 compute - the caller gathers).  flags / xchg: per-rank symmetric windows (3 * 16 uint32 / 2 * 16 floats), zero-initialised once.
-// partials: >= 2048 floats, bcast: 2 floats (device scratch).  n % (8 * world) == 0.
+// partials: >= 2048 floats, bcast: 2 floats (device scratch).  skipped: the optimizer's int32 [2] skipped-step counter
+// (adamw_bias_corrections, common.cuh).  n % (8 * world) == 0.
 ODB_EXPORT int odb_zero_fused_step(void* p, void* m, void* v, void* grad_local, void* grad_mc, void* shadow_mc, int shadow_mode,
                                    const void* const* flag_ptrs, const void* const* xchg_ptrs, int rank, int world, long long n,
-                                   const void* hp, void* partials, void* bcast, int check_inf, void* found_inf, void* out_stats,
-                                   unsigned seq, void* timeout_flag, cudaStream_t st) {
+                                   const void* hp, void* partials, void* bcast, int check_inf, void* found_inf, void* skipped,
+                                   void* out_stats, unsigned seq, void* timeout_flag, cudaStream_t st) {
   using namespace zero;
   if (world > kMaxPeers || world < 1 || n % (8ll * world) || grad_mc == nullptr) return -1;
   PeerPtrs fp{}, xp{};
@@ -243,8 +248,8 @@ ODB_EXPORT int odb_zero_fused_step(void* p, void* m, void* v, void* grad_local, 
   float* a0 = (float*)p; float* a1 = (float*)m; float* a2 = (float*)v; float* a3 = (float*)grad_local;
   const float* a4 = (const float*)grad_mc; __nv_bfloat16* a5 = (__nv_bfloat16*)shadow_mc;
   const float* a6 = (const float*)hp; float* a7 = (float*)partials; float* a8 = (float*)bcast; int* a9 = (int*)found_inf;
-  float* a10 = (float*)out_stats; int* a11 = (int*)timeout_flag;
-  void* args[] = {&a0, &a1, &a2, &a3, &a4, &a5, &fp, &xp, &rank, &world, &n, &a6, &a7, &a8, &check_inf, &a9, &a10, &seq, &a11};
+  float* a10 = (float*)out_stats; int* a11 = (int*)timeout_flag; int* a12 = (int*)skipped;
+  void* args[] = {&a0, &a1, &a2, &a3, &a4, &a5, &fp, &xp, &rank, &world, &n, &a6, &a7, &a8, &check_inf, &a9, &a12, &a10, &seq, &a11};
   e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(512), args, 0, st);
   return (int)e;
 }

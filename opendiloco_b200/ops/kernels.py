@@ -9,6 +9,7 @@ All ops take pre-allocated outputs where the training engine owns the buffers.
 from __future__ import annotations
 
 import math
+import struct
 
 import torch
 
@@ -323,8 +324,44 @@ def lce_score_finalize(pmax: torch.Tensor, psum: torch.Tensor, pidx: torch.Tenso
 
 # ------------------------------------------------------------------------------------------------ optimizer kernels
 HP_LR, HP_B1, HP_B2, HP_EPS, HP_WD, HP_BC1, HP_BC2, HP_MAXNORM, HP_INVSCALE = range(9)
+HP_STEP, HP_B1_LO, HP_B2_LO = 13, 14, 15       # host step count and the betas' fp32 residuals (skipped-step accounting)
 HP_SIZE = 16
 MAX_PARTIALS = 2048
+
+
+def _f32(x: float) -> float:
+    return struct.unpack("<f", struct.pack("<f", x))[0]
+
+
+def adamw_hp(lr: float, betas: tuple[float, float], eps: float, weight_decay: float, step: int, max_norm: float) -> dict:
+    """The AdamW slots of the device hyper-parameter block for the host's ``step``-th call (1-based).
+
+    The bias corrections are the host's, for ``step``; the kernels redo them for ``step`` minus the steps a non-finite
+    gradient skipped so far (the device counter of ``adamw_step``), from the betas rebuilt as fp32 slot + residual."""
+    b1, b2 = betas
+    return {HP_LR: lr, HP_B1: b1, HP_B2: b2, HP_EPS: eps, HP_WD: weight_decay, HP_BC1: 1.0 - b1 ** step,
+            HP_BC2: 1.0 - b2 ** step, HP_MAXNORM: max_norm, HP_INVSCALE: 1.0, HP_STEP: float(step),
+            HP_B1_LO: b1 - _f32(b1), HP_B2_LO: b2 - _f32(b2)}
+
+
+def bias_corrections(hp: torch.Tensor, skipped: torch.Tensor | None) -> tuple[float, float]:
+    """(1 - beta1^t, 1 - beta2^t) for the t updates actually applied: reference of ``adamw_bias_corrections`` (common.cuh)."""
+    bc1, bc2 = float(hp[HP_BC1]), float(hp[HP_BC2])
+    if skipped is None:
+        return bc1, bc2
+    t = int(hp[HP_STEP])
+    s = int(skipped[t & 1])
+    if s == 0:
+        return bc1, bc2
+    b1, b2 = float(hp[HP_B1]) + float(hp[HP_B1_LO]), float(hp[HP_B2]) + float(hp[HP_B2_LO])
+    return _f32(1.0 - b1 ** (t - s)), _f32(1.0 - b2 ** (t - s))
+
+
+def count_skip(hp: torch.Tensor, skipped: torch.Tensor | None, skip: bool) -> None:
+    """skipped[(t + 1) & 1] = skipped[t & 1] + skip: reference of ``adamw_count_skip`` (common.cuh)."""
+    if skipped is not None:
+        t = int(hp[HP_STEP])
+        skipped[(t + 1) & 1] = skipped[t & 1] + int(skip)
 
 
 def grad_sqnorm(g: torch.Tensor, partials: torch.Tensor, flag: torch.Tensor) -> int:
@@ -345,8 +382,10 @@ def grad_sqnorm(g: torch.Tensor, partials: torch.Tensor, flag: torch.Tensor) -> 
 
 def adamw_step(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tensor, shadow: torch.Tensor | None,
                hp: torch.Tensor, partials: torch.Tensor, n_partials: int, found_inf: torch.Tensor | None,
-               stats: torch.Tensor | None, zero_grad: bool = True) -> None:
+               stats: torch.Tensor | None, zero_grad: bool = True, skipped: torch.Tensor | None = None) -> None:
     """Fused clip + AdamW + bf16 shadow + zero-grad over the flat arena.  hp: fp32 [HP_SIZE] on the same device.
+    ``skipped``: int32 [2] device counter of the steps ``found_inf`` skipped so far (see ``adamw_hp``); None: hp's bias
+    corrections are used as they are.
 
     Math is torch.optim.AdamW's (decoupled decay, lerp'd first moment, bias-corrected): reference inner optimizer
     train_fsdp.py:250 / train_diloco_torch.py:186 ; clipping = clip_grad_norm_(1.0) train_fsdp.py:395.
@@ -355,10 +394,12 @@ def adamw_step(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tenso
     if p.is_cuda:
         assert n % 4 == 0
         _lib.check(_lib.cuda_lib().odb_adamw_step(_p(p), _p(g), _p(m), _p(v), _p(shadow), n, _p(hp), _p(partials), n_partials,
-                                                  _p(found_inf), _p(stats), int(zero_grad), _lib.stream_ptr(p)), "adamw_step")
+                                                  _p(found_inf), _p(skipped), _p(stats), int(zero_grad), _lib.stream_ptr(p)),
+                   "adamw_step")
         _lib.count_launch()
         return
-    lr, b1, b2, eps, wd, bc1, bc2, max_norm, inv_scale = (float(hp[i]) for i in range(9))
+    lr, b1, b2, eps, wd, _, _, max_norm, inv_scale = (float(hp[i]) for i in range(9))
+    bc1, bc2 = bias_corrections(hp, skipped)
     gnorm = math.sqrt(float(partials[:n_partials].sum())) * inv_scale
     coef, clip = inv_scale, 1.0
     if max_norm > 0:
@@ -367,6 +408,7 @@ def adamw_step(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tenso
     if stats is not None:
         stats[0], stats[1] = gnorm, clip
     skip = found_inf is not None and int(found_inf.item()) != 0
+    count_skip(hp, skipped, skip)
     if not skip:
         gr = g * coef
         p.mul_(1 - lr * wd)

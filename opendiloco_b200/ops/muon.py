@@ -27,7 +27,7 @@ _lib.register_optional("odb_muon_prepare", [_v, _v, _v, _i, _v, _v, _i, _v, _v, 
 _lib.register_optional("odb_muon_scale", [_v, _i, _v, _v, _i, _v, _v, _f, _v])
 _lib.register_optional("odb_muon_normalize", [_v, _v, _v, _i, _i, _i, _v, _v, _v, _v])
 _lib.register_optional("odb_muon_apply", [_v, _v, _v, _v, _i, _i, _i, _v, _v, _v, _i, _v])
-_lib.register_optional("odb_adamw_segments", [_v, _v, _v, _v, _v, _v, _i, _v, _v, _i, _v, _i, _v])
+_lib.register_optional("odb_adamw_segments", [_v, _v, _v, _v, _v, _v, _i, _v, _v, _i, _v, _v, _i, _v])
 
 
 def _p(t: torch.Tensor | None) -> int | None:
@@ -144,9 +144,11 @@ def muon_apply(p: torch.Tensor, g: torch.Tensor, shadow: torch.Tensor | None, ta
 
 def adamw_segments(p: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tensor, shadow: torch.Tensor | None,
                    chunks: torch.Tensor, hp: torch.Tensor, gpart: torch.Tensor, n_gpart: int, found_inf: torch.Tensor | None,
-                   zero_grad: bool) -> None:
-    """CUDA: adamw_step's update on the chunks (int64 [n, 2] = flat offset, length) of the flat arena, one launch."""
+                   zero_grad: bool, skipped: torch.Tensor | None = None) -> None:
+    """CUDA: adamw_step's update on the chunks (int64 [n, 2] = flat offset, length) of the flat arena, one launch; ``skipped``
+    is adamw_step's skipped-step counter."""
     _lib.check(_lib.cuda_lib().odb_adamw_segments(_p(p), _p(g), _p(m), _p(v), _p(shadow), _p(chunks), chunks.shape[0], _p(hp),
-                                                  _p(gpart), n_gpart, _p(found_inf), int(zero_grad), _lib.stream_ptr(p)),
+                                                  _p(gpart), n_gpart, _p(found_inf), _p(skipped), int(zero_grad),
+                                                  _lib.stream_ptr(p)),
                "adamw_segments")
     _lib.count_launch()

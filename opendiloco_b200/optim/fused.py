@@ -182,7 +182,11 @@ class FusedAdamW(torch.optim.Optimizer):
         self.exp_avg_sq = torch.zeros(fv.hi - fv.lo, dtype=torch.float32, device=dev)
         self.max_grad_norm = max_grad_norm
         self.zero_grad_in_step = zero_grad_in_step
-        self._step = 0
+        self._step = 0                                                # step() calls, skipped ones included
+        # steps a non-finite gradient skipped so far, counted by the step kernels themselves (two slots, see
+        # adamw_bias_corrections in csrc/common.cuh): the bias corrections follow the updates actually applied, as torch's
+        # AdamW under a GradScaler does, without the host ever reading the verdict
+        self._skipped = torch.zeros(2, dtype=torch.int32, device=dev)
         # per-step scalars travel through a RING of pinned slots, each guarded by an event recorded after its H2D copy: the
         # host may run ahead of the GPU by several steps (only rank 0 reads the loss), and a single slot would be
         # rewritten before the asynchronous copy of an earlier step has read it
@@ -219,9 +223,19 @@ class FusedAdamW(torch.optim.Optimizer):
             self.state[p] = {"step": torch.tensor(float(self._step)), "exp_avg": fv.view_of(self.exp_avg, i),
                              "exp_avg_sq": fv.view_of(self.exp_avg_sq, i)}
 
+    def applied_steps(self) -> int:
+        """Updates actually applied (torch's ``state["step"]``): step() calls minus the skipped ones.  Reads the device."""
+        return self._step - int(self._skipped[(self._step + 1) & 1])
+
+    def restore_step_count(self, step: int) -> None:
+        """Continue from ``step`` applied updates (a checkpoint's count)."""
+        self._step = step
+        self._skipped.zero_()
+
     def state_dict(self):
+        step = self.applied_steps()
         for st in self.state.values():
-            st["step"] = torch.tensor(float(self._step))
+            st["step"] = torch.tensor(float(step))
         return super().state_dict()
 
     def load_state_dict(self, state_dict) -> None:
@@ -241,7 +255,7 @@ class FusedAdamW(torch.optim.Optimizer):
                     fv.view_of(self.exp_avg, i).copy_(st["exp_avg"])
                     fv.view_of(self.exp_avg_sq, i).copy_(st["exp_avg_sq"])
                     step = int(float(st.get("step", 0)))
-        self._step = step
+        self.restore_step_count(step)
         self.state.clear()
         self._init_state_views()
 
@@ -351,7 +365,6 @@ class FusedAdamW(torch.optim.Optimizer):
         fv = self.fv
         g = self.param_groups[0]
         self._step += 1
-        b1, b2 = g["betas"]
         max_norm = self.max_grad_norm
         n_part = 0
         if self._pending is not None:
@@ -361,20 +374,18 @@ class FusedAdamW(torch.optim.Optimizer):
             n_part = -1
         elif (max_norm is not None and max_norm > 0) or _check_inf:
             n_part = self._norm_partials()
-        self._upload_hp({K.HP_LR: g["lr"], K.HP_B1: b1, K.HP_B2: b2, K.HP_EPS: g["eps"], K.HP_WD: g["weight_decay"],
-                         K.HP_BC1: 1.0 - b1 ** self._step, K.HP_BC2: 1.0 - b2 ** self._step,
-                         K.HP_MAXNORM: max_norm if (max_norm is not None and max_norm > 0 and n_part != 0) else 0.0,
-                         K.HP_INVSCALE: 1.0})
+        self._upload_hp(K.adamw_hp(g["lr"], g["betas"], g["eps"], g["weight_decay"], self._step,
+                                   max_norm if (max_norm is not None and max_norm > 0 and n_part != 0) else 0.0))
         if self._inv_scale is not None:           # device-side 1/scale (no host read of the GradScaler's scale)
             self._hp[K.HP_INVSCALE:K.HP_INVSCALE + 1].copy_(self._inv_scale.reshape(1))
             self._inv_scale = None
         if self._zero is not None:
-            self._zero.step(self._hp, _check_inf, self._flag, self.stats)       # gradients are zeroed by the kernel
+            self._zero.step(self._hp, _check_inf, self._flag, self._skipped, self.stats)   # gradients are zeroed by the kernel
             self._grads_synced = False
             return loss
         K.adamw_step(fv.own(fv.flat), fv.own(fv.grad), self.exp_avg, self.exp_avg_sq, fv.own_shadow(), self._hp,
                      self._partials, n_part, self._flag if _check_inf else None, self.stats,
-                     zero_grad=self.zero_grad_in_step and not fv.sharded)
+                     zero_grad=self.zero_grad_in_step and not fv.sharded, skipped=self._skipped)
         fv.gather_compute_weights()
         if self.zero_grad_in_step and fv.sharded:
             fv.grad.zero_()

@@ -144,14 +144,15 @@ class FusedMuon(FusedAdamW):
                                         "exp_avg_sq": fv.view_of(self.exp_avg_sq, i)}
 
     def state_dict(self):
+        step = self.applied_steps()
         for st in self.state.values():
             if "step" in st:
-                st["step"] = torch.tensor(float(self._step))
+                st["step"] = torch.tensor(float(step))
         return torch.optim.Optimizer.state_dict(self)
 
     def load_state_dict(self, state_dict) -> None:
         torch.optim.Optimizer.load_state_dict(self, state_dict)
-        fv, step = self.fv, self._step
+        fv, step = self.fv, self.applied_steps()
         for i in self._muon_idx:
             st = self.state.get(fv.params[i], {})
             if "momentum_buffer" in st:
@@ -162,7 +163,7 @@ class FusedMuon(FusedAdamW):
                 fv.view_of(self.exp_avg, i).copy_(st["exp_avg"])
                 fv.view_of(self.exp_avg_sq, i).copy_(st["exp_avg_sq"])
                 step = int(float(st.get("step", 0)))
-        self._step = step
+        self.restore_step_count(step)
         self.state.clear()
         self._init_state_views()
 
@@ -177,7 +178,6 @@ class FusedMuon(FusedAdamW):
         fv = self.fv
         mg, ag = self.param_groups
         self._step += 1
-        b1, b2 = ag["betas"]
         max_norm = self.max_grad_norm
         n_part = 0
         if self._pending is not None:
@@ -185,11 +185,11 @@ class FusedMuon(FusedAdamW):
             self._pending = None
         elif (max_norm is not None and max_norm > 0) or _check_inf:
             n_part = self._norm_partials()
-        self._upload_hp({K.HP_LR: ag["lr"], K.HP_B1: b1, K.HP_B2: b2, K.HP_EPS: ag["eps"], K.HP_WD: ag["weight_decay"],
-                         K.HP_BC1: 1.0 - b1 ** self._step, K.HP_BC2: 1.0 - b2 ** self._step,
-                         K.HP_MAXNORM: max_norm if (max_norm is not None and max_norm > 0 and n_part != 0) else 0.0,
-                         K.HP_INVSCALE: 1.0, M.HP_MLR: mg["lr"], M.HP_MOM: mg["momentum"], M.HP_MWD: mg["weight_decay"],
-                         M.HP_NESTEROV: float(bool(mg["nesterov"]))})
+        hp = K.adamw_hp(ag["lr"], ag["betas"], ag["eps"], ag["weight_decay"], self._step,
+                        max_norm if (max_norm is not None and max_norm > 0 and n_part != 0) else 0.0)
+        hp.update({M.HP_MLR: mg["lr"], M.HP_MOM: mg["momentum"], M.HP_MWD: mg["weight_decay"],
+                   M.HP_NESTEROV: float(bool(mg["nesterov"]))})
+        self._upload_hp(hp)
         if self._inv_scale is not None:
             self._hp[K.HP_INVSCALE:K.HP_INVSCALE + 1].copy_(self._inv_scale.reshape(1))
             self._inv_scale = None
@@ -202,7 +202,7 @@ class FusedMuon(FusedAdamW):
                 sl = slice(fv.offsets[i], fv.offsets[i] + fv.params[i].numel())
                 K.adamw_step(fv.flat[sl], fv.grad[sl], self.exp_avg[sl], self.exp_avg_sq[sl],
                              None if fv.shadow is None else fv.shadow[sl], self._hp, self._partials, n_part, flag, self.stats,
-                             zero_grad=zero)
+                             zero_grad=zero, skipped=self._skipped)
         self._step_reference(mg, n_part, flag, zero)
         self._grads_synced = False
         return loss
@@ -211,7 +211,7 @@ class FusedMuon(FusedAdamW):
         fv, pl = self.fv, self._plan
         if pl["adamw"] is not None:
             M.adamw_segments(fv.flat, fv.grad, self.exp_avg, self.exp_avg_sq, fv.shadow, pl["adamw"], self._hp, self._partials,
-                             n_part, flag, zero)
+                             n_part, flag, zero, skipped=self._skipped)
         if pl["prep"] is None:
             return
         coeffs, steps, eps, _ = self._ns

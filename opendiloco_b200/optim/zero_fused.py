@@ -19,8 +19,8 @@ from ..utils.logger import get_logger
 
 c_void_p, c_int, c_ll, c_uint = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_uint
 _lib.register_optional("odb_zero_fused_step", [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
-                                              c_int, c_int, c_ll, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_uint,
-                                              c_void_p, c_void_p])
+                                              c_int, c_int, c_ll, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                              c_uint, c_void_p, c_void_p])
 _lib.register_optional("odb_zero_set_timeout_ms", [c_int])
 logger = get_logger()
 MAX_PEERS = 16
@@ -102,7 +102,7 @@ class FusedZeroStep:
             return None
 
     @torch.no_grad()
-    def step(self, hp: torch.Tensor, check_inf: bool, found_inf: torch.Tensor, stats: torch.Tensor) -> None:
+    def step(self, hp: torch.Tensor, check_inf: bool, found_inf: torch.Tensor, skipped: torch.Tensor, stats: torch.Tensor) -> None:
         opt, fv = self.opt, self.opt.fv
         self.poll_timeout(block=False)
         if self.shadow_mode == 1:
@@ -115,8 +115,8 @@ class FusedZeroStep:
         rc = _lib.cuda_lib().odb_zero_fused_step(
             fv.own(fv.flat).data_ptr(), opt.exp_avg.data_ptr(), opt.exp_avg_sq.data_ptr(), fv.grad.data_ptr(), self.grad_mc, sh,
             self.shadow_mode, self._flag_ptrs, self._xchg_ptrs, self.rank, self.world, self.n, hp.data_ptr(),
-            self.partials.data_ptr(), self.bcast.data_ptr(), int(check_inf), found_inf.data_ptr(), stats.data_ptr(), self.seq,
-            self.timeout_flag.data_ptr(), _lib.stream_ptr(fv.flat))
+            self.partials.data_ptr(), self.bcast.data_ptr(), int(check_inf), found_inf.data_ptr(), skipped.data_ptr(),
+            stats.data_ptr(), self.seq, self.timeout_flag.data_ptr(), _lib.stream_ptr(fv.flat))
         _lib.check(rc, "zero_fused_step")
         _lib.count_launch()
         self.seq += 1

@@ -172,13 +172,13 @@ class _Lookup8(Codec):
         x = x.contiguous()
         q = self._codes(x)
         sums = torch.zeros(256, dtype=torch.float32, device=x.device)
-        cnts = torch.zeros(256, dtype=torch.float32, device=x.device)
+        cnts = torch.zeros(256, dtype=torch.int32, device=x.device)          # exact past 2^24 members per bucket
         if x.is_cuda:
             _call("odb_bucket_stats", x.data_ptr(), q.data_ptr(), x.numel(), sums.data_ptr(), cnts.data_ptr(), _lib.stream_ptr(x))
         else:
             qi = q.long()
             sums.index_add_(0, qi, x)
-            cnts.index_add_(0, qi, torch.ones_like(x))
+            cnts.index_add_(0, qi, torch.ones_like(qi, dtype=torch.int32))
         return q, sums / cnts.clamp_min(1.0)
 
     def decompress_into(self, payload, meta, out, alpha=1.0, accumulate=False):
@@ -239,9 +239,16 @@ class BlockwiseQuantization(Codec):
     def meta_size(self, n):
         return n // QBLOCK
 
+    @staticmethod
+    def _check_blocks(n: int) -> None:
+        # one absmax per whole block: a partial block would have no slot for its scale
+        if n % QBLOCK:
+            raise ValueError(f"blockwise8bit works on whole {QBLOCK}-element blocks; got {n} elements")
+
     def compress(self, x):
         x = x.contiguous()
         n = x.numel()
+        self._check_blocks(n)
         q = torch.empty(n, dtype=torch.int8, device=x.device)
         absmax = torch.empty(n // QBLOCK, dtype=torch.float32, device=x.device)
         if x.is_cuda:
@@ -255,6 +262,7 @@ class BlockwiseQuantization(Codec):
 
     def decompress_into(self, payload, meta, out, alpha=1.0, accumulate=False):
         payload = payload.view(torch.int8)
+        self._check_blocks(out.numel())
         if out.is_cuda:
             _call("odb_dequant_blockwise8", payload.data_ptr(), meta.data_ptr(), out.data_ptr(), out.numel(), float(alpha),
                   int(accumulate), _lib.stream_ptr(out))

@@ -152,7 +152,7 @@ def save_checkpoint(checkpoint_path: str, model: torch.nn.Module, optimizer: tor
         if writes:
             shard.update(lo=lo, hi=hi, numel=fv.numel, model=fv.flat[lo:hi].detach().cpu(),
                          exp_avg=inner.exp_avg.detach().cpu(), exp_avg_sq=inner.exp_avg_sq.detach().cpu(),
-                         step=int(inner._step), param_groups=[{k: v for k, v in g.items() if k != "params"} for g in inner.param_groups])
+                         step=inner.applied_steps(), param_groups=[{k: v for k, v in g.items() if k != "params"} for g in inner.param_groups])
             if diloco is not None:
                 sa = diloco.state_averager
                 if hasattr(diloco, "_sync_outer_state"):
@@ -239,7 +239,7 @@ def load_checkpoint(checkpoint_path: str, model: torch.nn.Module, optimizer: tor
         if m is not None:
             inner.exp_avg.copy_(m)
             inner.exp_avg_sq.copy_(v)
-        inner._step = int(first.get("step", 0))
+        inner.restore_step_count(int(first.get("step", 0)))
         # publish the restored weights to the compute copy (and to the worker's other GPUs when sharded)
         arena = getattr(model, "arena", None)
         if fv.sharded:
